@@ -6,19 +6,24 @@ on synthetic 16384x4 clouds, batch 16 per GPU (BASELINE.json configs[1]).
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
     python bench.py --impl reference ...      # the CPU restatement of the same path on the host cores
 
-One JSON line on rank 0.  A "step" is one batch of 16 scenes per GPU.  Every timed region times EXACTLY K steps between
-a barrier + synchronize on both sides (CUDA events, max over ranks) and is REPEATED R >= 3 times so that at least
-~1 s is timed per leg; the line reports the median repeat (and min / max).
+One JSON line on rank 0.  A "step" is one batch of 16 scenes per GPU.  Every timed region times EXACTLY K = --steps
+steps between a barrier + synchronize on both sides (CUDA events, max over ranks).
+
+    --dump-outputs DIR   after the timed steps, writes what the timed paths computed in their last step as float32 .npy
+                         files: features_sample.npy (a fixed, seeded sample of 4096 of the 16384 points of every scene of the
+                         backbone features, all 128 channels), features_sample_idx.npy (the sampled point indices),
+                         rois.npy and roi_scores.npy (the proposals of the RPN stage).  Inputs are seeded, so two builds can
+                         be compared output for output.
 
   value         device-resident throughput: K steps through pointrcnn_b200.pipeline.BatchPipeline with `--inflight`
-                independent batches in flight (one CUDA graph per slot); inputs rotate through a pool larger than L2.
+                independent batches in flight (one CUDA graph per slot); inputs rotate through a pool larger than the 50 MB L2.
   e2e           the whole RPN stage a caller runs (backbone -> fused cls/reg heads -> proposal layer, TEST quotas) from
                 pinned HOST input: H2D of every step's points and D2H of every step's proposals (B,100,7)+(B,100)
                 inside the timed region, handed to a host consumer per batch.
   e2e_features  backbone only, returning the full (B,128,16384) feature tensor to the host (PCIe bound; secondary).
   single_batch  one batch at a time on one stream with an L2 flush in between (per-batch latency view).
   roofline / kernels   per-kernel-family device times from CUDA events on the launching stream (sequential pass).
-  ref_cuda      the reference's own CUDA kernels (oracle/_ref, rebuilt for sm_100a) + stock cuDNN MLP in the reference's
+  ref_cuda      the reference's own CUDA kernels (oracle/_ref, rebuilt for sm_90a) + stock cuDNN MLP in the reference's
                 call order, same process, same inputs: once single-stream, once with the same number of batches in
                 flight; vs_ref_cuda = ours / theirs for both.
   strong_scaling  (N > 1) global batch 16: 16/N scenes per GPU per step, same pipeline.
@@ -211,21 +216,22 @@ class ClockSampler:
 
 
 def peaks():
-    path = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(path):
-        p = json.load(open(path))
-        return dict(hbm=p["hbm_gbs"], bf16=p["bf16_tflops"], bf16_sustained=p.get("bf16_tflops_sustained"), src="measured")
-    return dict(hbm=6650.0, bf16=1590.0, bf16_sustained=1400.0, src="fallback")
+    """H100 SXM data-sheet figures (700 W card): HBM3 bandwidth in GB/s, dense BF16 TFLOP/s.  A card set to a lower power
+    limit reaches less; the line records the card's name and power limit beside the fractions computed from these."""
+    return dict(hbm=3350.0, bf16=989.0, src="H100 SXM data sheet")
 
 
-def ncu_traffic():
-    """DRAM bytes per step of each kernel family, from the committed ncu --set full capture (profiles/r2_traffic.json:
-    dram__bytes_read.sum + dram__bytes_write.sum summed over the family's launches of one step), or {}"""
-    path = os.path.join(ROOT, "profiles", "r2_traffic.json")
+def device_info(dev):
+    import torch
+    info = {"name": torch.cuda.get_device_name(dev), "power_limit_w": None}
     try:
-        return json.load(open(path))
+        import pynvml
+        pynvml.nvmlInit()
+        h = pynvml.nvmlDeviceGetHandleByIndex(torch.cuda.current_device())
+        info["power_limit_w"] = pynvml.nvmlDeviceGetEnforcedPowerLimit(h) / 1000.0
     except Exception:
-        return {}
+        pass
+    return info
 
 
 def run_reference_arm(args):
@@ -254,23 +260,6 @@ def run_reference_arm(args):
     print(json.dumps(line))
 
 
-def tuned_plans():
-    """measured build choice per chain shape (prb_debug_tuned_plans): CTAs per SM of the faster build"""
-    import ctypes
-    from pointrcnn_b200 import _cabi
-    buf = (ctypes.c_int * (18 * 64))()
-    n = _cabi.lib().prb_debug_tuned_plans(buf, 64)
-    kinds_in, kinds_out = ("sa", "fp", "rows"), ("rows", "sa_max", "fp")
-    builds = {2: "2 CTAs x (4 epilogue + 4 gather warps)", 1: "1 CTA x (8 + 8)", 3: "1 CTA x (8 + 12)", 4: "3 CTAs x (4 + 4)"}
-    out = []
-    for i in range(n):
-        r = buf[18 * i:18 * i + 18]
-        out.append({"in": kinds_in[r[0]], "out": kinds_out[r[1]], "nsample": r[3], "k_chunks": r[4], "tiles": r[5],
-                    "np": [x for x in r[6:6 + r[2]]], "build": builds.get(r[9], r[9]),
-                    "measured_us": {builds.get(r[10 + 2 * c], r[10 + 2 * c]): r[11 + 2 * c] for c in range(4) if r[10 + 2 * c]}})
-    return out
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -285,8 +274,8 @@ def main():
     ap.add_argument("--no-eval", action="store_true", help="skip the end-to-end two-stage evaluation leg (BASELINE configs[4])")
     ap.add_argument("--inflight", type=int, default=6, help="independent batches in flight (CUDA streams); 1 = sequential")
     ap.add_argument("--graphs", type=int, default=1, help="1: one CUDA graph per pipeline slot (default), 0: eager launches")
-    ap.add_argument("--min-seconds", type=float, default=1.0, help="each leg repeats its K-step region until this much is timed (>= 3 repeats)")
-    ap.add_argument("--pool", type=int, default=40, help="distinct input batches rotated through (40 x 4.2 MB > 126 MB L2)")
+    ap.add_argument("--pool", type=int, default=40, help="distinct input batches rotated through (40 x 4.2 MB > 50 MB L2)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR", help="write the last timed step's outputs to DIR as .npy")
     ap.add_argument("--profile-out", default=None, help="write the line as indented JSON here as well")
     args = ap.parse_args()
     if args.impl == "reference":
@@ -313,11 +302,11 @@ def main():
 
     net = build_model(dev)
     stage = build_rpn_stage(dev, net)
-    # input pool: distinct batches, together larger than the 126 MB L2, rotated through -> no step finds its input in L2
+    # input pool: distinct batches, together larger than the 50 MB L2, rotated through -> no step finds its input in L2
     P = max(1, args.pool)
     host_pool = [torch.from_numpy(make_scenes((rank * P + i) * BATCH, BATCH)).pin_memory() for i in range(P)]
     dev_pool = [h.to(dev) for h in host_pool]
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 126 MB L2 (sequential pass)
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)   # > 50 MB L2 (sequential pass)
     pipe = BatchPipeline(lambda x: net(x)[1], inflight=F, device=dev, graphs=G)
     pipe_rpn = BatchPipeline(lambda x: stage(x), inflight=F, device=dev, graphs=G)
     pipe_feat = BatchPipeline(lambda x: net(x)[1], inflight=min(F, 3), device=dev, graphs=G)
@@ -326,37 +315,34 @@ def main():
         if world > 1:
             dist.barrier()
 
-    def timed(run_k, min_seconds):
-        """repeat the K-step region (barrier + sync on both sides, CUDA events, max over ranks) until min_seconds are
-        timed, at least 3 times; returns the list of ms per step"""
+    def timed(run_k):
+        """one region of exactly K steps (barrier + sync on both sides, CUDA events, max over ranks); returns ms per step
+        as a one-element list"""
         t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        out, total, offset = [], 0.0, 0
-        while len(out) < 3 or (total < min_seconds and len(out) < 200):
-            barrier(); torch.cuda.synchronize()
-            t0.record()
-            run_k(offset)
-            t1.record()
-            torch.cuda.synchronize(); barrier()
-            ms = max_over_ranks(t0.elapsed_time(t1), device=dev)      # identical on every rank -> same repeat count
-            out.append(ms / K)
-            total += ms * 1e-3
-            offset += K
-        return out
+        barrier(); torch.cuda.synchronize()
+        t0.record()
+        run_k(0)
+        t1.record()
+        torch.cuda.synchronize(); barrier()
+        return [max_over_ranks(t0.elapsed_time(t1), device=dev) / K]
 
     def summary(ms_list):
         return {"n": len(ms_list), "ms_per_step_median": statistics.median(ms_list), "ms_per_step_min": min(ms_list),
                 "ms_per_step_max": max(ms_list), "timed_seconds": sum(ms_list) * K * 1e-3}
 
     checksum = [0.0]
+    last_rois = [None]
 
     def consume_rois(i, res):
         rois, scores = res
         checksum[0] += float(scores.numpy().sum())       # the host consumer: touches every batch's proposals
+        if i == K - 1:
+            last_rois[0] = (rois.clone(), scores.clone())
         return None
 
     sampler = ClockSampler(local) if rank == 0 else None
     with torch.no_grad():
-        net(dev_pool[0])                                                    # first call: the chain plans are measured here
+        net(dev_pool[0])
         torch.cuda.synchronize()
         launches0 = _cabi.launch_count()
         net(dev_pool[0])
@@ -374,18 +360,23 @@ def main():
             sampler.mark()
 
         # ---------------- device-resident throughput: K steps, F independent batches in flight
-        ms_list = timed(lambda off: pipe.run([dev_pool[(off + i) % P] for i in range(K)], keep=False), args.min_seconds)
+        ms_list = timed(lambda off: pipe.run([dev_pool[(off + i) % P] for i in range(K)], keep=False))
         ms = statistics.median(ms_list)
+        if args.dump_outputs and rank == 0:
+            # with graphs the last step's features are still in its slot's static output buffer; eager launches are
+            # deterministic, so the last step's batch is run once more
+            last = pipe.slots[(K - 1) % F].static_out[0] if G else pipe.run([dev_pool[(K - 1) % P]])[0]
+            last_features = last.float().cpu().numpy()
 
         # ---------------- end to end: pinned host input -> H2D -> backbone -> heads -> proposals -> D2H -> host consumer
         e2e_list = timed(lambda off: pipe_rpn.run([host_pool[(off + i) % P] for i in range(K)], to_host=True, consume=consume_rois),
-                         args.min_seconds)
+                         )
         ms_e2e = statistics.median(e2e_list)
         d2h_bytes = BATCH * 100 * 7 * 4 + BATCH * 100 * 4
 
         # ---------------- secondary: the full feature tensor back on the host (PCIe bound)
         feat_list = timed(lambda off: pipe_feat.run([host_pool[(off + i) % P] for i in range(K)], to_host=True,
-                                                    consume=lambda i, r: None), 0.0)
+                                                    consume=lambda i, r: None))
         ms_feat = statistics.median(feat_list)
 
         # ---------------- strong scaling: global batch 16 -> 16/world scenes per GPU per step
@@ -396,7 +387,7 @@ def main():
             pipe_s = BatchPipeline(lambda x: net(x)[1], inflight=Fs, device=dev, graphs=G)
             small = [d[:bs] for d in dev_pool]
             pipe_s.run([small[i % P] for i in range(2 * Fs)], keep=False)
-            s_list = timed(lambda off: pipe_s.run([small[(off + i) % P] for i in range(K)], keep=False), args.min_seconds)
+            s_list = timed(lambda off: pipe_s.run([small[(off + i) % P] for i in range(K)], keep=False))
             ms_s = statistics.median(s_list)
             strong = {"global_batch": BATCH, "scenes_per_gpu_per_step": bs, "batches_in_flight": Fs, "ms_per_step": ms_s,
                       "value": BATCH / (ms_s * 1e-3), "unit": "scenes/s", "repeats": summary(s_list),
@@ -565,7 +556,7 @@ def main():
                     b_.record()
                     torch.cuda.synchronize()
                     ms_ref_pipe = a.elapsed_time(b_) / KP
-                ref_cuda = {"impl": "reference CUDA kernels (oracle/_ref, unmodified sources rebuilt for sm_100a) + torch cuDNN/cuBLAS MLP, "
+                ref_cuda = {"impl": "reference CUDA kernels (oracle/_ref, unmodified sources rebuilt for sm_90a) + torch cuDNN/cuBLAS MLP, "
                                     "reference call order (pointnet2_modules.py:19-55,127-156)",
                             "single_stream": {"ms_per_step": ms_ref_single, "value": BATCH / (ms_ref_single * 1e-3), "steps": KR},
                             "pipelined": {"ms_per_step": ms_ref_pipe, "value": BATCH / (ms_ref_pipe * 1e-3), "steps": KP,
@@ -581,9 +572,8 @@ def main():
 
     pk = peaks()
     sa_flops, fp_flops = mlp_flops_per_scene(net)
-    tf32_peak = pk["bf16"] / 2.0          # tcgen05 kind::tf32 runs at half the bf16 rate; bf16 figure is the measured one
+    tf32_peak = pk["bf16"] / 2.0          # dense TF32 wgmma runs at half the BF16 rate
     fam_ms = {k: v[0] / KS_FAM for k, v in fam.items()}
-    traffic = ncu_traffic()
     kernels = []
     if "sa_mlp" in fam_ms:
         kernels.append({"name": "mlp_chain kernels (SA: gather + SharedMLP + max-pool)", "family": "sa_mlp", "ms_per_step": fam_ms["sa_mlp"],
@@ -610,8 +600,6 @@ def main():
         if "achieved" in k:
             k["frac"] = k["achieved"] / k["peak"]
         k["share"] = k["ms_per_step"] / ms_seq     # share of the sequential (single batch) step
-        if k.get("family") in traffic:
-            k["traffic"] = traffic[k["family"]]
     # Dominant kernel of the PIPELINED step = largest share of SM-time: a chain launch fills the GPU, while the
     # sampling kernels hold one CTA per scene (16 of the SMs) for their duration.
     n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
@@ -623,10 +611,9 @@ def main():
     roofline = None
     if dom:
         roofline = {"kernel": dom["name"], "bound": dom["bound"], "achieved": dom["achieved"], "peak": dom["peak"], "unit": dom["unit"],
-                    "frac": dom["frac"], "traffic": dom.get("traffic"),
-                    "traffic_source": traffic.get("_source") if dom.get("traffic") is not None else None,
+                    "frac": dom["frac"],
                     "algorithmic_flops_per_step": (sa_flops if dom.get("family") == "sa_mlp" else fp_flops) * BATCH if dom["bound"] == "tensor" else None,
-                    "peak_source": pk["src"] + (" bf16/2" if dom["bound"] == "tensor" else " copy"),
+                    "peak_source": pk["src"] + (" bf16/2" if dom["bound"] == "tensor" else " HBM3"),
                     "share_of_step": dom["share"],
                     "share_of_sm_time": dom["sm_time_ms"] / sum(k.get("sm_time_ms", k["ms_per_step"]) for k in kernels if "family" in k),
                     "timing": "CUDA events around the family's launches, sequential pass with L2 flush (single_batch), median of %d steps" % KS}
@@ -650,7 +637,7 @@ def main():
             "dtype": "f32 (tf32 tensor-core MLP, fp32 accumulate)", "data": "synthetic",
             "config": workload_config(world),
             "pipeline": {"batches_in_flight": F, "cuda_graphs": G,
-                         "l2": "inputs rotate through %d distinct batches (%.0f MB > 126 MB L2)" % (P, P * BATCH * POINTS * CHANNELS * 4 / 1e6)},
+                         "l2": "inputs rotate through %d distinct batches (%.0f MB > 50 MB L2)" % (P, P * BATCH * POINTS * CHANNELS * 4 / 1e6)},
             "repeats": summary(ms_list),
             "single_batch": {"ms_per_step": ms_seq, "value": single_val, "unit": "scenes/s", "ms_per_step_planned": ms_plan,
                              "ms_per_step_min_max": [min(ms_seq_all), max(ms_seq_all)],
@@ -664,11 +651,24 @@ def main():
                              "h2d_bytes_per_step": host_pool[0].numel() * 4, "d2h_bytes_per_step": BATCH * 128 * POINTS * 4,
                              "what": "backbone only, full (B,128,16384) features copied to pinned host memory every step (PCIe bound)",
                              "repeats": summary(feat_list)},
-            "gpu_launches": launches, "chain_plans": tuned_plans(), "clocks": clocks, "roofline": roofline, "kernels": kernels, "cpu_baseline": cpu,
+            "device": device_info(dev), "gpu_launches": launches, "clocks": clocks, "roofline": roofline, "kernels": kernels, "cpu_baseline": cpu,
             "ref_cuda": ref_cuda, "vs_ref_cuda": vs_ref, "strong_scaling": strong, "train_step": train, "rcnn_stage": rcnn, "eval_e2e": eval_e2e}
     if args.profile_out:
         json.dump(line, open(args.profile_out, "w"), indent=1)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, last_features, last_rois[0])
     print(json.dumps(line))
+
+
+def dump_outputs(out_dir, features, rois):
+    """features: (B, 128, 16384) of the last timed backbone step; rois: (boxes (B, 100, 7), scores (B, 100)) of the last
+    timed RPN step.  The point sample is fixed (seed 0), so it is the same in every run."""
+    os.makedirs(out_dir, exist_ok=True)
+    idx = np.sort(np.random.default_rng(0).choice(features.shape[2], 4096, replace=False))
+    np.save(os.path.join(out_dir, "features_sample.npy"), np.ascontiguousarray(features[:, :, idx], dtype=np.float32))
+    np.save(os.path.join(out_dir, "features_sample_idx.npy"), idx.astype(np.float64))
+    np.save(os.path.join(out_dir, "rois.npy"), rois[0].numpy().astype(np.float32))
+    np.save(os.path.join(out_dir, "roi_scores.npy"), rois[1].numpy().astype(np.float32))
 
 
 if __name__ == "__main__":

@@ -1,5 +1,5 @@
 /*
- * pointrcnn_b200.h -- C ABI of libpointrcnn_b200.so: B200 (sm_100a) kernels for PointRCNN's
+ * pointrcnn_b200.h -- C ABI of libpointrcnn_b200.so: H100 (sm_90a) kernels for PointRCNN's
  * per-scene point-cloud operator path.
  *
  * This is the drop-in boundary.  Every entry point takes plain device pointers, sizes and a
@@ -51,25 +51,23 @@ typedef struct prb_options {
     int fps_prune;     /* 0: never use the pruned single-CTA kernel; 1: for 4097..16384 points; 2: also 2049..4096 */
     int fps_threads;   /* threads per CTA of the rank kernel; 0 = heuristic */
     int fps_generic;   /* 1: force the generic (reference-shaped) kernel */
-    int mlp_gather;    /* layer-0 row gather of the chain kernel: 0 registers (+tf32 rounding), 1 cp.async.cg, 2 cp.async.ca */
-    int mlp_ng;        /* row groups per CTA (legacy kernel); 0 = heuristic */
-    int mlp_occ;       /* 1: one CTA per SM; 3: the three-CTA build where it applies (narrow SA chains); 0 = plan rule / measured */
+    /* the chain kernel reads only mlp_occ and mlp_sms; the other mlp_* fields have no effect and keep the block's layout */
+    int mlp_gather;
+    int mlp_ng;
+    int mlp_occ;       /* >= 1: at most this many chain-kernel CTAs per SM; 0 = as many as registers and shared memory allow */
     int mlp_sms;       /* size the persistent grid for this many SMs; 0 = all */
-    int mlp_atmem;     /* 1: layers >= 1 take their A operand from tensor memory (legacy kernel) */
-    int mlp_sleepy;    /* bit 0: MMA issuer waits with a suspend hint, bit 1: weight producer does */
-    int mlp_trace;     /* 1: record the phase trace read by prb_debug_mlp_trace */
-    int mlp_pipeline;  /* 1: role-specialised pipelined chain kernel (gather of tile i+1 overlaps tile i); 0: legacy */
-    int mlp_ne, mlp_ngw;   /* pipelined kernel: epilogue (1, 2) / gather (1, 2, 3) warp groups per CTA; 0 = plan rule */
-    int mlp_zs, mlp_nbuf;  /* pipelined kernel: last-layer slice width (multiple of 32) / slice buffers (1 or 2); 0 = plan rule */
-    int mlp_brows;     /* pipelined kernel: rows per weight stage / MMA N (32..256); 0 = 64 */
-    int mlp_pool;      /* SA max-pool over 16..128 samples: 0 = quad tensor-memory layout (2 rows x 4 columns per thread, 3 exchange
-                        * stages), 1 = shuffle butterfly, 2 = CREDUX (warp-wide max per channel), 3 = staged tile for 64/128 samples */
-    int mlp_resident;  /* 1 (default): chains whose weight stages all fit in shared memory load them once per CTA instead of per tile */
-    int mlp_lazy_ns;   /* poll interval (ns) of the run-ahead roles (gather warps, weight producers) in the narrow builds; 0 = 400 */
-    int mlp_fill;      /* 1 (default): single-layer launches with fewer tiles than SMs are dealt to more column groups until every
-                        * SM has one (lower latency, each group re-gathers its rows); 0: only as many groups as tensor memory needs */
-    int mlp_tune;      /* 1 (default): the first eager launch of a chain shape times the two-CTA and the one-CTA build and
-                        * caches the faster one per device and shape; 0: rule-based plan only */
+    int mlp_atmem;
+    int mlp_sleepy;
+    int mlp_trace;
+    int mlp_pipeline;
+    int mlp_ne, mlp_ngw;
+    int mlp_zs, mlp_nbuf;
+    int mlp_brows;
+    int mlp_pool;
+    int mlp_resident;
+    int mlp_lazy_ns;
+    int mlp_fill;
+    int mlp_tune;
     int roipool_exhaustive;  /* 1: roipool3d pass A tests every point against every box (no x-z binning) */
     int roipool_parts;     /* roipool3d pass B: CTAs per box (1..8); 0 = 1 */
     int roipool_stage_kb;  /* roipool3d pass B: shared staging area per CTA in KB (8..160); 0 = 48 */
@@ -154,7 +152,7 @@ PRB_API int prb_transpose_bcn_to_bnc(int b, int c, int n, const float *in, float
  * New natives behind PointnetSAModuleMSG.forward / PointnetFPModule.forward
  * (pointnet2_modules.py:19-55, 127-156).  Eval-mode BatchNorm is folded by the host into a
  * per-channel (scale, shift); every layer is y = relu(scale * (W x) + shift).
- * Weights are passed pre-packed by prb_mlp_pack_weights (tile images in the tcgen05 shared-
+ * Weights are passed pre-packed by prb_mlp_pack_weights (tile images in the wgmma shared-
  * memory operand layout), so the kernel stages them with plain bulk copies. */
 
 typedef struct prb_mlp_desc {
@@ -242,18 +240,6 @@ PRB_API size_t prb_rpn_proposals_workspace_bytes(int b, int post_nms_top_n);
 PRB_API int prb_rpn_proposals(int b, int n, const float *boxes, const float *scores, const long long *order,
                               int distance_based, int pre_nms_top_n, int post_nms_top_n, float nms_thresh, int normal_nms,
                               float *out_boxes, float *out_scores, void *workspace, size_t workspace_bytes, void *stream);
-
-/* diagnostics (PRB_MLP_TRACE=1): clock64 stamps of CTA 0 at the phase boundaries of its first 32 tiles (32 x 16) */
-PRB_API int prb_debug_mlp_trace(long long *dst);
-/* pipelined kernel (prb_options.mlp_trace): cycles CTA 0's roles spent in each class of barrier wait during the last traced
- * launch, 8 x 8 int64 (slot 7 of a row = total cycles of the role's loop): issuer A {x/z_free, a_full, b0_full}, issuer B
- * {z_free, ready, b1_full, fence, mma issue, commit}, weight producer 0 {b0_empty}, producer 1 {b1_empty}, gather warp 0
- * {a_empty}, epilogue warp 0 {r_full, z_full} */
-PRB_API int prb_debug_pipe_trace(long long *dst);
-/* measured plan choices so far: up to max_entries rows of 18 ints {mode_in, mode_out, layers, nsample, K chunks of layer 0,
- * tiles, np0, np1, np2, winning build, then 4 x (candidate build, measured microseconds; 0 = no candidate)}; builds: 2 = two
- * CTAs per SM (4 epilogue + 4 gather warps), 1 = one CTA 8 + 8, 3 = one CTA 8 + 12, 4 = three CTAs 4 + 4; returns the rows */
-PRB_API int prb_debug_tuned_plans(int *dst, int max_entries);
 
 /* --- uniform-grid neighbour search: same results, bit for bit, as prb_ball_query(_msg2) / prb_three_nn
  * (first-nsample-in-index-order and lexicographic (d2, idx) rules kept; queries the grid cannot answer

@@ -1,10 +1,10 @@
 """oracle/bench_ref_cuda.py -- time the reference's own CUDA-extension pipeline on the bench workload (B-ref of
-BASELINE.md): the UNMODIFIED reference kernels (oracle/_ref, rebuilt for sm_100a) called in exactly the order
+BASELINE.md): the UNMODIFIED reference kernels (oracle/_ref, rebuilt for sm_90a) called in exactly the order
 pointnet2_modules.py calls them (ref:pointnet2_modules.py:19-55,127-156, pointnet2_utils.py:241-264), with the
 MLP through stock torch.nn Conv2d/BatchNorm2d/ReLU/max_pool2d (cuDNN/cuBLAS, torch defaults incl. TF32 convs).
 
 TEST / BASELINE INFRASTRUCTURE ONLY.  Usage on the GPU box:  python oracle/bench_ref_cuda.py [--steps 10]
-Prints one JSON line (also the per-family event timings) -- recorded under profiles/.
+Prints one JSON line (also the per-family event timings).
 """
 import argparse
 import json
@@ -48,7 +48,7 @@ def main():
         prof.disable()
     ms = sum(s.elapsed_time(e) for s, e in ev) / a.steps
     fam = {k: v[0] / a.steps for k, v in prof.collect().items()}
-    print(json.dumps({"impl": "reference CUDA-extension build (oracle/_ref kernels, sm_100a, + torch cuDNN MLP)",
+    print(json.dumps({"impl": "reference CUDA-extension build (oracle/_ref kernels, sm_90a, + torch cuDNN MLP)",
                       "metric": "scenes/sec RPN backbone fwd (16384 pts)", "value": bench.BATCH / (ms * 1e-3), "unit": "scenes/s",
                       "ms_per_step": ms, "steps": a.steps, "batch": bench.BATCH, "family_ms_per_step": fam,
                       "cudnn_allow_tf32": torch.backends.cudnn.allow_tf32, "checksum": float(feats.double().mean())}))

@@ -19,7 +19,7 @@
  *   orc_nms_mask / orc_nms  lib/utils/iou3d/src/iou3d_kernel.cu:250-348 + iou3d.cpp:100-116
  *
  * Arithmetic contract: fp32 everywhere the kernels are fp32, with the FMA contraction the
- * reference's sm_100a SASS shows for the three distance kernels (nvcc 12.9 -O2):
+ * reference's SASS shows for the three distance kernels (nvcc 12.9 -O2):
  *     d = fmaf(dz, dz, fmaf(dx, dx, dy * dy))
  * so FPS / ball-query / three_nn indices are bit-exact against the GPU.  This file must be
  * compiled with -ffp-contract=off so that gcc adds no contraction of its own.
@@ -29,7 +29,7 @@
  * GPU and with a stated tolerance / borderline filter against this file.
  *
  * Parity pin: the reference ships no golden vectors (SURVEY.md section 4).  This oracle is
- * pinned against outputs of the reference's own kernels (oracle/_ref, run on a B200 through
+ * pinned against outputs of the reference's own kernels (oracle/_ref, run on a GPU through
  * gpurun) committed under tests/golden/ by oracle/make_golden.py.
  */
 #include <math.h>
@@ -207,7 +207,7 @@ ORC_API void orc_three_nn(int b, int n, int m, const float *unknown, const float
         }
 }
 
-/* out = w0*p0 + w1*p1 + w2*p2 ; reference SASS (sm_100a, nvcc 12.9 -O2): FMUL(w1,p1) -> FFMA(w0,p0,.) -> FFMA(w2,p2,.) */
+/* out = w0*p0 + w1*p1 + w2*p2 ; reference SASS (nvcc 12.9 -O2): FMUL(w1,p1) -> FFMA(w0,p0,.) -> FFMA(w2,p2,.) */
 ORC_API void orc_three_interpolate(int b, int c, int m, int n, const float *points, const int *idx,
                                    const float *weight, float *out) {
 #pragma omp parallel for collapse(2)
@@ -253,7 +253,7 @@ ORC_API int orc_pt_in_box3d(float x, float y, float z, float cx, float bottom_y,
     if ((fabsf(x - cx) > max_dis) || (fabsf(y - cy) > h / 2.0) || (fabsf(z - cz) > max_dis)) return 0;
     cosa = cosf(angle);
     sina = sinf(angle);
-    /* reference SASS (assign_pts_to_box3d, sm_100a, nvcc 12.9 -O2):
+    /* reference SASS (assign_pts_to_box3d, nvcc 12.9 -O2):
      *   x_rot = FFMA(dx, cosa, -(FMUL(dz, sina)));  z_rot = FFMA(dz, cosa, FMUL(dx, sina)) */
     float dx = x - cx, dz = z - cz;
     x_rot = fmaf(dx, cosa, -(dz * sina));

@@ -1,5 +1,5 @@
 """oracle/ref_backbone.py -- the reference's own CUDA-extension pipeline for the RPN backbone (B-ref of BASELINE.md):
-the UNMODIFIED reference kernels (oracle/_ref, rebuilt for sm_100a) called in exactly the order
+the UNMODIFIED reference kernels (oracle/_ref, rebuilt for sm_90a) called in exactly the order
 pointnet2_modules.py calls them (ref:pointnet2_modules.py:19-55,127-156, pointnet2_utils.py:241-264), with the
 MLP through stock torch.nn Conv2d/BatchNorm2d/ReLU/max_pool2d (cuDNN/cuBLAS, torch defaults incl. TF32 convs).
 

@@ -1,4 +1,4 @@
-"""pointrcnn_b200 -- B200 (sm_100a) kernels for PointRCNN's point-cloud operator path.
+"""pointrcnn_b200 -- H100 (sm_90a) kernels for PointRCNN's point-cloud operator path.
 
 Layout
   csrc/      hand-written CUDA + the C ABI (include/pointrcnn_b200.h) -> libpointrcnn_b200.so

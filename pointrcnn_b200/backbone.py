@@ -73,9 +73,8 @@ class Pointnet2MSG(nn.Module):
     # Same kernels, same results as the level-by-level loop.
     def _plannable(self, xyz, features):
         from . import config
-        # opt-in: measured on B200 (profiles/r1_notes.md) the side-stream plan does not pay at batch 16 -- every
-        # kernel except the small FPS levels already fills the GPU, and the persistent MLP CTAs queue behind the
-        # neighbour-search CTAs they share SMs with (7.66 ms planned vs 6.95 ms level-by-level).
+        # opt-in: at batch 16 every kernel except the small FPS levels already fills the GPU, and the persistent MLP
+        # CTAs queue behind the neighbour-search CTAs they share SMs with, so the side-stream plan is not the default.
         if not config.get("enable_plan") or not xyz.is_cuda:
             return False
         if not all(m._can_fuse(xyz, features, None) for m in self.SA_modules):

@@ -1,9 +1,9 @@
-"""Build libpointrcnn_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libpointrcnn_b200.so in-tree with nvcc for sm_90a (H100) (cross-compiles without a GPU).
 
     python -m pointrcnn_b200.build [--force]
 
 One object per csrc/*.cu (compiled in parallel), linked into pointrcnn_b200/libpointrcnn_b200.so.
-The .so is git-ignored but travels to the GPU box with the repo snapshot.
+The .so and the objects are build products (git-ignored).
 """
 import concurrent.futures
 import glob
@@ -16,7 +16,7 @@ CSRC = os.path.join(HERE, "csrc")
 OBJ = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "libpointrcnn_b200.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
          "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden", "--expt-relaxed-constexpr"]
 
 
@@ -52,7 +52,7 @@ def build(force=False, verbose=False):
                     sys.stderr.write(log)
     objs = [os.path.join(OBJ, os.path.basename(s)[:-3] + ".o") for s in srcs]
     if force or jobs or _stale(LIB, objs):
-        cmd = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB] + objs + ["-lcudart"]
+        cmd = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB] + objs + ["-lcudart"]
         r = subprocess.run(cmd, capture_output=True, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n%s" % r.stderr)

@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for libpointrcnn_b200 (sm_100a only).
+// common.cuh -- shared helpers for libpointrcnn_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -6,8 +6,8 @@
 
 #include "../../include/pointrcnn_b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libpointrcnn_b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ != 900)
+#error "libpointrcnn_b200 is written for sm_90a (H100) only"
 #endif
 
 namespace prb {
@@ -46,7 +46,7 @@ inline int check_launch(const char *what) {
 __host__ __device__ constexpr int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
 // The squared distance of the three reference distance kernels, in the contraction order their
-// sm_100a SASS shows (FMUL(dy,dy) -> FFMA(dx,dx,.) -> FFMA(dz,dz,.)).  Explicit intrinsics so the
+// SASS shows (FMUL(dy,dy) -> FFMA(dx,dx,.) -> FFMA(dz,dz,.)).  Explicit intrinsics so the
 // optimiser cannot pick another order: FPS / ball-query / three_nn indices depend on it.
 __device__ __forceinline__ float dist2_ref(float dx, float dy, float dz) {
     return __fmaf_rn(dz, dz, __fmaf_rn(dx, dx, __fmul_rn(dy, dy)));

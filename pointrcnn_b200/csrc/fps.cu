@@ -1,4 +1,4 @@
-// fps.cu -- furthest point sampling for sm_100a: register-resident, cluster-parallel.
+// fps.cu -- furthest point sampling for sm_90a: register-resident, cluster-parallel.
 //
 // Replaces furthest_point_sampling_wrapper (pointnet2_lib/pointnet2/src/sampling.cpp:36-46 ->
 // sampling_gpu.cu:93-253) and the gather_operation that follows it (pointnet2_modules.py:32-35).
@@ -82,8 +82,6 @@ __device__ __forceinline__ void mbar_wait_cluster(uint32_t bar, uint32_t parity)
         : "memory");
 }
 // 16-byte store into a peer CTA's shared memory that completes 16 tx-bytes on the peer's mbarrier.
-// (Measured alternatives, profiles/r1_fps_sweep.json: plain remote stores + tag polling, cluster barriers and
-//  per-warp direct pushes are all 1.3-5x slower per round than st.async + mbarrier complete_tx.)
 __device__ __forceinline__ void st_async_v4(uint32_t remote_addr, uint32_t a, uint32_t b, uint32_t c, uint32_t d, uint32_t remote_bar) {
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v4.b32 [%0], {%1, %2, %3, %4}, [%5];" ::"r"(remote_addr),
                  "r"(a), "r"(b), "r"(c), "r"(d), "r"(remote_bar)
@@ -470,15 +468,19 @@ __global__ void __launch_bounds__(1024, 1) fps_sort_kernel(const FpsParams p, co
     }
 }
 
+// Warp-wide float max / min as one integer REDUX: sm_90 has no float redux, but the map below is an order-preserving
+// involution from floats to signed ints (negative floats get their magnitude bits flipped), so the integer extremum
+// maps back to the float extremum exactly.
+__device__ __forceinline__ int float_order_key(float v) {
+    const int i = __float_as_int(v);
+    return i >= 0 ? i : i ^ 0x7fffffff;
+}
+__device__ __forceinline__ float float_from_order_key(int i) { return __int_as_float(i >= 0 ? i : i ^ 0x7fffffff); }
 __device__ __forceinline__ float redux_max_f32(float v) {
-    float r;
-    asm volatile("redux.sync.max.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(v));
-    return r;
+    return float_from_order_key(__reduce_max_sync(0xffffffffu, float_order_key(v)));
 }
 __device__ __forceinline__ float redux_min_f32(float v) {
-    float r;
-    asm volatile("redux.sync.min.f32 %0, %1, 0xffffffff;" : "=f"(r) : "f"(v));
-    return r;
+    return float_from_order_key(__reduce_min_sync(0xffffffffu, float_order_key(v)));
 }
 
 // one slot of the pruned round: update my point of group (J, warp), refresh the group's cached best.
@@ -496,8 +498,7 @@ __device__ __forceinline__ float redux_min_f32(float v) {
 
 // W warps x NS slots per lane cover the W * NS groups of a scene: <32,16> is the default for 16384 points.  <16,32> (1024
 // threads, prb_options.fps_threads = 1024: fewer touched slots on the busiest warp but a wider CTA arg-max and twice the
-// instruction issue per round) measured SLOWER: 543 vs 490 ns per round at 16 x 16384 -> 4096, 499 vs 425 at 8192 -> 2048
-// (profiles/r2_notes.md): the round is bound by the fixed arg-max / barrier chain, not by the slot updates.
+// instruction issue per round) is an option, not the default: the round is bound by the fixed arg-max / barrier chain.
 template <int NS, int W>
 __global__ void __launch_bounds__(32 * W, 1) fps_pruned_kernel(const FpsParams p, const FpsSorted s) {
     constexpr int NP = W * NS * 32;
@@ -673,8 +674,7 @@ static int fps_run(int b, int n, int m, const float *xyz, float *temp, int *idx,
 
     // configuration: cluster size, threads per CTA, points per thread
     // A cluster of CS CTAs per scene cuts the per-round compute CS-fold; each CTA mirrors only its own slice of the
-    // scene in shared memory (<= 48 KB).  Measured (profiles/r1_fps_sweep.json, n=16384, m=4096, ns per round):
-    // b=2: CS=8 538, CS=4 614, CS=2 803;  b=16: CS=8 691 (CTAs start sharing SMs), CS=4 617;  b=32: CS=4 617.
+    // scene in shared memory (<= 48 KB); large batches use smaller clusters so that CTAs do not start sharing SMs.
     int cs = opts().fps_cluster;
     if (cs != 0 && n_pad < 4096) cs = 1;       // the override is meant for the big levels only
     if (cs == 0) {

@@ -39,8 +39,7 @@ struct GridView {
 // the points grouped by bucket.  A bucket is then a contiguous run of 16-byte nodes: its loads are independent of each
 // other, where a linked list is one L2 round trip per candidate.  Order inside a bucket is arbitrary (atomics) and does
 // not matter: both searches are order independent by construction (see above).
-// MEASURED (profiles/r2_notes.md): slower than the lists at the RPN shapes -- ball query 0.205 vs 0.135 ms, 3-NN 0.417 vs
-// 0.271 ms per batch.  With 2n buckets a bucket holds 0-2 points, so there is no chain to chase, while the single-CTA
+// Not the default at the RPN shapes.  With 2n buckets a bucket holds 0-2 points, so there is no chain to chase, while the single-CTA
 // counting sort adds a serial build per level and the 27 range pairs cost the 3-NN kernel its occupancy.  Kept for dense
 // clouds (many points per cell), where runs do win.
 constexpr int GB_THREADS = 1024;
@@ -516,7 +515,7 @@ __global__ void __launch_bounds__(GR_THREADS) three_nn_grid_kernel(const GridNnP
 // the next cell that can still hold a better neighbour, or processes one node; all lanes run the same short body.  Bucket
 // heads live in shared memory ([cell][thread], conflict free), the visiting order in a 27-entry shared table.  Same cells,
 // same order per query, same pruning and certification: identical results.
-// Result (profiles/r2_notes.md): 3-NN family 0.474 ms against 0.260 ms for the unrolled kernel.  The divergence of the
+// Slower than the unrolled kernel: the divergence of the
 // unrolled form is not waste: with independent thread scheduling the diverged lane groups of a warp cover each other's
 // dependent L2 loads like extra warps would; the convergent loop waits for every load with all 32 lanes.
 __global__ void __launch_bounds__(GR_THREADS) three_nn_walk_kernel(const GridNnParams p) {
@@ -835,7 +834,7 @@ PRB_API int prb_three_nn_grid(int b, int n, int m, const float *unknown, const f
     PRB_CUDA(cudaMemsetAsync(w.overflow, 0, 4, st));
     // cell edge = factor * mean point spacing.  A query is certified only if its third neighbour is closer than one
     // cell, everything else falls back to the exhaustive scan; the centre-out walk skips cells beyond the current
-    // third distance.  Measured on the RPN backbone (profiles/r1_notes.md): 1.3 -> 0.285 ms, 1.6 -> 0.272, 2.0 -> 0.288.
+    // third distance.
     double factor = opts().nn_cell > 0.2f && opts().nn_cell < 50.f ? (double)opts().nn_cell : 1.6;
     grid_cell_from_bbox_kernel<<<b, 256, 0, st>>>(m, known, factor, w.inv_h, w.h);
     if (int rc = check_launch("grid_cell_from_bbox_kernel")) return rc;

@@ -83,7 +83,7 @@ __global__ void __launch_bounds__(NN_THREADS) three_nn_kernel(int n, int m, cons
 }
 
 // out[b,c,j] = w0*p[c,i0] + w1*p[c,i1] + w2*p[c,i2]; one CTA owns a block of channels of one scene
-// (rows stay L1-resident); reference contraction (its sm_100a SASS): FMUL(w1,p1) -> FFMA(w0,p0,.) -> FFMA(w2,p2,.)
+// (rows stay L1-resident); reference contraction (its SASS): FMUL(w1,p1) -> FFMA(w0,p0,.) -> FFMA(w2,p2,.)
 constexpr int TI_THREADS = 256;
 constexpr int TI_CH = 8;
 

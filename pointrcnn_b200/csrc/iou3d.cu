@@ -48,8 +48,8 @@ __global__ void __launch_bounds__(PM_T * PM_T) pair_matrix_kernel(int num_a, con
 // columns l and l+32 of the row and two ballots assemble the 64-bit mask word (the reference and the round-1 kernel: one
 // thread per row, 64 pairs in sequence).  Rotated: the boxes of the tile are precomputed once; axis-aligned: plain extents.
 // RT = 64 for the cheap axis-aligned test.  RT = 8 for the rotated test (one row per warp, two polygon clippings per
-// thread): with 64-row tiles a thread clipped 16 polygons in sequence and N = 1000 gave only 136 busy CTAs -- 176 us at
-// 8.7 % SM utilisation (profiles/r2_ncu_ops_summary.csv); short tiles trade 72 box precomputations per 512 pairs for 8x the CTAs.
+// thread): with 64-row tiles a thread clipped 16 polygons in sequence and N = 1000 gave only 136 busy CTAs;
+// short tiles trade 72 box precomputations per 512 pairs for 8x the CTAs.
 constexpr int NM_THREADS = 256;
 template <bool NORMAL, int RT>
 __global__ void __launch_bounds__(NM_THREADS) nms_mask_kernel(int n, float thresh, const float *__restrict__ boxes,

@@ -62,7 +62,7 @@ __global__ void __launch_bounds__(256) kitti_prepare_kernel(int b, int total, co
     }
     if (counts) {
         // one atomic per warp and scene (a warp nearly always lies inside one scene): per-point atomics on the 2*b counters
-        // serialised the whole kernel (665 us for 960 k points, profiles/r2_ncu_ops_summary.csv)
+        // serialise the whole kernel
         const unsigned grp = __match_any_sync(0xffffffffu, s);
         const unsigned okm = __ballot_sync(0xffffffffu, ok) & grp;
         const unsigned farm = __ballot_sync(0xffffffffu, ok && !near) & grp;

@@ -1,4 +1,4 @@
-// mlp_tc.cu -- the per-group / per-point shared MLP as a tcgen05 (5th-gen tensor core) layer chain.
+// mlp_tc.cu -- the per-group / per-point shared MLP as a wgmma (Hopper tensor core) layer chain.
 //
 // Replaces, for eval-mode forward, everything between the ball query and the next level's features:
 //   grouping_operation x2 + cat + SharedMLP (Conv2d 1x1 -> BN -> ReLU) x L + max_pool2d
@@ -6,22 +6,20 @@
 //   three_interpolate + cat + SharedMLP x L
 //     (pointnet2_modules.py:144-156)
 // The reference materialises every (B,C,npoint,nsample) tensor in HBM between ~10 library kernels per
-// scale; here a 128-row tile never leaves the SM between its gather and its pooled output.
+// scale; here a 64-row tile never leaves the SM between its gather and its pooled output.
 //
-// Structure (one CTA per SM, persistent over 128-row tiles; rows = (centre, sample) pairs or points):
-//   warps 0-3  "row threads": build the A operand of every layer, chunk by chunk (32 K-columns =
-//              one 128-byte swizzle row), into a ring of shared-memory stages:
-//                layer 0  : gathered neighbour features / interpolated + skip features / plain rows
-//                layer l>0: tcgen05.ld of layer l-1's accumulator columns -> scale/shift/ReLU -> tf32
-//              and run the final epilogue (max over nsample / channel-major store).
-//   warp 4     weight producer: one thread streams pre-packed weight tiles (already in the UMMA
-//              K-major SWIZZLE_128B image, see prb_mlp_pack_weights) with cp.async.bulk + mbarrier tx.
-//   warp 5     MMA issuer: one thread issues tcgen05.mma kind::tf32 (M=128, N<=256, K=8) with fp32
-//              accumulators in TMEM; tcgen05.commit releases stages / publishes finished layers.
-// TMEM plan: layer 0 at column 0, layer 1 at the top (512-N1), layer 2 at column 0 again; chains that
-// do not fit (N_l + N_{l+1} > 512) are split into several launches by the host wrapper.
-// Precision: operands are rounded to TF32 (cvt.rna), products accumulate in fp32 -- the same contract
-// as the reference's cuDNN convolutions under torch's default allow_tf32=True (SURVEY.md 8c).
+// Structure (persistent CTAs over 64-row tiles; rows = (centre, sample) pairs or points):
+//   warpgroups 0, 1  gather layer 0's A operand chunk by chunk (32 K-columns = one 128-byte swizzle row) into a
+//                    ring of three shared-memory slots, issue wgmma m64n32k8 tf32 with fp32 register accumulators --
+//                    the layer's output columns are split between the two warpgroups -- and run the epilogues:
+//                    layer l < L-1 writes relu(acc + shift) as tf32 into the resident activation buffer (the next
+//                    layer's A operand, all of its K chunks), the last layer pools / stores.
+//   warp 8           weight producer: one thread streams pre-packed weight chunks (already in the K-major
+//                    SWIZZLE_128B image, see prb_mlp_pack_weights) with cp.async.bulk + mbarrier transaction counts.
+// Chains whose activation buffer and weight stages do not fit in shared memory are split into several launches by
+// the host wrapper (rows materialised in between).
+// Precision: operands are rounded to TF32 (cvt.rn), products accumulate in fp32 -- the same contract as the
+// reference's cuDNN convolutions under torch's default allow_tf32=True (SURVEY.md 8c).
 #include <string.h>
 
 #include <vector>
@@ -31,620 +29,365 @@
 namespace prb {
 
 // ------------------------------------------------------------------------------------------------ kernel
-// NG row groups of 4 warps each (warp w: TMEM lane quarter w%4, group w/4) + producer warp + MMA warp.
-// The A chunks (and the 16-column epilogue batches) of a tile are dealt round-robin to the groups, so 4*NG warps
-// hide each other's latencies while the stage order seen by the MMA issuer stays sequential.
-// optional phase trace (PRB_MLP_TRACE=1): CTA 0 stamps clock64 at the phase boundaries of its first 32 tiles
-__device__ long long g_trace[32 * 16];
-#define PRB_TRACE(slot) do { if (p.trace && blockIdx.x == 0 && tcount < 32 && r == 0) g_trace[tcount * 16 + (slot)] = clock64(); } while (0)
-
-template <int NG, int MINB>
-__global__ void __launch_bounds__(128 * NG + 64, MINB) mlp_chain_kernel(const ChainParams p) {
-    constexpr int NTHREADS = 128 * NG + 64;
+// NS: 32-column subtiles per warpgroup of the widest layer (accumulator registers: 16 * NS per thread)
+template <int NS, int MINB>
+__global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const ChainParams p) {
     extern __shared__ uint8_t smem_raw[];
     __shared__ SmemFixed S;
-    // keep the pointer arithmetic on the __shared__ symbol itself so the compiler emits LDS/STS, not generic accesses
     uint8_t *base = smem_raw + ((1024u - (s2u(smem_raw) & 1023u)) & 1023u);
     const int L = p.num_layers;
     int np_total = 0, sc_off[MAX_LAYERS];
     for (int l = 0; l < L; ++l) { sc_off[l] = np_total; np_total += p.np[l]; }
-    uint8_t *sA = base;
-    uint8_t *sB = sA + (size_t)p.na * A_STAGE_BYTES;
+    // work region, by phase of a tile: layer-0 A slots -> resident activations (layers >= 1) -> pool staging
+    uint8_t *sW = base;
+    uint8_t *sB = sW + p.work_bytes;
     float *s_scale = reinterpret_cast<float *>(sB + (size_t)p.nb * p.b_stage_bytes);
     float *s_shift = s_scale + np_total;
-    float *s_pool = s_shift + np_total;                                  // NG x (TM x POOL_STRIDE + 8 x 16)
+    float *s_carry = s_shift + np_total;     // SA max over several tiles: partial maxima of the last layer
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int NA = p.na, NB = p.nb;
+    const int NB = p.nb;
 
     if (tid == 0) {
-        for (int i = 0; i < NA; ++i) { mbar_init(s2u(&S.a_full[i]), 128); mbar_init(s2u(&S.a_empty[i]), 1); }
-        for (int i = 0; i < NB; ++i) { mbar_init(s2u(&S.b_full[i]), 1); mbar_init(s2u(&S.b_empty[i]), 1); }
-        for (int i = 0; i < MAX_LAYERS; ++i) mbar_init(s2u(&S.d_full[i]), 1);
+        for (int i = 0; i < NB; ++i) { mbar_init(s2u(&S.b_full[i]), 1); mbar_init(s2u(&S.b_empty[i]), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 4 * NG + 1) tmem_alloc(s2u(&S.tmem_base), (uint32_t)p.tmem_cols);
     for (int l = 0; l < L; ++l)
-        for (int i = tid; i < p.np[l]; i += NTHREADS) { s_scale[sc_off[l] + i] = p.unit_scale ? 1.f : p.scale[l][i]; s_shift[sc_off[l] + i] = p.shift[l][i]; }
-    tc_fence_before();
+        for (int i = tid; i < p.np[l]; i += CHAIN_THREADS) {
+            s_scale[sc_off[l] + i] = p.unit_scale ? 1.f : p.scale[l][i];
+            s_shift[sc_off[l] + i] = p.shift[l][i];
+        }
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = S.tmem_base;
 
-    if (warp == 4 * NG) {
+    if (warp == 8) {
         // ===================================================== weight producer
         if (lane == 0) {
             RingPos rb = {0, 0};
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-                for (int l = 0; l < L; ++l) {
-                    const int halves = (p.np[l] + B_TILE_ROWS - 1) / B_TILE_ROWS;
-                    for (int kc = 0; kc < p.nchunks[l]; ++kc)
-                        for (int h = 0; h < halves; ++h) {
-                            const int rows = min(B_TILE_ROWS, p.np[l] - h * B_TILE_ROWS);
-                            const uint32_t bytes = (uint32_t)rows * KC * 4;
-                            if (p.sleepy & 2) mbar_wait_sleepy(s2u(&S.b_empty[rb.stage]), rb.phase ^ 1); else mbar_wait(s2u(&S.b_empty[rb.stage]), rb.phase ^ 1);
+            for (int item = blockIdx.x; item < p.num_items; item += gridDim.x)
+                for (int s = 0; s < p.tiles_per_item && item * p.tiles_per_item + s < p.num_tiles; ++s)
+                    for (int l = 0; l < L; ++l)
+                        for (int kc = 0; kc < p.nchunks[l]; ++kc) {
+                            const uint32_t bytes = (uint32_t)p.np[l] * KC * 4;
+                            mbar_wait(s2u(&S.b_empty[rb.stage]), rb.phase ^ 1);
                             mbar_expect_tx(s2u(&S.b_full[rb.stage]), bytes);
-                            const float *src = p.w[l] + ((size_t)kc * p.np[l] + (size_t)h * B_TILE_ROWS) * KC;
-                            bulk_g2s(s2u(sB + (size_t)rb.stage * p.b_stage_bytes), src, bytes, s2u(&S.b_full[rb.stage]));
+                            bulk_g2s(s2u(sB + (size_t)rb.stage * p.b_stage_bytes), p.w[l] + (size_t)kc * p.np[l] * KC, bytes,
+                                     s2u(&S.b_full[rb.stage]));
                             rb.advance(NB);
                         }
-                }
-            }
         }
-    } else if (warp == 4 * NG + 1) {
-        // ===================================================== MMA issuer
-        if (lane == 0) {
-            RingPos ra = {0, 0}, rb = {0, 0};
-            for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-                for (int l = 0; l < L; ++l) {
-                    const int halves = (p.np[l] + B_TILE_ROWS - 1) / B_TILE_ROWS;
-                    for (int kc = 0; kc < p.nchunks[l]; ++kc) {
-                        // valid K in this chunk -> number of K=8 steps
-                        int valid = KC;
-                        if (l == 0) {
-                            int c = kc, s = 0;
-                            if (p.nseg > 1 && c >= p.seg_chunks[0]) { c -= p.seg_chunks[0]; s = 1; }
-                            valid = min(KC, p.seg_width[s] - c * KC);
-                        }
-                        const int ksteps = (valid + 7) >> 3;
-                        if (p.sleepy & 1) mbar_wait_sleepy(s2u(&S.a_full[ra.stage]), ra.phase); else mbar_wait(s2u(&S.a_full[ra.stage]), ra.phase);
-                        const uint64_t adesc = make_desc(s2u(sA + (size_t)ra.stage * A_STAGE_BYTES));
-                        for (int h = 0; h < halves; ++h) {
-                            const int rows = min(B_TILE_ROWS, p.np[l] - h * B_TILE_ROWS);
-                            if (p.sleepy & 1) mbar_wait_sleepy(s2u(&S.b_full[rb.stage]), rb.phase); else mbar_wait(s2u(&S.b_full[rb.stage]), rb.phase);
-                            tc_fence_after();
-                            const uint64_t bdesc = make_desc(s2u(sB + (size_t)rb.stage * p.b_stage_bytes));
-                            const uint32_t idesc = make_idesc(rows);
-                            const uint32_t d = tmem + (uint32_t)(p.dcol[l] + h * B_TILE_ROWS);
-                            if (p.a_tmem && l > 0) {   // A = the rewritten accumulator of layer l-1: columns kc*32 + ks*8 ...
-                                const uint32_t a_t = tmem + (uint32_t)(p.dcol[l - 1] + kc * KC);
-                                for (int ks = 0; ks < ksteps; ++ks)
-                                    umma_tf32_ts(d, a_t + (uint32_t)(8 * ks), bdesc + (uint64_t)(2 * ks), idesc, (kc > 0 || ks > 0) ? 1u : 0u);
-                            } else {
-                                for (int ks = 0; ks < ksteps; ++ks)  // +32 bytes (= 2 x 16 B) per K=8 step inside the swizzle row
-                                    umma_tf32(d, adesc + (uint64_t)(2 * ks), bdesc + (uint64_t)(2 * ks), idesc, (kc > 0 || ks > 0) ? 1u : 0u);
-                            }
-                            umma_commit(s2u(&S.b_empty[rb.stage]));
-                            rb.advance(NB);
-                        }
-                        umma_commit(s2u(&S.a_empty[ra.stage]));
-                        ra.advance(NA);
-                    }
-                    umma_commit(s2u(&S.d_full[l]));
-                }
-            }
-        }
-    } else {
-        // ===================================================== row threads (warps 0 .. 4*NG-1)
-        RingPos ra = {0, 0};
-        uint32_t dphase = 0;
-        const int wq = warp & 3, grp = warp >> 2;
-        const int r = wq * 32 + lane;       // my row inside the tile / my TMEM lane
-        const uint32_t lane_base = (uint32_t)(wq * 32) << 16;
-        const int j8 = lane & 7;            // my 16-byte unit inside a 128-byte row (gathers)
-        const int rsub = lane >> 3;         // which of the 4 rows a warp-wide gather step covers
-        uint32_t cc = 0;                    // chunk counter: chunk cc belongs to group cc % NG
-        float *pool = s_pool + grp * (TM * POOL_STRIDE + 128);
-        float *pool2 = pool + TM * POOL_STRIDE;   // 8 x 16 partial maxima (nsample > 32)
+        return;
+    }
 
-        // tile metadata is fetched one tile ahead (global loads of idx / centres / weights overlap the MMAs)
-        int m_src[3] = {0, 0, 0};
-        float m_aux[3] = {0.f, 0.f, 0.f};
-        bool m_valid = false;
-        int m_scene = 0, m_u = 0;            // FP: scene / point index of my row
-        auto fetch_meta = [&](int tile) {
-            const unsigned R = (unsigned)tile * TM + r;          // total_rows < 2^31 (checked on the host)
-            m_valid = tile < p.num_tiles && (long)R < p.total_rows;
-            if (p.mode_in == IN_SA) {
-                const unsigned pr = m_valid ? (R >> p.log_ns) : 0u;     // global centre index (nsample is a power of two)
-                const unsigned scene = pr / (unsigned)p.npoint;
-                m_src[0] = (int)scene * p.n + (m_valid ? __ldg(p.idx + R) : 0);
-                m_aux[0] = __ldg(p.new_xyz + (size_t)pr * 3 + 0);
-                m_aux[1] = __ldg(p.new_xyz + (size_t)pr * 3 + 1);
-                m_aux[2] = __ldg(p.new_xyz + (size_t)pr * 3 + 2);
-            } else if (p.mode_in == IN_FP || p.mode_out == OUT_FP) {
-                const unsigned rr = m_valid ? R : 0u;
-                const unsigned scene = rr / (unsigned)p.n;
-                m_scene = (int)scene; m_u = (int)(rr - scene * (unsigned)p.n);
-                if (p.mode_in == IN_FP) {
+    // ===================================================== MMA / epilogue warpgroups
+    const int wg = warp >> 2, wq = warp & 3;
+    const int g = lane >> 2, t4 = lane & 3;      // accumulator fragment: rows 16 wq + g (+8), columns 2 t4 (+1) of each 8
+    const int tw = tid & 127;                    // thread inside the warpgroup
+    RingPos rb = {0, 0};
+    int aslot = 0;
+    float acc[NS][16];
+    const float lo = p.linear_last ? -CUDART_INF_F : 0.f;   // ReLU = max(., 0); a linear last layer keeps the sign
+    const bool pool_raw = p.unit_scale && p.mode_out == OUT_SA_MAX;
+
+    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
+        for (int s = 0; s < p.tiles_per_item; ++s) {
+            const int tile = item * p.tiles_per_item + s;
+            if (tile >= p.num_tiles) break;
+            bar_mma();   // the previous tile's readers of S.row_* and of the pool staging are done
+            if (tid < TM) {
+                const long R = (long)tile * TM + tid;
+                const bool valid = R < p.total_rows;
+                int src[3] = {0, 0, 0};
+                float aux[3] = {0.f, 0.f, 0.f};
+                if (p.mode_in == IN_SA) {
+                    const long pr = valid ? (R >> p.log_ns) : 0;      // global centre index (nsample is a power of two)
+                    const int scene = (int)(pr / p.npoint);
+                    src[0] = scene * p.n + (valid ? __ldg(p.idx + R) : 0);
+#pragma unroll
+                    for (int q = 0; q < 3; ++q) aux[q] = __ldg(p.new_xyz + (size_t)pr * 3 + q);
+                } else if (p.mode_in == IN_FP) {
+                    const long rr = valid ? R : 0;
+                    const int scene = (int)(rr / p.n);
 #pragma unroll
                     for (int q = 0; q < 3; ++q) {
-                        m_src[q] = (int)scene * p.m + __ldg(p.idx + (size_t)rr * 3 + q);
-                        m_aux[q] = __ldg(p.weight + (size_t)rr * 3 + q);
+                        src[q] = scene * p.m + __ldg(p.idx + (size_t)rr * 3 + q);
+                        aux[q] = __ldg(p.weight + (size_t)rr * 3 + q);
                     }
                 }
+                S.row_valid[tid] = valid;
+#pragma unroll
+                for (int q = 0; q < 3; ++q) { S.row_src[tid][q] = src[q]; S.row_aux[tid][q] = aux[q]; }
             }
-        };
-        fetch_meta(blockIdx.x);
+            bar_mma();
 
-        int tcount = -1;
-        for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
-            ++tcount;
-            PRB_TRACE(0);
-            const long R = (long)tile * TM + r;
-            const bool valid = m_valid;
-            const int my_scene = m_scene, my_u = m_u;
-            bar_rows<NG>();  // previous tile's readers of S.row_* are done
-            if (grp == 0) {
-                S.row_valid[r] = valid;
+            for (int l = 0; l < L; ++l) {
+                const int nsub_all = p.np[l] >> 5, nsub0 = (nsub_all + 1) >> 1;
+                const int nsub = wg == 0 ? nsub0 : nsub_all - nsub0;
+                const int col0 = wg == 0 ? 0 : nsub0 * 32;            // first output column of this warpgroup
+                int prev_stage = -1;
+                for (int kc = 0; kc < p.nchunks[l]; ++kc) {
+                    uint32_t a_addr;
+                    int ksteps = KC / 8;
+                    if (l == 0) {
+                        // ---- gather chunk kc of the tile's input rows into A slot `aslot`
+                        int c = kc, seg = 0;
+                        if (p.nseg > 1 && c >= p.seg_chunks[0]) { c -= p.seg_chunks[0]; seg = 1; }
+                        const int k0 = c * KC;                         // first column of this chunk inside its segment
+                        const int width = p.seg_width[seg];
+                        ksteps = (min(KC, width - k0) + 7) >> 3;       // K=8 steps that hold data (the rest is padding)
+                        uint8_t *A = sW + (size_t)aslot * A_STAGE_BYTES;
+                        const bool rows_seg = (p.mode_in == IN_DIRECT) || (p.mode_in == IN_SA && seg == 0 && p.c_feat > 5) ||
+                                              (p.mode_in == IN_FP && seg == 0);
+                        if (rows_seg) {
+                            // point-major sources: 8 threads cover one row's 128 bytes, 256 threads 32 rows per step, 2 steps
+                            const int j8 = tid & 7, kk = k0 + 4 * j8;
+                            float4 v[2];
+                            if (p.mode_in == IN_FP) {
+                                const int C = p.c_known;
+                                const bool vec = (C & 3) == 0;
 #pragma unroll
-                for (int q = 0; q < 3; ++q) { S.row_src[r][q] = m_src[q]; S.row_aux[r][q] = m_aux[q]; }
-            }
-            bar_rows<NG>();
-
-            // ---- layer 0: build A chunks from global memory
-            // Feature rows with a 16-byte aligned pitch are gathered with cp.async straight into the swizzled stage
-            // (no registers, up to two chunks of loads in flight per group); their fp32 bits reach the tensor core
-            // unrounded, which then drops the low 13 mantissa bits itself.
-            uint32_t pend_bar[2] = {0u, 0u};
-            int npend = 0;
-            // publish every chunk whose cp.async copies are still pending (all of them: groups complete in order)
-            auto retire_all = [&]() {
-                if (npend > 0) {
-                    cp_async_wait<0>();
-                    fence_async_smem();
-                    mbar_arrive(pend_bar[0]);
-                    if (npend == 2) mbar_arrive(pend_bar[1]);
-                    npend = 0;
-                }
-            };
-            // claim the next ring stage.  Never block on the consumer while own chunks are unpublished: the stage we
-            // wait for may only be released after one of them has been consumed (deadlock otherwise).
-            auto acquire_stage = [&]() {
-                if (!mbar_test(s2u(&S.a_empty[ra.stage]), ra.phase ^ 1)) {
-                    retire_all();
-                    mbar_wait(s2u(&S.a_empty[ra.stage]), ra.phase ^ 1);
-                }
-            };
-            for (int kc = 0; kc < p.nchunks[0]; ++kc, ++cc, ra.advance(NA)) {
-                if ((int)(cc % NG) != grp) continue;
-                int c = kc, seg = 0;
-                if (p.nseg > 1 && c >= p.seg_chunks[0]) { c -= p.seg_chunks[0]; seg = 1; }
-                const int k0 = c * KC;                       // first column of this chunk inside its segment
-                const int width = p.seg_width[seg];
-                uint8_t *A = sA + (size_t)ra.stage * A_STAGE_BYTES;
-                const bool rows_seg = (p.mode_in == IN_DIRECT) || (p.mode_in == IN_SA && seg == 0 && p.c_feat > 5) ||
-                                      (p.mode_in == IN_FP && seg == 0);
-                if (rows_seg) {
-                    // point-major sources: 8 lanes cover one row's 128 bytes, a warp covers 4 rows per step, 8 steps.
-                    // All loads of the chunk are issued before the first use (memory-level parallelism).
-                    const int kk = k0 + 4 * j8;
-                    if (p.mode_in == IN_FP) {
-                        const int C = p.c_known;
-                        const bool vec = (C & 3) == 0;
+                                for (int i = 0; i < 2; ++i) {
+                                    const int rr = (tid >> 3) + 32 * i;
+                                    float4 t0 = make_float4(0.f, 0.f, 0.f, 0.f), t1 = t0, t2 = t0;
+                                    const float w0 = S.row_aux[rr][0], w1 = S.row_aux[rr][1], w2 = S.row_aux[rr][2];
+                                    if (S.row_valid[rr] && kk < width) {
+                                        const float *s0 = p.known_pm + (size_t)S.row_src[rr][0] * C + kk;
+                                        const float *s1 = p.known_pm + (size_t)S.row_src[rr][1] * C + kk;
+                                        const float *s2 = p.known_pm + (size_t)S.row_src[rr][2] * C + kk;
+                                        if (vec) {
+                                            t0 = __ldg((const float4 *)s0); t1 = __ldg((const float4 *)s1); t2 = __ldg((const float4 *)s2);
+                                        } else {
+                                            float a0[4], a1[4], a2[4];
 #pragma unroll
-                        for (int half = 0; half < 2; ++half) {
-                            float4 t0[4], t1[4], t2[4];
-                            float w0[4], w1[4], w2[4];
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const int rr = wq * 32 + rsub + 4 * (half * 4 + i);
-                                t0[i] = t1[i] = t2[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                                w0[i] = S.row_aux[rr][0]; w1[i] = S.row_aux[rr][1]; w2[i] = S.row_aux[rr][2];
-                                if (S.row_valid[rr] && kk < width) {
-                                    const float *s0 = p.known_pm + (size_t)S.row_src[rr][0] * C + kk;
-                                    const float *s1 = p.known_pm + (size_t)S.row_src[rr][1] * C + kk;
-                                    const float *s2 = p.known_pm + (size_t)S.row_src[rr][2] * C + kk;
-                                    if (vec) {
-                                        t0[i] = __ldg((const float4 *)s0); t1[i] = __ldg((const float4 *)s1); t2[i] = __ldg((const float4 *)s2);
-                                    } else {
-                                        float a0[4], a1[4], a2[4];
-#pragma unroll
-                                        for (int q = 0; q < 4; ++q) {
-                                            const bool in = kk + q < width;
-                                            a0[q] = in ? __ldg(s0 + q) : 0.f; a1[q] = in ? __ldg(s1 + q) : 0.f; a2[q] = in ? __ldg(s2 + q) : 0.f;
+                                            for (int q = 0; q < 4; ++q) {
+                                                const bool in = kk + q < width;
+                                                a0[q] = in ? __ldg(s0 + q) : 0.f; a1[q] = in ? __ldg(s1 + q) : 0.f; a2[q] = in ? __ldg(s2 + q) : 0.f;
+                                            }
+                                            t0 = make_float4(a0[0], a0[1], a0[2], a0[3]);
+                                            t1 = make_float4(a1[0], a1[1], a1[2], a1[3]);
+                                            t2 = make_float4(a2[0], a2[1], a2[2], a2[3]);
                                         }
-                                        t0[i] = make_float4(a0[0], a0[1], a0[2], a0[3]);
-                                        t1[i] = make_float4(a1[0], a1[1], a1[2], a1[3]);
-                                        t2[i] = make_float4(a2[0], a2[1], a2[2], a2[3]);
+                                    }
+                                    // same contraction as three_interpolate (reference SASS): fma(w2,p2, fma(w0,p0, w1*p1))
+                                    v[i].x = __fmaf_rn(w2, t2.x, __fmaf_rn(w0, t0.x, __fmul_rn(w1, t1.x)));
+                                    v[i].y = __fmaf_rn(w2, t2.y, __fmaf_rn(w0, t0.y, __fmul_rn(w1, t1.y)));
+                                    v[i].z = __fmaf_rn(w2, t2.z, __fmaf_rn(w0, t0.z, __fmul_rn(w1, t1.z)));
+                                    v[i].w = __fmaf_rn(w2, t2.w, __fmaf_rn(w0, t0.w, __fmul_rn(w1, t1.w)));
+                                }
+                            } else {
+                                const float *srcb = p.mode_in == IN_DIRECT ? (seg ? p.x2_rows : p.x_rows) : p.feats_pm;
+                                const int pitch = p.mode_in == IN_DIRECT ? (seg ? p.x2_pitch : p.x_pitch) : p.c_feat;
+                                const bool vec = (pitch & 3) == 0 && (reinterpret_cast<uintptr_t>(srcb) & 15) == 0;
+#pragma unroll
+                                for (int i = 0; i < 2; ++i) {
+                                    const int rr = (tid >> 3) + 32 * i;
+                                    v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+                                    if (S.row_valid[rr] && kk < width) {
+                                        const size_t row = p.mode_in == IN_DIRECT ? (size_t)tile * TM + rr : (size_t)S.row_src[rr][0];
+                                        const float *src = srcb + row * pitch + kk;
+                                        if (vec) {
+                                            v[i] = __ldg((const float4 *)src);
+                                        } else {
+                                            float o[4];
+#pragma unroll
+                                            for (int q = 0; q < 4; ++q) o[q] = (kk + q < width) ? __ldg(src + q) : 0.f;
+                                            v[i] = make_float4(o[0], o[1], o[2], o[3]);
+                                        }
                                     }
                                 }
                             }
-                            if (half == 0) acquire_stage();
+#pragma unroll
+                            for (int i = 0; i < 2; ++i) {
+                                const int rr = (tid >> 3) + 32 * i;
+                                *reinterpret_cast<float4 *>(A + swz(rr, j8)) =
+                                    make_float4(to_tf32(v[i].x), to_tf32(v[i].y), to_tf32(v[i].z), to_tf32(v[i].w));
+                            }
+                        } else if (p.mode_in == IN_SA) {
+                            // relative xyz segment: [x - cx, y - cy, z - cz, (<= 5 feature channels,) 0 ...]; one K=8 step
+                            if (tid < TM) {
+                                const int r = tid;
+                                float4 v = make_float4(0.f, 0.f, 0.f, 0.f), v2 = make_float4(0.f, 0.f, 0.f, 0.f);
+                                if (S.row_valid[r]) {
+                                    const float *q = p.xyz + (size_t)S.row_src[r][0] * 3;
+                                    v.x = to_tf32(__ldg(q + 0) - S.row_aux[r][0]);
+                                    v.y = to_tf32(__ldg(q + 1) - S.row_aux[r][1]);
+                                    v.z = to_tf32(__ldg(q + 2) - S.row_aux[r][2]);
+                                    if (p.c_feat > 0 && p.c_feat <= 5) {
+                                        const float *f = p.feats_pm + (size_t)S.row_src[r][0] * p.c_feat;
+                                        v.w = to_tf32(__ldg(f));
+                                        if (p.c_feat > 1) v2.x = to_tf32(__ldg(f + 1));
+                                        if (p.c_feat > 2) v2.y = to_tf32(__ldg(f + 2));
+                                        if (p.c_feat > 3) v2.z = to_tf32(__ldg(f + 3));
+                                        if (p.c_feat > 4) v2.w = to_tf32(__ldg(f + 4));
+                                    }
+                                }
+                                *reinterpret_cast<float4 *>(A + swz(r, 0)) = v;
+                                *reinterpret_cast<float4 *>(A + swz(r, 1)) = v2;
+                            }
+                        } else {
+                            // FP skip segment: channel-major (b, c_skip, n); 4 threads per row (8 channels each), the
+                            // threads of a warp run along consecutive points
+                            const int r = tid & (TM - 1), q8 = tid >> 6;
+                            const long R = (long)tile * TM + r;
+                            float o[8];
+                            if (S.row_valid[r]) {
+                                const int scene = (int)(R / p.n), u = (int)(R - (long)scene * p.n);
+                                const float *bsrc = p.skip + (size_t)scene * p.c_skip * p.n + u;
+#pragma unroll
+                                for (int q = 0; q < 8; ++q) {
+                                    const int ch = k0 + 8 * q8 + q;
+                                    o[q] = ch < width ? to_tf32(__ldg(bsrc + (size_t)ch * p.n)) : 0.f;
+                                }
+                            } else {
+#pragma unroll
+                                for (int q = 0; q < 8; ++q) o[q] = 0.f;
+                            }
+                            *reinterpret_cast<float4 *>(A + swz(r, 2 * q8)) = make_float4(o[0], o[1], o[2], o[3]);
+                            *reinterpret_cast<float4 *>(A + swz(r, 2 * q8 + 1)) = make_float4(o[4], o[5], o[6], o[7]);
+                        }
+                        fence_async_smem();
+                        // slot `aslot` is complete.  It was last read by the MMAs of chunk kc-3, which both warpgroups
+                        // retired (wgmma_wait<1> of chunk kc-2) before the barrier of chunk kc-1.
+                        bar_mma();
+                        a_addr = s2u(A);
+                        aslot = aslot == A_SLOTS - 1 ? 0 : aslot + 1;
+                    } else {
+                        a_addr = s2u(sW + (size_t)kc * A_STAGE_BYTES);
+                    }
+                    mbar_wait(s2u(&S.b_full[rb.stage]), rb.phase);
+                    const uint32_t b_addr = s2u(sB + (size_t)rb.stage * p.b_stage_bytes) + (uint32_t)col0 * (KC * 4);
+                    wgmma_fence();
+#pragma unroll
+                    for (int ks = 0; ks < KC / 8; ++ks) {
+                        if (ks < ksteps) {
+                            const uint64_t adesc = make_desc(a_addr) + (uint64_t)(2 * ks);
+#pragma unroll
+                            for (int j = 0; j < NS; ++j)
+                                if (j < nsub)
+                                    wgmma_tf32_n32(acc[j], adesc, make_desc(b_addr + (uint32_t)j * 32 * KC * 4) + (uint64_t)(2 * ks),
+                                                   (kc > 0 || ks > 0) ? 1u : 0u);
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();     // the previous chunk's MMAs are done: release its weight stage
+                    if (prev_stage >= 0 && lane == 0) mbar_arrive(s2u(&S.b_empty[prev_stage]));
+                    prev_stage = (int)rb.stage;
+                    rb.advance(NB);
+                }
+                wgmma_wait<0>();
+#pragma unroll
+                for (int j = 0; j < NS; ++j) reg_fence(acc[j]);
+                if (lane == 0) mbar_arrive(s2u(&S.b_empty[prev_stage]));
+                bar_mma();   // both warpgroups' MMAs of layer l have read their A operand: the work region is free
+
+                if (l + 1 < L) {
+                    // ---- relu(acc * scale + shift) -> tf32 -> resident activations = the next layer's K chunks
+                    const float *sc = s_scale + sc_off[l], *sh = s_shift + sc_off[l];
+#pragma unroll
+                    for (int j = 0; j < NS; ++j) {
+                        if (j >= nsub) continue;
+#pragma unroll
+                        for (int i = 0; i < 4; ++i) {
+                            const int c = col0 + 32 * j + 8 * i + 2 * t4;
+                            uint8_t *chunk = sW + (size_t)(c >> 5) * A_STAGE_BYTES;
+                            const int ju = (c & 31) >> 2, within = (c & 3) * 4;
+#pragma unroll
+                            for (int h = 0; h < 2; ++h) {
+                                const int r = 16 * wq + g + 8 * h;
+                                float2 o;
+                                if (p.unit_scale) {
+                                    o.x = relu_to_tf32(acc[j][4 * i + 2 * h] + sh[c]);
+                                    o.y = relu_to_tf32(acc[j][4 * i + 2 * h + 1] + sh[c + 1]);
+                                } else {
+                                    o.x = relu_to_tf32(fmaf(acc[j][4 * i + 2 * h], sc[c], sh[c]));
+                                    o.y = relu_to_tf32(fmaf(acc[j][4 * i + 2 * h + 1], sc[c + 1], sh[c + 1]));
+                                }
+                                *reinterpret_cast<float2 *>(chunk + swz(r, ju) + within) = o;
+                            }
+                        }
+                    }
+                    fence_async_smem();
+                    bar_mma();   // the next layer's A operand is complete
+                    continue;
+                }
+
+                // ---- final epilogue
+                const int Cl = p.c_last;
+                const float *sc = s_scale + sc_off[l], *sh = s_shift + sc_off[l];
+                auto value = [&](float a, int c) -> float {
+                    if (pool_raw) return a;   // max_s relu(x_s + t) == relu(max_s x_s + t): shift / ReLU after the max
+                    return p.unit_scale ? fmaxf(a + sh[c], lo) : fmaxf(fmaf(a, sc[c], sh[c]), lo);
+                };
+                if (p.mode_out == OUT_SA_MAX) {
+                    // max over the nsample consecutive rows of each centre, one 32-column subtile at a time through this
+                    // warpgroup's staging tile; a centre spanning several tiles keeps its partial maxima in s_carry
+                    float *stg = reinterpret_cast<float *>(sW) + wg * (TM * POOL_STRIDE);
+                    const int nse = p.ns < TM ? p.ns : TM, per = p.ns > TM ? p.ns / TM : 1;
+                    const int sub = tile % per, ncent = TM / nse;
+#pragma unroll
+                    for (int j = 0; j < NS; ++j) {
+                        if (j >= nsub) continue;
+#pragma unroll
+                        for (int i = 0; i < 4; ++i)
+#pragma unroll
+                            for (int h = 0; h < 2; ++h)
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    const int cs = 8 * i + 2 * t4 + e;
+                                    stg[(16 * wq + g + 8 * h) * POOL_STRIDE + cs] = value(acc[j][4 * i + 2 * h + e], col0 + 32 * j + cs);
+                                }
+                        bar_wg(wg);
+                        for (int o = tw; o < ncent * 32; o += 128) {
+                            const int ci = o >> 5, cs = o & 31, c = col0 + 32 * j + cs;
+                            float x = stg[(ci * nse) * POOL_STRIDE + cs];
+                            for (int r = 1; r < nse; ++r) x = fmaxf(x, stg[(ci * nse + r) * POOL_STRIDE + cs]);
+                            if (per > 1) {
+                                if (sub > 0) x = fmaxf(x, s_carry[c]);
+                                if (sub < per - 1) { s_carry[c] = x; continue; }
+                            }
+                            if (pool_raw) x = fmaxf(x + sh[c], lo);
+                            const long Rg = (long)tile * TM + ci * nse;    // a row of the centre (whole centres per tile)
+                            if (Rg < p.total_rows && c < Cl) {
+                                const long pr = Rg >> p.log_ns;
+                                const int scene = (int)(pr / p.npoint), pp = (int)(pr - (long)scene * p.npoint);
+                                p.out[((size_t)scene * p.out_stride_c + p.out_c_off + c) * p.npoint + pp] = x;
+                                if (p.out_pm) p.out_pm[((size_t)scene * p.npoint + pp) * p.out_stride_c + p.out_c_off + c] = x;
+                            }
+                        }
+                        bar_wg(wg);
+                    }
+                } else {
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const long R = (long)tile * TM + 16 * wq + g + 8 * h;
+                        if (R >= p.total_rows) continue;
+                        int scene = 0, u = 0;
+                        if (p.mode_out == OUT_FP) { scene = (int)(R / p.n); u = (int)(R - (long)scene * p.n); }
+#pragma unroll
+                        for (int j = 0; j < NS; ++j) {
+                            if (j >= nsub) continue;
 #pragma unroll
                             for (int i = 0; i < 4; ++i) {
-                                const int rr = wq * 32 + rsub + 4 * (half * 4 + i);
-                                // same contraction as three_interpolate (reference SASS): fma(w2,p2, fma(w0,p0, w1*p1))
-                                float4 v;
-                                v.x = to_tf32(__fmaf_rn(w2[i], t2[i].x, __fmaf_rn(w0[i], t0[i].x, __fmul_rn(w1[i], t1[i].x))));
-                                v.y = to_tf32(__fmaf_rn(w2[i], t2[i].y, __fmaf_rn(w0[i], t0[i].y, __fmul_rn(w1[i], t1[i].y))));
-                                v.z = to_tf32(__fmaf_rn(w2[i], t2[i].z, __fmaf_rn(w0[i], t0[i].z, __fmul_rn(w1[i], t1[i].z))));
-                                v.w = to_tf32(__fmaf_rn(w2[i], t2[i].w, __fmaf_rn(w0[i], t0[i].w, __fmul_rn(w1[i], t1[i].w))));
-                                *reinterpret_cast<float4 *>(A + swz(rr, j8)) = v;
-                            }
-                        }
-                    } else {
-                        const int pitch = p.mode_in == IN_DIRECT ? p.x_pitch : p.c_feat;
-                        if ((pitch & 3) == 0 && p.gather_mode != 0) {
-                            // asynchronous path: width is a multiple of 4 too, so a unit is either all data or all padding
-                            acquire_stage();
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                const int rr = wq * 32 + rsub + 4 * i;
-                                const bool ok = S.row_valid[rr] && kk < width;
-                                const float *src = p.mode_in == IN_DIRECT ? p.x_rows + ((size_t)tile * TM + rr) * pitch + kk
-                                                                          : p.feats_pm + (size_t)S.row_src[rr][0] * pitch + kk;
-                                if (p.gather_mode == 1) cp_async16(s2u(A + swz(rr, j8)), ok ? src : (const float *)p.w[0], ok ? 16u : 0u);
-                                else cp_async16_ca(s2u(A + swz(rr, j8)), ok ? src : (const float *)p.w[0], ok ? 16u : 0u);
-                            }
-                            cp_async_commit();
-                            if (npend == 2) {          // retire the oldest chunk: its copies have landed
-                                cp_async_wait<2>();
-                                fence_async_smem();
-                                mbar_arrive(pend_bar[0]);
-                                pend_bar[0] = pend_bar[1];
-                                npend = 1;
-                            }
-                            pend_bar[npend++] = s2u(&S.a_full[ra.stage]);
-                            continue;                  // (the for-increment advances cc and the ring)
-                        }
-                        float4 t[8];
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const int rr = wq * 32 + rsub + 4 * i;
-                            t[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                            if (S.row_valid[rr] && kk < width) {
-                                const float *src = p.mode_in == IN_DIRECT ? p.x_rows + ((size_t)tile * TM + rr) * pitch + kk
-                                                                          : p.feats_pm + (size_t)S.row_src[rr][0] * pitch + kk;
-                                if ((pitch & 3) == 0) {
-                                    t[i] = __ldg((const float4 *)src);
+                                const int c = col0 + 32 * j + 8 * i + 2 * t4;
+                                float v0 = value(acc[j][4 * i + 2 * h], c), v1 = value(acc[j][4 * i + 2 * h + 1], c + 1);
+                                if (p.mode_out == OUT_ROWS) {
+                                    if (p.round_out) { v0 = to_tf32(v0); v1 = to_tf32(v1); }   // the next launch's A operand
+                                    *reinterpret_cast<float2 *>(p.out + (size_t)R * p.out_pitch + c) = make_float2(v0, v1);
                                 } else {
-                                    float o[4];
-#pragma unroll
-                                    for (int q = 0; q < 4; ++q) o[q] = (kk + q < width) ? __ldg(src + q) : 0.f;
-                                    t[i] = make_float4(o[0], o[1], o[2], o[3]);
+                                    float *o = p.out + ((size_t)scene * p.out_stride_c + p.out_c_off + c) * p.n + u;
+                                    if (c < Cl) o[0] = v0;
+                                    if (c + 1 < Cl) o[p.n] = v1;
+                                    if (p.out_pm) {   // point-major copy for the next consumer (no transpose kernel)
+                                        float *o2 = p.out_pm + (size_t)R * p.out_stride_c + p.out_c_off + c;
+                                        if (c < Cl) o2[0] = v0;
+                                        if (c + 1 < Cl) o2[1] = v1;
+                                    }
                                 }
                             }
                         }
-                        acquire_stage();
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const int rr = wq * 32 + rsub + 4 * i;
-                            float4 v = t[i];
-                            v.x = to_tf32(v.x); v.y = to_tf32(v.y); v.z = to_tf32(v.z); v.w = to_tf32(v.w);
-                            *reinterpret_cast<float4 *>(A + swz(rr, j8)) = v;
-                        }
-                    }
-                } else if (p.mode_in == IN_SA) {
-                    // relative xyz segment: [x - cx, y - cy, z - cz, (<= 5 feature channels,) 0 ...]; one K=8 step
-                    float4 v = make_float4(0.f, 0.f, 0.f, 0.f), v2 = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (valid) {
-                        const float *q = p.xyz + (size_t)m_src[0] * 3;
-                        v.x = to_tf32(__ldg(q + 0) - m_aux[0]);
-                        v.y = to_tf32(__ldg(q + 1) - m_aux[1]);
-                        v.z = to_tf32(__ldg(q + 2) - m_aux[2]);
-                        if (p.c_feat > 0 && p.c_feat <= 5) {
-                            const float *f = p.feats_pm + (size_t)m_src[0] * p.c_feat;
-                            v.w = to_tf32(__ldg(f));
-                            if (p.c_feat > 1) v2.x = to_tf32(__ldg(f + 1));
-                            if (p.c_feat > 2) v2.y = to_tf32(__ldg(f + 2));
-                            if (p.c_feat > 3) v2.z = to_tf32(__ldg(f + 3));
-                            if (p.c_feat > 4) v2.w = to_tf32(__ldg(f + 4));
-                        }
-                    }
-                    acquire_stage();
-                    *reinterpret_cast<float4 *>(A + swz(r, 0)) = v;
-                    *reinterpret_cast<float4 *>(A + swz(r, 1)) = v2;
-                } else {
-                    // FP skip segment: channel-major (b, c_skip, n); lanes run along consecutive points
-                    const float *bsrc = p.skip + (size_t)my_scene * p.c_skip * p.n + my_u;
-                    float o[32];
-#pragma unroll
-                    for (int q = 0; q < 32; ++q) {
-                        const int ch = k0 + q;
-                        o[q] = (valid && ch < width) ? __ldg(bsrc + (size_t)ch * p.n) : 0.f;
-                    }
-                    acquire_stage();
-#pragma unroll
-                    for (int j = 0; j < 8; ++j)
-                        *reinterpret_cast<float4 *>(A + swz(r, j)) =
-                            make_float4(to_tf32(o[4 * j]), to_tf32(o[4 * j + 1]), to_tf32(o[4 * j + 2]), to_tf32(o[4 * j + 3]));
-                }
-                fence_async_smem();
-                mbar_arrive(s2u(&S.a_full[ra.stage]));
-            }
-
-            retire_all();
-            PRB_TRACE(1);
-
-            // next tile's metadata: issue the loads now, consume them at the top of the next iteration
-            fetch_meta(tile + gridDim.x);
-
-            // ---- layers 1..L-1: previous accumulator -> scale/shift/ReLU -> next A operand
-            for (int l = 1; l < L; ++l) {
-                mbar_wait(s2u(&S.d_full[l - 1]), dphase);
-                tc_fence_after();
-                PRB_TRACE(2 * l);
-                for (int kc = 0; kc < p.nchunks[l]; ++kc, ++cc, ra.advance(NA)) {
-                    if ((int)(cc % NG) != grp) continue;
-                    mbar_wait(s2u(&S.a_empty[ra.stage]), ra.phase ^ 1);
-                    uint8_t *A = sA + (size_t)ra.stage * A_STAGE_BYTES;
-                    if (p.a_tmem) {
-                        // in place: D_{l-1}[:, chunk] -> relu(. + shift) as tf32 bit patterns -> the same TMEM columns
-#pragma unroll
-                        for (int hh = 0; hh < 2; ++hh) {
-                            const uint32_t col = tmem + lane_base + (uint32_t)(p.dcol[l - 1] + kc * KC + hh * 16);
-                            uint32_t acc[16];
-                            tmem_ld16(col, acc);
-                            const float4 *sc4 = reinterpret_cast<const float4 *>(s_scale + sc_off[l - 1] + kc * KC + hh * 16);
-                            const float4 *sh4 = reinterpret_cast<const float4 *>(s_shift + sc_off[l - 1] + kc * KC + hh * 16);
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const float4 a = sc4[j], b = sh4[j];
-                                acc[4 * j + 0] = __float_as_uint(relu_to_tf32(fmaf(__uint_as_float(acc[4 * j + 0]), a.x, b.x)));
-                                acc[4 * j + 1] = __float_as_uint(relu_to_tf32(fmaf(__uint_as_float(acc[4 * j + 1]), a.y, b.y)));
-                                acc[4 * j + 2] = __float_as_uint(relu_to_tf32(fmaf(__uint_as_float(acc[4 * j + 2]), a.z, b.z)));
-                                acc[4 * j + 3] = __float_as_uint(relu_to_tf32(fmaf(__uint_as_float(acc[4 * j + 3]), a.w, b.w)));
-                            }
-                            tmem_st16(col, acc);
-                        }
-                        tmem_st_wait();
-                        tc_fence_before();
-                        mbar_arrive(s2u(&S.a_full[ra.stage]));
-                        continue;
-                    }
-#pragma unroll
-                    for (int hh = 0; hh < 2; ++hh) {
-                        uint32_t acc[16];
-                        tmem_ld16(tmem + lane_base + (uint32_t)(p.dcol[l - 1] + kc * KC + hh * 16), acc);
-                        const float4 *sc4 = reinterpret_cast<const float4 *>(s_scale + sc_off[l - 1] + kc * KC + hh * 16);
-                        const float4 *sh4 = reinterpret_cast<const float4 *>(s_shift + sc_off[l - 1] + kc * KC + hh * 16);
-                        if (p.unit_scale) {
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const float4 b = sh4[j];                 // broadcast LDS.128
-                                float4 o;
-                                o.x = relu_to_tf32(__uint_as_float(acc[4 * j + 0]) + b.x);
-                                o.y = relu_to_tf32(__uint_as_float(acc[4 * j + 1]) + b.y);
-                                o.z = relu_to_tf32(__uint_as_float(acc[4 * j + 2]) + b.z);
-                                o.w = relu_to_tf32(__uint_as_float(acc[4 * j + 3]) + b.w);
-                                *reinterpret_cast<float4 *>(A + swz(r, hh * 4 + j)) = o;
-                            }
-                        } else {
-#pragma unroll
-                            for (int j = 0; j < 4; ++j) {
-                                const float4 a = sc4[j], b = sh4[j];     // broadcast LDS.128
-                                float4 o;
-                                o.x = relu_to_tf32(fmaf(__uint_as_float(acc[4 * j + 0]), a.x, b.x));
-                                o.y = relu_to_tf32(fmaf(__uint_as_float(acc[4 * j + 1]), a.y, b.y));
-                                o.z = relu_to_tf32(fmaf(__uint_as_float(acc[4 * j + 2]), a.z, b.z));
-                                o.w = relu_to_tf32(fmaf(__uint_as_float(acc[4 * j + 3]), a.w, b.w));
-                                *reinterpret_cast<float4 *>(A + swz(r, hh * 4 + j)) = o;
-                            }
-                        }
-                    }
-                    tc_fence_before();
-                    fence_async_smem();
-                    mbar_arrive(s2u(&S.a_full[ra.stage]));
-                }
-                PRB_TRACE(2 * l + 1);
-            }
-
-            // ---- final epilogue: 16-column batches dealt round-robin to the row groups
-            mbar_wait(s2u(&S.d_full[L - 1]), dphase);
-            tc_fence_after();
-            PRB_TRACE(2 * L);
-            const int Cl = p.c_last;
-            const float *sc = s_scale + sc_off[L - 1], *sh = s_shift + sc_off[L - 1];
-            // SA max-pool: thread (g16, q) owns 16-row segment g16 and channel q of every batch
-            size_t e_off = 0, e_pm = 0;
-            bool e_ok = false;
-            // butterfly pooling (nsample 16 / 32): my centre is the one my own row belongs to
-            size_t b_off = 0, b_pm = 0;
-            bool b_ok = false;
-            if (p.mode_out == OUT_SA_MAX && (p.ns == 16 || p.ns == 32)) {
-                const unsigned Rg = (unsigned)tile * TM + (unsigned)r;
-                b_ok = (long)Rg < p.total_rows;
-                const unsigned pr = Rg >> p.log_ns, scene = pr / (unsigned)p.npoint, pp = pr - scene * (unsigned)p.npoint;
-                b_off = ((size_t)scene * p.out_stride_c + p.out_c_off) * p.npoint + pp;
-                b_pm = ((size_t)scene * p.npoint + pp) * p.out_stride_c + p.out_c_off;
-            }
-            if (p.mode_out == OUT_SA_MAX && p.ns >= 16) {
-                const unsigned Rg = (unsigned)tile * TM + (unsigned)(r >> 4) * 16u;
-                e_ok = (long)Rg < p.total_rows && (((r >> 4) & ((p.ns >> 4) - 1)) == 0);
-                const unsigned pr = Rg >> p.log_ns, scene = pr / (unsigned)p.npoint, pp = pr - scene * (unsigned)p.npoint;
-                e_off = ((size_t)scene * p.out_stride_c + p.out_c_off + (r & 15)) * p.npoint + pp;
-                e_pm = ((size_t)scene * p.npoint + pp) * p.out_stride_c + p.out_c_off + (r & 15);
-            }
-            for (int c0 = grp * 16; c0 < Cl; c0 += 16 * NG) {
-                uint32_t acc[16];
-                tmem_ld16(tmem + lane_base + (uint32_t)(p.dcol[L - 1] + c0), acc);
-                float v[16];
-                // folded scale + max-pool: max_s relu(x_s + t) == relu(max_s x_s + t), so the raw accumulators are
-                // pooled and shift / ReLU are applied once per (centre, channel) after the reduction
-                const bool pool_raw = p.unit_scale && p.mode_out == OUT_SA_MAX;
-                const float lo = p.linear_last ? -CUDART_INF_F : 0.f;    // ReLU = max(., 0); a linear last layer keeps the sign
-                if (pool_raw) {
-#pragma unroll
-                    for (int q = 0; q < 16; ++q) v[q] = __uint_as_float(acc[q]);
-                } else if (p.unit_scale) {
-                    const float4 *sh4 = reinterpret_cast<const float4 *>(sh + c0);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float4 b = sh4[j];
-                        v[4 * j + 0] = fmaxf(__uint_as_float(acc[4 * j + 0]) + b.x, lo);
-                        v[4 * j + 1] = fmaxf(__uint_as_float(acc[4 * j + 1]) + b.y, lo);
-                        v[4 * j + 2] = fmaxf(__uint_as_float(acc[4 * j + 2]) + b.z, lo);
-                        v[4 * j + 3] = fmaxf(__uint_as_float(acc[4 * j + 3]) + b.w, lo);
-                    }
-                } else {
-                    const float4 *sc4 = reinterpret_cast<const float4 *>(sc + c0), *sh4 = reinterpret_cast<const float4 *>(sh + c0);
-#pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const float4 a = sc4[j], b = sh4[j];
-                        v[4 * j + 0] = fmaxf(fmaf(__uint_as_float(acc[4 * j + 0]), a.x, b.x), lo);
-                        v[4 * j + 1] = fmaxf(fmaf(__uint_as_float(acc[4 * j + 1]), a.y, b.y), lo);
-                        v[4 * j + 2] = fmaxf(fmaf(__uint_as_float(acc[4 * j + 2]), a.z, b.z), lo);
-                        v[4 * j + 3] = fmaxf(fmaf(__uint_as_float(acc[4 * j + 3]), a.w, b.w), lo);
-                    }
-                }
-                if (p.mode_out == OUT_ROWS) {
-                    if (valid) {
-                        float *o = p.out + (size_t)R * p.out_pitch + c0;
-                        if (p.round_out) {   // the next launch of a split chain reads these rows as its A operand
-#pragma unroll
-                            for (int q = 0; q < 16; ++q) v[q] = to_tf32(v[q]);
-                        }
-#pragma unroll
-                        for (int q = 0; q < 16; q += 4)
-                            *reinterpret_cast<float4 *>(o + q) = make_float4(v[q], v[q + 1], v[q + 2], v[q + 3]);
-                    }
-                } else if (p.mode_out == OUT_FP) {
-                    if (valid) {
-                        float *o = p.out + ((size_t)my_scene * p.out_stride_c + p.out_c_off + c0) * p.n + my_u;
-#pragma unroll
-                        for (int q = 0; q < 16; ++q)
-                            if (c0 + q < Cl) o[(size_t)q * p.n] = v[q];
-                        if (p.out_pm) {   // point-major copy for the next consumer (no transpose kernel)
-                            float *o2 = p.out_pm + (size_t)R * p.out_stride_c + p.out_c_off + c0;
-                            if ((p.out_stride_c & 3) == 0 && c0 + 16 <= Cl) {
-#pragma unroll
-                                for (int q = 0; q < 16; q += 4) *reinterpret_cast<float4 *>(o2 + q) = make_float4(v[q], v[q + 1], v[q + 2], v[q + 3]);
-                            } else {
-#pragma unroll
-                                for (int q = 0; q < 16; ++q)
-                                    if (c0 + q < Cl) o2[q] = v[q];
-                            }
-                        }
-                    }
-                } else {
-                    // max over the nsample consecutive rows of each centre, through a shared staging tile:
-                    // thread (seg, q) reduces the <=16 rows of one segment for channel c0+q; segments of a centre
-                    // with nsample > 16 are combined with one shuffle (32) or a second tiny tile (64, 128).
-                    // Groups are whole (total_rows is a multiple of nsample): tail groups past total_rows are skipped.
-                    const int ns = p.ns;
-                    const int g16 = r >> 4, q = r & 15;          // (segment of 16 rows, channel) handled by this thread
-                    if (ns == 32 || ns == 16) {
-                        // The nsample rows of a centre are lanes of ONE warp: halving butterfly, no staging tile and
-                        // no barriers.  Each step a lane keeps half of its channels (chosen by one lane-id bit),
-                        // sends the other half to its partner and takes the max -- 8+4+2+1 shuffles leave one channel
-                        // per lane: channel (lane>>1)&15 for 32 samples (one more step joins lanes 2k, 2k+1), channel
-                        // lane&15 for 16 samples.  (Measured per 16-column batch under load, scripts/mlp_trace.py:
-                        // staged tile + two named barriers ~1000 cycles, 16 CREDUX ~860, this butterfly see notes.)
-                        float w8[8], w4[4], w2[2], x;
-                        if (ns == 32) {
-                            const bool b4 = lane & 16;
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                const float keep = b4 ? v[i + 8] : v[i], send = b4 ? v[i] : v[i + 8];
-                                w8[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 16));
-                            }
-                            const bool b3 = lane & 8;
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const float keep = b3 ? w8[i + 4] : w8[i], send = b3 ? w8[i] : w8[i + 4];
-                                w4[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 8));
-                            }
-                            const bool b2 = lane & 4;
-#pragma unroll
-                            for (int i = 0; i < 2; ++i) {
-                                const float keep = b2 ? w4[i + 2] : w4[i], send = b2 ? w4[i] : w4[i + 2];
-                                w2[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 4));
-                            }
-                            const bool b1 = lane & 2;
-                            x = fmaxf(b1 ? w2[1] : w2[0], __shfl_xor_sync(0xffffffffu, b1 ? w2[0] : w2[1], 2));
-                            x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 1));
-                        } else {
-                            const bool b3 = lane & 8;
-#pragma unroll
-                            for (int i = 0; i < 8; ++i) {
-                                const float keep = b3 ? v[i + 8] : v[i], send = b3 ? v[i] : v[i + 8];
-                                w8[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 8));
-                            }
-                            const bool b2 = lane & 4;
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const float keep = b2 ? w8[i + 4] : w8[i], send = b2 ? w8[i] : w8[i + 4];
-                                w4[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 4));
-                            }
-                            const bool b1 = lane & 2;
-#pragma unroll
-                            for (int i = 0; i < 2; ++i) {
-                                const float keep = b1 ? w4[i + 2] : w4[i], send = b1 ? w4[i] : w4[i + 2];
-                                w2[i] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 2));
-                            }
-                            const bool b0 = lane & 1;
-                            x = fmaxf(b0 ? w2[1] : w2[0], __shfl_xor_sync(0xffffffffu, b0 ? w2[0] : w2[1], 1));
-                        }
-                        // my channel and whether I store it: 32 samples -> even lanes, channel (lane >> 1) & 15;
-                        // 16 samples -> every lane, channel = the bit pattern the halving steps selected
-                        const int ch = ns == 32 ? ((lane >> 1) & 15) : (((lane >> 3) & 1) * 8 + ((lane >> 2) & 1) * 4 + ((lane >> 1) & 1) * 2 + (lane & 1));
-                        if (pool_raw) x = fmaxf(x + sh[c0 + ch], lo);
-                        if (b_ok && (ns == 16 || (lane & 1) == 0) && c0 + ch < Cl) {
-                            p.out[b_off + (size_t)(c0 + ch) * p.npoint] = x;
-                            if (p.out_pm) p.out_pm[b_pm + c0 + ch] = x;
-                        }
-                        continue;
-                    }
-                    bar_group(grp);                              // previous readers of the staging tile are done
-#pragma unroll
-                    for (int j = 0; j < 4; ++j)
-                        *reinterpret_cast<float4 *>(pool + r * POOL_STRIDE + 4 * j) = make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-                    bar_group(grp);
-                    if (ns >= 16) {
-                        float x = pool[(g16 * 16) * POOL_STRIDE + q];
-#pragma unroll
-                        for (int s = 1; s < 16; ++s) x = fmaxf(x, pool[(g16 * 16 + s) * POOL_STRIDE + q]);
-                        if (ns == 32) x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, 16));
-                        if (ns > 32) {
-                            pool2[g16 * 16 + q] = x;
-                            bar_group(grp);
-                            const int per = ns >> 4;
-                            if ((g16 % per) == 0) {
-                                for (int s = 1; s < per; ++s) x = fmaxf(x, pool2[(g16 + s) * 16 + q]);
-                            }
-                        }
-                        if (pool_raw) x = fmaxf(x + sh[c0 + q], lo);
-                        if (e_ok && c0 + q < Cl) {
-                            p.out[e_off + (size_t)c0 * p.npoint] = x;
-                            if (p.out_pm) p.out_pm[e_pm + c0] = x;
-                        }
-                    } else {
-                        // nsample 4 or 8: 128/ns centres per tile, 16 channels each -> (16/ns) items per thread
-                        const int per16 = 16 / ns;
-                        for (int t = 0; t < per16; ++t) {
-                            const int row0 = g16 * 16 + t * ns;
-                            float x = pool[row0 * POOL_STRIDE + q];
-                            for (int s = 1; s < ns; ++s) x = fmaxf(x, pool[(row0 + s) * POOL_STRIDE + q]);
-                            if (pool_raw) x = fmaxf(x + sh[c0 + q], lo);
-                            const unsigned Rg = (unsigned)tile * TM + (unsigned)row0;
-                            if ((long)Rg < p.total_rows && c0 + q < Cl) {
-                                const unsigned pr = Rg >> p.log_ns, scene = pr / (unsigned)p.npoint, pp = pr - scene * (unsigned)p.npoint;
-                                p.out[((size_t)scene * p.out_stride_c + p.out_c_off + c0 + q) * p.npoint + pp] = x;
-                                if (p.out_pm) p.out_pm[((size_t)scene * p.npoint + pp) * p.out_stride_c + p.out_c_off + c0 + q] = x;
-                            }
-                        }
                     }
                 }
             }
-            tc_fence_before();
-            dphase ^= 1;
-            PRB_TRACE(2 * L + 1);
         }
     }
-
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 4 * NG + 1) tmem_dealloc(tmem, (uint32_t)p.tmem_cols);
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -770,99 +513,69 @@ int prb_mlp_pack_weights(int num_layers, int c_in, const int *c_out, const float
 
 namespace prb {
 
-int launch_chain_pipe(ChainParams &p, cudaStream_t st);   // mlp_pipe.cu
-
-// the pipelined kernel takes every segment unless the caller asks for the legacy one (prb_options.mlp_pipeline = 0) or
-// for the cp.async gather experiment, which only the legacy kernel implements
-static bool use_pipe() { return opts().mlp_pipeline != 0 && opts().mlp_gather == 0; }
-
-// launch one fused segment of the chain: size rings / TMEM to the segment, pick the CTAs-per-SM it allows
-static int launch_chain(ChainParams &p, cudaStream_t st) {
-    if (use_pipe()) return launch_chain_pipe(p, st);
-    int max_optin = 0;
-    {
-        int dev = 0;
-        PRB_CUDA(cudaGetDevice(&dev));
-        PRB_CUDA(cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+// dynamic shared memory of a fused segment [l0, l1) with an nb-deep weight ring
+static size_t segment_smem(const int *np, int n, int nb, int *work_bytes, int *b_stage_bytes) {
+    int np_total = 0, np_max = 0, mid_max = 0;
+    for (int i = 0; i < n; ++i) {
+        np_total += np[i];
+        np_max = np[i] > np_max ? np[i] : np_max;
+        if (i + 1 < n && np[i] > mid_max) mid_max = np[i];
     }
+    int work = A_SLOTS * A_STAGE_BYTES;                                    // >= the pool staging of both warpgroups
+    if (TM * mid_max * 4 > work) work = TM * mid_max * 4;
+    if (work_bytes) *work_bytes = work;
+    if (b_stage_bytes) *b_stage_bytes = np_max * KC * 4;
+    return chain_smem_bytes(work, nb, np_max * KC * 4, np_total, np[n - 1]) + sizeof(SmemFixed);
+}
+
+// launch one fused segment of the chain: size the weight ring to the segment, pick the CTAs per SM it allows
+static int launch_chain(ChainParams &p, cudaStream_t st) {
+    int max_optin = 0, dev = 0;
+    PRB_CUDA(cudaGetDevice(&dev));
+    PRB_CUDA(cudaDeviceGetAttribute(&max_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     p.num_tiles = (int)((p.total_rows + TM - 1) / TM);
     if (p.num_tiles == 0) return 0;
-    p.gather_mode = opts().mlp_gather;   // default 0; measured (profiles/r1_notes.md): register gather 1.53 ms, cp.async.cg 1.66, cp.async.ca 1.67 per batch of SA chains
+    p.tiles_per_item = (p.mode_out == OUT_SA_MAX && p.ns > TM) ? p.ns / TM : 1;
+    p.num_items = (p.num_tiles + p.tiles_per_item - 1) / p.tiles_per_item;
     const int L = p.num_layers;
-    int np_total = 0, np_max = 0;
-    for (int l = 0; l < L; ++l) { np_total += p.np[l]; np_max = p.np[l] > np_max ? p.np[l] : np_max; }
-    p.b_stage_bytes = (np_max < B_TILE_ROWS ? np_max : B_TILE_ROWS) * KC * 4;
-    int need = p.np[0];
-    if (L >= 2) need = p.np[0] + p.np[1];
-    if (L >= 3 && p.np[1] + p.np[2] > need) need = p.np[1] + p.np[2];
-    int cols = 32;
-    while (cols < need) cols <<= 1;
-    p.tmem_cols = cols;
-    p.dcol[0] = 0;
-    if (L >= 2) p.dcol[1] = cols - p.np[1];
-    if (L >= 3) p.dcol[2] = 0;
-    // Row-thread parallelism: NG groups of 4 row warps in one CTA (chunks dealt round-robin), or -- when TMEM and
-    // shared memory allow several CTAs per SM -- NG=1 with 2 or 3 independent CTAs (the 3-CTA build is capped at 112
-    // registers per thread).
-    const int sm_smem = 227 * 1024;
-    int ng = opts().mlp_ng;
-    const bool ng_forced = ng != 0;
-    int occ = 1;
-    if (ng == 0) ng = (cols <= 256) ? 1 : 2;
-    if (ng == 1) occ = 512 / cols > 3 ? 3 : 512 / cols;
-    // 129..256 TMEM columns: two CTAs fit either way, and two CTAs of 8 row warps beat two of 4 (measured per level,
-    // profiles/r1_notes.md: FP0 0.201 -> 0.165 ms, SA2 0.311 -> 0.295); the 3-CTA build stays best below 128 columns
-    if (!ng_forced && ng == 1 && occ == 2) ng = 2;
-    if (ng == 2) occ = 512 / cols >= 2 ? 2 : 1;
-    if (const int o = opts().mlp_occ; o >= 1 && o < occ) occ = o;
-    size_t smem = 0;
-    for (;; --occ) {
-        int depth = occ >= 2 ? 3 : 4;
-        for (; depth >= 2; --depth) {
-            smem = chain_smem_bytes(ng, depth, depth, p.b_stage_bytes, np_total);
-            if ((smem + 1024 + 3744) * occ <= (size_t)sm_smem && smem <= (size_t)max_optin) { p.na = p.nb = depth; break; }
-        }
-        if (depth >= 2 || occ == 1) break;
+    int np_total = 0, ns_max = 1;
+    for (int l = 0; l < L; ++l) {
+        np_total += p.np[l];
+        const int nsub0 = ((p.np[l] >> 5) + 1) >> 1;
+        ns_max = nsub0 > ns_max ? nsub0 : ns_max;
     }
-    PRB_REQUIRE(smem <= (size_t)max_optin, "mlp: %zu bytes of shared memory needed, %d available", smem, max_optin);
-    // Tiles are dealt statically (tile += gridDim.x), so a CTA that cannot start with the first wave doubles the
-    // kernel's duration.  When other streams hold SMs (BatchPipeline: the single-CTA-per-scene FPS of the next
-    // batches), PRB_MLP_SMS sizes the grid for the SMs that are actually free.
-    int sms = num_sms();
-    if (const int v = opts().mlp_sms; v >= 1 && v < sms) sms = v;
-    int grid = sms * occ;
-    if (grid > p.num_tiles) grid = p.num_tiles;
-#define PRB_LAUNCH_CHAIN(NGV, MB)                                                                                              \
-    do {                                                                                                                       \
-        PRB_CUDA(cudaFuncSetAttribute(mlp_chain_kernel<NGV, MB>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
-        mlp_chain_kernel<NGV, MB><<<grid, 128 * NGV + 64, smem, st>>>(p);                                                     \
-    } while (0)
-    if (ng == 1 && occ >= 3) PRB_LAUNCH_CHAIN(1, 3);
-    else if (ng == 1) PRB_LAUNCH_CHAIN(1, 2);
-    else if (ng == 2 && occ >= 2) PRB_LAUNCH_CHAIN(2, 2);
-    else if (ng == 2) PRB_LAUNCH_CHAIN(2, 1);
-    else PRB_LAUNCH_CHAIN(3, 1);
-#undef PRB_LAUNCH_CHAIN
-    return check_launch("mlp_chain_kernel");
+    // deepest weight ring that fits (a stage is one K chunk of the widest layer)
+    size_t smem = 0;
+    for (p.nb = NB_MAX; p.nb >= 2; --p.nb) {
+        smem = segment_smem(p.np, L, p.nb, &p.work_bytes, &p.b_stage_bytes) - sizeof(SmemFixed);
+        if (smem + sizeof(SmemFixed) <= (size_t)max_optin) break;
+    }
+    PRB_REQUIRE(p.nb >= 2, "mlp: %zu bytes of shared memory needed, %d available", smem + sizeof(SmemFixed), max_optin);
+    // the accumulators of the widest layer set the register budget, and with it how many CTAs share an SM: several
+    // CTAs of a narrow chain overlap one another's latency-bound gathers
+    auto go = [&](auto kern) -> int {
+        PRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        int occ = 0;
+        PRB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, CHAIN_THREADS, smem));
+        if (occ < 1) occ = 1;
+        if (const int o = opts().mlp_occ; o >= 1 && o < occ) occ = o;
+        int sms = num_sms();
+        if (const int v = opts().mlp_sms; v >= 1 && v < sms) sms = v;
+        const int grid = p.num_items < sms * occ ? p.num_items : sms * occ;
+        kern<<<grid, CHAIN_THREADS, smem, st>>>(p);
+        return check_launch("mlp_chain_kernel");
+    };
+    if (ns_max <= 2) return go(mlp_chain_kernel<2, 3>);
+    if (ns_max <= 4) return go(mlp_chain_kernel<4, 2>);
+    return go(mlp_chain_kernel<8, 1>);
 }
 
-// TMEM feasibility of fusing layers [l0, l1).  Legacy kernel: accumulators ping-pong between column 0 and the top.
-// Pipelined kernel: every mid layer owns a region, the last layer needs at least one 32-column slice buffer.
-static bool fits_legacy(const LayerGeom *g, int l0, int l1) {
-    const int n = l1 - l0;
-    if (n == 1) return g[l0].np <= 512;
-    if (n == 2) return g[l0].np + g[l0 + 1].np <= 512;
-    return g[l0].np + g[l0 + 1].np <= 512 && g[l0 + 2].np + g[l0 + 1].np <= 512;
+// can layers [l0, l1) run as one launch: the activations of the widest inner layer and two weight stages in shared memory
+static bool fits(const LayerGeom *g, int l0, int l1) {
+    int np[MAX_LAYERS];
+    for (int l = l0; l < l1; ++l) np[l - l0] = g[l].np;
+    return segment_smem(np, l1 - l0, 2, nullptr, nullptr) <= 227 * 1024;
 }
-static bool fits_pipe(const LayerGeom *g, int l0, int l1) {
-    int mid = 0;
-    for (int l = l0; l + 1 < l1; ++l) mid += g[l].np;
-    // keep at least two 64-column slice buffers (or the whole last layer) next to the mid regions
-    const int last = g[l1 - 1].np;
-    const int z = last < 64 ? last : 64;
-    return g[l1 - 1].np <= 512 && mid + (l1 - l0 > 1 ? 2 * z : 0) <= 512;
-}
-static bool fits(const LayerGeom *g, int l0, int l1) { return use_pipe() ? fits_pipe(g, l0, l1) : fits_legacy(g, l0, l1); }
 
 struct ChainIO {
     int kind, split;          // packing kind (0 SA, 1 FP, 2 DIRECT) and its split argument
@@ -878,12 +591,12 @@ static size_t chain_workspace_bytes(long rows, int L, int kind, int c_in, int sp
     // worst case: two ping-pong row buffers of the widest padded layer
     int wmax = 0;
     for (int l = 0; l < L; ++l) wmax = g[l].np > wmax ? g[l].np : wmax;
-    bool split_needed = !fits_legacy(g, 0, L) || !fits_pipe(g, 0, L);   // either kernel may be chosen at launch time
+    const bool split_needed = !fits(g, 0, L);
     const size_t rows_pad = (size_t)((rows + TM - 1) / TM * TM);
     return split_needed ? 2 * (rows_pad * wmax * sizeof(float) + 256) : 256;
 }
 
-// run the whole chain, splitting where TMEM cannot hold two consecutive accumulators
+// run the whole chain, splitting where shared memory cannot hold a segment's activations and weight stages
 static int run_chain(const ChainIO &io, const prb_mlp_desc *mlp, void *workspace, size_t workspace_bytes, cudaStream_t st) {
     const int L = mlp->num_layers;
     PRB_REQUIRE(io.rows < 0x7fffff00L, "mlp: %ld rows exceed the 2^31 row limit", io.rows);
@@ -908,9 +621,6 @@ static int run_chain(const ChainIO &io, const prb_mlp_desc *mlp, void *workspace
         ChainParams p = io.base;
         p.unit_scale = mlp->scale ? 0 : 1;
         p.linear_last = (l1 == L && (mlp->flags & 1)) ? 1 : 0;
-        p.trace = opts().mlp_trace ? 1 : 0;
-        p.a_tmem = opts().mlp_atmem ? 1 : 0;   // default 1; measured (profiles/r1_notes.md): SA chains 1.124 -> 1.088 ms per batch; 0 = shared-memory stages
-        p.sleepy = opts().mlp_sleepy;
         p.total_rows = io.rows;
         p.num_layers = l1 - l0;
         for (int l = l0; l < l1; ++l) {
@@ -960,15 +670,6 @@ static int run_chain(const ChainIO &io, const prb_mlp_desc *mlp, void *workspace
 }  // namespace prb
 
 extern "C" {
-
-// debug: copy the phase trace of the last traced launch (32 tiles x 16 stamps, clock64 of CTA 0's row thread 0)
-PRB_API int prb_debug_mlp_trace(long long *dst) {
-    PRB_CUDA(cudaDeviceSynchronize());
-    PRB_CUDA(cudaMemcpyFromSymbol(dst, g_trace, sizeof(long long) * 32 * 16));
-    static long long zeros[32 * 16];
-    PRB_CUDA(cudaMemcpyToSymbol(g_trace, zeros, sizeof(zeros)));
-    return 0;
-}
 
 PRB_API size_t prb_sa_workspace_bytes(int b, int npoint, int nsample, int c_feat, int num_layers, const int *c_out) {
     return chain_workspace_bytes((long)b * npoint * nsample, num_layers, 0, 3 + c_feat, c_feat, c_out);
@@ -1047,7 +748,6 @@ PRB_API int prb_mlp_rows2(long rows, int c_a, const float *a_rows, int a_pitch, 
     PRB_REQUIRE(rows >= 0 && c_a > 0 && a_rows && a_pitch >= c_a && mlp && out_rows, "mlp_rows2: bad arguments");
     PRB_REQUIRE(c_b >= 0 && (c_b == 0 || (b_rows && b_pitch >= c_b)), "mlp_rows2: bad second segment");
     PRB_REQUIRE(mlp->c_in == c_a + c_b, "mlp_rows2: c_in %d != %d + %d", mlp->c_in, c_a, c_b);
-    PRB_REQUIRE(c_b == 0 || use_pipe(), "mlp_rows2: two input segments need the pipelined kernel (mlp_pipeline = 1, mlp_gather = 0)");
     const int np_last = (mlp->c_out[mlp->num_layers - 1] + 31) / 32 * 32;
     PRB_REQUIRE(out_pitch >= np_last && (out_pitch & 3) == 0, "mlp_rows2: out_pitch %d must be >= %d and a multiple of 4", out_pitch, np_last);
     if (rows == 0) return 0;

@@ -375,8 +375,8 @@ struct FusedAssign { const int *sorted_idx, *cell_start; const SceneGrid *grids;
 // flat, the output IS the cnt x (3+C) source block repeated -- out[e] = block[e mod (cnt*(3+C))].  The block is staged in
 // shared memory once (coalesced row reads, canonical transform applied there) and streamed out with 128-bit stores;
 // boxes with more points than the staging area holds take the direct path (sources through L1).
-constexpr int RB_STAGE_FLOATS = 12 * 1024;   // 48 KB: 92 rows of 133 floats.  Data dependent (profiles/r2_notes.md): 24 KB is 3 % faster when boxes
-                                             // hold a few points, 48 KB 20 % faster with ~60 points per enlarged RoI (the RCNN stage's regime)
+constexpr int RB_STAGE_FLOATS = 12 * 1024;   // 48 KB: 92 rows of 133 floats.  Data dependent: a smaller area suits boxes that
+                                             // hold a few points, 48 KB the ~60 points per enlarged RoI of the RCNN stage
 
 __global__ void __launch_bounds__(RP_THREADS) roipool3d_copy_kernel(int N, int M, int C, int S, const float *__restrict__ xyz,
                                                                     const float *__restrict__ pts_feature,

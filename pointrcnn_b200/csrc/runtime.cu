@@ -21,7 +21,7 @@ void count_launch(int n) { g_launches.fetch_add((unsigned long long)n, std::memo
 int num_sms() {
     static std::atomic<int> cache[64];   // per device ordinal; 0 = not queried yet
     int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 148;  // B200
+    if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;  // H100 SXM
     int sms = cache[dev].load(std::memory_order_relaxed);
     if (sms == 0) {
         if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) sms = 148;

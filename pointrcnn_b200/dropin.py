@@ -1,4 +1,4 @@
-"""Register the B200 implementations under the reference's import names.
+"""Register the H100 implementations under the reference's import names.
 
     import pointrcnn_b200.dropin as dropin; dropin.activate()
 

@@ -1,6 +1,6 @@
 """`roipool3d_cuda` -- same exports as lib/utils/roipool3d/src/roipool3d.cpp:198-203.
 
-`forward` / `forward_slow` run the one-pass B200 kernel.  The two CPU twins the reference exports for its
+`forward` / `forward_slow` run the one-pass H100 kernel.  The two CPU twins the reference exports for its
 dataloader (`pts_in_boxes3d_cpu`, `roipool3d_cpu`, roipool3d.cpp:97-195) are host functions by contract;
 they are restated here in numpy on top of the same predicate arithmetic.
 """

@@ -1,5 +1,5 @@
 """Mirror of lib/utils/iou3d/iou3d_utils.py (reference :6-87): boxes_iou_bev, boxes_iou3d_gpu, nms_gpu,
-nms_normal_gpu -- same signatures and return values, on top of the B200 `iou3d_cuda` natives.
+nms_normal_gpu -- same signatures and return values, on top of the H100 `iou3d_cuda` natives.
 
 nms_gpu / nms_normal_gpu keep the reference contract (sorted by score, returns original indices of the kept
 boxes, int64 on the GPU) but run the greedy scan on the device: one 4-byte D2H for the count instead of a

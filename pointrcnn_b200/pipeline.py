@@ -1,11 +1,9 @@
 """Batch pipelining: consecutive, independent batches on alternating CUDA streams, optionally as CUDA graphs.
 
 Furthest-point sampling is a dependency chain (4095 serial rounds for the first RPN level) that runs as one CTA per
-scene (16 of 148 SMs), and nothing else of the SAME batch can run before it ends.  Consecutive batches are
+scene (16 of 132 SMs), and nothing else of the SAME batch can run before it ends.  Consecutive batches are
 independent (the reference's eval loop processes them one after another), so batch i+1's sampling chain can
-overlap batch i's neighbour searches and tensor-core MLPs.  Measured on B200 (RPN backbone, 16 scenes of 16384
-points per batch): 4.68 ms per batch back to back on one stream, 2.13 ms with six batches in flight
-(profiles/r1_notes.md).  Results are identical to the sequential loop, bit for bit -- only the stream assignment
+overlap batch i's neighbour searches and tensor-core MLPs.  Results are identical to the sequential loop, bit for bit -- only the stream assignment
 differs (tests/test_gpu_mlp.py::test_batch_pipeline_matches_sequential).
 
 `graphs=True` captures `fn` once per slot (stream) into a CUDA graph and replays it: the ~45 native launches and the
@@ -49,7 +47,7 @@ class BatchPipeline:
         """run fn on x (already on the slot's stream); returns the output tuple.
         With several batches in flight the library runs in THROUGHPUT mode (`prb_options.mlp_fill = 0`): small single-layer
         chain launches are not dealt to extra column groups just to fill idle SMs -- those SMs belong to the other batches
-        (+1.2 % at 16 scenes per batch, profiles/r2_notes.md; baked into the graph at capture)."""
+        (baked into the graph at capture)."""
         from . import _cabi
         if len(self.slots) > 1 and _cabi.lib() is not None:
             with _cabi.options(mlp_fill=0):

@@ -1,4 +1,4 @@
-"""Two-stage inference on the B200 path without the reference tree: the eval branch of lib/net/point_rcnn.py:26-70 (RPN ->
+"""Two-stage inference on the H100 path without the reference tree: the eval branch of lib/net/point_rcnn.py:26-70 (RPN ->
 proposal layer -> RCNN) and the detection post-processing of tools/eval_rcnn.py:485-620 (decode -> score threshold ->
 rotated NMS) with the NMS scan on the device.  Sub-module names are the reference's (`rpn.*` = lib.net.rpn.RPN keys,
 `rcnn_net.*` = lib.net.rcnn_net.RCNNNet keys), so a PointRCNN checkpoint loads as it is.

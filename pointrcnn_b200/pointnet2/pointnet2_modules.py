@@ -7,7 +7,7 @@ Two execution paths per module, chosen per call:
            FPS(+new_xyz) -> [one ball-query scan for both radii] -> per scale ONE tensor-core kernel that
            gathers the neighbourhood, runs the whole SharedMLP and max-pools (csrc/mlp_tc.cu).  FP modules:
            three_nn(+weights) -> ONE kernel that interpolates, concatenates the skip features and runs the MLP.
-  unfused  (training / anything else): the reference's op-by-op sequence on the B200 natives with
+  unfused  (training / anything else): the reference's op-by-op sequence on the H100 natives with
            torch.nn convolutions, full autograd support.
 `config.override(disable_fused=True)` forces the unfused path (used by tests to cross-check the two).
 """
@@ -391,8 +391,7 @@ class PointnetFPModule(nn.Module):
         c1 = list(self.mlp.children())[0].conv.out_channels
         # interpolation commutes with the (linear) first layer: project the m known points once instead of gathering
         # c_known floats for each of the 3 neighbours of every one of the n >= m unknown points
-        # measured (profiles/r2_notes.md): pays at the finest level (262144 rows: 0.267 -> 0.231 ms incl. the projection launch),
-        # not at the coarse ones, where the extra launch costs more than the narrower gather saves
+        # only worth it at the finest level: at the coarse ones the extra launch costs more than the narrower gather saves
         project = (self.project_known and config.get("fp_project") and _fold_scale() and c1 < c_known and n >= m
                    and B * n >= config.get("fp_project_min_rows"))
         desc = self._fused.get(self.mlp, 1, c_known, dev, project_known=project)

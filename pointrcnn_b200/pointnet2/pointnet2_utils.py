@@ -1,6 +1,6 @@
 """Mirror of pointnet2_lib/pointnet2/pointnet2_utils.py (reference :10-290): the autograd Functions
 furthest_point_sample / gather_operation / three_nn / three_interpolate / grouping_operation / ball_query
-and the QueryAndGroup / GroupAll modules, on top of the B200 `pointnet2_cuda` natives.
+and the QueryAndGroup / GroupAll modules, on top of the H100 `pointnet2_cuda` natives.
 
 Same names, argument order, output shapes/dtypes and zero-/1e10-fill obligations as the reference.
 Extras (used by the fused module paths, not part of the reference API): furthest_point_sample_xyz,

@@ -1,4 +1,4 @@
-"""The RCNN (stage-2) network of lib/net/rcnn_net.py:14-190 on the B200 path, eval / inference branch, without the
+"""The RCNN (stage-2) network of lib/net/rcnn_net.py:14-190 on the H100 path, eval / inference branch, without the
 reference tree or its global EasyDict:
 
     roipool3d (+ canonical transform, fused) -> xyz_up_layer + merge_down_layer -> 3 PointnetSAModule -> cls / reg heads

@@ -1,5 +1,5 @@
 """Mirror of lib/utils/roipool3d/roipool3d_utils.py (reference :7-108): roipool3d_gpu, pts_in_boxes3d_cpu,
-roipool_pc_cpu, roipool3d_cpu -- same signatures, on top of the B200 `roipool3d_cuda` natives.
+roipool_pc_cpu, roipool3d_cpu -- same signatures, on top of the H100 `roipool3d_cuda` natives.
 
 Extra: roipool3d_gpu(..., canonical_rois=rois) fuses the canonical transform of lib/net/rcnn_net.py:146-152
 into the pooling kernel's store.

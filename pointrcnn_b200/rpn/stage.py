@@ -1,4 +1,4 @@
-"""The whole RPN stage of lib/net/rpn.py:11-94 on the B200 path, without the reference tree or its global EasyDict:
+"""The whole RPN stage of lib/net/rpn.py:11-94 on the H100 path, without the reference tree or its global EasyDict:
 
     Pointnet2MSG backbone -> rpn_cls_layer / rpn_reg_layer -> ProposalLayer (eval: rois + roi scores)
 

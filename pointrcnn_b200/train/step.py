@@ -1,10 +1,10 @@
-"""One RPN training step on the B200 path (BASELINE configs[2]; reference: tools/train_rcnn.py:199-233 +
+"""One RPN training step on the H100 path (BASELINE configs[2]; reference: tools/train_rcnn.py:199-233 +
 lib/net/train_functions.py:12-52): forward in training mode (batch-statistics BatchNorm, Dropout), bin-based loss,
 backward, gradient all-reduce over the data-parallel ranks, optimizer step.
 
 Forward / backward use the reference-shaped op-by-op path of the mirror modules: this repo's sampling / neighbour / grouping
 / interpolation natives with their scatter backward kernels (gather_points_grad, group_points_grad,
-three_interpolate_grad), the shared MLPs through cuDNN / cuBLAS with torch autograd.  (The fused tcgen05 chain is an
+three_interpolate_grad), the shared MLPs through cuDNN / cuBLAS with torch autograd.  (The fused tensor-core chain is an
 eval-mode kernel: batch-statistics BatchNorm couples all tiles of a launch.)  What this module adds over the reference's
 loop: no `.item()` inside the loss, per-rank processes instead of nn.DataParallel's per-step replicate / scatter / gather,
 and the bucketed all-reduce of `parallel_utils.GradBucketReducer` overlapped with backward.

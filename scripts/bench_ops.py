@@ -1,6 +1,6 @@
 """Secondary measurements for SURVEY 8 rows a12-a16 (BASELINE configs 4/5 shapes): roipool3d, IoU matrices, NMS --
 this repo's kernels next to the reference's own kernels (oracle/_ref), CUDA events, inputs resident on the device.
-Prints one JSON object; recorded under profiles/."""
+Prints one JSON object."""
 import json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -11,7 +11,7 @@ from pointrcnn_b200.ext import iou3d_cuda, roipool3d_cuda
 from pointrcnn_b200.iou3d import iou3d_utils
 
 dev = torch.device("cuda:0")
-peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))) if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else {"hbm_gbs": 6650.0}
+peaks = {"hbm_gbs": 3350.0}   # H100 SXM data sheet (700 W card)
 flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)
 
 

@@ -20,7 +20,7 @@ from pointrcnn_b200.rpn.proposal_layer import ProposalLayer, decode_rpn_proposal
 
 
 def loop_reference_shape(scores, proposals, pre_tot, post_tot, thresh, nms_type):
-    """the reference's per-scene control flow (proposal_layer.py:34-118) on the B200 NMS natives"""
+    """the reference's per-scene control flow (proposal_layer.py:34-118) on the H100 NMS natives"""
     B = scores.shape[0]
     ret_b = scores.new_zeros(B, post_tot, 7)
     ret_s = scores.new_zeros(B, post_tot)

@@ -1,5 +1,5 @@
 """Full RPN stage (backbone -> cls/reg heads -> proposal layer, TEST quotas), B=16 x 16384 points, pipelined:
-everything on the B200 path against the same backbone followed by torch heads + the reference-shaped Python proposal
+everything on the H100 path against the same backbone followed by torch heads + the reference-shaped Python proposal
 loop on this repo's NMS natives.  Random weights, synthetic scenes (scores are not meaningful, the work is)."""
 import json
 import os

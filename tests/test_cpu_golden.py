@@ -1,5 +1,5 @@
 """CPU suite: the oracle against the golden vectors produced by the reference's own CUDA kernels
-(oracle/make_golden.py run on a B200 through gpurun; tests/golden/reference_kernels.npz)."""
+(oracle/make_golden.py run on a GPU; tests/golden/reference_kernels.npz)."""
 import os
 import sys
 

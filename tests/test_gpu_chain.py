@@ -1,5 +1,5 @@
 """End-to-end chain (BASELINE configs[3]/[4], VERDICT r1 item 6): RPN backbone -> heads -> proposal layer -> roipool3d
-(+ canonical transform) -> RCNN SA stack -> decode -> final rotated NMS, from the repo's own modules on the B200
+(+ canonical transform) -> RCNN SA stack -> decode -> final rotated NMS, from the repo's own modules on the H100
 natives, against the SAME chain on the reference's own kernels (oracle/_ref) + stock torch ops.
 
 MLP outputs carry TF32 rounding, so stage N+1 of both chains is fed THIS repo's stage-N output: every index / keep /
@@ -74,7 +74,7 @@ def test_rpn_stage_against_reference_kernels(cuda, chain):
         rel = (out["backbone_features"] - rfeats).abs().max().item() / rfeats.abs().max().item()
         assert torch.equal(out["backbone_xyz"], rxyz)
         assert rel <= TOL_BACKBONE, "backbone features vs reference kernels + fp32 cuDNN: %g" % rel
-        # heads on OUR features: fused tcgen05 heads vs the torch modules
+        # heads on OUR features: fused tensor-core heads vs the torch modules
         cls_t = _fp32(lambda: model.rpn.rpn_cls_layer(out["backbone_features"]).transpose(1, 2).contiguous())
         reg_t = _fp32(lambda: model.rpn.rpn_reg_layer(out["backbone_features"]).transpose(1, 2).contiguous())
     assert (out["rpn_cls"] - cls_t).abs().max().item() <= TOL * cls_t.abs().max().item()
@@ -121,7 +121,7 @@ def test_roipool_and_rcnn_stage_against_reference_kernels(cuda, chain):
         assert (got[..., 0:3] - rp[..., 0:3]).abs().max().item() <= 2e-5, "canonical xyz differ"
         nonempty = int((empty == 0).sum())
         assert nonempty >= 8 * 20, "too few non-empty RoIs (%d) for a meaningful stage-2 check" % nonempty
-        # RCNN SA stack on OUR pooled points: fused tcgen05 path vs the op-by-op path (our index natives + fp32 cuDNN)
+        # RCNN SA stack on OUR pooled points: fused tensor-core path vs the op-by-op path (our index natives + fp32 cuDNN)
         cls_f, reg_f = rcnn.forward_pts(pts_input)
         with config.override(disable_fused=True):
             cls_u, reg_u = _fp32(lambda: rcnn.forward_pts(pts_input))

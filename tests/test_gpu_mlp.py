@@ -1,4 +1,4 @@
-"""GPU tests of the tcgen05 MLP chain and of the fused SA / FP module paths.
+"""GPU tests of the wgmma MLP chain and of the fused SA / FP module paths.
 
 Tolerances.  The reference's MLP is torch.nn.Conv2d (cuDNN, TF32 allowed by torch's default) and is not
 pinned by any reference test (SURVEY.md 8c).  Two checks:
@@ -118,7 +118,7 @@ ROW_CASES = [
     (1000, [40, 48]),                # K and N not multiples of 32, tail tile
     (4096, [99, 64, 64, 128]),       # SA2 scale 0 shape
     (3000, [259, 128, 196, 256]),    # SA3: N padded 196 -> 224
-    (2000, [515, 256, 256, 512]),    # SA4 s0: split after two layers (N=512 needs the whole TMEM)
+    (2000, [515, 256, 256, 512]),    # SA4 s0: split after two layers (N=512 layers: one launch each)
     (1500, [515, 256, 384, 512]),    # SA4 s1: every layer its own launch
     (20000, [257, 128, 128]),        # FP0, many tiles per CTA (ring wrap-around, phase bits)
     (700, [1536, 512, 512]),         # FP3: two N halves per K chunk
@@ -455,7 +455,7 @@ def test_c1_single_sa_layer_at_baseline_shape(cuda):
 
 
 def test_training_path_autograd(cuda):
-    """grad-enabled calls take the op-by-op path and back-propagate through the B200 scatter kernels"""
+    """grad-enabled calls take the op-by-op path and back-propagate through the H100 scatter kernels"""
     torch.manual_seed(4)
     sa = pm.PointnetSAModuleMSG(npoint=64, radii=[0.3], nsamples=[16], mlps=[[8, 16, 32]], bn=True).to(cuda).train()
     fp = pm.PointnetFPModule(mlp=[32 + 8, 16]).to(cuda).train()

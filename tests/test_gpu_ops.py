@@ -1,6 +1,6 @@
-"""GPU parity tests (run with -m gpu on the B200 box): every native of the C ABI against
+"""GPU parity tests (run with -m gpu on an H100): every native of the C ABI against
   (1) the CPU oracle (oracle/pointops_oracle.c, bit-exact for index work), and
-  (2) the reference's own CUDA kernels rebuilt for sm_100a (oracle/_ref) when that library is present.
+  (2) the reference's own CUDA kernels rebuilt for sm_90a (oracle/_ref) when that library is present.
 Calls go through the reference-named extension modules / Python wrappers, i.e. through the C ABI.
 """
 import os

@@ -1,4 +1,4 @@
-"""Training path on the B200 natives (BASELINE configs[2], VERDICT r1 row x1): gradients through the op-by-op path -- this
+"""Training path on the H100 natives (BASELINE configs[2], VERDICT r1 row x1): gradients through the op-by-op path -- this
 repo's gather / grouping / interpolation forward kernels and their atomic scatter backward kernels, cuDNN MLPs -- against
 the same network with every index op expressed in plain torch (advanced indexing, torch autograd), and the RPN training
 step (batch-statistics BN, bin-based loss, bucketed gradient reducer, fused Adam)."""

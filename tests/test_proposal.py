@@ -142,7 +142,7 @@ def test_fused_rpn_heads_match_torch(cuda, n_pts, with_twin):
 def test_golden_holds_with_the_reference_nms_kernel(cuda, gold, case, monkeypatch):
     """The golden vectors were produced by the reference's own Python with the CPU oracle standing in for its NMS
     extension (no GPU in the build container).  Here every NMS call of that pipeline is served by the reference's OWN
-    kernel + host scan (oracle/_ref: nmsLauncher / nmsNormalLauncher, iou3d.cpp:73-170) on the B200 and the result must
+    kernel + host scan (oracle/_ref: nmsLauncher / nmsNormalLauncher, iou3d.cpp:73-170) on the H100 and the result must
     be the committed golden, rotated cases included -- i.e. the goldens are what the reference produces end to end."""
     from oracle import refgpu as R
     if not R.available():
