@@ -13,7 +13,7 @@ constexpr int A_SLOTS = 3;           // layer-0 A chunks in flight (gather of ch
 constexpr int NB_MAX = 4;            // weight ring depth upper bound (runtime depth in ChainParams)
 constexpr int MAX_LAYERS = 3;
 constexpr int MAX_NP = 512;
-constexpr int NSUB_MAX = 8;          // 32-column MMA subtiles per warpgroup (2 warpgroups x 8 x 32 = MAX_NP)
+constexpr int NSUB_MAX = 8;          // 32-column subtiles per warpgroup (2 warpgroups x 8 x 32 = MAX_NP; wgmma N <= 256)
 constexpr int POOL_STRIDE = 33;      // floats per row of a warpgroup's 64 x 32 max-pool staging tile (conflict-free columns)
 constexpr int CHAIN_THREADS = 2 * 128 + 32;       // two MMA / epilogue warpgroups + one weight-producer warp
 
@@ -95,22 +95,74 @@ __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_grou
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 // the accumulator registers are written asynchronously: keep the compiler from moving their uses across a wait
-__device__ __forceinline__ void reg_fence(float (&d)[16]) {
+template <int N>
+__device__ __forceinline__ void reg_fence(float (&d)[N]) {
 #pragma unroll
-    for (int i = 0; i < 16; ++i) asm volatile("" : "+f"(d[i])::"memory");
+    for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-// D(64x32, fp32 registers) (+)= A(64x8, smem desc) * B(32x8, smem desc)^T, tf32 operands, both K-major.
-// Register q of thread T in warp w of the warpgroup: row 16w + T/4 + 8*((q>>1)&1), column 8*(q>>2) + 2*(T%4) + (q&1).
-__device__ __forceinline__ void wgmma_tf32_n32(float (&d)[16], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %18, 0;\n\t"
-        "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 "
-        "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
-          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+
+// D(64 x 32*NSUB, fp32 registers) (+)= A(64x8, smem desc) * B(32*NSUB x 8, smem desc)^T, tf32 operands, both K-major:
+// one wgmma m64nNk8 (N = 32*NSUB) on the first 16*NSUB registers of the flat accumulator d.  Register 16j + q of
+// thread T in warp w of the warpgroup: row 16w + T/4 + 8*((q>>1)&1), column 32j + 8*(q>>2) + 2*(T%4) + (q&1) -- the
+// m64nN fragment is NSUB m64n32 fragments side by side.
+#define PRB_REGS0 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15"
+#define PRB_REGS1 "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+#define PRB_REGS2 "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47"
+#define PRB_REGS3 "%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+#define PRB_REGS4 "%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79"
+#define PRB_REGS5 "%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95"
+#define PRB_REGS6 "%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111"
+#define PRB_REGS7 "%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+#define PRB_ACC4(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3])
+#define PRB_ACC16(i) PRB_ACC4(i), PRB_ACC4(i + 4), PRB_ACC4(i + 8), PRB_ACC4(i + 12)
+// N: instruction width; REGS: the accumulator operands; IA, IB, IS: operand numbers of a_desc, b_desc, accumulate
+#define PRB_WGMMA_TF32(N, REGS, IA, IB, IS, ...)                                                                 \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %" IS ", 0;\n\t"                                           \
+                 "wgmma.mma_async.sync.aligned.m64n" N "k8.f32.tf32.tf32 {" REGS "}, %" IA ", %" IB ", p, 1, 1;\n\t}" \
+                 : __VA_ARGS__                                                                                     \
+                 : "l"(a_desc), "l"(b_desc), "r"(accumulate))
+template <int NSUB, int NS>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[16 * NS], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    static_assert(NSUB >= 1 && NSUB <= NS && NS <= NSUB_MAX, "wgmma_tf32: 1 <= NSUB <= NS <= NSUB_MAX");
+    if constexpr (NSUB == 1) {
+        PRB_WGMMA_TF32("32", PRB_REGS0, "16", "17", "18", PRB_ACC16(0));
+    } else if constexpr (NSUB == 2) {
+        PRB_WGMMA_TF32("64", PRB_REGS0 "," PRB_REGS1, "32", "33", "34", PRB_ACC16(0), PRB_ACC16(16));
+    } else if constexpr (NSUB == 3) {
+        PRB_WGMMA_TF32("96", PRB_REGS0 "," PRB_REGS1 "," PRB_REGS2, "48", "49", "50", PRB_ACC16(0), PRB_ACC16(16),
+                       PRB_ACC16(32));
+    } else if constexpr (NSUB == 4) {
+        PRB_WGMMA_TF32("128", PRB_REGS0 "," PRB_REGS1 "," PRB_REGS2 "," PRB_REGS3, "64", "65", "66", PRB_ACC16(0),
+                       PRB_ACC16(16), PRB_ACC16(32), PRB_ACC16(48));
+    } else if constexpr (NSUB == 5) {
+        PRB_WGMMA_TF32("160", PRB_REGS0 "," PRB_REGS1 "," PRB_REGS2 "," PRB_REGS3 "," PRB_REGS4, "80", "81", "82",
+                       PRB_ACC16(0), PRB_ACC16(16), PRB_ACC16(32), PRB_ACC16(48), PRB_ACC16(64));
+    } else if constexpr (NSUB == 6) {
+        PRB_WGMMA_TF32("192", PRB_REGS0 "," PRB_REGS1 "," PRB_REGS2 "," PRB_REGS3 "," PRB_REGS4 "," PRB_REGS5, "96", "97",
+                       "98", PRB_ACC16(0), PRB_ACC16(16), PRB_ACC16(32), PRB_ACC16(48), PRB_ACC16(64), PRB_ACC16(80));
+    } else if constexpr (NSUB == 7) {
+        PRB_WGMMA_TF32("224", PRB_REGS0 "," PRB_REGS1 "," PRB_REGS2 "," PRB_REGS3 "," PRB_REGS4 "," PRB_REGS5 "," PRB_REGS6,
+                       "112", "113", "114", PRB_ACC16(0), PRB_ACC16(16), PRB_ACC16(32), PRB_ACC16(48), PRB_ACC16(64),
+                       PRB_ACC16(80), PRB_ACC16(96));
+    } else {
+        PRB_WGMMA_TF32("256",
+                       PRB_REGS0 "," PRB_REGS1 "," PRB_REGS2 "," PRB_REGS3 "," PRB_REGS4 "," PRB_REGS5 "," PRB_REGS6
+                                 "," PRB_REGS7,
+                       "128", "129", "130", PRB_ACC16(0), PRB_ACC16(16), PRB_ACC16(32), PRB_ACC16(48), PRB_ACC16(64),
+                       PRB_ACC16(80), PRB_ACC16(96), PRB_ACC16(112));
+    }
 }
+#undef PRB_WGMMA_TF32
+#undef PRB_ACC16
+#undef PRB_ACC4
+#undef PRB_REGS0
+#undef PRB_REGS1
+#undef PRB_REGS2
+#undef PRB_REGS3
+#undef PRB_REGS4
+#undef PRB_REGS5
+#undef PRB_REGS6
+#undef PRB_REGS7
 
 // relu + round-to-nearest-even to tf32 in ONE instruction
 __device__ __forceinline__ float relu_to_tf32(float x) {

@@ -10,10 +10,15 @@
 //
 // Structure (persistent CTAs over 64-row tiles; rows = (centre, sample) pairs or points):
 //   warpgroups 0, 1  gather layer 0's A operand chunk by chunk (32 K-columns = one 128-byte swizzle row) into a
-//                    ring of three shared-memory slots, issue wgmma m64n32k8 tf32 with fp32 register accumulators --
-//                    the layer's output columns are split between the two warpgroups -- and run the epilogues:
-//                    layer l < L-1 writes relu(acc + shift) as tf32 into the resident activation buffer (the next
-//                    layer's A operand, all of its K chunks), the last layer pools / stores.
+//                    ring of three shared-memory slots, issue wgmma tf32 with fp32 register accumulators -- the
+//                    layer's output columns are split between the two warpgroups, and each warpgroup covers its
+//                    nsub * 32 columns with ONE m64n(32 nsub)k8 instruction per K=8 step, so the A slice is read
+//                    from shared memory once per step -- and run the epilogues: layer l < L-1 writes
+//                    relu(acc + shift) as tf32 into the resident activation buffer (the next layer's A operand, all
+//                    of its K chunks), the last layer pools / stores.
+//                    A chunk's MMAs are one commit group and stay in flight: the warpgroup waits for the previous
+//                    chunk's group only (wgmma_wait<1>), then releases that chunk's weight stage and gathers the
+//                    next chunk while the current one runs.  The whole layer is drained before its epilogue.
 //   warp 8           weight producer: one thread streams pre-packed weight chunks (already in the K-major
 //                    SWIZZLE_128B image, see prb_mlp_pack_weights) with cp.async.bulk + mbarrier transaction counts.
 // Chains whose activation buffer and weight stages do not fit in shared memory are split into several launches by
@@ -29,6 +34,53 @@
 namespace prb {
 
 // ------------------------------------------------------------------------------------------------ kernel
+// element l of a per-layer parameter array, by selects: indexing the kernel parameter with a runtime l would copy
+// the array to local memory
+template <typename T>
+__device__ __forceinline__ T per_layer(const T (&a)[MAX_LAYERS], int l) {
+    static_assert(MAX_LAYERS == 3, "per_layer: one select per layer");
+    return l == 0 ? a[0] : l == 1 ? a[1] : a[2];
+}
+
+// The MMAs of one K chunk over a warpgroup's nsub * 32 output columns: one m64n(32*NSUB)k8 instruction per K=8 step,
+// KSTEPS steps in K order, straight-line.  nsub and ksteps are warp-uniform and select the sequence before the first
+// wgmma, so no predicate sits between wgmma_fence and wgmma_commit (a divergent one makes ptxas serialise every
+// wgmma behind its own arrive / wait).
+template <int NSUB, int KSTEPS, int NS>
+__device__ __forceinline__ void mma_steps(float (&acc)[16 * NS], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+#pragma unroll
+    for (int ks = 0; ks < KSTEPS; ++ks)
+        wgmma_tf32<NSUB, NS>(acc, adesc + (uint64_t)(2 * ks), bdesc + (uint64_t)(2 * ks), ks > 0 ? 1u : accumulate);
+}
+template <int NSUB, int NS>
+__device__ __forceinline__ void mma_chunk_n(float (&acc)[16 * NS], int ksteps, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    static_assert(KC / 8 == 4, "mma_chunk_n: one case per K=8 step of a chunk");
+    switch (ksteps) {   // fewer than 4 only for the last chunk of a layer-0 segment (the rest of the chunk is padding)
+        case 1: mma_steps<NSUB, 1, NS>(acc, adesc, bdesc, accumulate); break;
+        case 2: mma_steps<NSUB, 2, NS>(acc, adesc, bdesc, accumulate); break;
+        case 3: mma_steps<NSUB, 3, NS>(acc, adesc, bdesc, accumulate); break;
+        default: mma_steps<NSUB, 4, NS>(acc, adesc, bdesc, accumulate); break;
+    }
+}
+template <int NS>
+__device__ __forceinline__ void mma_chunk(float (&acc)[16 * NS], int nsub, int ksteps, uint64_t adesc, uint64_t bdesc,
+                                          uint32_t accumulate) {
+    // both are warp-uniform already; the broadcast keeps ptxas from losing track of that under register pressure
+    nsub = __shfl_sync(0xffffffffu, nsub, 0);
+    ksteps = __shfl_sync(0xffffffffu, ksteps, 0);
+    switch (nsub) {
+        case 1: mma_chunk_n<1, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 2: if constexpr (NS >= 2) mma_chunk_n<2, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 3: if constexpr (NS >= 3) mma_chunk_n<3, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 4: if constexpr (NS >= 4) mma_chunk_n<4, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 5: if constexpr (NS >= 5) mma_chunk_n<5, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 6: if constexpr (NS >= 6) mma_chunk_n<6, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 7: if constexpr (NS >= 7) mma_chunk_n<7, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 8: if constexpr (NS >= 8) mma_chunk_n<8, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
+        default: break;   // the warpgroup owns no columns of this layer (np = 32: all of them go to warpgroup 0)
+    }
+}
+
 // NS: 32-column subtiles per warpgroup of the widest layer (accumulator registers: 16 * NS per thread)
 template <int NS, int MINB>
 __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const ChainParams p) {
@@ -36,8 +88,9 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
     __shared__ SmemFixed S;
     uint8_t *base = smem_raw + ((1024u - (s2u(smem_raw) & 1023u)) & 1023u);
     const int L = p.num_layers;
-    int np_total = 0, sc_off[MAX_LAYERS];
-    for (int l = 0; l < L; ++l) { sc_off[l] = np_total; np_total += p.np[l]; }
+    int np_total = 0;
+#pragma unroll
+    for (int l = 0; l < MAX_LAYERS; ++l) np_total += l < L ? p.np[l] : 0;
     // work region, by phase of a tile: layer-0 A slots -> resident activations (layers >= 1) -> pool staging
     uint8_t *sW = base;
     uint8_t *sB = sW + p.work_bytes;
@@ -51,39 +104,51 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
         for (int i = 0; i < NB; ++i) { mbar_init(s2u(&S.b_full[i]), 1); mbar_init(s2u(&S.b_empty[i]), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    for (int l = 0; l < L; ++l)
-        for (int i = tid; i < p.np[l]; i += CHAIN_THREADS) {
-            s_scale[sc_off[l] + i] = p.unit_scale ? 1.f : p.scale[l][i];
-            s_shift[sc_off[l] + i] = p.shift[l][i];
+    {
+        int off = 0;
+#pragma unroll
+        for (int l = 0; l < MAX_LAYERS; ++l) {
+            if (l >= L) break;
+            for (int i = tid; i < p.np[l]; i += CHAIN_THREADS) {
+                s_scale[off + i] = p.unit_scale ? 1.f : p.scale[l][i];
+                s_shift[off + i] = p.shift[l][i];
+            }
+            off += p.np[l];
         }
+    }
     __syncthreads();
 
-    if (warp == 8) {
+    // the broadcast tells the compiler that wg -- and with it every column range and MMA width -- is warp-uniform
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
+    if (wg == 2) {
         // ===================================================== weight producer
         if (lane == 0) {
             RingPos rb = {0, 0};
             for (int item = blockIdx.x; item < p.num_items; item += gridDim.x)
                 for (int s = 0; s < p.tiles_per_item && item * p.tiles_per_item + s < p.num_tiles; ++s)
-                    for (int l = 0; l < L; ++l)
-                        for (int kc = 0; kc < p.nchunks[l]; ++kc) {
-                            const uint32_t bytes = (uint32_t)p.np[l] * KC * 4;
+                    for (int l = 0; l < L; ++l) {
+                        const int np_l = per_layer(p.np, l), nch = per_layer(p.nchunks, l);
+                        const float *w = per_layer(p.w, l);
+                        for (int kc = 0; kc < nch; ++kc) {
+                            const uint32_t bytes = (uint32_t)np_l * KC * 4;
                             mbar_wait(s2u(&S.b_empty[rb.stage]), rb.phase ^ 1);
                             mbar_expect_tx(s2u(&S.b_full[rb.stage]), bytes);
-                            bulk_g2s(s2u(sB + (size_t)rb.stage * p.b_stage_bytes), p.w[l] + (size_t)kc * p.np[l] * KC, bytes,
+                            bulk_g2s(s2u(sB + (size_t)rb.stage * p.b_stage_bytes), w + (size_t)kc * np_l * KC, bytes,
                                      s2u(&S.b_full[rb.stage]));
                             rb.advance(NB);
                         }
+                    }
         }
         return;
     }
 
     // ===================================================== MMA / epilogue warpgroups
-    const int wg = warp >> 2, wq = warp & 3;
+    const int wq = warp & 3;
     const int g = lane >> 2, t4 = lane & 3;      // accumulator fragment: rows 16 wq + g (+8), columns 2 t4 (+1) of each 8
     const int tw = tid & 127;                    // thread inside the warpgroup
     RingPos rb = {0, 0};
     int aslot = 0;
-    float acc[NS][16];
+    float acc[16 * NS];                          // subtile j (32 columns) = registers 16 j .. 16 j + 15
     const float lo = p.linear_last ? -CUDART_INF_F : 0.f;   // ReLU = max(., 0); a linear last layer keeps the sign
     const bool pool_raw = p.unit_scale && p.mode_out == OUT_SA_MAX;
 
@@ -118,12 +183,15 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
             }
             bar_mma();
 
+            int sc_base = 0;   // layer l's scale / shift in s_scale / s_shift
             for (int l = 0; l < L; ++l) {
-                const int nsub_all = p.np[l] >> 5, nsub0 = (nsub_all + 1) >> 1;
+                const int np_l = per_layer(p.np, l);
+                const int nsub_all = np_l >> 5, nsub0 = (nsub_all + 1) >> 1;
                 const int nsub = wg == 0 ? nsub0 : nsub_all - nsub0;
                 const int col0 = wg == 0 ? 0 : nsub0 * 32;            // first output column of this warpgroup
+                const int nch = per_layer(p.nchunks, l);
                 int prev_stage = -1;
-                for (int kc = 0; kc < p.nchunks[l]; ++kc) {
+                for (int kc = 0; kc < nch; ++kc) {
                     uint32_t a_addr;
                     int ksteps = KC / 8;
                     if (l == 0) {
@@ -131,7 +199,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                         int c = kc, seg = 0;
                         if (p.nseg > 1 && c >= p.seg_chunks[0]) { c -= p.seg_chunks[0]; seg = 1; }
                         const int k0 = c * KC;                         // first column of this chunk inside its segment
-                        const int width = p.seg_width[seg];
+                        const int width = seg ? p.seg_width[1] : p.seg_width[0];
                         ksteps = (min(KC, width - k0) + 7) >> 3;       // K=8 steps that hold data (the rest is padding)
                         uint8_t *A = sW + (size_t)aslot * A_STAGE_BYTES;
                         const bool rows_seg = (p.mode_in == IN_DIRECT) || (p.mode_in == IN_SA && seg == 0 && p.c_feat > 5) ||
@@ -255,17 +323,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                     mbar_wait(s2u(&S.b_full[rb.stage]), rb.phase);
                     const uint32_t b_addr = s2u(sB + (size_t)rb.stage * p.b_stage_bytes) + (uint32_t)col0 * (KC * 4);
                     wgmma_fence();
-#pragma unroll
-                    for (int ks = 0; ks < KC / 8; ++ks) {
-                        if (ks < ksteps) {
-                            const uint64_t adesc = make_desc(a_addr) + (uint64_t)(2 * ks);
-#pragma unroll
-                            for (int j = 0; j < NS; ++j)
-                                if (j < nsub)
-                                    wgmma_tf32_n32(acc[j], adesc, make_desc(b_addr + (uint32_t)j * 32 * KC * 4) + (uint64_t)(2 * ks),
-                                                   (kc > 0 || ks > 0) ? 1u : 0u);
-                        }
-                    }
+                    mma_chunk<NS>(acc, nsub, ksteps, make_desc(a_addr), make_desc(b_addr), kc > 0 ? 1u : 0u);
                     wgmma_commit();
                     wgmma_wait<1>();     // the previous chunk's MMAs are done: release its weight stage
                     if (prev_stage >= 0 && lane == 0) mbar_arrive(s2u(&S.b_empty[prev_stage]));
@@ -273,14 +331,14 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                     rb.advance(NB);
                 }
                 wgmma_wait<0>();
-#pragma unroll
-                for (int j = 0; j < NS; ++j) reg_fence(acc[j]);
+                reg_fence(acc);
                 if (lane == 0) mbar_arrive(s2u(&S.b_empty[prev_stage]));
                 bar_mma();   // both warpgroups' MMAs of layer l have read their A operand: the work region is free
+                const float *sc = s_scale + sc_base, *sh = s_shift + sc_base;
+                sc_base += np_l;
 
                 if (l + 1 < L) {
                     // ---- relu(acc * scale + shift) -> tf32 -> resident activations = the next layer's K chunks
-                    const float *sc = s_scale + sc_off[l], *sh = s_shift + sc_off[l];
 #pragma unroll
                     for (int j = 0; j < NS; ++j) {
                         if (j >= nsub) continue;
@@ -293,12 +351,13 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                             for (int h = 0; h < 2; ++h) {
                                 const int r = 16 * wq + g + 8 * h;
                                 float2 o;
+                                const float a0 = acc[16 * j + 4 * i + 2 * h], a1 = acc[16 * j + 4 * i + 2 * h + 1];
                                 if (p.unit_scale) {
-                                    o.x = relu_to_tf32(acc[j][4 * i + 2 * h] + sh[c]);
-                                    o.y = relu_to_tf32(acc[j][4 * i + 2 * h + 1] + sh[c + 1]);
+                                    o.x = relu_to_tf32(a0 + sh[c]);
+                                    o.y = relu_to_tf32(a1 + sh[c + 1]);
                                 } else {
-                                    o.x = relu_to_tf32(fmaf(acc[j][4 * i + 2 * h], sc[c], sh[c]));
-                                    o.y = relu_to_tf32(fmaf(acc[j][4 * i + 2 * h + 1], sc[c + 1], sh[c + 1]));
+                                    o.x = relu_to_tf32(fmaf(a0, sc[c], sh[c]));
+                                    o.y = relu_to_tf32(fmaf(a1, sc[c + 1], sh[c + 1]));
                                 }
                                 *reinterpret_cast<float2 *>(chunk + swz(r, ju) + within) = o;
                             }
@@ -311,7 +370,6 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
 
                 // ---- final epilogue
                 const int Cl = p.c_last;
-                const float *sc = s_scale + sc_off[l], *sh = s_shift + sc_off[l];
                 auto value = [&](float a, int c) -> float {
                     if (pool_raw) return a;   // max_s relu(x_s + t) == relu(max_s x_s + t): shift / ReLU after the max
                     return p.unit_scale ? fmaxf(a + sh[c], lo) : fmaxf(fmaf(a, sc[c], sh[c]), lo);
@@ -332,7 +390,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
 #pragma unroll
                                 for (int e = 0; e < 2; ++e) {
                                     const int cs = 8 * i + 2 * t4 + e;
-                                    stg[(16 * wq + g + 8 * h) * POOL_STRIDE + cs] = value(acc[j][4 * i + 2 * h + e], col0 + 32 * j + cs);
+                                    stg[(16 * wq + g + 8 * h) * POOL_STRIDE + cs] = value(acc[16 * j + 4 * i + 2 * h + e], col0 + 32 * j + cs);
                                 }
                         bar_wg(wg);
                         for (int o = tw; o < ncent * 32; o += 128) {
@@ -367,7 +425,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
 #pragma unroll
                             for (int i = 0; i < 4; ++i) {
                                 const int c = col0 + 32 * j + 8 * i + 2 * t4;
-                                float v0 = value(acc[j][4 * i + 2 * h], c), v1 = value(acc[j][4 * i + 2 * h + 1], c + 1);
+                                float v0 = value(acc[16 * j + 4 * i + 2 * h], c), v1 = value(acc[16 * j + 4 * i + 2 * h + 1], c + 1);
                                 if (p.mode_out == OUT_ROWS) {
                                     if (p.round_out) { v0 = to_tf32(v0); v1 = to_tf32(v1); }   // the next launch's A operand
                                     *reinterpret_cast<float2 *>(p.out + (size_t)R * p.out_pitch + c) = make_float2(v0, v1);
@@ -565,8 +623,9 @@ static int launch_chain(ChainParams &p, cudaStream_t st) {
         kern<<<grid, CHAIN_THREADS, smem, st>>>(p);
         return check_launch("mlp_chain_kernel");
     };
-    if (ns_max <= 2) return go(mlp_chain_kernel<2, 3>);
-    if (ns_max <= 4) return go(mlp_chain_kernel<4, 2>);
+    // register bounds without spills: <2,2> 96, <4,1> 168 (the weight ring of a 256-wide chain leaves room for one CTA)
+    if (ns_max <= 2) return go(mlp_chain_kernel<2, 2>);
+    if (ns_max <= 4) return go(mlp_chain_kernel<4, 1>);
     return go(mlp_chain_kernel<8, 1>);
 }
 
