@@ -342,6 +342,38 @@ PRB_API int prb_kitti_image_boxes_batch(int b, int m, const float *boxes3d, cons
 PRB_API size_t prb_kitti_format_detections(const char *cls_name, int n, const float *boxes3d, const float *img_boxes,
                                    const float *alpha, const float *scores, const int *valid, char *buf, size_t cap);
 
+/* GT-paste augmentation (kitti_rcnn_dataset.py:273-282, 408-511, apply_gt_aug_to_one_scene), between
+ * prb_kitti_prepare_points and prb_kitti_draw_points.  The host draws each scene's candidate list (the database entries
+ * that reach the collision test, in draw order, with their boxes moved onto the road plane); the device decides and pastes.
+ * Candidates are indexed flat, c = scene * k + j.  cand_first (b*k+1) int32: exclusive prefix of the candidates' point
+ * counts in that order (unused slots count 0 points); cand_first[b*k] = cand_total.
+ *
+ * select: one CTA per scene tests candidate j's box, w and l enlarged by 0.5, against the scene's collision boxes
+ * coll_boxes (b,m,7) (first coll_count[s] rows, enlarged the same way) and the candidates accepted before it: rejected
+ * when a 3D IoU >= 1e-8 (BEV overlap of the rotated rectangles, height range [-y, -y+h]).  An empty collision list
+ * accepts.  cand_boxes (b,k,7) moved boxes, cand_count (b).  place (b,k) int32: -1 = rejected or no candidate, else the
+ * offset of the candidate's first point among the scene's pasted points; stats (b,2) int32: accepted candidates, pasted
+ * points; counts (b,2) or NULL: zeroed for prb_gt_paste_points.  gt_out (b,g+k,7) or NULL: per scene the first
+ * gt_count[s] rows of gt_rows (b,g,7) (all g when gt_count is NULL), then the cand_rows (b,k,7) of the accepted
+ * candidates in order, zero padded; gt_count_out (b) their number.  k <= 128, m <= 1024, g + k <= 128 with gt_out. */
+PRB_API int prb_gt_paste_select(int b, int k, int m, int g, const float *cand_boxes, const int *cand_count, const int *cand_first,
+                        const float *coll_boxes, const int *coll_count, const float *gt_rows, const int *gt_count,
+                        const float *cand_rows, int *place, int *stats, float *gt_out, int *gt_count_out, int *counts,
+                        void *stream);
+/* paste: the post-paste ragged cloud.  offsets_out (b+1); per scene first its raw segment (rect, flags as
+ * prb_kitti_prepare_points wrote them, intensity = lidar column 3 when stride > 3 else 0) with bit 0 cleared on the
+ * valid points inside an accepted box with h + 2 (pts_in_boxes3d_cpu's predicate), then the accepted candidates' points
+ * in acceptance order: db_points (.,4) [rect x, y, z, intensity] rows cand_src[c] ... + count, y moved by
+ * (float)((double)y - moves[c]), valid, near = z < 40.  rect_out (total+cand_total,3), points_out (total+cand_total,4)
+ * [x, y, z, intensity] (the lidar operand of prb_kitti_gather_points with stride 4), flags_out (total+cand_total):
+ * rows past offsets_out[b] are unused.  counts (b,2), zeroed by select: post-paste valid / valid far points.
+ * points_out and db_points 16-byte aligned. */
+PRB_API int prb_gt_paste_points(int b, int total, int k, int cand_total, const int *offsets, const float *rect, const float *lidar,
+                        int stride, const unsigned char *flags, const float *cand_boxes, const int *cand_first,
+                        const int *cand_src, const double *moves, const int *place, const int *stats, const float *db_points,
+                        int *offsets_out, float *rect_out, float *points_out, unsigned char *flags_out, int *counts,
+                        void *stream);
+
 #ifdef __cplusplus
 }
 #endif
