@@ -374,6 +374,36 @@ PRB_API int prb_gt_paste_points(int b, int total, int k, int cand_total, const i
                         int *offsets_out, float *rect_out, float *points_out, unsigned char *flags_out, int *counts,
                         void *stream);
 
+/* ------------------------------------------------------------------ KITTI AP evaluation ------
+ * tools/kitti_object_eval_python/eval.py:608-678 (get_official_eval_result's statistics) for a whole split on the device.
+ * Annotations are row tables of 16 doubles, ragged by per-image offsets (device int32, n_img+1):
+ *   x1 y1 x2 y2 (image box), alpha, truncated, occluded, l h w, x y z (camera frame), rotation_y, score, class code
+ * class code: 0 car, 1 pedestrian, 2 cyclist, 3 van, 4 person_sitting (names compared case-insensitively), 5 DontCare
+ * (exact name), -1 anything else.  gt (n_gt,16) with gt_off; dt (n_dt,16) with dt_off: image i owns rows
+ * dt_off[i] .. dt_off[i+1] of which the first dt_count[i] (device) are detections; max_det >= every dt_off[i+1]-dt_off[i]
+ * (<= 1024).  pair_off (n_img+1) int64 device: prefix of (gt rows x dt rows owned) per image; overlaps (3, n_pairs) double
+ * receives the (dt x gt) matrices (image box IoU in double, BEV IoU in fp32, 3D IoU rounded to fp32 as the reference stores
+ * them), row-major per image at pair_off[i].  classes (num_classes) HOST: 0..2; min_overlaps HOST (2, 3, num_classes)
+ * [overlap set][metric][class].  out (18*num_classes*41*8 + 1 + 18*num_classes) double: per config
+ * q = ((metric*num_classes + class)*3 + difficulty)*2 + overlap set and per threshold t < 41:
+ * tp, fp, fn, similarity, recall, precision, orientation (the last three after the suffix maxima), threshold; then the
+ * AOS flag (the reference's rule: the first image with detections decides, AOS unless its first alpha is -10), then the
+ * number of thresholds per config.  Six launches and a memset, no host synchronisation; the same inputs give the same bits. */
+PRB_API size_t prb_kitti_eval_workspace_bytes(int n_img, int n_gt, int n_dt, int num_classes);
+PRB_API int prb_kitti_eval(int n_img, int num_classes, const int *classes, const double *min_overlaps, const double *gt,
+                           const int *gt_off, int n_gt, const double *dt, const int *dt_off, const int *dt_count, int n_dt,
+                           int max_det, const long long *pair_off, long long n_pairs, double *overlaps, double *out,
+                           void *workspace, size_t workspace_bytes, void *stream);
+/* the rows save_kitti_format would write for a batch of scenes (valid[k,j] && select[k,j], in row order) appended as
+ * detection rows of image slot[k] (b, device int32), starting at row 0 of its range; dt_count[slot[k]] = their number.
+ * boxes3d (b,m,7) [x,y,z,h,w,l,ry], scores (b,m), img_boxes (b,m,4), alpha (b,m), valid / select (b,m) int32, as
+ * prb_kitti_image_boxes_batch produces them.  text_rounding != 0: every field is rint((double)f*1e4)/1e4, the value the
+ * "%.4f" text parses back to. */
+PRB_API int prb_kitti_eval_add_detections(int b, int m, const float *boxes3d, const float *scores, const float *img_boxes,
+                                          const float *alpha, const int *valid, const int *select, const int *slot,
+                                          int text_rounding, int class_code, double *dt, const int *dt_off, int *dt_count,
+                                          void *stream);
+
 #ifdef __cplusplus
 }
 #endif

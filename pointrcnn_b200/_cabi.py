@@ -59,7 +59,8 @@ def lib():
         L.prb_launch_count.restype = ctypes.c_ulonglong
         for name in ("prb_nms_workspace_bytes", "prb_mlp_packed_bytes", "prb_mlp_packed_bytes_ex",
                      "prb_sa_workspace_bytes", "prb_fp_workspace_bytes", "prb_rows_workspace_bytes", "prb_rows2_workspace_bytes", "prb_grid_workspace_bytes",
-                     "prb_fps_workspace_bytes", "prb_fps_ordered_workspace_bytes", "prb_kitti_format_detections", "prb_rpn_proposals_workspace_bytes", "prb_roipool3d_workspace_bytes"):
+                     "prb_fps_workspace_bytes", "prb_fps_ordered_workspace_bytes", "prb_kitti_format_detections", "prb_rpn_proposals_workspace_bytes", "prb_roipool3d_workspace_bytes",
+                     "prb_kitti_eval_workspace_bytes"):
             getattr(L, name).restype = c_size_t
         L.prb_options_init.restype = None
         L.prb_get_thread_options.restype = None

@@ -8,6 +8,7 @@ After this, with the reference tree on sys.path, `lib/net/*.py` and `tools/*.py`
     lib.utils.iou3d.iou3d_utils, lib.utils.roipool3d.roipool3d_utils       -> pointrcnn_b200.{iou3d,roipool3d}.*
     lib.rpn.proposal_layer (ProposalLayer)                                 -> pointrcnn_b200.rpn.proposal_layer
     lib.rpn.proposal_target_layer (ProposalTargetLayer)                    -> pointrcnn_b200.rpn.proposal_target_layer
+    tools.kitti_object_eval_python.{evaluate,eval}                          -> pointrcnn_b200.datasets.kitti_eval
 Optionally (compat=True) also provides the tiny stand-ins the 2019-era reference needs on a modern stack:
 `easydict`, `tensorboardX.SummaryWriter` (no-op), `fire`, and a default Loader for `yaml.load`
 (SURVEY.md section 0) -- none of them is on the operator path.
@@ -63,6 +64,17 @@ def activate(compat=False):
     _alias("lib.rpn.proposal_layer", proposal_layer)
     # rank 2: the RCNN target layer (one IoU launch per batch, batched jitter loop); lib/net/rcnn_net.py imports it by name
     _alias("lib.rpn.proposal_target_layer", proposal_target_layer)
+    # the KITTI AP evaluator (tools/eval_rcnn.py:11 imports evaluate): same import-or-stub rule for the tools packages
+    for pkg in ("tools", "tools.kitti_object_eval_python"):
+        try:
+            importlib.import_module(pkg)
+        except ImportError:
+            m = types.ModuleType(pkg)
+            m.__path__ = []
+            _alias(pkg, m)
+    from .datasets import kitti_eval
+    _alias("tools.kitti_object_eval_python.evaluate", kitti_eval)
+    _alias("tools.kitti_object_eval_python.eval", kitti_eval)
 
 
 def _install_compat():
