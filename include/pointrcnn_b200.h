@@ -404,6 +404,41 @@ PRB_API int prb_kitti_eval_add_detections(int b, int m, const float *boxes3d, co
                                           int text_rounding, int class_code, double *dt, const int *dt_off, int *dt_count,
                                           void *stream);
 
+/* ------------------------------------------------------------------ offline RCNN training samples ------
+ * lib/datasets/kitti_rcnn_dataset.py:876-1077 (get_rcnn_training_sample_batch, sample_bg_inds, aug_roi_by_noise_batch) for a
+ * batch: prb_boxes_iou3d (b,m,g), prb_rcnn_sample_rois, prb_roipool3d_ws on pool_boxes (rois_canonical
+ * NULL, zero_fill_empty 1), prb_rcnn_roi_targets.  No host synchronisation.  Random draws are counter-based hashes of
+ * (seed, scene, stage, roi, try, slot): the reference's distribution, not its np.random stream.
+ *
+ * sample: one CTA per scene.  iou (b,m,g) from prb_boxes_iou3d; rois (b,m,7), gt_boxes (b,g,7); the first roi_count[s] /
+ * gt_count[s] (device int32) rows are real.  fg = RoIs with max IoU >= min(reg_fg, cls_fg) in index order, then each GT's
+ * first-max RoI (GTs with max IoU > 0), duplicates kept; easy bg < cls_bg_lo; hard bg in [cls_bg_lo, cls_bg).  fg and bg
+ * present: min(fg_per_image, |fg|) fg rows without replacement, the rest bg with replacement, int(bg * hard_bg_ratio) of
+ * them hard when both bg lists are non-empty; fg only: roi_per_image fg rows with replacement; bg only: all bg.  Each row
+ * runs the jitter loop: fg rows up to fg_aug_times tries, bg rows one; a try keeps the source box with p = 0.2, else
+ * aug_method (0 single, 1 multiple, 2 normal) jitters it; the loop stops when the 3D IoU with the assigned GT reaches
+ * min(reg_fg, cls_fg), and the last box and its IoU are kept.  Outputs (b, roi_per_image, .): rois_out 7, gt_out 7,
+ * iou_out 1, pool_boxes 7 (enlarge_box3d by pool_extra_width), sel 3 int32 (source RoI, GT, tries; -1 -1 0 on ignored
+ * rows); status (b): 0 ok, 1 neither fg nor bg RoIs, 2 no RoI or no GT -- the rows of such a scene are zero with a
+ * pool box no point is inside.  m <= 4096, g <= 256, roi_per_image <= 1024, fg_aug_times < 64.
+ *
+ * targets: one CTA per row k of the (b * roi_per_image) rows.  rows (b*roi_per_image, S, W) pooled [x, y, z, ...] in the
+ * original frame; rois / gt_boxes (b*roi_per_image, 7) from sample, updated in place.  With aug_data: rotation
+ * U(-pi/aug_rot_range, pi/aug_rot_range) of the points and of both boxes with their observation angle kept
+ * (aug_rotation), scaling U(0.95, 1.05) of the points and box[0:6] (aug_scaling), x flip with ry -> sign(ry) pi - ry when
+ * 1 - u < flip_prob (aug_flip).  Then labels from iou (before augmentation) and empty_flag: reg_valid_mask = iou > reg_fg
+ * and not empty, cls_label = iou > cls_fg, -1 inside (cls_bg, cls_fg) or when empty; then the canonical transform of the
+ * xyz columns (centre, rotation by ry mod 2 pi) and gt_boxes_ct. */
+PRB_API int prb_rcnn_sample_rois(int b, int m, int g, const float *iou, const float *rois, const int *roi_count, const float *gt_boxes,
+                                 const int *gt_count, int roi_per_image, int fg_per_image, float reg_fg_thresh, float cls_fg_thresh,
+                                 float cls_bg_thresh, float cls_bg_thresh_lo, double hard_bg_ratio, int aug_method, int fg_aug_times,
+                                 float pool_extra_width, unsigned seed, float *rois_out, float *gt_out, float *iou_out,
+                                 float *pool_boxes, int *sel, int *status, void *stream);
+PRB_API int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes, const float *iou,
+                                 const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling, int aug_flip,
+                                 float aug_rot_range, float flip_prob, float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh,
+                                 unsigned seed, float *gt_boxes_ct, int *cls_label, int *reg_valid_mask, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

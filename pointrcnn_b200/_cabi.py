@@ -62,6 +62,9 @@ def lib():
                      "prb_fps_workspace_bytes", "prb_fps_ordered_workspace_bytes", "prb_kitti_format_detections", "prb_rpn_proposals_workspace_bytes", "prb_roipool3d_workspace_bytes",
                      "prb_kitti_eval_workspace_bytes"):
             getattr(L, name).restype = c_size_t
+        P, I, F, U = c_void_p, c_int, c_float, ctypes.c_uint
+        L.prb_rcnn_sample_rois.argtypes = [I, I, I, P, P, P, P, P, I, I, F, F, F, F, ctypes.c_double, I, I, F, U, P, P, P, P, P, P, P]
+        L.prb_rcnn_roi_targets.argtypes = [I, I, I, I, P, P, P, P, P, I, I, I, I, F, F, F, F, F, U, P, P, P, P]
         L.prb_options_init.restype = None
         L.prb_get_thread_options.restype = None
         if L.prb_abi_version() != 5:

@@ -52,6 +52,15 @@ __device__ __forceinline__ float dist2_ref(float dx, float dy, float dz) {
     return __fmaf_rn(dz, dz, __fmaf_rn(dx, dx, __fmul_rn(dy, dy)));
 }
 
+// counter-based random draws (kitti_io.cu's npoints draw, rcnn_sample.cu): a 32-bit hash of (seed, scene, i, salt)
+__device__ __forceinline__ uint32_t mix32(uint32_t x) {
+    x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16;
+    return x;
+}
+__device__ __forceinline__ uint32_t draw_key(uint32_t seed, uint32_t scene, uint32_t i, uint32_t salt) {
+    return mix32(mix32(seed ^ (scene * 0x9e3779b9u) ^ salt) + i * 0x85ebca6bu);
+}
+
 int num_sms();   // SM count of the CURRENT device (cached per device)
 
 // per-thread tuning block (include/pointrcnn_b200.h: prb_options).  Environment variables seed the DEFAULTS once,

@@ -223,26 +223,7 @@ __global__ void __launch_bounds__(SCAN_THREADS) nms_scan_global_kernel(int n, co
 // it; every torch op of the reference is one fp32 rounding here too (explicit _rn intrinsics: no FMA contraction), so
 // the values equal the reference's op sequence on its own overlap kernel bit for bit.
 //   mode 0: matrix, out[s][i][j] = iou(a[s][i], b[s][j]) for s < batch; mode 1: aligned pairs, out[k] = iou(a[k], b[k])
-__device__ __forceinline__ void box7_to_bev(const float *b, float *bev) {
-    const float half_l = __fmul_rn(b[5], 0.5f), half_w = __fmul_rn(b[4], 0.5f);
-    bev[0] = __fsub_rn(b[0], half_l); bev[1] = __fsub_rn(b[2], half_w);
-    bev[2] = __fadd_rn(b[0], half_l); bev[3] = __fadd_rn(b[2], half_w);
-    bev[4] = b[6];
-}
-__device__ __forceinline__ float iou3d_pair(const float *a, const float *b, float *px, float *py, float *pa, int stride) {
-    float abev[5], bbev[5];
-    box7_to_bev(a, abev);
-    box7_to_bev(b, bbev);
-    BoxPre A, Bp;
-    box_pre(abev, A);
-    box_pre(bbev, Bp);
-    const float ov_bev = box_overlap_pre(A, Bp, px, py, pa, stride);
-    const float a_min = __fsub_rn(a[1], a[3]), b_min = __fsub_rn(b[1], b[3]);       // y - h .. y (y points down)
-    const float ov_h = fmaxf(__fsub_rn(fminf(a[1], b[1]), fmaxf(a_min, b_min)), 0.f);
-    const float ov3d = __fmul_rn(ov_bev, ov_h);
-    const float va = __fmul_rn(__fmul_rn(a[3], a[4]), a[5]), vb = __fmul_rn(__fmul_rn(b[3], b[4]), b[5]);
-    return __fdiv_rn(ov3d, fmaxf(__fsub_rn(__fadd_rn(va, vb), ov3d), 1e-7f));
-}
+// (the per-pair arithmetic, box7_to_bev / iou3d_pair, is in iou3d_dev.cuh)
 __global__ void __launch_bounds__(128) iou3d_kernel(int mode, int batch, int na, int nb, const float *__restrict__ boxes_a,
                                                     const float *__restrict__ boxes_b, float *__restrict__ out) {
     __shared__ float s_poly[3 * POLY_SLOTS * 128];

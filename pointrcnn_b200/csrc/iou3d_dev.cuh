@@ -237,4 +237,28 @@ __device__ __forceinline__ float iou_bev_pre(const BoxPre &A, const BoxPre &B, f
     return s_overlap / fmaxf(sa + sb - s_overlap, EPS);
 }
 
+// ---------------------------------------------------------------------------------------------- fused 3D IoU of one pair
+// iou3d_utils.boxes_iou3d_gpu's op sequence for [x,y,z,h,w,l,ry] boxes, every torch op one fp32 rounding (iou3d.cu's
+// iou3d_kernel, rcnn_sample.cu's jitter loop)
+__device__ __forceinline__ void box7_to_bev(const float *b, float *bev) {
+    const float half_l = __fmul_rn(b[5], 0.5f), half_w = __fmul_rn(b[4], 0.5f);
+    bev[0] = __fsub_rn(b[0], half_l); bev[1] = __fsub_rn(b[2], half_w);
+    bev[2] = __fadd_rn(b[0], half_l); bev[3] = __fadd_rn(b[2], half_w);
+    bev[4] = b[6];
+}
+__device__ __forceinline__ float iou3d_pair(const float *a, const float *b, float *px, float *py, float *pa, int stride) {
+    float abev[5], bbev[5];
+    box7_to_bev(a, abev);
+    box7_to_bev(b, bbev);
+    BoxPre A, Bp;
+    box_pre(abev, A);
+    box_pre(bbev, Bp);
+    const float ov_bev = box_overlap_pre(A, Bp, px, py, pa, stride);
+    const float a_min = __fsub_rn(a[1], a[3]), b_min = __fsub_rn(b[1], b[3]);       // y - h .. y (y points down)
+    const float ov_h = fmaxf(__fsub_rn(fminf(a[1], b[1]), fmaxf(a_min, b_min)), 0.f);
+    const float ov3d = __fmul_rn(ov_bev, ov_h);
+    const float va = __fmul_rn(__fmul_rn(a[3], a[4]), a[5]), vb = __fmul_rn(__fmul_rn(b[3], b[4]), b[5]);
+    return __fdiv_rn(ov3d, fmaxf(__fsub_rn(__fadd_rn(va, vb), ov3d), 1e-7f));
+}
+
 }  // namespace prb

@@ -74,14 +74,6 @@ __global__ void __launch_bounds__(256) kitti_prepare_kernel(int b, int total, co
 }
 
 // ---------------------------------------------------------------------------------------------------- draw
-__device__ __forceinline__ uint32_t mix32(uint32_t x) {
-    x ^= x >> 16; x *= 0x7feb352du; x ^= x >> 15; x *= 0x846ca68bu; x ^= x >> 16;
-    return x;
-}
-__device__ __forceinline__ uint32_t draw_key(uint32_t seed, uint32_t scene, uint32_t i, uint32_t salt) {
-    return mix32(mix32(seed ^ (scene * 0x9e3779b9u) ^ salt) + i * 0x85ebca6bu);
-}
-
 // block-wide exclusive scan of one int per thread (1024 threads); returns the exclusive prefix, total in *sum
 __device__ __forceinline__ int block_excl_scan(int v, int *s_warp, int *sum) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;

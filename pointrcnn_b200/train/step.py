@@ -94,9 +94,26 @@ class RCNNTrainer:
                          self.mean_size, loc_scope=c["LOC_SCOPE"], loc_bin_size=c["LOC_BIN_SIZE"], num_head_bin=c["NUM_HEAD_BIN"],
                          loc_y_by_bin=c["LOC_Y_BY_BIN"], loc_y_scope=c["LOC_Y_SCOPE"], loc_y_bin_size=c["LOC_Y_BIN_SIZE"])
 
+    def forward_loss_offline(self, batch):
+        """the ROI_SAMPLE_JIT=False branch of rcnn_net.forward (:155-163) + get_rcnn_loss on a batch of
+        datasets.rcnn_offline.RCNNOfflineSampler.prepare_batch: the network reads the pooled rows as they are (no
+        torch.cat of pts_input and pts_features), the targets are the batch's labels and canonical GT boxes"""
+        rcnn_cls, rcnn_reg = self.model.forward_pts(batch["rows"])
+        c = self.model.cfg
+        return rcnn_loss(rcnn_cls, rcnn_reg, batch["cls_label"], batch["reg_valid_mask"], batch["roi_boxes3d"], batch["gt_boxes3d_ct"],
+                         self.mean_size, loc_scope=c["LOC_SCOPE"], loc_bin_size=c["LOC_BIN_SIZE"], num_head_bin=c["NUM_HEAD_BIN"],
+                         loc_y_by_bin=c["LOC_Y_BY_BIN"], loc_y_scope=c["LOC_Y_SCOPE"], loc_y_bin_size=c["LOC_Y_BIN_SIZE"])
+
+    def step_offline(self, batch, grad_norm_clip=None):
+        """one offline-recipe training step (tools/train_rcnn.py --train_mode rcnn_offline) on a prepared batch"""
+        return self._step(self.forward_loss_offline, (batch,), grad_norm_clip)
+
     def step(self, pts_input, gt_boxes3d, grad_norm_clip=None):
+        return self._step(self.forward_loss, (pts_input, gt_boxes3d), grad_norm_clip)
+
+    def _step(self, forward_loss, args, grad_norm_clip):
         self.reducer.reset()
-        loss, terms = self.forward_loss(pts_input, gt_boxes3d)
+        loss, terms = forward_loss(*args)
         loss.backward()
         self.reducer.finish()
         if grad_norm_clip:
