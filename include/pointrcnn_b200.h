@@ -51,7 +51,8 @@ typedef struct prb_options {
     int fps_prune;     /* 0: never use the pruned single-CTA kernel; 1: for 4097..16384 points; 2: also 2049..4096 */
     int fps_threads;   /* threads per CTA of the rank kernel; 0 = heuristic */
     int fps_generic;   /* 1: force the generic (reference-shaped) kernel */
-    /* the chain kernel reads only mlp_occ and mlp_sms; the other mlp_* fields have no effect and keep the block's layout */
+    /* the chain kernels read only mlp_occ, mlp_sms and mlp_resident; the other mlp_* fields have no effect and keep the
+     * block's layout */
     int mlp_gather;
     int mlp_ng;
     int mlp_occ;       /* >= 1: at most this many chain-kernel CTAs per SM; 0 = as many as registers and shared memory allow */
@@ -64,7 +65,7 @@ typedef struct prb_options {
     int mlp_zs, mlp_nbuf;
     int mlp_brows;
     int mlp_pool;
-    int mlp_resident;
+    int mlp_resident;  /* 1 (default): chain launches whose weights fit run on the resident-weight kernel; 0: always stream */
     int mlp_lazy_ns;
     int mlp_fill;
     int mlp_tune;

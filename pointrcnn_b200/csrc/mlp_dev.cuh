@@ -1,4 +1,4 @@
-// mlp_dev.cuh -- constants, launch parameters and PTX wrappers of the tensor-core chain kernel (mlp_tc.cu).
+// mlp_dev.cuh -- constants, launch parameters and PTX wrappers of the tensor-core chain kernels (mlp_tc.cu).
 #pragma once
 #include <math_constants.h>
 
@@ -16,6 +16,8 @@ constexpr int MAX_NP = 512;
 constexpr int NSUB_MAX = 8;          // 32-column subtiles per warpgroup (2 warpgroups x 8 x 32 = MAX_NP; wgmma N <= 256)
 constexpr int POOL_STRIDE = 33;      // floats per row of a warpgroup's 64 x 32 max-pool staging tile (conflict-free columns)
 constexpr int CHAIN_THREADS = 2 * 128 + 32;       // two MMA / epilogue warpgroups + one weight-producer warp
+constexpr int RES_NP_MAX = 128;      // resident kernel: widest layer (one warpgroup covers it: <= 64 accumulator registers)
+constexpr int RES_WG_MAX = 5;        // resident kernel: warpgroups per CTA, at most
 
 enum { IN_SA = 0, IN_FP = 1, IN_DIRECT = 2 };
 enum { OUT_ROWS = 0, OUT_SA_MAX = 1, OUT_FP = 2 };
@@ -190,10 +192,15 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t smem_addr) {
 // byte offset of (row r, 16-byte unit j) inside a K-major SWIZZLE_128B chunk
 __device__ __forceinline__ uint32_t swz(int r, int j) { return (uint32_t)(r * 128 + ((j ^ (r & 7)) << 4)); }
 
+// the source rows of one 64-row tile, filled before its layer-0 gather
+struct TileRows {
+    int src[TM][3];      // SA: global point row (slot 0); FP: 3 known rows
+    float aux[TM][3];    // SA: centre xyz; FP: 3 weights
+    int valid[TM];
+};
+
 struct SmemFixed {
-    int row_src[TM][3];      // SA: global point row (slot 0); FP: 3 known rows
-    float row_aux[TM][3];    // SA: centre xyz; FP: 3 weights
-    int row_valid[TM];
+    TileRows rows;
     uint64_t b_full[NB_MAX], b_empty[NB_MAX];
 };
 
@@ -209,11 +216,20 @@ struct RingPos {
     }
 };
 
-// barrier over the two MMA warpgroups / over one of them
+// barrier over the two MMA warpgroups of the streaming kernel
 __device__ __forceinline__ void bar_mma() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-__device__ __forceinline__ void bar_wg(int wg) {
-    if (wg == 0) asm volatile("bar.sync 2, 128;" ::: "memory");
-    else asm volatile("bar.sync 3, 128;" ::: "memory");
+// barrier over the 128 threads of one warpgroup: named barrier `id` (streaming kernel: 2 + wg; resident kernel: 1 + wg)
+// (immediate ids: ptxas then reserves only the barriers a kernel uses)
+__device__ __forceinline__ void bar_wg_id(int id) {
+    static_assert(RES_WG_MAX <= 5, "bar_wg_id: ids 1..6");
+    switch (id) {
+        case 1: asm volatile("bar.sync 1, 128;" ::: "memory"); break;
+        case 2: asm volatile("bar.sync 2, 128;" ::: "memory"); break;
+        case 3: asm volatile("bar.sync 3, 128;" ::: "memory"); break;
+        case 4: asm volatile("bar.sync 4, 128;" ::: "memory"); break;
+        case 5: asm volatile("bar.sync 5, 128;" ::: "memory"); break;
+        default: asm volatile("bar.sync 6, 128;" ::: "memory"); break;
+    }
 }
 
 }  // namespace prb

@@ -8,7 +8,23 @@
 // The reference materialises every (B,C,npoint,nsample) tensor in HBM between ~10 library kernels per
 // scale; here a 64-row tile never leaves the SM between its gather and its pooled output.
 //
-// Structure (persistent CTAs over 64-row tiles; rows = (centre, sample) pairs or points):
+// Two kernels run a launch (one fused segment of a chain); they share the tile stages -- the row lookup, the layer-0
+// gather, the inner-layer epilogue and the final epilogues -- issue the same MMA sequence per K chunk, and give
+// bit-identical outputs.  launch_chain picks one by shape:
+//   resident   every layer <= 128 wide; input / output one of SA -> max-pool, FP -> FP, rows -> rows; the packed weight
+//              image at most half of a CTA's shared memory; prb_options.mlp_resident != 0 (the default).
+//   streaming  every other launch.
+//
+// Resident kernel (mlp_resident_kernel; persistent CTAs of nwg warpgroups, no producer warp): at CTA start one thread
+// loads the segment's whole packed image with cp.async.bulk on one mbarrier, which every warpgroup waits on once.  Each
+// warpgroup then runs its own 64-row tiles (strided over the grid; the tiles of a pooled SA centre stay together)
+// through every layer at full width -- one m64n(np)k8 instruction per K=8 step -- in a private work region (layer-0 A
+// slots -> activations -> pool staging, as below), synchronising only on its own named barrier, so one warpgroup's
+// gather and epilogues overlap another's MMAs.  The B operand of chunk kc of layer l is the image at the layer's offset
+// + kc * np * 128 bytes.  Warpgroups per CTA and CTAs per SM are the pair the occupancy calculator allows the most
+// warpgroups per SM for (registers: 96 for 32-wide chains, 128 otherwise).
+//
+// Streaming kernel (mlp_chain_kernel; persistent CTAs over 64-row tiles; rows = (centre, sample) pairs or points):
 //   warpgroups 0, 1  gather layer 0's A operand chunk by chunk (32 K-columns = one 128-byte swizzle row) into a
 //                    ring of three shared-memory slots, issue wgmma tf32 with fp32 register accumulators -- the
 //                    layer's output columns are split between the two warpgroups, and each warpgroup covers its
@@ -81,6 +97,298 @@ __device__ __forceinline__ void mma_chunk(float (&acc)[16 * NS], int nsub, int k
     }
 }
 
+// ------------------------------------------------------------------------------------------------ tile stages
+// The stages of a tile that do not depend on how the weights reach shared memory, shared by both kernels.  NT is the
+// number of threads that run a stage together (the streaming kernel's two warpgroups: 256; one resident warpgroup: 128),
+// t the thread's index among them.
+
+// the tile's source rows (threads t < TM)
+__device__ __forceinline__ void load_tile_rows(const ChainParams &p, int tile, int t, TileRows &M) {
+    if (t >= TM) return;
+    const long R = (long)tile * TM + t;
+    const bool valid = R < p.total_rows;
+    int src[3] = {0, 0, 0};
+    float aux[3] = {0.f, 0.f, 0.f};
+    if (p.mode_in == IN_SA) {
+        const long pr = valid ? (R >> p.log_ns) : 0;      // global centre index (nsample is a power of two)
+        const int scene = (int)(pr / p.npoint);
+        src[0] = scene * p.n + (valid ? __ldg(p.idx + R) : 0);
+#pragma unroll
+        for (int q = 0; q < 3; ++q) aux[q] = __ldg(p.new_xyz + (size_t)pr * 3 + q);
+    } else if (p.mode_in == IN_FP) {
+        const long rr = valid ? R : 0;
+        const int scene = (int)(rr / p.n);
+#pragma unroll
+        for (int q = 0; q < 3; ++q) {
+            src[q] = scene * p.m + __ldg(p.idx + (size_t)rr * 3 + q);
+            aux[q] = __ldg(p.weight + (size_t)rr * 3 + q);
+        }
+    }
+    M.valid[t] = valid;
+#pragma unroll
+    for (int q = 0; q < 3; ++q) { M.src[t][q] = src[q]; M.aux[t][q] = aux[q]; }
+}
+
+// gather K chunk kc of the tile's layer-0 input rows, rounded to tf32, into the A chunk at A; returns the K=8 steps that
+// hold data (the rest of the chunk is padding)
+template <int NT>
+__device__ __forceinline__ int gather_chunk(const ChainParams &p, int tile, int kc, int t, const TileRows &M, uint8_t *A) {
+    static_assert(NT == 128 || NT == 256, "gather_chunk: one or two warpgroups");
+    int c = kc, seg = 0;
+    if (p.nseg > 1 && c >= p.seg_chunks[0]) { c -= p.seg_chunks[0]; seg = 1; }
+    const int k0 = c * KC;                         // first column of this chunk inside its segment
+    const int width = seg ? p.seg_width[1] : p.seg_width[0];
+    const int ksteps = (min(KC, width - k0) + 7) >> 3;
+    const bool rows_seg = (p.mode_in == IN_DIRECT) || (p.mode_in == IN_SA && seg == 0 && p.c_feat > 5) ||
+                          (p.mode_in == IN_FP && seg == 0);
+    if (rows_seg) {
+        // point-major sources: 8 threads cover one row's 128 bytes, NT threads NT/8 rows per step, two steps in flight
+        constexpr int RS = NT / 8, STEPS = 2;
+        const int j8 = t & 7, kk = k0 + 4 * j8;
+#pragma unroll 1
+        for (int r0 = 0; r0 < TM; r0 += STEPS * RS) {
+            float4 v[STEPS];
+            if (p.mode_in == IN_FP) {
+                const int C = p.c_known;
+                const bool vec = (C & 3) == 0;
+#pragma unroll
+                for (int i = 0; i < STEPS; ++i) {
+                    const int rr = r0 + (t >> 3) + RS * i;
+                    float4 t0 = make_float4(0.f, 0.f, 0.f, 0.f), t1 = t0, t2 = t0;
+                    const float w0 = M.aux[rr][0], w1 = M.aux[rr][1], w2 = M.aux[rr][2];
+                    if (M.valid[rr] && kk < width) {
+                        const float *s0 = p.known_pm + (size_t)M.src[rr][0] * C + kk;
+                        const float *s1 = p.known_pm + (size_t)M.src[rr][1] * C + kk;
+                        const float *s2 = p.known_pm + (size_t)M.src[rr][2] * C + kk;
+                        if (vec) {
+                            t0 = __ldg((const float4 *)s0); t1 = __ldg((const float4 *)s1); t2 = __ldg((const float4 *)s2);
+                        } else {
+                            float a0[4], a1[4], a2[4];
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) {
+                                const bool in = kk + q < width;
+                                a0[q] = in ? __ldg(s0 + q) : 0.f; a1[q] = in ? __ldg(s1 + q) : 0.f; a2[q] = in ? __ldg(s2 + q) : 0.f;
+                            }
+                            t0 = make_float4(a0[0], a0[1], a0[2], a0[3]);
+                            t1 = make_float4(a1[0], a1[1], a1[2], a1[3]);
+                            t2 = make_float4(a2[0], a2[1], a2[2], a2[3]);
+                        }
+                    }
+                    // same contraction as three_interpolate (reference SASS): fma(w2,p2, fma(w0,p0, w1*p1))
+                    v[i].x = __fmaf_rn(w2, t2.x, __fmaf_rn(w0, t0.x, __fmul_rn(w1, t1.x)));
+                    v[i].y = __fmaf_rn(w2, t2.y, __fmaf_rn(w0, t0.y, __fmul_rn(w1, t1.y)));
+                    v[i].z = __fmaf_rn(w2, t2.z, __fmaf_rn(w0, t0.z, __fmul_rn(w1, t1.z)));
+                    v[i].w = __fmaf_rn(w2, t2.w, __fmaf_rn(w0, t0.w, __fmul_rn(w1, t1.w)));
+                }
+            } else {
+                const float *srcb = p.mode_in == IN_DIRECT ? (seg ? p.x2_rows : p.x_rows) : p.feats_pm;
+                const int pitch = p.mode_in == IN_DIRECT ? (seg ? p.x2_pitch : p.x_pitch) : p.c_feat;
+                const bool vec = (pitch & 3) == 0 && (reinterpret_cast<uintptr_t>(srcb) & 15) == 0;
+#pragma unroll
+                for (int i = 0; i < STEPS; ++i) {
+                    const int rr = r0 + (t >> 3) + RS * i;
+                    v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+                    if (M.valid[rr] && kk < width) {
+                        const size_t row = p.mode_in == IN_DIRECT ? (size_t)tile * TM + rr : (size_t)M.src[rr][0];
+                        const float *src = srcb + row * pitch + kk;
+                        if (vec) {
+                            v[i] = __ldg((const float4 *)src);
+                        } else {
+                            float o[4];
+#pragma unroll
+                            for (int q = 0; q < 4; ++q) o[q] = (kk + q < width) ? __ldg(src + q) : 0.f;
+                            v[i] = make_float4(o[0], o[1], o[2], o[3]);
+                        }
+                    }
+                }
+            }
+#pragma unroll
+            for (int i = 0; i < STEPS; ++i) {
+                const int rr = r0 + (t >> 3) + RS * i;
+                *reinterpret_cast<float4 *>(A + swz(rr, j8)) =
+                    make_float4(to_tf32(v[i].x), to_tf32(v[i].y), to_tf32(v[i].z), to_tf32(v[i].w));
+            }
+        }
+    } else if (p.mode_in == IN_SA) {
+        // relative xyz segment: [x - cx, y - cy, z - cz, (<= 5 feature channels,) 0 ...]; one K=8 step
+        if (t < TM) {
+            const int r = t;
+            float4 v = make_float4(0.f, 0.f, 0.f, 0.f), v2 = make_float4(0.f, 0.f, 0.f, 0.f);
+            if (M.valid[r]) {
+                const float *q = p.xyz + (size_t)M.src[r][0] * 3;
+                v.x = to_tf32(__ldg(q + 0) - M.aux[r][0]);
+                v.y = to_tf32(__ldg(q + 1) - M.aux[r][1]);
+                v.z = to_tf32(__ldg(q + 2) - M.aux[r][2]);
+                if (p.c_feat > 0 && p.c_feat <= 5) {
+                    const float *f = p.feats_pm + (size_t)M.src[r][0] * p.c_feat;
+                    v.w = to_tf32(__ldg(f));
+                    if (p.c_feat > 1) v2.x = to_tf32(__ldg(f + 1));
+                    if (p.c_feat > 2) v2.y = to_tf32(__ldg(f + 2));
+                    if (p.c_feat > 3) v2.z = to_tf32(__ldg(f + 3));
+                    if (p.c_feat > 4) v2.w = to_tf32(__ldg(f + 4));
+                }
+            }
+            *reinterpret_cast<float4 *>(A + swz(r, 0)) = v;
+            *reinterpret_cast<float4 *>(A + swz(r, 1)) = v2;
+        }
+    } else {
+        // FP skip segment: channel-major (b, c_skip, n); 4 threads per row (8 channels each), the threads of a warp run
+        // along consecutive points
+        const int r = t & (TM - 1);
+        const long R = (long)tile * TM + r;
+#pragma unroll 1
+        for (int i = 0; i < 256 / NT; ++i) {
+            const int q8 = (t >> 6) + i * (NT / 64);
+            float o[8];
+            if (M.valid[r]) {
+                const int scene = (int)(R / p.n), u = (int)(R - (long)scene * p.n);
+                const float *bsrc = p.skip + (size_t)scene * p.c_skip * p.n + u;
+#pragma unroll
+                for (int q = 0; q < 8; ++q) {
+                    const int ch = k0 + 8 * q8 + q;
+                    o[q] = ch < width ? to_tf32(__ldg(bsrc + (size_t)ch * p.n)) : 0.f;
+                }
+            } else {
+#pragma unroll
+                for (int q = 0; q < 8; ++q) o[q] = 0.f;
+            }
+            *reinterpret_cast<float4 *>(A + swz(r, 2 * q8)) = make_float4(o[0], o[1], o[2], o[3]);
+            *reinterpret_cast<float4 *>(A + swz(r, 2 * q8 + 1)) = make_float4(o[4], o[5], o[6], o[7]);
+        }
+    }
+    return ksteps;
+}
+
+// The accumulator fragment of a warpgroup that covers columns col0 .. col0 + 32 nsub of the layer: thread (wq, g, t4)
+// holds rows 16 wq + g (+8), columns 2 t4 (+1) of each 8.
+// Inner layer: relu(acc * scale + shift) -> tf32 -> the resident activations in `work` (the next layer's K chunks).
+template <int NS>
+__device__ __forceinline__ void store_activations(const ChainParams &p, const float (&acc)[16 * NS], int nsub, int col0, int wq,
+                                                  int g, int t4, const float *sc, const float *sh, uint8_t *work) {
+#pragma unroll
+    for (int j = 0; j < NS; ++j) {
+        if (j >= nsub) continue;
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const int c = col0 + 32 * j + 8 * i + 2 * t4;
+            uint8_t *chunk = work + (size_t)(c >> 5) * A_STAGE_BYTES;
+            const int ju = (c & 31) >> 2, within = (c & 3) * 4;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = 16 * wq + g + 8 * h;
+                float2 o;
+                const float a0 = acc[16 * j + 4 * i + 2 * h], a1 = acc[16 * j + 4 * i + 2 * h + 1];
+                if (p.unit_scale) {
+                    o.x = relu_to_tf32(a0 + sh[c]);
+                    o.y = relu_to_tf32(a1 + sh[c + 1]);
+                } else {
+                    o.x = relu_to_tf32(fmaf(a0, sc[c], sh[c]));
+                    o.y = relu_to_tf32(fmaf(a1, sc[c + 1], sh[c + 1]));
+                }
+                *reinterpret_cast<float2 *>(chunk + swz(r, ju) + within) = o;
+            }
+        }
+    }
+}
+
+// Last layer: SA max-pool, FP (channel-major + optional point-major copy) or rows.  The SA pool goes through the
+// warpgroup's 64 x 32 staging tile `stg` one 32-column subtile at a time (named barrier bar_id over the warpgroup's
+// 128 threads, tw = thread inside the warpgroup); a centre spanning several tiles keeps its partial maxima in s_carry
+// (indexed by column).
+template <int NS>
+__device__ __forceinline__ void final_epilogue(const ChainParams &p, const float (&acc)[16 * NS], int nsub, int col0, int wq,
+                                               int g, int t4, int tw, int tile, const float *sc, const float *sh, float *stg,
+                                               float *s_carry, int bar_id) {
+    const float lo = p.linear_last ? -CUDART_INF_F : 0.f;   // ReLU = max(., 0); a linear last layer keeps the sign
+    const bool pool_raw = p.unit_scale && p.mode_out == OUT_SA_MAX;
+    const int Cl = p.c_last;
+    auto value = [&](float a, int c) -> float {
+        if (pool_raw) return a;   // max_s relu(x_s + t) == relu(max_s x_s + t): shift / ReLU after the max
+        return p.unit_scale ? fmaxf(a + sh[c], lo) : fmaxf(fmaf(a, sc[c], sh[c]), lo);
+    };
+    if (p.mode_out == OUT_SA_MAX) {
+        const int nse = p.ns < TM ? p.ns : TM, per = p.ns > TM ? p.ns / TM : 1;
+        const int sub = tile % per, ncent = TM / nse;
+#pragma unroll
+        for (int j = 0; j < NS; ++j) {
+            if (j >= nsub) continue;
+#pragma unroll
+            for (int i = 0; i < 4; ++i)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int e = 0; e < 2; ++e) {
+                        const int cs = 8 * i + 2 * t4 + e;
+                        stg[(16 * wq + g + 8 * h) * POOL_STRIDE + cs] = value(acc[16 * j + 4 * i + 2 * h + e], col0 + 32 * j + cs);
+                    }
+            bar_wg_id(bar_id);
+            for (int o = tw; o < ncent * 32; o += 128) {
+                const int ci = o >> 5, cs = o & 31, c = col0 + 32 * j + cs;
+                float x = stg[(ci * nse) * POOL_STRIDE + cs];
+                for (int r = 1; r < nse; ++r) x = fmaxf(x, stg[(ci * nse + r) * POOL_STRIDE + cs]);
+                if (per > 1) {
+                    if (sub > 0) x = fmaxf(x, s_carry[c]);
+                    if (sub < per - 1) { s_carry[c] = x; continue; }
+                }
+                if (pool_raw) x = fmaxf(x + sh[c], lo);
+                const long Rg = (long)tile * TM + ci * nse;    // a row of the centre (whole centres per tile)
+                if (Rg < p.total_rows && c < Cl) {
+                    const long pr = Rg >> p.log_ns;
+                    const int scene = (int)(pr / p.npoint), pp = (int)(pr - (long)scene * p.npoint);
+                    p.out[((size_t)scene * p.out_stride_c + p.out_c_off + c) * p.npoint + pp] = x;
+                    if (p.out_pm) p.out_pm[((size_t)scene * p.npoint + pp) * p.out_stride_c + p.out_c_off + c] = x;
+                }
+            }
+            bar_wg_id(bar_id);
+        }
+    } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const long R = (long)tile * TM + 16 * wq + g + 8 * h;
+            if (R >= p.total_rows) continue;
+            int scene = 0, u = 0;
+            if (p.mode_out == OUT_FP) { scene = (int)(R / p.n); u = (int)(R - (long)scene * p.n); }
+#pragma unroll
+            for (int j = 0; j < NS; ++j) {
+                if (j >= nsub) continue;
+#pragma unroll
+                for (int i = 0; i < 4; ++i) {
+                    const int c = col0 + 32 * j + 8 * i + 2 * t4;
+                    float v0 = value(acc[16 * j + 4 * i + 2 * h], c), v1 = value(acc[16 * j + 4 * i + 2 * h + 1], c + 1);
+                    if (p.mode_out == OUT_ROWS) {
+                        if (p.round_out) { v0 = to_tf32(v0); v1 = to_tf32(v1); }   // the next launch's A operand
+                        *reinterpret_cast<float2 *>(p.out + (size_t)R * p.out_pitch + c) = make_float2(v0, v1);
+                    } else {
+                        float *o = p.out + ((size_t)scene * p.out_stride_c + p.out_c_off + c) * p.n + u;
+                        if (c < Cl) o[0] = v0;
+                        if (c + 1 < Cl) o[p.n] = v1;
+                        if (p.out_pm) {   // point-major copy for the next consumer (no transpose kernel)
+                            float *o2 = p.out_pm + (size_t)R * p.out_stride_c + p.out_c_off + c;
+                            if (c < Cl) o2[0] = v0;
+                            if (c + 1 < Cl) o2[1] = v1;
+                        }
+                    }
+                }
+            }
+        }
+    }
+}
+
+// per-layer scale / shift into shared memory (the scale is 1 where it is folded into the weights)
+__device__ __forceinline__ void load_scale_shift(const ChainParams &p, float *s_scale, float *s_shift, int t, int nt) {
+    int off = 0;
+#pragma unroll
+    for (int l = 0; l < MAX_LAYERS; ++l) {
+        if (l >= p.num_layers) break;
+        for (int i = t; i < p.np[l]; i += nt) {
+            s_scale[off + i] = p.unit_scale ? 1.f : p.scale[l][i];
+            s_shift[off + i] = p.shift[l][i];
+        }
+        off += p.np[l];
+    }
+}
+
+// ------------------------------------------------------------------------------------------------ streaming kernel
 // NS: 32-column subtiles per warpgroup of the widest layer (accumulator registers: 16 * NS per thread)
 template <int NS, int MINB>
 __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const ChainParams p) {
@@ -104,18 +412,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
         for (int i = 0; i < NB; ++i) { mbar_init(s2u(&S.b_full[i]), 1); mbar_init(s2u(&S.b_empty[i]), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    {
-        int off = 0;
-#pragma unroll
-        for (int l = 0; l < MAX_LAYERS; ++l) {
-            if (l >= L) break;
-            for (int i = tid; i < p.np[l]; i += CHAIN_THREADS) {
-                s_scale[off + i] = p.unit_scale ? 1.f : p.scale[l][i];
-                s_shift[off + i] = p.shift[l][i];
-            }
-            off += p.np[l];
-        }
-    }
+    load_scale_shift(p, s_scale, s_shift, tid, CHAIN_THREADS);
     __syncthreads();
 
     // the broadcast tells the compiler that wg -- and with it every column range and MMA width -- is warp-uniform
@@ -149,38 +446,13 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
     RingPos rb = {0, 0};
     int aslot = 0;
     float acc[16 * NS];                          // subtile j (32 columns) = registers 16 j .. 16 j + 15
-    const float lo = p.linear_last ? -CUDART_INF_F : 0.f;   // ReLU = max(., 0); a linear last layer keeps the sign
-    const bool pool_raw = p.unit_scale && p.mode_out == OUT_SA_MAX;
 
     for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
         for (int s = 0; s < p.tiles_per_item; ++s) {
             const int tile = item * p.tiles_per_item + s;
             if (tile >= p.num_tiles) break;
-            bar_mma();   // the previous tile's readers of S.row_* and of the pool staging are done
-            if (tid < TM) {
-                const long R = (long)tile * TM + tid;
-                const bool valid = R < p.total_rows;
-                int src[3] = {0, 0, 0};
-                float aux[3] = {0.f, 0.f, 0.f};
-                if (p.mode_in == IN_SA) {
-                    const long pr = valid ? (R >> p.log_ns) : 0;      // global centre index (nsample is a power of two)
-                    const int scene = (int)(pr / p.npoint);
-                    src[0] = scene * p.n + (valid ? __ldg(p.idx + R) : 0);
-#pragma unroll
-                    for (int q = 0; q < 3; ++q) aux[q] = __ldg(p.new_xyz + (size_t)pr * 3 + q);
-                } else if (p.mode_in == IN_FP) {
-                    const long rr = valid ? R : 0;
-                    const int scene = (int)(rr / p.n);
-#pragma unroll
-                    for (int q = 0; q < 3; ++q) {
-                        src[q] = scene * p.m + __ldg(p.idx + (size_t)rr * 3 + q);
-                        aux[q] = __ldg(p.weight + (size_t)rr * 3 + q);
-                    }
-                }
-                S.row_valid[tid] = valid;
-#pragma unroll
-                for (int q = 0; q < 3; ++q) { S.row_src[tid][q] = src[q]; S.row_aux[tid][q] = aux[q]; }
-            }
+            bar_mma();   // the previous tile's readers of S.rows and of the pool staging are done
+            load_tile_rows(p, tile, tid, S.rows);
             bar_mma();
 
             int sc_base = 0;   // layer l's scale / shift in s_scale / s_shift
@@ -195,122 +467,8 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                     uint32_t a_addr;
                     int ksteps = KC / 8;
                     if (l == 0) {
-                        // ---- gather chunk kc of the tile's input rows into A slot `aslot`
-                        int c = kc, seg = 0;
-                        if (p.nseg > 1 && c >= p.seg_chunks[0]) { c -= p.seg_chunks[0]; seg = 1; }
-                        const int k0 = c * KC;                         // first column of this chunk inside its segment
-                        const int width = seg ? p.seg_width[1] : p.seg_width[0];
-                        ksteps = (min(KC, width - k0) + 7) >> 3;       // K=8 steps that hold data (the rest is padding)
                         uint8_t *A = sW + (size_t)aslot * A_STAGE_BYTES;
-                        const bool rows_seg = (p.mode_in == IN_DIRECT) || (p.mode_in == IN_SA && seg == 0 && p.c_feat > 5) ||
-                                              (p.mode_in == IN_FP && seg == 0);
-                        if (rows_seg) {
-                            // point-major sources: 8 threads cover one row's 128 bytes, 256 threads 32 rows per step, 2 steps
-                            const int j8 = tid & 7, kk = k0 + 4 * j8;
-                            float4 v[2];
-                            if (p.mode_in == IN_FP) {
-                                const int C = p.c_known;
-                                const bool vec = (C & 3) == 0;
-#pragma unroll
-                                for (int i = 0; i < 2; ++i) {
-                                    const int rr = (tid >> 3) + 32 * i;
-                                    float4 t0 = make_float4(0.f, 0.f, 0.f, 0.f), t1 = t0, t2 = t0;
-                                    const float w0 = S.row_aux[rr][0], w1 = S.row_aux[rr][1], w2 = S.row_aux[rr][2];
-                                    if (S.row_valid[rr] && kk < width) {
-                                        const float *s0 = p.known_pm + (size_t)S.row_src[rr][0] * C + kk;
-                                        const float *s1 = p.known_pm + (size_t)S.row_src[rr][1] * C + kk;
-                                        const float *s2 = p.known_pm + (size_t)S.row_src[rr][2] * C + kk;
-                                        if (vec) {
-                                            t0 = __ldg((const float4 *)s0); t1 = __ldg((const float4 *)s1); t2 = __ldg((const float4 *)s2);
-                                        } else {
-                                            float a0[4], a1[4], a2[4];
-#pragma unroll
-                                            for (int q = 0; q < 4; ++q) {
-                                                const bool in = kk + q < width;
-                                                a0[q] = in ? __ldg(s0 + q) : 0.f; a1[q] = in ? __ldg(s1 + q) : 0.f; a2[q] = in ? __ldg(s2 + q) : 0.f;
-                                            }
-                                            t0 = make_float4(a0[0], a0[1], a0[2], a0[3]);
-                                            t1 = make_float4(a1[0], a1[1], a1[2], a1[3]);
-                                            t2 = make_float4(a2[0], a2[1], a2[2], a2[3]);
-                                        }
-                                    }
-                                    // same contraction as three_interpolate (reference SASS): fma(w2,p2, fma(w0,p0, w1*p1))
-                                    v[i].x = __fmaf_rn(w2, t2.x, __fmaf_rn(w0, t0.x, __fmul_rn(w1, t1.x)));
-                                    v[i].y = __fmaf_rn(w2, t2.y, __fmaf_rn(w0, t0.y, __fmul_rn(w1, t1.y)));
-                                    v[i].z = __fmaf_rn(w2, t2.z, __fmaf_rn(w0, t0.z, __fmul_rn(w1, t1.z)));
-                                    v[i].w = __fmaf_rn(w2, t2.w, __fmaf_rn(w0, t0.w, __fmul_rn(w1, t1.w)));
-                                }
-                            } else {
-                                const float *srcb = p.mode_in == IN_DIRECT ? (seg ? p.x2_rows : p.x_rows) : p.feats_pm;
-                                const int pitch = p.mode_in == IN_DIRECT ? (seg ? p.x2_pitch : p.x_pitch) : p.c_feat;
-                                const bool vec = (pitch & 3) == 0 && (reinterpret_cast<uintptr_t>(srcb) & 15) == 0;
-#pragma unroll
-                                for (int i = 0; i < 2; ++i) {
-                                    const int rr = (tid >> 3) + 32 * i;
-                                    v[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-                                    if (S.row_valid[rr] && kk < width) {
-                                        const size_t row = p.mode_in == IN_DIRECT ? (size_t)tile * TM + rr : (size_t)S.row_src[rr][0];
-                                        const float *src = srcb + row * pitch + kk;
-                                        if (vec) {
-                                            v[i] = __ldg((const float4 *)src);
-                                        } else {
-                                            float o[4];
-#pragma unroll
-                                            for (int q = 0; q < 4; ++q) o[q] = (kk + q < width) ? __ldg(src + q) : 0.f;
-                                            v[i] = make_float4(o[0], o[1], o[2], o[3]);
-                                        }
-                                    }
-                                }
-                            }
-#pragma unroll
-                            for (int i = 0; i < 2; ++i) {
-                                const int rr = (tid >> 3) + 32 * i;
-                                *reinterpret_cast<float4 *>(A + swz(rr, j8)) =
-                                    make_float4(to_tf32(v[i].x), to_tf32(v[i].y), to_tf32(v[i].z), to_tf32(v[i].w));
-                            }
-                        } else if (p.mode_in == IN_SA) {
-                            // relative xyz segment: [x - cx, y - cy, z - cz, (<= 5 feature channels,) 0 ...]; one K=8 step
-                            if (tid < TM) {
-                                const int r = tid;
-                                float4 v = make_float4(0.f, 0.f, 0.f, 0.f), v2 = make_float4(0.f, 0.f, 0.f, 0.f);
-                                if (S.row_valid[r]) {
-                                    const float *q = p.xyz + (size_t)S.row_src[r][0] * 3;
-                                    v.x = to_tf32(__ldg(q + 0) - S.row_aux[r][0]);
-                                    v.y = to_tf32(__ldg(q + 1) - S.row_aux[r][1]);
-                                    v.z = to_tf32(__ldg(q + 2) - S.row_aux[r][2]);
-                                    if (p.c_feat > 0 && p.c_feat <= 5) {
-                                        const float *f = p.feats_pm + (size_t)S.row_src[r][0] * p.c_feat;
-                                        v.w = to_tf32(__ldg(f));
-                                        if (p.c_feat > 1) v2.x = to_tf32(__ldg(f + 1));
-                                        if (p.c_feat > 2) v2.y = to_tf32(__ldg(f + 2));
-                                        if (p.c_feat > 3) v2.z = to_tf32(__ldg(f + 3));
-                                        if (p.c_feat > 4) v2.w = to_tf32(__ldg(f + 4));
-                                    }
-                                }
-                                *reinterpret_cast<float4 *>(A + swz(r, 0)) = v;
-                                *reinterpret_cast<float4 *>(A + swz(r, 1)) = v2;
-                            }
-                        } else {
-                            // FP skip segment: channel-major (b, c_skip, n); 4 threads per row (8 channels each), the
-                            // threads of a warp run along consecutive points
-                            const int r = tid & (TM - 1), q8 = tid >> 6;
-                            const long R = (long)tile * TM + r;
-                            float o[8];
-                            if (S.row_valid[r]) {
-                                const int scene = (int)(R / p.n), u = (int)(R - (long)scene * p.n);
-                                const float *bsrc = p.skip + (size_t)scene * p.c_skip * p.n + u;
-#pragma unroll
-                                for (int q = 0; q < 8; ++q) {
-                                    const int ch = k0 + 8 * q8 + q;
-                                    o[q] = ch < width ? to_tf32(__ldg(bsrc + (size_t)ch * p.n)) : 0.f;
-                                }
-                            } else {
-#pragma unroll
-                                for (int q = 0; q < 8; ++q) o[q] = 0.f;
-                            }
-                            *reinterpret_cast<float4 *>(A + swz(r, 2 * q8)) = make_float4(o[0], o[1], o[2], o[3]);
-                            *reinterpret_cast<float4 *>(A + swz(r, 2 * q8 + 1)) = make_float4(o[4], o[5], o[6], o[7]);
-                        }
+                        ksteps = gather_chunk<2 * 128>(p, tile, kc, tid, S.rows, A);
                         fence_async_smem();
                         // slot `aslot` is complete.  It was last read by the MMAs of chunk kc-3, which both warpgroups
                         // retired (wgmma_wait<1> of chunk kc-2) before the barrier of chunk kc-1.
@@ -338,114 +496,129 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                 sc_base += np_l;
 
                 if (l + 1 < L) {
-                    // ---- relu(acc * scale + shift) -> tf32 -> resident activations = the next layer's K chunks
-#pragma unroll
-                    for (int j = 0; j < NS; ++j) {
-                        if (j >= nsub) continue;
-#pragma unroll
-                        for (int i = 0; i < 4; ++i) {
-                            const int c = col0 + 32 * j + 8 * i + 2 * t4;
-                            uint8_t *chunk = sW + (size_t)(c >> 5) * A_STAGE_BYTES;
-                            const int ju = (c & 31) >> 2, within = (c & 3) * 4;
-#pragma unroll
-                            for (int h = 0; h < 2; ++h) {
-                                const int r = 16 * wq + g + 8 * h;
-                                float2 o;
-                                const float a0 = acc[16 * j + 4 * i + 2 * h], a1 = acc[16 * j + 4 * i + 2 * h + 1];
-                                if (p.unit_scale) {
-                                    o.x = relu_to_tf32(a0 + sh[c]);
-                                    o.y = relu_to_tf32(a1 + sh[c + 1]);
-                                } else {
-                                    o.x = relu_to_tf32(fmaf(a0, sc[c], sh[c]));
-                                    o.y = relu_to_tf32(fmaf(a1, sc[c + 1], sh[c + 1]));
-                                }
-                                *reinterpret_cast<float2 *>(chunk + swz(r, ju) + within) = o;
-                            }
-                        }
-                    }
+                    store_activations<NS>(p, acc, nsub, col0, wq, g, t4, sc, sh, sW);
                     fence_async_smem();
                     bar_mma();   // the next layer's A operand is complete
                     continue;
                 }
-
-                // ---- final epilogue
-                const int Cl = p.c_last;
-                auto value = [&](float a, int c) -> float {
-                    if (pool_raw) return a;   // max_s relu(x_s + t) == relu(max_s x_s + t): shift / ReLU after the max
-                    return p.unit_scale ? fmaxf(a + sh[c], lo) : fmaxf(fmaf(a, sc[c], sh[c]), lo);
-                };
-                if (p.mode_out == OUT_SA_MAX) {
-                    // max over the nsample consecutive rows of each centre, one 32-column subtile at a time through this
-                    // warpgroup's staging tile; a centre spanning several tiles keeps its partial maxima in s_carry
-                    float *stg = reinterpret_cast<float *>(sW) + wg * (TM * POOL_STRIDE);
-                    const int nse = p.ns < TM ? p.ns : TM, per = p.ns > TM ? p.ns / TM : 1;
-                    const int sub = tile % per, ncent = TM / nse;
-#pragma unroll
-                    for (int j = 0; j < NS; ++j) {
-                        if (j >= nsub) continue;
-#pragma unroll
-                        for (int i = 0; i < 4; ++i)
-#pragma unroll
-                            for (int h = 0; h < 2; ++h)
-#pragma unroll
-                                for (int e = 0; e < 2; ++e) {
-                                    const int cs = 8 * i + 2 * t4 + e;
-                                    stg[(16 * wq + g + 8 * h) * POOL_STRIDE + cs] = value(acc[16 * j + 4 * i + 2 * h + e], col0 + 32 * j + cs);
-                                }
-                        bar_wg(wg);
-                        for (int o = tw; o < ncent * 32; o += 128) {
-                            const int ci = o >> 5, cs = o & 31, c = col0 + 32 * j + cs;
-                            float x = stg[(ci * nse) * POOL_STRIDE + cs];
-                            for (int r = 1; r < nse; ++r) x = fmaxf(x, stg[(ci * nse + r) * POOL_STRIDE + cs]);
-                            if (per > 1) {
-                                if (sub > 0) x = fmaxf(x, s_carry[c]);
-                                if (sub < per - 1) { s_carry[c] = x; continue; }
-                            }
-                            if (pool_raw) x = fmaxf(x + sh[c], lo);
-                            const long Rg = (long)tile * TM + ci * nse;    // a row of the centre (whole centres per tile)
-                            if (Rg < p.total_rows && c < Cl) {
-                                const long pr = Rg >> p.log_ns;
-                                const int scene = (int)(pr / p.npoint), pp = (int)(pr - (long)scene * p.npoint);
-                                p.out[((size_t)scene * p.out_stride_c + p.out_c_off + c) * p.npoint + pp] = x;
-                                if (p.out_pm) p.out_pm[((size_t)scene * p.npoint + pp) * p.out_stride_c + p.out_c_off + c] = x;
-                            }
-                        }
-                        bar_wg(wg);
-                    }
-                } else {
-#pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const long R = (long)tile * TM + 16 * wq + g + 8 * h;
-                        if (R >= p.total_rows) continue;
-                        int scene = 0, u = 0;
-                        if (p.mode_out == OUT_FP) { scene = (int)(R / p.n); u = (int)(R - (long)scene * p.n); }
-#pragma unroll
-                        for (int j = 0; j < NS; ++j) {
-                            if (j >= nsub) continue;
-#pragma unroll
-                            for (int i = 0; i < 4; ++i) {
-                                const int c = col0 + 32 * j + 8 * i + 2 * t4;
-                                float v0 = value(acc[16 * j + 4 * i + 2 * h], c), v1 = value(acc[16 * j + 4 * i + 2 * h + 1], c + 1);
-                                if (p.mode_out == OUT_ROWS) {
-                                    if (p.round_out) { v0 = to_tf32(v0); v1 = to_tf32(v1); }   // the next launch's A operand
-                                    *reinterpret_cast<float2 *>(p.out + (size_t)R * p.out_pitch + c) = make_float2(v0, v1);
-                                } else {
-                                    float *o = p.out + ((size_t)scene * p.out_stride_c + p.out_c_off + c) * p.n + u;
-                                    if (c < Cl) o[0] = v0;
-                                    if (c + 1 < Cl) o[p.n] = v1;
-                                    if (p.out_pm) {   // point-major copy for the next consumer (no transpose kernel)
-                                        float *o2 = p.out_pm + (size_t)R * p.out_stride_c + p.out_c_off + c;
-                                        if (c < Cl) o2[0] = v0;
-                                        if (c + 1 < Cl) o2[1] = v1;
-                                    }
-                                }
-                            }
-                        }
-                    }
-                }
+                final_epilogue<NS>(p, acc, nsub, col0, wq, g, t4, tw, tile, sc, sh,
+                                   reinterpret_cast<float *>(sW) + wg * (TM * POOL_STRIDE), s_carry, 2 + wg);
             }
         }
     }
+}
+
+// ------------------------------------------------------------------------------------------------ resident kernel
+// NS: 32-column subtiles of the widest layer, all of them in one warpgroup (np <= RES_NP_MAX).  blockDim.x = 128 * nwg.
+template <int NS, int NWG, int MINB>
+__global__ void __launch_bounds__(NWG * 128, MINB) mlp_resident_kernel(const ChainParams p) {
+    static_assert(NWG <= RES_WG_MAX, "mlp_resident_kernel: one named barrier per warpgroup");
+    static_assert(NS * 32 <= RES_NP_MAX, "mlp_resident_kernel: one warpgroup covers the widest layer");
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ uint64_t w_full;
+    uint8_t *base = smem_raw + ((1024u - (s2u(smem_raw) & 1023u)) & 1023u);
+    const int L = p.num_layers, nwg = blockDim.x >> 7;
+    int np_total = 0, w_bytes = 0;
+#pragma unroll
+    for (int l = 0; l < MAX_LAYERS; ++l) {
+        np_total += l < L ? p.np[l] : 0;
+        w_bytes += l < L ? p.nchunks[l] * p.np[l] * KC * 4 : 0;
+    }
+    const int np_last = per_layer(p.np, L - 1);
+    // [weight image of every layer | nwg work regions | scale | shift | nwg pool carries | nwg tile-row tables]
+    uint8_t *sWt = base;
+    uint8_t *sWork = sWt + w_bytes;
+    float *s_scale = reinterpret_cast<float *>(sWork + (size_t)nwg * p.work_bytes);
+    float *s_shift = s_scale + np_total;
+    float *s_carry_all = s_shift + np_total;
+    TileRows *rows_all = reinterpret_cast<TileRows *>(s_carry_all + nwg * np_last);
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+
+    if (tid == 0) {
+        mbar_init(s2u(&w_full), 1);
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    load_scale_shift(p, s_scale, s_shift, tid, blockDim.x);
+    __syncthreads();
+    if (tid == 0) {
+        // the whole packed image, chunk by chunk, on one mbarrier; it stays for every tile of the CTA
+        mbar_expect_tx(s2u(&w_full), (uint32_t)w_bytes);
+        uint32_t off = 0;
+        for (int l = 0; l < L; ++l) {
+            const int np_l = per_layer(p.np, l), nch = per_layer(p.nchunks, l);
+            const float *w = per_layer(p.w, l);
+            const uint32_t bytes = (uint32_t)np_l * KC * 4;
+            for (int kc = 0; kc < nch; ++kc, off += bytes)
+                bulk_g2s(s2u(sWt + off), w + (size_t)kc * np_l * KC, bytes, s2u(&w_full));
+        }
+    }
+
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
+    const int wq = warp & 3;
+    const int g = lane >> 2, t4 = lane & 3;
+    const int tw = tid & 127;
+    const int bar_id = 1 + wg;
+    uint8_t *W = sWork + (size_t)wg * p.work_bytes;   // this warpgroup's A slots / activations / pool staging
+    float *s_carry = s_carry_all + wg * np_last;
+    TileRows &M = rows_all[wg];
+    const int nslots = p.nchunks[0] < A_SLOTS ? p.nchunks[0] : A_SLOTS;
+    bool w_ready = false;
+    float acc[16 * NS];
+
+    // warpgroups take items in a strided order over the whole grid; an item's tiles stay with one warpgroup
+    for (int item = blockIdx.x * nwg + wg; item < p.num_items; item += gridDim.x * nwg) {
+        for (int s = 0; s < p.tiles_per_item; ++s) {
+            const int tile = item * p.tiles_per_item + s;
+            if (tile >= p.num_tiles) break;
+            bar_wg_id(bar_id);   // the previous tile's readers of M and of the pool staging are done
+            load_tile_rows(p, tile, tw, M);
+            bar_wg_id(bar_id);
+
+            int sc_base = 0;
+            uint32_t w_off = 0;   // layer l's image in sWt
+            for (int l = 0; l < L; ++l) {
+                const int np_l = per_layer(p.np, l), nsub = np_l >> 5;
+                const int nch = per_layer(p.nchunks, l);
+                int aslot = 0;
+                for (int kc = 0; kc < nch; ++kc) {
+                    uint32_t a_addr;
+                    int ksteps = KC / 8;
+                    if (l == 0) {
+                        uint8_t *A = W + (size_t)aslot * A_STAGE_BYTES;
+                        ksteps = gather_chunk<128>(p, tile, kc, tw, M, A);
+                        fence_async_smem();
+                        // slot `aslot` was last read by the MMAs of chunk kc-3, which every warp of the warpgroup
+                        // retired (wgmma_wait<1> of chunk kc-2) before the barrier of chunk kc-1
+                        bar_wg_id(bar_id);
+                        a_addr = s2u(A);
+                        aslot = aslot == nslots - 1 ? 0 : aslot + 1;
+                    } else {
+                        a_addr = s2u(W + (size_t)kc * A_STAGE_BYTES);
+                    }
+                    if (!w_ready) { mbar_wait(s2u(&w_full), 0); w_ready = true; }
+                    const uint32_t b_addr = s2u(sWt) + w_off + (uint32_t)kc * np_l * (KC * 4);
+                    wgmma_fence();
+                    mma_chunk<NS>(acc, nsub, ksteps, make_desc(a_addr), make_desc(b_addr), kc > 0 ? 1u : 0u);
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                }
+                w_off += (uint32_t)nch * np_l * (KC * 4);
+                wgmma_wait<0>();
+                reg_fence(acc);
+                bar_wg_id(bar_id);   // the warpgroup's MMAs of layer l have read their A operand: the work region is free
+                const float *sc = s_scale + sc_base, *sh = s_shift + sc_base;
+                sc_base += np_l;
+                if (l + 1 < L) {
+                    store_activations<NS>(p, acc, nsub, 0, wq, g, t4, sc, sh, W);
+                    fence_async_smem();
+                    bar_wg_id(bar_id);   // the next layer's A operand is complete
+                    continue;
+                }
+                final_epilogue<NS>(p, acc, nsub, 0, wq, g, t4, tw, tile, sc, sh, reinterpret_cast<float *>(W), s_carry, bar_id);
+            }
+        }
+    }
+    if (tid == 0 && !w_ready) mbar_wait(s2u(&w_full), 0);   // no CTA exits with its weight copy in flight
 }
 
 // ------------------------------------------------------------------------------------------------ host side
@@ -586,7 +759,72 @@ static size_t segment_smem(const int *np, int n, int nb, int *work_bytes, int *b
     return chain_smem_bytes(work, nb, np_max * KC * 4, np_total, np[n - 1]) + sizeof(SmemFixed);
 }
 
-// launch one fused segment of the chain: size the weight ring to the segment, pick the CTAs per SM it allows
+// Resident variant of one launch, if it applies: every layer at most RES_NP_MAX wide, one of the three plain mode pairs,
+// and the whole packed image plus one warpgroup's working set within the shared memory of a CTA.  Warpgroups per CTA
+// and CTAs per SM are the pair that keeps the most warpgroups on an SM (registers, shared memory and threads as the
+// occupancy calculator counts them); on a tie, the fewer CTAs, so fewer copies of the image.  Returns false if the
+// launch is for the streaming kernel.
+static bool launch_resident(ChainParams &p, int max_optin, cudaStream_t st, int *rc) {
+    if (!opts().mlp_resident) return false;
+    const bool modes = (p.mode_in == IN_SA && p.mode_out == OUT_SA_MAX) || (p.mode_in == IN_FP && p.mode_out == OUT_FP) ||
+                       (p.mode_in == IN_DIRECT && p.mode_out == OUT_ROWS);
+    if (!modes) return false;
+    const int L = p.num_layers;
+    int np_total = 0, np_max = 0, mid_max = 0;
+    size_t w_bytes = 0;
+    for (int l = 0; l < L; ++l) {
+        np_total += p.np[l];
+        np_max = p.np[l] > np_max ? p.np[l] : np_max;
+        if (l + 1 < L && p.np[l] > mid_max) mid_max = p.np[l];
+        w_bytes += (size_t)p.nchunks[l] * p.np[l] * KC * 4;
+    }
+    if (np_max > RES_NP_MAX) return false;
+    // the image takes at most half of a CTA's shared memory, so at least three warpgroups' work regions fit beside it.
+    // Measured on an H100 80GB HBM3 (600 W limit): the two larger images of the RPN backbone -- the FP0 chain, 144 KB
+    // (2 warpgroups per SM), and its projection, 128 KB (3) -- ran 1.33x and 1.16x slower resident than streamed.
+    if (2 * w_bytes > (size_t)max_optin) return false;
+    // a warpgroup's work region: its layer-0 A slots, the activations of the widest inner layer, its pool staging
+    const int slots = p.nchunks[0] < A_SLOTS ? p.nchunks[0] : A_SLOTS;
+    int work = slots * A_STAGE_BYTES;
+    if (TM * mid_max * 4 > work) work = TM * mid_max * 4;
+    if (TM * POOL_STRIDE * 4 > work) work = TM * POOL_STRIDE * 4;
+    work = round_up(work, 1024);
+    const int np_last = p.np[L - 1];
+    auto smem_for = [&](int nwg) -> size_t {
+        return 1024 /*alignment slack*/ + w_bytes + 2 * (size_t)np_total * sizeof(float) +
+               (size_t)nwg * (work + np_last * sizeof(float) + sizeof(TileRows));
+    };
+    if (smem_for(1) + 64 /*static: the weight mbarrier*/ > (size_t)max_optin) return false;
+    p.work_bytes = work;
+    auto go = [&](auto kern, int nwg_max) -> int {
+        cudaFuncAttributes fa;
+        PRB_CUDA(cudaFuncGetAttributes(&fa, kern));
+        const size_t dyn_max = (size_t)max_optin - fa.sharedSizeBytes;
+        PRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn_max));
+        int best_nwg = 1, best_occ = 1, best_total = 0;
+        for (int nwg = 1; nwg <= nwg_max; ++nwg) {
+            if (smem_for(nwg) > dyn_max) break;
+            int occ = 0;
+            PRB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, nwg * 128, smem_for(nwg)));
+            if (const int o = opts().mlp_occ; o >= 1 && o < occ) occ = o;
+            if (occ * nwg >= best_total && occ >= 1) { best_nwg = nwg; best_occ = occ; best_total = occ * nwg; }
+        }
+        int sms = num_sms();
+        if (const int v = opts().mlp_sms; v >= 1 && v < sms) sms = v;
+        const int ctas = (p.num_items + best_nwg - 1) / best_nwg;   // every CTA has an item for its warpgroup 0
+        const int grid = ctas < sms * best_occ ? ctas : sms * best_occ;
+        kern<<<grid, best_nwg * 128, smem_for(best_nwg), st>>>(p);
+        return check_launch("mlp_resident_kernel");
+    };
+    const int ns = np_max >> 5;
+    // register bounds without spills: <1, 5> 96 (five warpgroups per SM), <4, 4> 128 (four); a 64-wide chain takes the
+    // <4, 4> build, whose m64n64 path needs no more registers than the <2, *> builds that were tried and spilled
+    *rc = ns <= 1 ? go(mlp_resident_kernel<1, 5, 1>, 5) : go(mlp_resident_kernel<4, 4, 1>, 4);
+    return true;
+}
+
+// launch one fused segment of the chain: the resident kernel where it applies, else the streaming kernel with the
+// weight ring sized to the segment and the CTAs per SM it allows
 static int launch_chain(ChainParams &p, cudaStream_t st) {
     int max_optin = 0, dev = 0;
     PRB_CUDA(cudaGetDevice(&dev));
@@ -595,6 +833,7 @@ static int launch_chain(ChainParams &p, cudaStream_t st) {
     if (p.num_tiles == 0) return 0;
     p.tiles_per_item = (p.mode_out == OUT_SA_MAX && p.ns > TM) ? p.ns / TM : 1;
     p.num_items = (p.num_tiles + p.tiles_per_item - 1) / p.tiles_per_item;
+    if (int rc = 0; launch_resident(p, max_optin, st, &rc)) return rc;
     const int L = p.num_layers;
     int np_total = 0, ns_max = 1;
     for (int l = 0; l < L; ++l) {
