@@ -215,7 +215,8 @@ PRB_API int prb_fp_interp_mlp_ws(int b, int n, int m, int c_known, int c_skip, c
 PRB_API int prb_mlp_rows(long rows, int c_in, const float *x_rows, const prb_mlp_desc *mlp, float *out_rows,
                          int out_pitch, void *workspace, size_t workspace_bytes, void *stream);
 /* the same with strided inputs and an optional second K segment: layer 0 reads [a_rows[:, :c_a] | b_rows[:, :c_b]] (row
- * pitches in floats, any alignment; 128-bit loads when base and pitch are 16-byte aligned).  With c_b > 0 the weights are
+ * pitches in floats, any alignment; 128-bit loads when base and pitch are 16-byte aligned; columns past c_a / c_b are never
+ * read, so they may hold anything, NaN included).  With c_b > 0 the weights are
  * packed with prb_mlp_pack_weights_ex(kind 1, split c_a), else kind 2.  This is merge_down_layer on cat(xyz_feature,
  * rpn_feature) (lib/net/rcnn_net.py:171-175) without materialising the concatenation, and xyz_up_layer on a column
  * slice of the pooled rows. */

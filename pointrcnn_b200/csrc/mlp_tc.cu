@@ -183,7 +183,9 @@ __device__ __forceinline__ int gather_chunk(const ChainParams &p, int tile, int 
             } else {
                 const float *srcb = p.mode_in == IN_DIRECT ? (seg ? p.x2_rows : p.x_rows) : p.feats_pm;
                 const int pitch = p.mode_in == IN_DIRECT ? (seg ? p.x2_pitch : p.x_pitch) : p.c_feat;
-                const bool vec = (pitch & 3) == 0 && (reinterpret_cast<uintptr_t>(srcb) & 15) == 0;
+                // a 128-bit load only where the whole group of 4 columns lies inside the segment: a direct-rows segment may
+                // be narrower than its pitch, and the columns past it must not be read (0 * NaN would reach the output)
+                const bool vec = (pitch & 3) == 0 && (reinterpret_cast<uintptr_t>(srcb) & 15) == 0 && kk + 4 <= width;
 #pragma unroll
                 for (int i = 0; i < STEPS; ++i) {
                     const int rr = r0 + (t >> 3) + RS * i;

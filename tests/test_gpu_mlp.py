@@ -49,26 +49,11 @@ def tf32_rn(x):
     return u.astype(np.uint32).view(np.float32)
 
 
-def tf32_trunc(x):
-    """what the tensor core does to raw fp32 operand bits: the low 13 mantissa bits are dropped"""
-    u = np.ascontiguousarray(x, dtype=np.float32).view(np.uint32).copy()
-    u &= 0xFFFFE000
-    return u.view(np.float32)
-
-
 def mlp_tf32_ref(x, layers):
-    """weights are rounded at pack time (host, ties away), every A operand built in registers with cvt.rn (ties even).  With the
-    optional cp.async gather (prb_options.mlp_gather = 1/2) layer-0 rows of 16-byte aligned pitch reach the tensor core
-    unrounded and are truncated there."""
-    import ctypes
-    from pointrcnn_b200 import _cabi
-    o = _cabi.Options()
-    _cabi.lib().prb_get_thread_options(ctypes.byref(o))
-    async_gather = o.mlp_gather in (1, 2)
+    """weights are rounded at pack time (host, ties away), every A operand built in registers with cvt.rn (ties even)"""
     h = x.astype(np.float32)
-    for li, (W, sc, sh) in enumerate(layers):
-        a = tf32_trunc(h) if (async_gather and li == 0 and x.shape[1] % 4 == 0) else tf32_rn(h)
-        h = a @ tf32(W).T
+    for W, sc, sh in layers:
+        h = tf32_rn(h) @ tf32(W).T
         h = np.maximum(h * sc[None] + sh[None], 0).astype(np.float32)
     return h
 
@@ -301,34 +286,11 @@ def test_sa_module_scale_fold_modes_agree(cuda, ns):
     assert (outs["0"] - outs["1"]).abs().max().item() <= TOL * scale
 
 
-@pytest.mark.parametrize("fold", [True, False])
-@pytest.mark.parametrize("ns,widths", [(16, [24, 32, 48]), (32, [64, 96, 128]), (64, [32, 32, 80]), (128, [32, 64]), (32, [16, 200])])
-def test_sa_pooling_layouts_bit_identical(cuda, ns, widths, fold):
-    """max-pool epilogues of the chain kernel (prb_options.mlp_pool): 0 quad tensor-memory layout (default), 1 shuffle
-    butterfly, 2 warp-wide CREDUX, 3 staged tile (64 / 128 samples) -- a max is exact, so every layout must give the same bits
-    (channel counts that are not multiples of 16, both scale modes)"""
-    from pointrcnn_b200 import _cabi as C, config
-    torch.manual_seed(ns)
-    mod = pm.PointnetSAModuleMSG(npoint=150, radii=[0.3], nsamples=[ns], mlps=[[20] + widths], bn=True).to(cuda).eval()
-    _randomise_bn(mod, 5)
-    x = torch.from_numpy(synth.u_cube(2, 2500, 31)).to(cuda)
-    f = torch.randn(2, 20, 2500, device=cuda)
-    outs = []
-    for mode in (0, 1, 2, 3):
-        with torch.no_grad(), config.override(fold_scale=fold), C.options(mlp_pool=mode):
-            outs.append(mod(x, f)[1].clone())
-    for mode in (1, 2, 3):
-        assert torch.equal(outs[0], outs[mode]), "pooling layout %d differs from the quad layout" % mode
-    with torch.no_grad():
-        ref = _unfused(lambda: mod(x, f))[1]
-    assert (outs[0] - ref).abs().max().item() <= TOL * ref.abs().max().item()
-
-
 @pytest.mark.parametrize("ns,widths", [(16, [16, 16, 32]), (32, [32, 32, 64])])
 def test_sa_builds_bit_identical(cuda, ns, widths):
-    """the builds of the chain kernel (CTAs per SM x row warps; prb_options.mlp_occ / mlp_ne / mlp_ngw) compute the same bits: K
-    order and per-element arithmetic do not depend on the plan -- the premise of the measured build choice.  SA1-shaped chains
-    (xyz + 1 feature channel), which is where the three-CTA build applies."""
+    """the launch plans of the chain (CTAs per SM, SMs of the persistent grid, resident or streamed weights;
+    prb_options.mlp_occ / mlp_sms / mlp_resident) compute the same bits: K order and per-element arithmetic do not depend on
+    the plan.  SA1-shaped chains (xyz + 1 feature channel) through the module."""
     from pointrcnn_b200 import _cabi as C
     torch.manual_seed(3 + ns)
     mod = pm.PointnetSAModuleMSG(npoint=700, radii=[0.3], nsamples=[ns], mlps=[[1] + widths], bn=True).to(cuda).eval()
@@ -336,7 +298,7 @@ def test_sa_builds_bit_identical(cuda, ns, widths):
     x = torch.from_numpy(synth.u_cube(3, 4000, 13)).to(cuda)
     f = torch.randn(3, 1, 4000, device=cuda)
     outs = []
-    for opt in ({"mlp_tune": 0}, {"mlp_occ": 3}, {"mlp_occ": 1}, {"mlp_occ": 1, "mlp_ne": 2, "mlp_ngw": 3}):
+    for opt in ({}, {"mlp_occ": 3}, {"mlp_occ": 1}, {"mlp_sms": 7}, {"mlp_resident": 0}, {"mlp_resident": 0, "mlp_occ": 1}):
         with torch.no_grad(), C.options(**opt):
             outs.append(mod(x, f)[1].clone())
     for k in range(1, len(outs)):
