@@ -11,34 +11,26 @@ Two execution paths per module, chosen per call:
            torch.nn convolutions, full autograd support.
 `config.override(disable_fused=True)` forces the unfused path (used by tests to cross-check the two).
 """
-import ctypes
 from typing import List
 
-import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from .. import _cabi as C
 from .. import config
-from .. import prof
+from .. import mlp_chain
 from . import pointnet2_utils
 from . import pytorch_utils as pt_utils
 
 
-def _round_up(a, b):
-    return (a + b - 1) // b * b
-
-
 class _FusedMLP:
-    """Device-side image of one SharedMLP for the tensor-core chain: packed weights + folded BN scale/shift.
-    Rebuilt whenever a parameter / buffer version changes (optimizer step, load_state_dict, .to())."""
+    """The mlp_chain.Chain of one SharedMLP (folded BN, packed weights on the device), rebuilt whenever a parameter / buffer
+    version changes (optimizer step, load_state_dict, .to())."""
 
     def __init__(self):
         self.key = None
-        self.desc = None
-        self.tensors = None
-        self.c_out = None
+        self.chain = None
+        self.proj = None
 
     @staticmethod
     def supported(mlp: nn.Sequential):
@@ -59,7 +51,8 @@ class _FusedMLP:
         return True
 
     def get(self, mlp: nn.Sequential, kind: int, split: int, device, project_known: bool = False):
-        """project_known (FP chains, kind 1): layer 0 is split by linearity -- interp(known) @ W0k^T == interp(known @ W0k^T) --
+        """-> the chain of `mlp`, packed as (kind, split) on `device`.
+        project_known (FP chains, kind FP): layer 0 is split by linearity -- interp(known) @ W0k^T == interp(known @ W0k^T) --
         into a per-KNOWN-point projection (a separate, 4x smaller row GEMM: `self.proj`, linear, no shift) and a main chain
         whose layer 0 reads [interp(projected rows) | skip] through the weight [I | W0s]: the gather moves c_out0 instead of
         c_known floats per neighbour and layer 0 contracts over c_out0 + c_skip instead of c_known + c_skip columns."""
@@ -72,73 +65,24 @@ class _FusedMLP:
                 tensors += [bn.weight, bn.bias, bn.running_mean, bn.running_var]
         key = (kind, split, str(device), _fold_scale(), project_known) + tuple((id(t), t._version) if t is not None else None for t in tensors)
         if key == self.key:
-            return self.desc
-        L = len(layers)
-        c_in = layers[0].conv.in_channels
-        c_out = [layer.conv.out_channels for layer in layers]
-        ws, scales, shifts = [], [], []
-        with torch.no_grad():
-            for layer in layers:
-                conv = layer.conv
-                W = conv.weight.detach().reshape(conv.out_channels, -1).float().cpu().contiguous()
-                co = conv.out_channels
-                if hasattr(layer, "bn"):
-                    bn = layer.bn.bn
-                    inv = (bn.weight.detach().float() / torch.sqrt(bn.running_var.detach().float() + bn.eps)).cpu()
-                    sh = (bn.bias.detach().float().cpu() - bn.running_mean.detach().float().cpu() * inv)
-                    if conv.bias is not None:
-                        sh = sh + inv * conv.bias.detach().float().cpu()
-                else:
-                    inv = torch.ones(co)
-                    sh = conv.bias.detach().float().cpu() if conv.bias is not None else torch.zeros(co)
-                pad = _round_up(co, 32) - co
-                if _fold_scale():
-                    W = (W * inv[:, None]).contiguous()     # BN scale folded into the weights before TF32 rounding
-                ws.append(W)
-                scales.append(F.pad(inv, (0, pad)))
-                shifts.append(F.pad(sh, (0, pad)))
-        lib = C.lib()
+            return self.chain
+        fold_scale = key[3]
+        folded = [mlp_chain.fold(layer.conv, layer.bn.bn if hasattr(layer, "bn") else None, fold_scale) for layer in layers]
+        ws = [W for W, _, _ in folded]
+        shifts = [t for _, _, t in folded]
+        scales = None if fold_scale else [s for _, s, _ in folded]
         self.proj = None
         if project_known:
             # ws[0] is (c_out0, c_known + c_skip) with the BN scale already folded in: W0k -> projection, W0s stays
+            assert scales is None, "project_known needs the BN scale folded into the weights"
             W0 = ws[0]
             c1, c_known = W0.shape[0], split
-            self.proj = self._pack(lib, 2, 0, c_known, [c1], [W0[:, :c_known].contiguous()], torch.zeros(_round_up(c1, 32)), device, flags=1)
-            ws[0] = torch.cat([torch.eye(c1), W0[:, c_known:]], dim=1).contiguous()
-            c_in, split = c1 + (c_in - c_known), c1
-        co_arr = (ctypes.c_int * 3)(*(c_out + [0] * (3 - L)))
-        nbytes = lib.prb_mlp_packed_bytes_ex(kind, split, L, c_in, co_arr)
-        host = np.zeros(nbytes // 4, dtype=np.float32)
-        wp = (ctypes.c_void_p * L)(*[w.data_ptr() for w in ws])
-        C.check(lib.prb_mlp_pack_weights_ex(kind, split, L, c_in, co_arr, wp, host.ctypes.data_as(ctypes.c_void_p)), "mlp_pack")
-        packed = torch.from_numpy(host).to(device)
-        scale = torch.cat(scales).contiguous().to(device)
-        shift = torch.cat(shifts).contiguous().to(device)
-        desc = C.MlpDesc()
-        desc.num_layers, desc.c_in = L, c_in
-        for i in range(3):
-            desc.c_out[i] = c_out[i] if i < L else 0
-        desc.packed_w, desc.scale, desc.shift = packed.data_ptr(), (None if _fold_scale() else scale.data_ptr()), shift.data_ptr()
-        self.key, self.desc, self.tensors, self.c_out = key, desc, (packed, scale, shift), c_out
-        return desc
-
-    @staticmethod
-    def _pack(lib, kind, split, c_in, c_out, ws, shift, device, flags=0):
-        """pack a chain whose scale is already folded into `ws`; returns dict(desc, keep-alive tensors, c_out)"""
-        L = len(ws)
-        co_arr = (ctypes.c_int * 3)(*(c_out + [0] * (3 - L)))
-        nbytes = lib.prb_mlp_packed_bytes_ex(kind, split, L, c_in, co_arr)
-        host = np.zeros(nbytes // 4, dtype=np.float32)
-        wp = (ctypes.c_void_p * L)(*[w.data_ptr() for w in ws])
-        C.check(lib.prb_mlp_pack_weights_ex(kind, split, L, c_in, co_arr, wp, host.ctypes.data_as(ctypes.c_void_p)), "mlp_pack")
-        packed = torch.from_numpy(host).to(device)
-        shift = shift.contiguous().to(device)
-        desc = C.MlpDesc()
-        desc.num_layers, desc.c_in = L, c_in
-        for i in range(3):
-            desc.c_out[i] = c_out[i] if i < L else 0
-        desc.packed_w, desc.scale, desc.shift, desc.flags = packed.data_ptr(), None, shift.data_ptr(), flags
-        return dict(desc=desc, keep=(packed, shift, ws), c_out=c_out, co_arr=co_arr)
+            self.proj = mlp_chain.Chain(mlp_chain.ROWS, 0, [W0[:, :c_known]], [torch.zeros(c1)], linear_last=True, device=device)
+            ws[0] = torch.cat([torch.eye(c1), W0[:, c_known:]], dim=1)
+            split = c1
+        self.chain = mlp_chain.Chain(kind, split, ws, shifts, scales, device=device)
+        self.key = key
+        return self.chain
 
 
 def _attach_pm(t, pm):
@@ -160,24 +104,9 @@ def rows_mlp(fused: "_FusedMLP", mlp: nn.Sequential, a: torch.Tensor, b: torch.T
     unit column stride and any row pitch (e.g. column slices of the pooled RoI rows); layer 0 reads [a | b] without the
     concatenation ever existing in memory.  Returns (rows, c_out) row-major.  Replaces pt_utils.SharedMLP on (B,C,N,1)
     tensors (lib/net/rcnn_net.py:58-66,171-175)."""
-    lib = C.lib()
-    dev = a.device
-    rows, c_a = a.shape
-    c_b = 0 if b is None else b.size(1)
-    assert a.stride(1) == 1 and (b is None or (b.stride(1) == 1 and b.size(0) == rows))
-    desc = fused.get(mlp, 1 if c_b else 2, c_a if c_b else 0, dev)
-    c_out = fused.c_out
-    pitch = _round_up(c_out[-1], 32)
-    out = torch.empty((rows, pitch), dtype=torch.float32, device=dev)
-    co_arr = (ctypes.c_int * 3)(*(c_out + [0] * (3 - len(c_out))))
-    with torch.cuda.device(dev):
-        wsb = lib.prb_rows2_workspace_bytes(C.c_long(rows), c_a, c_b, desc.num_layers, co_arr)
-        ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-        with prof.region(tag, "%d [%d+%d]+%s" % (rows, c_a, c_b, c_out)):
-            C.check(lib.prb_mlp_rows2(C.c_long(rows), c_a, C.ptr(a), a.stride(0), c_b, C.ptr(b) if c_b else None,
-                                      b.stride(0) if c_b else 0, ctypes.byref(desc), C.ptr(out), pitch, C.ptr(ws), C.c_size_t(wsb),
-                                      C.stream()), "mlp_rows2")
-    return out if pitch == c_out[-1] else out[:, :c_out[-1]]
+    chain = fused.get(mlp, *mlp_chain.rows_layout(a.size(1), 0 if b is None else b.size(1)), a.device)
+    out = chain.rows(a, b, tag)
+    return out if out.size(1) == chain.c_out[-1] else out[:, :chain.c_out[-1]]
 
 
 def _fold_scale():
@@ -260,29 +189,21 @@ class _PointnetSAModuleBase(nn.Module):
 
     def fused_mlp(self, xyz, features, centres, idxs, nss):
         """gather + SharedMLP + max-pool of every scale (one tensor-core kernel per scale) -> (B, sum C_out, npoint)"""
-        lib = C.lib()
-        B, N, _ = xyz.shape
+        B = xyz.size(0)
         dev = xyz.device
         npoint = centres.size(1)
         c_feat = 0 if features is None else features.size(1)
         feats_pm = _point_major(features) if features is not None else None
         if self._fused is None or len(self._fused) != len(self.mlps):
             self._fused = [_FusedMLP() for _ in self.mlps]
-        descs = [f.get(mlp, 0, c_feat, dev) for f, mlp in zip(self._fused, self.mlps)]
-        c_total = sum(f.c_out[-1] for f in self._fused)
+        chains = [f.get(mlp, mlp_chain.SA, c_feat, dev) for f, mlp in zip(self._fused, self.mlps)]
+        c_total = sum(chain.c_out[-1] for chain in chains)
         out = torch.empty((B, c_total, npoint), dtype=torch.float32, device=dev)
         out_pm = torch.empty((B, npoint, c_total), dtype=torch.float32, device=dev)   # twin for the next gather
         off = 0
-        with torch.cuda.device(dev):
-            for desc, fused, idx, ns in zip(descs, self._fused, idxs, nss):
-                co_arr = (ctypes.c_int * 3)(*(fused.c_out + [0] * (3 - len(fused.c_out))))
-                wsb = lib.prb_sa_workspace_bytes(B, npoint, ns, c_feat, desc.num_layers, co_arr)
-                ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-                with prof.region("sa_mlp", "%dx%d [%d]+%s" % (B * npoint, ns, 3 + c_feat, fused.c_out)):
-                    C.check(lib.prb_sa_group_mlp_max_ws(B, N, npoint, ns, c_feat, C.ptr(xyz), C.ptr(centres), C.ptr(feats_pm),
-                                                        C.ptr(idx), ctypes.byref(desc), C.ptr(out), C.ptr(out_pm), out.size(1), off,
-                                                        C.ptr(ws), C.c_size_t(wsb), C.stream()), "sa_group_mlp_max")
-                off += fused.c_out[-1]
+        for chain, idx, ns in zip(chains, idxs, nss):
+            chain.sa(xyz, centres, feats_pm, idx, ns, out, out_pm, off)
+            off += chain.c_out[-1]
         return _attach_pm(out, out_pm)
 
     def _forward_fused(self, xyz, features, new_xyz):
@@ -380,10 +301,8 @@ class PointnetFPModule(nn.Module):
         return idx, weight
 
     def fused_mlp(self, n, idx, weight, unknow_feats, known_feats):
-        lib = C.lib()
         dev = known_feats.device
         B, c_known, m = known_feats.shape
-        c_skip = 0 if unknow_feats is None else unknow_feats.size(1)
         known_pm = _point_major(known_feats)
         skip = unknow_feats.contiguous() if unknow_feats is not None else None
         if self._fused is None:
@@ -394,31 +313,14 @@ class PointnetFPModule(nn.Module):
         # only worth it at the finest level: at the coarse ones the extra launch costs more than the narrower gather saves
         project = (self.project_known and config.get("fp_project") and _fold_scale() and c1 < c_known and n >= m
                    and B * n >= config.get("fp_project_min_rows"))
-        desc = self._fused.get(self.mlp, 1, c_known, dev, project_known=project)
-        c_out = self._fused.c_out
+        chain = self._fused.get(self.mlp, mlp_chain.FP, c_known, dev, project_known=project)
         if project:
-            pj = self._fused.proj
-            pitch = _round_up(c1, 32)
-            rows = B * m
-            proj_rows = torch.empty((rows, pitch), dtype=torch.float32, device=dev)
-            with torch.cuda.device(dev):
-                wsb = lib.prb_rows_workspace_bytes(C.c_long(rows), c_known, 1, pj["co_arr"])
-                wsp = torch.empty(wsb, dtype=torch.uint8, device=dev)
-                with prof.region("fp_mlp", "%d proj [%d]+[%d]" % (rows, c_known, c1)):
-                    C.check(lib.prb_mlp_rows(C.c_long(rows), c_known, C.ptr(known_pm), ctypes.byref(pj["desc"]), C.ptr(proj_rows), pitch,
-                                             C.ptr(wsp), C.c_size_t(wsb), C.stream()), "mlp_rows(fp projection)")
-            known_pm = proj_rows if pitch == c1 else proj_rows[:, :c1].contiguous()
-            c_known = c1
-        out = torch.empty((B, c_out[-1], n), dtype=torch.float32, device=dev)
-        out_pm = torch.empty((B, n, c_out[-1]), dtype=torch.float32, device=dev) if self.emit_point_major else None
-        co_arr = (ctypes.c_int * 3)(*(c_out + [0] * (3 - len(c_out))))
-        with torch.cuda.device(dev):
-            wsb = lib.prb_fp_workspace_bytes(B, n, c_known, c_skip, desc.num_layers, co_arr)
-            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-            with prof.region("fp_mlp", "%d [%d+%d]+%s" % (B * n, c_known, c_skip, c_out)):
-                C.check(lib.prb_fp_interp_mlp_ws(B, n, m, c_known, c_skip, C.ptr(known_pm), C.ptr(idx), C.ptr(weight), C.ptr(skip),
-                                                 ctypes.byref(desc), C.ptr(out), C.ptr(out_pm), C.ptr(ws), C.c_size_t(wsb), C.stream()),
-                        "fp_interp_mlp")
+            proj = self._fused.proj.rows(known_pm.view(B * m, c_known), tag="fp_mlp", detail="%d proj [%d]+[%d]" % (B * m, c_known, c1))
+            known_pm = proj[:, :c1].contiguous().view(B, m, c1)
+        c_last = chain.c_out[-1]
+        out = torch.empty((B, c_last, n), dtype=torch.float32, device=dev)
+        out_pm = torch.empty((B, n, c_last), dtype=torch.float32, device=dev) if self.emit_point_major else None
+        chain.fp(known_pm, idx, weight, skip, out, out_pm)
         return _attach_pm(out, out_pm) if out_pm is not None else out
 
     def _forward_fused(self, unknown, known, unknow_feats, known_feats):

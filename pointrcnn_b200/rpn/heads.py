@@ -8,13 +8,10 @@ are ONE two-layer MLP over point-major rows: layer 0 stacks the two hidden layer
 weights, ReLU), layer 1 is block diagonal (256 -> 1 + reg_channel, linear: `prb_mlp_desc.flags & 1`).  The rows are
 the point-major twin the last FP level already wrote, the output rows are already (B,N,·): no transposes, one launch.
 """
-import ctypes
-
-import numpy as np
 import torch
 import torch.nn as nn
 
-from .. import _cabi as C
+from .. import mlp_chain
 from ..pointnet2 import pointnet2_modules as pm
 
 
@@ -29,21 +26,13 @@ def _layers(seq):
     return out
 
 
-def _fold(conv, bn):
-    W = conv.weight.detach().reshape(conv.out_channels, -1).float().cpu()
-    b = conv.bias.detach().float().cpu() if conv.bias is not None else torch.zeros(conv.out_channels)
-    if bn is None:
-        return W, b
-    inv = (bn.weight.detach().float() / torch.sqrt(bn.running_var.detach().float() + bn.eps)).cpu()
-    return W * inv[:, None], (bn.bias.detach().float().cpu() - bn.running_mean.detach().float().cpu() * inv) + inv * b
-
-
 class FusedRPNHeads:
-    """cache of the packed two-layer image of (rpn_cls_layer, rpn_reg_layer); rebuilt when a parameter changes"""
+    """cache of the packed two-layer chain of (rpn_cls_layer, rpn_reg_layer); rebuilt when a parameter changes"""
 
     def __init__(self):
         self.key = None
-        self.state = None
+        self.chain = None
+        self.n_cls = None
 
     @staticmethod
     def supported(cls_seq, reg_seq):
@@ -56,55 +45,34 @@ class FusedRPNHeads:
         ok = ok and all(bn is None or not bn.training for _, bn, _ in a + b)
         return ok and all(tuple(c.kernel_size) in ((1,), (1, 1)) for c, _, _ in a + b)
 
-    def _build(self, cls_seq, reg_seq, device):
+    @staticmethod
+    def _build(cls_seq, reg_seq, device):
+        """-> (chain, number of classification channels)"""
         (c0, cb0, _), (c1, _, _) = _layers(cls_seq)
         (r0, rb0, _), (r1, _, _) = _layers(reg_seq)
-        Wc0, sc0 = _fold(c0, cb0)
-        Wr0, sr0 = _fold(r0, rb0)
-        Wc1, sc1 = _fold(c1, None)
-        Wr1, sr1 = _fold(r1, None)
+        Wc0, _, sc0 = mlp_chain.fold(c0, cb0, zero_bias=True)
+        Wr0, _, sr0 = mlp_chain.fold(r0, rb0, zero_bias=True)
+        Wc1, _, sc1 = mlp_chain.fold(c1, None)
+        Wr1, _, sr1 = mlp_chain.fold(r1, None)
         hc, hr = Wc0.shape[0], Wr0.shape[0]
-        W0 = torch.cat([Wc0, Wr0], 0).contiguous()
+        W0 = torch.cat([Wc0, Wr0], 0)
         W1 = torch.zeros(Wc1.shape[0] + Wr1.shape[0], hc + hr)
         W1[:Wc1.shape[0], :hc] = Wc1
         W1[Wc1.shape[0]:, hc:] = Wr1
-        c_in, c_out = W0.shape[1], [W0.shape[0], W1.shape[0]]
-        lib = C.lib()
-        co = (ctypes.c_int * 3)(c_out[0], c_out[1], 0)
-        nbytes = lib.prb_mlp_packed_bytes_ex(2, 0, 2, c_in, co)
-        host = np.zeros(nbytes // 4, dtype=np.float32)
-        ws = [W0.contiguous(), W1.contiguous()]
-        wp = (ctypes.c_void_p * 2)(*[w.data_ptr() for w in ws])
-        C.check(lib.prb_mlp_pack_weights_ex(2, 0, 2, c_in, co, wp, host.ctypes.data_as(ctypes.c_void_p)), "mlp_pack")
-        pad = lambda v: torch.nn.functional.pad(v, (0, (-v.numel()) % 32))
-        packed = torch.from_numpy(host).to(device)
-        shift = torch.cat([pad(torch.cat([sc0, sr0])), pad(torch.cat([sc1, sr1]))]).contiguous().to(device)
-        desc = C.MlpDesc()
-        desc.num_layers, desc.c_in = 2, c_in
-        desc.c_out[0], desc.c_out[1], desc.c_out[2] = c_out[0], c_out[1], 0
-        desc.packed_w, desc.scale, desc.shift, desc.flags = packed.data_ptr(), None, shift.data_ptr(), 1
-        return dict(desc=desc, keep=(packed, shift), co=co, c_in=c_in, n_cls=Wc1.shape[0], n_out=c_out[1])
+        chain = mlp_chain.Chain(mlp_chain.ROWS, 0, [W0, W1], [torch.cat([sc0, sr0]), torch.cat([sc1, sr1])], linear_last=True,
+                                device=device)
+        return chain, Wc1.shape[0]
 
     def __call__(self, cls_seq, reg_seq, features):
         """features (B,C,N) -> rpn_cls (B,N,n_cls), rpn_reg (B,N,reg_channel), as lib/net/rpn.py:76-77"""
         tensors = [p for seq in (cls_seq, reg_seq) for p in list(seq.parameters()) + list(seq.buffers())]
         key = (str(features.device),) + tuple((id(t), t._version) for t in tensors)
         if key != self.key:
-            self.state, self.key = self._build(cls_seq, reg_seq, features.device), key
-        st = self.state
+            (self.chain, self.n_cls), self.key = self._build(cls_seq, reg_seq, features.device), key
         B, Cc, N = features.shape
-        assert Cc == st["c_in"]
         rows = pm._point_major(features)            # (B,N,C): the twin written by the last FP launch, or one transpose
-        lib = C.lib()
-        pitch = (st["n_out"] + 31) // 32 * 32
-        out = torch.empty((B * N, pitch), dtype=torch.float32, device=features.device)
-        wsb = lib.prb_rows_workspace_bytes(C.c_long(B * N), Cc, 2, st["co"])
-        ws = torch.empty(wsb, dtype=torch.uint8, device=features.device)
-        with torch.cuda.device(features.device):
-            C.check(lib.prb_mlp_rows(C.c_long(B * N), Cc, C.ptr(rows), ctypes.byref(st["desc"]), C.ptr(out), pitch, C.ptr(ws),
-                                     C.c_size_t(wsb), C.stream()), "mlp_rows(heads)")
-        out = out.view(B, N, pitch)
-        return out[:, :, :st["n_cls"]].contiguous(), out[:, :, st["n_cls"]:st["n_out"]].contiguous()
+        out = self.chain.rows(rows.view(B * N, Cc)).view(B, N, -1)
+        return out[:, :, :self.n_cls].contiguous(), out[:, :, self.n_cls:self.chain.c_out[-1]].contiguous()
 
 
 def rpn_heads(rpn_module, backbone_features):

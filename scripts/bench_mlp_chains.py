@@ -96,7 +96,7 @@ def main():
     def c_out_of(d):
         return [d.c_out[i] for i in range(d.num_layers)]
 
-    sa, fp, rows_fn = lib.prb_sa_group_mlp_max_ws, lib.prb_fp_interp_mlp_ws, lib.prb_mlp_rows
+    sa, fp, rows_fn = lib.prb_sa_group_mlp_max_ws, lib.prb_fp_interp_mlp_ws, lib.prb_mlp_rows2
 
     class Wrap:
         """stands in for the CDLL while the forward runs: the three chain entry points are timed, the rest pass through"""
@@ -118,11 +118,11 @@ def main():
             timed("fp", fp, a, "fp %d [%d+%d]+%s" % (B * n, c_known, c_skip, co), B * n, [c_known] + ([c_skip] if c_skip else []), co)
             return fp(*a)
 
-        def prb_mlp_rows(self, *a):
-            rws, c_in = a[0].value, int(a[1])
-            d = a[3]._obj
+        def prb_mlp_rows2(self, *a):
+            rws, c_a, c_b = a[0].value, int(a[1]), int(a[4])
+            d = a[7]._obj
             co = c_out_of(d)
-            timed("rows", rows_fn, a, "rows %d [%d]+%s" % (rws, c_in, co), rws, [c_in], co)
+            timed("rows", rows_fn, a, "rows %d [%d+%d]+%s" % (rws, c_a, c_b, co), rws, [c_a] + ([c_b] if c_b else []), co)
             return rows_fn(*a)
 
     torch.manual_seed(0)

@@ -21,9 +21,9 @@ carries a bound on |kernel - reference| per output element:
 The check is |got - ref| <= bound for every element.  emulate() is an fp32 model of the kernel's rounding points (used to
 show, without a GPU, that the bound holds for plausible accumulation orders and that it catches subtle mistakes).
 """
-import ctypes
-
 import numpy as np
+
+from pointrcnn_b200 import mlp_chain
 
 KC = 32                       # K columns per chunk of the packed image (one 128-byte swizzle row)
 U32 = 2.0 ** -24              # unit roundoff of one fp32 round-to-nearest
@@ -77,19 +77,6 @@ def k_order(kind, split, c_in):
     return np.array(cols, dtype=np.int64), [w for _, w in segs]
 
 
-def pack(lib, kind, split, c_in, weights):
-    """prb_mlp_pack_weights_ex on the host: the float32 image the kernel streams"""
-    L = len(weights)
-    c_out = [w.shape[0] for w in weights]
-    co = (ctypes.c_int * 3)(*(c_out + [0] * (3 - L)))
-    img = np.zeros(lib.prb_mlp_packed_bytes_ex(kind, split, L, c_in, co) // 4, dtype=np.float32)
-    ws = [np.ascontiguousarray(w, dtype=np.float32) for w in weights]
-    wp = (ctypes.c_void_p * L)(*[w.ctypes.data for w in ws])
-    rc = lib.prb_mlp_pack_weights_ex(kind, split, L, c_in, co, wp, img.ctypes.data_as(ctypes.c_void_p))
-    assert rc == 0, "prb_mlp_pack_weights_ex failed"
-    return img
-
-
 class Layer:
     """one layer read back from a packed image: W (c_out, k_in) in the caller's column order; Wk (np, k_pad) the tile rows in
     K order, kmap the caller column of every K index (-1: padding)"""
@@ -138,12 +125,9 @@ class Chain:
         self.scale = None if folded else [(rng.uniform(0.5, 1.5, co) * rng.choice([-1.0, 1.0], co)).astype(np.float32) for co in c_out]
         self.shift = [rng.normal(0, 0.2, co).astype(np.float32) for co in c_out]
 
-    def packed(self, lib):
-        img = pack(lib, self.kind, self.split, self.c_in, self.weights)
+    def packed(self):
+        img = mlp_chain.pack_image(self.kind, self.split, self.weights)
         return img, unpack(img, self.kind, self.split, self.c_in, self.c_out)
-
-    def padded(self, vs):
-        return np.concatenate([np.pad(v, (0, (-len(v)) % 32)) for v in vs]).astype(np.float32)
 
 
 def sa_inputs(rng, b, n, npoint, ns, c_feat):
@@ -463,7 +447,7 @@ PERSIST_OPTIONS = [dict(mlp_sms=1), dict(mlp_sms=1, mlp_occ=1)]
 
 
 def pack_args(case):
-    """(kind, split, c_in) of prb_mlp_pack_weights_ex for a case"""
+    """(kind, split, c_in) the chain of a case is packed with"""
     if case["kind"] == "sa":
         return 0, case["c_feat"], 3 + case["c_feat"]
     if case["kind"] == "fp":
@@ -485,12 +469,12 @@ def reduced(case):
     return c
 
 
-def make(case, lib, seed=0):
+def make(case, seed=0):
     """(chain, packed image, unpacked layers, host inputs) of a case"""
     rng = np.random.default_rng([seed] + [ord(ch) for ch in case["name"]])
     kind, split, c_in = pack_args(case)
     chain = Chain(rng, kind, split, c_in, case["c_out"], case["folded"], case["linear"])
-    img, layers = chain.packed(lib)
+    img, layers = chain.packed()
     if case["kind"] == "sa":
         inp = sa_inputs(rng, case["b"], case["n"], case["npoint"], case["ns"], case["c_feat"])
     elif case["kind"] == "fp":

@@ -4,7 +4,7 @@ import numpy as np
 import pytest
 
 import mlp_reference as R
-from pointrcnn_b200 import _cabi as C
+from pointrcnn_b200 import mlp_chain
 
 # --------------------------------------------------------------------------------------------- unpacker
 PACK_CASES = sorted({(R.pack_args(c), tuple(c["c_out"])) for c in R.CASES + R.PERSIST_CASES})
@@ -20,7 +20,7 @@ def test_unpack_inverts_the_packer(args, c_out):
     rng = np.random.default_rng(c_in * 7 + len(c_out))
     dims = [c_in] + list(c_out)
     ws = [rng.standard_normal((co, ci)).astype(np.float32) for ci, co in zip(dims[:-1], dims[1:])]
-    img = R.pack(C.lib(), kind, split, c_in, ws)
+    img = mlp_chain.pack_image(kind, split, ws)
     layers = R.unpack(img, kind, split, c_in, list(c_out))
     for W, ly in zip(ws, layers):
         assert ly.W.shape == W.shape
@@ -31,7 +31,7 @@ def test_unpack_rejects_a_wrong_layout():
     """the unpacker does not just mirror the packer: an image with a unit swizzled the wrong way is refused or differs"""
     rng = np.random.default_rng(1)
     W = rng.standard_normal((40, 37)).astype(np.float32)
-    img = R.pack(C.lib(), 2, 0, 37, [W])
+    img = mlp_chain.pack_image(2, 0, [W])
     bad = img.copy()
     bad[4:8], bad[8:12] = img[8:12], img[4:8]          # row 0, units 1 and 2 of the first chunk swapped
     assert np.array_equal(R.unpack(img, 2, 0, 37, [40])[0].W, R.tf32_rna(W))
@@ -49,7 +49,7 @@ def test_bound_holds_for_fp32_accumulation_orders(case):
     """an fp32 model of the kernel (its rounding points, fp32 accumulation per K chunk) sits inside the bound for every
     case shape, whichever order the products of a chunk are added in"""
     c = R.reduced(case)
-    chain, img, layers, inp = R.make(c, C.lib())
+    chain, img, layers, inp = R.make(c)
     ref, bound = R.expected(c["kind"], chain, layers, inp)
     worst = 0.0
     for order in R.ORDERS:
@@ -82,7 +82,7 @@ def test_every_mutant_has_a_case():
 @pytest.mark.parametrize("mutant", R.MUTANTS)
 def test_bound_catches_a_subtly_wrong_kernel(mutant):
     c = R.reduced(R.BY_NAME[MUTANT_CASES[mutant]])
-    chain, img, layers, inp = R.make(c, C.lib())
+    chain, img, layers, inp = R.make(c)
     ref, bound = R.expected(c["kind"], chain, layers, inp)
     assert R.check(R.emulate(c["kind"], chain, layers, inp), ref, bound)[0], "the unmutated model must pass"
     ok, ratio, bad = R.check(R.emulate(c["kind"], chain, layers, inp, mutant=mutant), ref, bound)

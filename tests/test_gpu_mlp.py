@@ -24,6 +24,7 @@ pytestmark = pytest.mark.gpu
 
 from pointrcnn_b200 import _cabi as C  # noqa: E402
 from pointrcnn_b200.backbone import Pointnet2MSG  # noqa: E402
+from pointrcnn_b200.mlp_chain import Chain  # noqa: E402
 from pointrcnn_b200.pointnet2 import pointnet2_modules as pm  # noqa: E402
 from pointrcnn_b200.pointnet2 import pointnet2_utils as pu  # noqa: E402
 
@@ -73,28 +74,10 @@ def _fold(layers):
     return [((W * sc[:, None]).astype(np.float32), np.ones_like(sc), sh) for W, sc, sh in layers]
 
 
-def _desc(layers, kind, split, dev, folded=False):
+def _chain(layers, kind, split, dev, folded=False):
     """folded: `layers` come from _fold(); the descriptor then carries scale = NULL"""
-    L = len(layers)
-    c_in = layers[0][0].shape[1]
-    c_out = [l[0].shape[0] for l in layers]
-    lib = C.lib()
-    co = (ctypes.c_int * 3)(*(c_out + [0] * (3 - L)))
-    nbytes = lib.prb_mlp_packed_bytes_ex(kind, split, L, c_in, co)
-    host = np.zeros(nbytes // 4, dtype=np.float32)
-    ws = [np.ascontiguousarray(l[0]) for l in layers]
-    wp = (ctypes.c_void_p * L)(*[w.ctypes.data for w in ws])
-    C.check(lib.prb_mlp_pack_weights_ex(kind, split, L, c_in, co, wp, host.ctypes.data_as(ctypes.c_void_p)), "pack")
-    pad = lambda v: np.pad(v, (0, (-len(v)) % 32))
-    keep = [torch.from_numpy(host).to(dev),
-            torch.from_numpy(np.concatenate([pad(l[1]) for l in layers])).to(dev),
-            torch.from_numpy(np.concatenate([pad(l[2]) for l in layers])).to(dev)]
-    d = C.MlpDesc()
-    d.num_layers, d.c_in = L, c_in
-    for i in range(3):
-        d.c_out[i] = c_out[i] if i < L else 0
-    d.packed_w, d.scale, d.shift = keep[0].data_ptr(), (None if folded else keep[1].data_ptr()), keep[2].data_ptr()
-    return d, keep, co
+    return Chain(kind, split, [l[0] for l in layers], [l[2] for l in layers], None if folded else [l[1] for l in layers],
+                 device=dev)
 
 
 ROW_CASES = [
@@ -130,14 +113,14 @@ def test_mlp_rows2_strided_segments(cuda, rows, c_a, c_b, off_a, off_b, width, d
         a_t, a_np = wt[:, off_a:off_a + c_a], wide[:, off_a:off_a + c_a]
     b_t = wt[:, off_b:off_b + c_b] if c_b else None
     x = np.concatenate([a_np] + ([wide[:, off_b:off_b + c_b]] if c_b else []), axis=1)
-    d, keep, co = _desc(layers, 1 if c_b else 2, c_a if c_b else 0, cuda, False)
+    ch = _chain(layers, 1 if c_b else 2, c_a if c_b else 0, cuda, False)
     lib = C.lib()
     np_last = (dims[-1] + 31) // 32 * 32
     out = torch.full((rows, np_last), float("nan"), device=cuda)
-    wsb = lib.prb_rows2_workspace_bytes(C.c_long(rows), c_a, c_b, len(layers), co)
+    wsb = lib.prb_rows2_workspace_bytes(C.c_long(rows), c_a, c_b, len(layers), ch.co)
     ws = torch.empty(wsb, dtype=torch.uint8, device=cuda)
     C.check(lib.prb_mlp_rows2(C.c_long(rows), c_a, C.ptr(a_t), a_t.stride(0), c_b, C.ptr(b_t) if c_b else None,
-                              b_t.stride(0) if c_b else 0, ctypes.byref(d), C.ptr(out), np_last, C.ptr(ws), C.c_size_t(wsb),
+                              b_t.stride(0) if c_b else 0, ctypes.byref(ch.desc), C.ptr(out), np_last, C.ptr(ws), C.c_size_t(wsb),
                               C.stream()), "mlp_rows2")
     torch.cuda.synchronize()
     got = out.cpu().numpy()[:, :dims[-1]]
@@ -156,14 +139,14 @@ def test_mlp_rows_tcgen05(cuda, rows, dims, folded):
     if folded:
         layers = _fold(layers)
     x = rng.standard_normal((rows, dims[0])).astype(np.float32)
-    d, keep, co = _desc(layers, 2, 0, cuda, folded)
+    ch = _chain(layers, 2, 0, cuda, folded)
     lib = C.lib()
     np_last = (dims[-1] + 31) // 32 * 32
     out = torch.full((rows, np_last), float("nan"), device=cuda)
-    wsb = lib.prb_rows_workspace_bytes(C.c_long(rows), dims[0], len(layers), co)
+    wsb = lib.prb_rows_workspace_bytes(C.c_long(rows), dims[0], len(layers), ch.co)
     ws = torch.empty(wsb, dtype=torch.uint8, device=cuda)
     xt = torch.from_numpy(x).to(cuda)
-    C.check(lib.prb_mlp_rows(C.c_long(rows), dims[0], C.ptr(xt), ctypes.byref(d), C.ptr(out), np_last, C.ptr(ws),
+    C.check(lib.prb_mlp_rows(C.c_long(rows), dims[0], C.ptr(xt), ctypes.byref(ch.desc), C.ptr(out), np_last, C.ptr(ws),
                              C.c_size_t(wsb), C.stream()), "mlp_rows")
     torch.cuda.synchronize()
     got = out.cpu().numpy()[:, :dims[-1]]

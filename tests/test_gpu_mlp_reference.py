@@ -18,6 +18,7 @@ import mlp_reference as R
 pytestmark = pytest.mark.gpu
 
 from pointrcnn_b200 import _cabi as C  # noqa: E402
+from pointrcnn_b200.mlp_chain import Chain  # noqa: E402
 
 SENTINEL = 7777.0
 GUARD = 64          # floats behind every output buffer
@@ -37,21 +38,11 @@ def _out(shape, dev):
 class Launch:
     """device operands, descriptor and sentinel-filled outputs of one case; run() launches the chain once"""
 
-    def __init__(self, case, chain, img, inp, dev):
+    def __init__(self, case, chain, inp, dev):
         lib = C.lib()
         self.case, self.lib = case, lib
-        self.keep = [_dev(img, dev), _dev(chain.padded(chain.shift), dev)]
-        d = C.MlpDesc()
-        d.num_layers, d.c_in = len(chain.c_out), chain.c_in
-        for i in range(3):
-            d.c_out[i] = chain.c_out[i] if i < len(chain.c_out) else 0
-        d.packed_w, d.shift = self.keep[0].data_ptr(), self.keep[1].data_ptr()
-        if chain.scale is not None:
-            self.keep.append(_dev(chain.padded(chain.scale), dev))
-            d.scale = self.keep[2].data_ptr()
-        d.flags = 1 if chain.linear else 0
-        self.desc = d
-        self.co = (ctypes.c_int * 3)(*[d.c_out[i] for i in range(3)])
+        self.chain = Chain(chain.kind, chain.split, chain.weights, chain.shift, chain.scale, chain.linear, dev)
+        self.desc, self.co = self.chain.desc, self.chain.co
         self.L, self.C = len(chain.c_out), chain.c_out[-1]
         self.inp = {k: (_dev(v, dev) if isinstance(v, np.ndarray) else v) for k, v in inp.items()}
         k = case["kind"]
@@ -127,9 +118,9 @@ class Launch:
 
 def _verify_case(case, dev, option_sets=({},)):
     lib = C.lib()
-    chain, img, layers, inp = R.make(case, lib)
+    chain, _, layers, inp = R.make(case)
     ref, bound = R.expected(case["kind"], chain, layers, inp)
-    launch = Launch(case, chain, img, inp, dev)
+    launch = Launch(case, chain, inp, dev)
     first, ratios = None, []
     for opts in option_sets:
         for resident in (1, 0):

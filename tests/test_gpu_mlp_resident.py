@@ -15,31 +15,18 @@ import torch
 pytestmark = pytest.mark.gpu
 
 from pointrcnn_b200 import _cabi as C  # noqa: E402
+from pointrcnn_b200.mlp_chain import Chain  # noqa: E402
 
 SENTINEL = -7.0   # outputs a kernel does not write keep this value in both runs
 
 
-def _desc(rng, dev, kind, split, c_in, c_out, folded, linear_last=False):
+def _chain(rng, dev, kind, split, c_in, c_out, folded, linear_last=False):
     """random weights packed for the chain; folded: no separate scale (scale = NULL in the descriptor)"""
-    lib = C.lib()
-    L = len(c_out)
     dims = [c_in] + list(c_out)
     ws = [(rng.standard_normal((co, ci)) * np.sqrt(2.0 / ci)).astype(np.float32) for ci, co in zip(dims[:-1], dims[1:])]
-    pad = lambda v: np.pad(v, (0, (-len(v)) % 32))
-    scale = np.concatenate([pad(rng.uniform(0.5, 1.5, co).astype(np.float32)) for co in c_out])
-    shift = np.concatenate([pad(rng.normal(0, 0.2, co).astype(np.float32)) for co in c_out])
-    co = (ctypes.c_int * 3)(*(list(c_out) + [0] * (3 - L)))
-    host = np.zeros(lib.prb_mlp_packed_bytes_ex(kind, split, L, c_in, co) // 4, dtype=np.float32)
-    wp = (ctypes.c_void_p * L)(*[w.ctypes.data for w in ws])
-    C.check(lib.prb_mlp_pack_weights_ex(kind, split, L, c_in, co, wp, host.ctypes.data_as(ctypes.c_void_p)), "pack")
-    keep = [torch.from_numpy(host).to(dev), torch.from_numpy(scale).to(dev), torch.from_numpy(shift).to(dev)]
-    d = C.MlpDesc()
-    d.num_layers, d.c_in = L, c_in
-    for i in range(3):
-        d.c_out[i] = c_out[i] if i < L else 0
-    d.packed_w, d.scale, d.shift = keep[0].data_ptr(), (None if folded else keep[1].data_ptr()), keep[2].data_ptr()
-    d.flags = 1 if linear_last else 0
-    return d, keep, co
+    scale = [rng.uniform(0.5, 1.5, co).astype(np.float32) for co in c_out]
+    shift = [rng.normal(0, 0.2, co).astype(np.float32) for co in c_out]
+    return Chain(kind, split, ws, shift, None if folded else scale, linear_last=linear_last, device=dev)
 
 
 def _both(run):
@@ -74,7 +61,7 @@ SA_CASES = [
 def test_sa_resident_bits(cuda, b, n, npoint, ns, c_feat, c_out, folded):
     rng = np.random.default_rng(b * 1000 + ns + c_feat)
     lib = C.lib()
-    d, keep, co = _desc(rng, cuda, 0, c_feat, 3 + c_feat, c_out, folded)
+    ch = _chain(rng, cuda, 0, c_feat, 3 + c_feat, c_out, folded)
     xyz = torch.from_numpy(rng.uniform(-1, 1, (b, n, 3)).astype(np.float32)).to(cuda)
     new_xyz = torch.from_numpy(rng.uniform(-1, 1, (b, npoint, 3)).astype(np.float32)).to(cuda)
     feats = torch.from_numpy(rng.standard_normal((b, n, c_feat)).astype(np.float32)).to(cuda) if c_feat else None
@@ -82,13 +69,13 @@ def test_sa_resident_bits(cuda, b, n, npoint, ns, c_feat, c_out, folded):
     C_out = c_out[-1]
     out = torch.empty((b, C_out, npoint), device=cuda)
     out_pm = torch.empty((b, npoint, C_out), device=cuda)
-    wsb = lib.prb_sa_workspace_bytes(b, npoint, ns, c_feat, len(c_out), co)
+    wsb = lib.prb_sa_workspace_bytes(b, npoint, ns, c_feat, len(c_out), ch.co)
     ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=cuda)
 
     def run():
         out.fill_(SENTINEL); out_pm.fill_(SENTINEL)
         C.check(lib.prb_sa_group_mlp_max_ws(b, n, npoint, ns, c_feat, C.ptr(xyz), C.ptr(new_xyz), C.ptr(feats), C.ptr(idx),
-                                            ctypes.byref(d), C.ptr(out), C.ptr(out_pm), C_out, 0, C.ptr(ws), C.c_size_t(wsb),
+                                            ctypes.byref(ch.desc), C.ptr(out), C.ptr(out_pm), C_out, 0, C.ptr(ws), C.c_size_t(wsb),
                                             C.stream()), "sa_group_mlp_max")
         return [out, out_pm]
 
@@ -110,7 +97,7 @@ FP_CASES = [
 def test_fp_resident_bits(cuda, b, n, m, c_known, c_skip, c_out, folded):
     rng = np.random.default_rng(n + c_known + c_skip)
     lib = C.lib()
-    d, keep, co = _desc(rng, cuda, 1, c_known, c_known + c_skip, c_out, folded)
+    ch = _chain(rng, cuda, 1, c_known, c_known + c_skip, c_out, folded)
     known_pm = torch.from_numpy(rng.standard_normal((b, m, c_known)).astype(np.float32)).to(cuda)
     idx = torch.from_numpy(rng.integers(0, m, (b, n, 3)).astype(np.int32)).to(cuda)
     w = rng.uniform(0.1, 1.0, (b, n, 3)).astype(np.float32)
@@ -119,13 +106,13 @@ def test_fp_resident_bits(cuda, b, n, m, c_known, c_skip, c_out, folded):
     C_out = c_out[-1]
     out = torch.empty((b, C_out, n), device=cuda)
     out_pm = torch.empty((b, n, C_out), device=cuda)
-    wsb = lib.prb_fp_workspace_bytes(b, n, c_known, c_skip, len(c_out), co)
+    wsb = lib.prb_fp_workspace_bytes(b, n, c_known, c_skip, len(c_out), ch.co)
     ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=cuda)
 
     def run():
         out.fill_(SENTINEL); out_pm.fill_(SENTINEL)
         C.check(lib.prb_fp_interp_mlp_ws(b, n, m, c_known, c_skip, C.ptr(known_pm), C.ptr(idx), C.ptr(weight), C.ptr(skip),
-                                         ctypes.byref(d), C.ptr(out), C.ptr(out_pm), C.ptr(ws), C.c_size_t(wsb), C.stream()),
+                                         ctypes.byref(ch.desc), C.ptr(out), C.ptr(out_pm), C.ptr(ws), C.c_size_t(wsb), C.stream()),
                 "fp_interp_mlp")
         return [out, out_pm]
 
@@ -148,16 +135,16 @@ ROW_CASES = [
 def test_rows_resident_bits(cuda, rows, c_in, c_out, linear, folded):
     rng = np.random.default_rng(rows + c_in)
     lib = C.lib()
-    d, keep, co = _desc(rng, cuda, 2, 0, c_in, c_out, folded, linear_last=linear)
+    ch = _chain(rng, cuda, 2, 0, c_in, c_out, folded, linear_last=linear)
     x = torch.from_numpy(rng.standard_normal((rows, c_in)).astype(np.float32)).to(cuda)
     pitch = (c_out[-1] + 31) // 32 * 32
     out = torch.empty((rows, pitch), device=cuda)
-    wsb = lib.prb_rows_workspace_bytes(C.c_long(rows), c_in, len(c_out), co)
+    wsb = lib.prb_rows_workspace_bytes(C.c_long(rows), c_in, len(c_out), ch.co)
     ws = torch.empty(max(wsb, 1), dtype=torch.uint8, device=cuda)
 
     def run():
         out.fill_(SENTINEL)
-        C.check(lib.prb_mlp_rows(C.c_long(rows), c_in, C.ptr(x), ctypes.byref(d), C.ptr(out), pitch, C.ptr(ws),
+        C.check(lib.prb_mlp_rows(C.c_long(rows), c_in, C.ptr(x), ctypes.byref(ch.desc), C.ptr(out), pitch, C.ptr(ws),
                                  C.c_size_t(wsb), C.stream()), "mlp_rows")
         return [out]
 
