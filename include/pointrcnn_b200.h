@@ -441,6 +441,31 @@ PRB_API int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *
                                  float aug_rot_range, float flip_prob, float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh,
                                  unsigned seed, float *gt_boxes_ct, int *cls_label, int *reg_valid_mask, void *stream);
 
+/* ------------------------------------------------------------------ evaluation statistics ------
+ * The recall, segmentation IoU and classification accuracy of tools/eval_rcnn.py's three evaluation loops
+ * (eval_one_epoch_rpn :179-201, eval_one_epoch_rcnn :337-367, eval_one_epoch_joint :541-573) for a batch of scenes.  Each
+ * entry point launches one kernel on `stream` (one CTA per scene), allocates nothing and never synchronises.
+ *
+ * box_recall: boxes (b,m,7), gt (b,g,7) [x,y,z,h,w,l,ry]; the first box_count[s] / gt_count[s] (device int32) rows are real,
+ * box_count NULL = all m rows.  The pair IoU is prb_boxes_iou3d's, bit for bit.  For every real GT, its max IoU over the
+ * scene's real boxes adds 1 to recalled[t] (int64) when it is > thresh[t] (a host array of n_thresh <= 16 values, passed
+ * by value); gt_total (int64) += gt_count[s].  box_max_iou (b,m), optional: each real row's max IoU over the scene's GT, 0
+ * for a scene without GT and for rows past box_count.  recalled / gt_total may be NULL.  m <= 512; integer atomics only.
+ *
+ * seg_iou: pred, label (b,n) int32 -> iou[s] = correct / max(#(label > 0) + #(pred > 0) - correct, 1), correct =
+ * #(pred == label & label > 0), counted in integers and divided once in fp32.  n <= 16384.
+ *
+ * cls_acc: over the first box_count[s] (NULL: m) RoIs of each scene, pred_cls (b,m) int32, gt_iou (b,m):
+ * acc[s] = #((pred == (gt_iou > cls_fg)) & valid) / max(#valid, 1), valid = gt_iou >= cls_fg | gt_iou <= cls_bg;
+ * acc_refined[s] = #(pred == (gt_iou >= refined_thresh)) * (1 / max(count, 1)) -- the reference divides that one by a
+ * Python number, which torch on the GPU computes as a product with the fp32 reciprocal. */
+PRB_API int prb_eval_box_recall(int b, int m, const float *boxes, const int *box_count, int g, const float *gt, const int *gt_count,
+                                int n_thresh, const float *thresh, long long *recalled, long long *gt_total, float *box_max_iou,
+                                void *stream);
+PRB_API int prb_eval_seg_iou(int b, int n, const int *pred, const int *label, float *iou, void *stream);
+PRB_API int prb_eval_cls_acc(int b, int m, const int *box_count, const int *pred_cls, const float *gt_iou, float cls_fg,
+                             float cls_bg, float refined_thresh, float *acc, float *acc_refined, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

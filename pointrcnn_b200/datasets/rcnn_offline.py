@@ -64,14 +64,17 @@ def read_rpn_features(feature_dir, sample_id, use_seg_score=False):
     return np.load(f("_xyz")), np.load(f("")), np.load(f("_intensity")).reshape(-1), seg
 
 
-def read_rois(roi_dir, sample_id):
-    """the proposals of one scene from a KITTI result file -> (M,7) float32 [x, y, z, h, w, l, ry] (objs_to_boxes3d)"""
+def read_rois(roi_dir, sample_id, with_scores=False):
+    """the proposals of one scene from a KITTI result file -> (M,7) float32 [x, y, z, h, w, l, ry] (objs_to_boxes3d);
+    with_scores: also the (M,) float32 score column, as get_proposal_from_file reads it (kitti_rcnn_dataset.py:800-803)"""
     a = read_label_anno(os.path.join(roi_dir, "%06d.txt" % sample_id))
     out = np.zeros((len(a["name"]), 7), np.float32)
     if len(out):
         out[:, 0:3] = a["location"]
         out[:, 3:6] = a["dimensions"][:, [1, 2, 0]]      # the parser stores l, h, w
         out[:, 6] = a["rotation_y"]
+    if with_scores:
+        return out, np.asarray(a["score"], np.float32).reshape(-1)
     return out
 
 
@@ -169,17 +172,11 @@ class RCNNOfflineSampler:
         counts = np.array([[b.shape[0] for b in rb], [b.shape[0] for b in gb]], np.int32)
         return xyz, feat, _pad(rb, M, 0.0), _pad(gb, G, 0.0), torch.from_numpy(counts).to(dev, non_blocking=True)
 
-    def prepare_batch(self, scenes, seed=0, mode="TRAIN"):
-        """scenes: list of dicts rpn_xyz (N,3), rpn_features (N,C), rpn_intensity (N,), seg_mask (N,), roi_boxes3d (M,7),
-        gt_boxes3d (G,7), numpy or CUDA.  -> dict of CUDA tensors over the flat RoI axis K = B * ROI_PER_IMAGE:
-        rows (K, NUM_POINTS, 3 + extra + C) the pooled buffer; pts_input / pts_features its [xyz | extra] / feature views;
-        cls_label (K) int32, reg_valid_mask (K) int32, gt_boxes3d_ct (K,7), roi_boxes3d (K,7), roi_size (K,3), gt_boxes3d
-        (K,7), gt_iou (K), sample_status (B) int32, sample_index (K,3) int32 [source RoI, GT, jitter tries]."""
-        cfg, r = self.cfg, self.cfg.RCNN
+    def _dims(self, scenes, what):
+        """-> B, N, M, G, C of a batch (M, G at least 1) and the packer for where its arrays live"""
         B = len(scenes)
         if B == 0:
-            raise ValueError("prepare_batch: empty batch")
-        dev = self.device
+            raise ValueError("%s: empty batch" % what)
         on_device = all(torch.is_tensor(s["rpn_xyz"]) and s["rpn_xyz"].is_cuda for s in scenes)
         shape = lambda v: tuple(v.shape)
         N = max(shape(s["rpn_xyz"])[0] for s in scenes)
@@ -187,12 +184,55 @@ class RCNNOfflineSampler:
         rows = lambda v: shape(v)[0] if len(shape(v)) == 2 else int(np.prod(shape(v))) // 7
         M = max(max(rows(s["roi_boxes3d"]) for s in scenes), 1)
         G = max(max(rows(s["gt_boxes3d"]) for s in scenes), 1)
-        E, R, S = self.num_extra, int(r.ROI_PER_IMAGE), int(r.NUM_POINTS)
         for s in scenes:
             if shape(s["rpn_features"])[1] != Cf or shape(s["rpn_features"])[0] != shape(s["rpn_xyz"])[0]:
-                raise ValueError("prepare_batch: rpn_features must be (N, C) with one C for the batch")
+                raise ValueError("%s: rpn_features must be (N, C) with one C for the batch" % what)
+        return B, N, M, G, Cf, (self._pack_device if on_device else self._pack_host)
+
+    def prepare_eval_batch(self, scenes):
+        """get_proposal_from_file (kitti_rcnn_dataset.py:790-874) for a batch, no sampling and no augmentation: every
+        proposal is pooled on its enlarged box with the canonical transform (RCNNStage.pool, rcnn_net.py:127-152, the
+        reference's default ROI_SAMPLE_JIT eval), and gt_iou is each proposal's max 3D IoU over the scene's GT (0 without GT).
+        scenes: dicts rpn_xyz (N,3), rpn_features (N,C), rpn_intensity (N,), seg_mask (N,), roi_boxes3d (M,7), roi_scores
+        (M,) (optional), gt_boxes3d (G,7), numpy or CUDA.  -> dict of CUDA tensors: rows (B*M, NUM_POINTS, 3 + extra + C),
+        roi_boxes3d (B,M,7), roi_scores (B,M), roi_count (B) int32, gt_boxes3d (B,G,7), gt_count (B) int32, gt_iou (B,M),
+        pooled_empty_flag (B,M) int32.  Padding RoIs (rows past roi_count) are zero boxes with gt_iou 0."""
+        from ..roipool3d import roipool3d_utils
+        r = self.cfg.RCNN
+        B, N, M, G, Cf, pack = self._dims(scenes, "prepare_eval_batch")
+        dev = self.device
         with torch.cuda.device(dev):
-            pack = self._pack_device if on_device else self._pack_host
+            xyz, feat, rois, gt, counts = pack(scenes, B, N, M, G, self.num_extra, Cf)
+            if pack == self._pack_device:
+                score = lambda s: s["roi_scores"] if s.get("roi_scores") is not None else torch.zeros(s["roi_boxes3d"].shape[0], device=dev)
+                scores = _pad([torch.as_tensor(score(s), device=dev).float().reshape(-1, 1) for s in scenes], M, 0.0)
+                scores = scores.view(B, M)
+            else:
+                host = np.zeros((B, M), np.float32)
+                for k, s in enumerate(scenes):
+                    if s.get("roi_scores") is not None:
+                        v = np.asarray(s["roi_scores"], np.float32).reshape(-1)
+                        host[k, :len(v)] = v
+                scores = torch.from_numpy(host).to(dev)
+            pooled, empty = roipool3d_utils.roipool3d_gpu(xyz, feat, rois, r.POOL_EXTRA_WIDTH, sampled_pt_num=int(r.NUM_POINTS),
+                                                          canonical_rois=rois)
+            gt_iou = torch.empty((B, M), dtype=torch.float32, device=dev)
+            C.check(C.lib().prb_eval_box_recall(B, M, C.ptr(rois), C.ptr(counts[0]), G, C.ptr(gt), C.ptr(counts[1]), 0, None, None, None,
+                                                C.ptr(gt_iou), C.stream()), "eval_box_recall")
+        return {"rows": pooled.view(B * M, pooled.shape[2], pooled.shape[3]), "roi_boxes3d": rois, "roi_scores": scores,
+                "roi_count": counts[0], "gt_boxes3d": gt, "gt_count": counts[1], "gt_iou": gt_iou, "pooled_empty_flag": empty}
+
+    def prepare_batch(self, scenes, seed=0, mode="TRAIN"):
+        """scenes: list of dicts rpn_xyz (N,3), rpn_features (N,C), rpn_intensity (N,), seg_mask (N,), roi_boxes3d (M,7),
+        gt_boxes3d (G,7), numpy or CUDA.  -> dict of CUDA tensors over the flat RoI axis K = B * ROI_PER_IMAGE:
+        rows (K, NUM_POINTS, 3 + extra + C) the pooled buffer; pts_input / pts_features its [xyz | extra] / feature views;
+        cls_label (K) int32, reg_valid_mask (K) int32, gt_boxes3d_ct (K,7), roi_boxes3d (K,7), roi_size (K,3), gt_boxes3d
+        (K,7), gt_iou (K), sample_status (B) int32, sample_index (K,3) int32 [source RoI, GT, jitter tries]."""
+        cfg, r = self.cfg, self.cfg.RCNN
+        B, N, M, G, Cf, pack = self._dims(scenes, "prepare_batch")
+        dev = self.device
+        E, R, S = self.num_extra, int(r.ROI_PER_IMAGE), int(r.NUM_POINTS)
+        with torch.cuda.device(dev):
             xyz, feat, rois, gt, counts = pack(scenes, B, N, M, G, E, Cf)
             L, st = C.lib(), C.stream()
             iou = torch.empty((B, M, G), dtype=torch.float32, device=dev)

@@ -35,18 +35,37 @@ class PointRCNNInference(nn.Module):
                    backbone_xyz=xyz, backbone_features=feats)
         return out
 
-    def detections(self, out):
-        """eval_rcnn.py:485-620: decode the RCNN regression relative to the RoIs, keep norm score > thresh, rotated NMS on
-        the raw scores.  Returns per scene (boxes (K,7), raw scores (K)) on the device, plus the decoded (B,M,7) boxes."""
+    def forward_offline(self, batch):
+        """the RCNN network on RCNNOfflineSampler.prepare_eval_batch's pooled rows (eval_one_epoch_rcnn from saved RPN
+        features and proposals) -> the `out` dict detections / detections_device take: rcnn_cls (B*M,), rcnn_reg (B*M, C),
+        rois (B,M,7), roi_scores_raw (B,M).  The rcnn_cls of padding RoIs (rows past roi_count) is -inf, so they are never
+        selected."""
+        rois = batch["roi_boxes3d"]
+        B, M = rois.shape[0], rois.shape[1]
+        rcnn_cls, rcnn_reg = self.rcnn_net.forward_pts(batch["rows"])
+        pad = torch.arange(M, device=rois.device).unsqueeze(0) >= batch["roi_count"].unsqueeze(1)
+        rcnn_cls = rcnn_cls.view(B, M, -1).masked_fill(pad.unsqueeze(2), float("-inf")).view(rcnn_cls.shape)
+        return {"rcnn_cls": rcnn_cls, "rcnn_reg": rcnn_reg, "rois": rois, "roi_scores_raw": batch["roi_scores"]}
+
+    def decode(self, out):
+        """decode_bbox_target of the RCNN regression relative to the RoIs (eval_rcnn.py:296-304) -> (B,M,7)"""
         rois = out["rois"]
         B, M = rois.shape[0], rois.shape[1]
         c = self.rcnn_net.cfg
-        rcnn_cls = out["rcnn_cls"].view(B, M, -1)
         rcnn_reg = out["rcnn_reg"].view(B, M, -1)
         pred = decode_bbox_target(rois.reshape(-1, 7), rcnn_reg.reshape(-1, rcnn_reg.shape[-1]), anchor_size=self.mean_size,
                                   loc_scope=c["LOC_SCOPE"], loc_bin_size=c["LOC_BIN_SIZE"], num_head_bin=c["NUM_HEAD_BIN"],
                                   get_xz_fine=True, get_y_by_bin=c["LOC_Y_BY_BIN"], loc_y_scope=c["LOC_Y_SCOPE"],
                                   loc_y_bin_size=c["LOC_Y_BIN_SIZE"], get_ry_fine=True).view(B, M, 7)
+        return pred
+
+    def detections(self, out):
+        """eval_rcnn.py:485-620: decode the RCNN regression relative to the RoIs, keep norm score > thresh, rotated NMS on
+        the raw scores.  Returns per scene (boxes (K,7), raw scores (K)) on the device, plus the decoded (B,M,7) boxes."""
+        rois = out["rois"]
+        B, M = rois.shape[0], rois.shape[1]
+        rcnn_cls = out["rcnn_cls"].view(B, M, -1)
+        pred = self.decode(out)
         raw = rcnn_cls[:, :, 0]
         keep_mask = torch.sigmoid(raw) > self.rcnn_score_thresh
         res = []
@@ -69,13 +88,8 @@ class PointRCNNInference(nn.Module):
         from .ext import iou3d_cuda
         rois = out["rois"]
         B, M = rois.shape[0], rois.shape[1]
-        c = self.rcnn_net.cfg
         rcnn_cls = out["rcnn_cls"].view(B, M, -1)
-        rcnn_reg = out["rcnn_reg"].view(B, M, -1)
-        pred = decode_bbox_target(rois.reshape(-1, 7), rcnn_reg.reshape(-1, rcnn_reg.shape[-1]), anchor_size=self.mean_size,
-                                  loc_scope=c["LOC_SCOPE"], loc_bin_size=c["LOC_BIN_SIZE"], num_head_bin=c["NUM_HEAD_BIN"],
-                                  get_xz_fine=True, get_y_by_bin=c["LOC_Y_BY_BIN"], loc_y_scope=c["LOC_Y_SCOPE"],
-                                  loc_y_bin_size=c["LOC_Y_BIN_SIZE"], get_ry_fine=True).view(B, M, 7)
+        pred = self.decode(out)
         raw = rcnn_cls[:, :, 0]
         above = torch.sigmoid(raw) > self.rcnn_score_thresh
         order = torch.where(above, raw, torch.full_like(raw, float("-inf"))).sort(dim=1, descending=True)[1]
