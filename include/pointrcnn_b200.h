@@ -440,6 +440,30 @@ PRB_API int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *
                                  const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling, int aug_flip,
                                  float aug_rot_range, float flip_prob, float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh,
                                  unsigned seed, float *gt_boxes_ct, int *cls_label, int *reg_valid_mask, void *stream);
+/* The same two stages with the recipe's choices as values, for the in-network target layer (lib/rpn/proposal_target_layer.py,
+ * ROI_SAMPLE_JIT) as well as the loader.  prb_rcnn_sample_rois is prb_rcnn_sample_rois_ex(..., gt_max_fg 1, fg_aug_times,
+ * bg_aug_times 1, kept_src_iou 0, ...) and prb_rcnn_roi_targets is prb_rcnn_roi_targets_ex(..., rot_lo -pi / aug_rot_range,
+ * rot_hi pi / aug_rot_range, flip_prob, pts_raw_ry 0, ...), draw for draw.
+ *
+ * sample_ex: roi_count NULL: all m rows of every scene are candidates (zero padding rows included: IoU 0, so easy bg).
+ * gt_count NULL: a scene's GT count is 1 + its last row with a non-zero value (trailing all-zero rows are padding).
+ * gt_max_fg 0: the fg list is only the RoIs over the threshold.  fg_aug_times / bg_aug_times: jitter tries of fg / bg rows,
+ * 0..63; a row with no try keeps its source box and the source's max IoU.  kept_src_iou != 0: a row whose last try kept
+ * the source box reports the source's max IoU (from iou) rather than the IoU recomputed for the kept box.
+ *
+ * targets_ex: the rotation angle is U[rot_lo, rot_hi) = rot_lo + (rot_hi - rot_lo) u, fp32; pts_raw_ry != 0: the points'
+ * canonical rotation uses the augmented RoI ry itself, the GT box's uses ry mod 2 pi (pts_raw_ry 0: both ry mod 2 pi). */
+PRB_API int prb_rcnn_sample_rois_ex(int b, int m, int g, const float *iou, const float *rois, const int *roi_count,
+                                    const float *gt_boxes, const int *gt_count, int roi_per_image, int fg_per_image,
+                                    float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh, float cls_bg_thresh_lo,
+                                    double hard_bg_ratio, int aug_method, int gt_max_fg, int fg_aug_times, int bg_aug_times,
+                                    int kept_src_iou, float pool_extra_width, unsigned seed, float *rois_out, float *gt_out,
+                                    float *iou_out, float *pool_boxes, int *sel, int *status, void *stream);
+PRB_API int prb_rcnn_roi_targets_ex(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
+                                    const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
+                                    int aug_flip, float rot_lo, float rot_hi, float flip_prob, int pts_raw_ry, float reg_fg_thresh,
+                                    float cls_fg_thresh, float cls_bg_thresh, unsigned seed, float *gt_boxes_ct, int *cls_label,
+                                    int *reg_valid_mask, void *stream);
 
 /* ------------------------------------------------------------------ evaluation statistics ------
  * The recall, segmentation IoU and classification accuracy of tools/eval_rcnn.py's three evaluation loops

@@ -65,6 +65,9 @@ def lib():
         P, I, F, U = c_void_p, c_int, c_float, ctypes.c_uint
         L.prb_rcnn_sample_rois.argtypes = [I, I, I, P, P, P, P, P, I, I, F, F, F, F, ctypes.c_double, I, I, F, U, P, P, P, P, P, P, P]
         L.prb_rcnn_roi_targets.argtypes = [I, I, I, I, P, P, P, P, P, I, I, I, I, F, F, F, F, F, U, P, P, P, P]
+        L.prb_rcnn_sample_rois_ex.argtypes = [I, I, I, P, P, P, P, P, I, I, F, F, F, F, ctypes.c_double, I, I, I, I, I, F, U, P, P, P, P, P,
+                                              P, P]
+        L.prb_rcnn_roi_targets_ex.argtypes = [I, I, I, I, P, P, P, P, P, I, I, I, I, F, F, F, I, F, F, F, U, P, P, P, P]
         L.prb_eval_box_recall.argtypes = [I, I, P, P, I, P, P, I, ctypes.POINTER(F), P, P, P, P]
         L.prb_eval_cls_acc.argtypes = [I, I, P, P, P, F, F, F, P, P, P]
         L.prb_options_init.restype = None

@@ -11,6 +11,8 @@ environment variables ONCE at import; at run time they are changed with `overrid
     fp_project_min_rows   ... for FP levels with at least this many unknown points in the batch (B * n)
     fps_ordered     SA modules whose input coordinates are the output of a previous sampling (nested encoder levels) take
                     the proven-prefix shortcut of prb_furthest_point_sampling_ordered_ws (same indices), default on
+    target_draw     which path ProposalTargetLayer(draw=None) takes: "torch" (the reference's random streams, default) or
+                    "device" (csrc/rcnn_sample.cu's hashed draws, no host synchronisation)
 """
 import contextlib
 import os
@@ -25,6 +27,7 @@ _DEFAULTS = dict(
     fp_project=os.environ.get("PRB_FP_PROJECT", "1") != "0",
     fp_project_min_rows=int(os.environ.get("PRB_FP_PROJECT_MIN_ROWS", "131072")),
     fps_ordered=os.environ.get("PRB_FPS_ORDERED", "1") != "0",
+    target_draw=os.environ.get("PRB_TARGET_DRAW", "torch"),
 )
 _local = threading.local()
 

@@ -6,6 +6,9 @@
 //            thread per sampled RoI runs the jitter loop with the 3D IoU computed inline (iou3d_dev.cuh's iou3d_pair)
 //   targets  one CTA per sampled RoI: stage-2 data augmentation of the pooled points and both boxes, labels from the
 //            pre-augmentation IoU, canonical transform
+// The _ex entry points take the recipe's choices as values, which also serves the in-network target layer
+// (lib/rpn/proposal_target_layer.py, ROI_SAMPLE_JIT): no GT-max RoIs in the fg list, per-class try counts, the source IoU
+// for a kept box, GT counts from trailing zero rows, an asymmetric rotation interval, points rotated by the raw ry.
 // Random draws are counter-based hashes keyed by (seed, scene, stage, roi, try, slot): the same distribution as the
 // reference's np.random stream, not the same stream.  oracle/rcnn_offline.py restates the keys, and the jitter arithmetic
 // below uses explicit _rn intrinsics so that an fp32 numpy restatement matches it bit for bit.
@@ -96,7 +99,9 @@ __device__ __forceinline__ void rs_jitter(const float *src, float *o, int method
 }
 
 struct RsCfg {
-    int R, fg_quota, method, fg_aug_times;
+    int R, fg_quota, method, fg_aug_times, bg_aug_times;
+    bool gt_max_fg;       // each GT's first-max RoI joins the fg list (the loader; the in-network layer leaves it out)
+    bool kept_src_iou;    // a row whose last try kept the source box reports the source's IoU (the in-network layer)
     float reg_fg, cls_fg, cls_bg, cls_bg_lo, extra_width;
     double hard_ratio;
     uint32_t seed;
@@ -117,8 +122,25 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
     __shared__ int s_src[kRsMaxRows];
     __shared__ int s_wc[kRsThreads / 32];
     __shared__ float s_poly[3 * POLY_SLOTS_RS * kRsThreads];
+    __shared__ int s_ng;
     const int scene = blockIdx.x, tid = threadIdx.x, R = cf.R;
-    const int n = min(roi_count[scene], m), ng = min(gt_count[scene], g);
+    const int n = roi_count ? min(roi_count[scene], m) : m;
+    int ng;
+    if (gt_count) {
+        ng = min(gt_count[scene], g);
+    } else {   // trailing all-zero GT rows are padding: ng = 1 + the last row with a non-zero value
+        if (tid == 0) s_ng = 0;
+        __syncthreads();
+        for (int j = tid; j < g; j += kRsThreads) {
+            const float *b = gts + ((size_t)scene * g + j) * 7;
+            bool nz = false;
+#pragma unroll
+            for (int q = 0; q < 7; ++q) nz |= b[q] != 0.f;
+            if (nz) atomicMax(&s_ng, j + 1);
+        }
+        __syncthreads();
+        ng = s_ng;
+    }
     const float fg_thresh = fminf(cf.reg_fg, cf.cls_fg);
 
     int st = 0, fg_rows = 0, hard_rows = 0, fg_num = 0, nh = 0, ne = 0;
@@ -138,7 +160,7 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
             s_maxov[i] = best;
             s_gtas[i] = arg;
         }
-        for (int j = tid; j < ng; j += kRsThreads) {
+        for (int j = tid; j < (cf.gt_max_fg ? ng : 0); j += kRsThreads) {
             float best = I[j];
             int arg = 0;
             for (int i = 1; i < n; ++i) {
@@ -150,7 +172,7 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
         __syncthreads();
         // fg: over the threshold in index order, then roi_assignment in GT order (duplicates kept); easy / hard bg
         fg_num = rs_append(n, [&](int i) { return s_maxov[i] >= fg_thresh; }, nullptr, s_fg, 0, s_wc);
-        fg_num = rs_append(ng, [&](int j) { return s_roias[j] >= 0; }, s_roias, s_fg, fg_num, s_wc);
+        if (cf.gt_max_fg) fg_num = rs_append(ng, [&](int j) { return s_roias[j] >= 0; }, s_roias, s_fg, fg_num, s_wc);
         ne = rs_append(n, [&](int i) { return s_maxov[i] < cf.cls_bg_lo; }, nullptr, s_easy, 0, s_wc);
         nh = rs_append(n, [&](int i) { return s_maxov[i] < cf.cls_bg && s_maxov[i] >= cf.cls_bg_lo; }, nullptr, s_hard, 0, s_wc);
         const int bg_num = ne + nh;
@@ -192,7 +214,7 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
     for (int r = tid; r < R; r += kRsThreads) {
         const size_t o = (size_t)scene * R + r;
         float box[7], gt[7];
-        float temp_iou = 0.f;
+        float temp_iou = 0.f, out_iou = 0.f;
         int cnt = 0, src = -1, ga = -1;
         if (st == 0) {
             src = s_src[r];
@@ -204,9 +226,11 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
                 gt[q] = gts[((size_t)scene * g + ga) * 7 + q];
                 box[q] = s[q];
             }
-            const int times = r < fg_rows ? cf.fg_aug_times : 1;
+            const int times = r < fg_rows ? cf.fg_aug_times : cf.bg_aug_times;
+            bool kept = false;
             while (temp_iou < pos_thresh && cnt < times) {
-                if (rs_u01(rs_key(cf.seed, scene, kSaltJitter, r, cnt, 0)) < 0.2f) {
+                kept = rs_u01(rs_key(cf.seed, scene, kSaltJitter, r, cnt, 0)) < 0.2f;
+                if (kept) {
 #pragma unroll
                     for (int q = 0; q < 7; ++q) box[q] = s[q];
                 } else {
@@ -215,6 +239,8 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
                 temp_iou = iou3d_pair(box, gt, px, py, pa, kRsThreads);
                 ++cnt;
             }
+            // no try: the source box with its source IoU
+            out_iou = (cnt == 0 || (cf.kept_src_iou && kept)) ? s_maxov[src] : temp_iou;
         } else {
 #pragma unroll
             for (int q = 0; q < 7; ++q) box[q] = gt[q] = 0.f;
@@ -224,7 +250,7 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
             rois_out[o * 7 + q] = box[q];
             gt_out[o * 7 + q] = gt[q];
         }
-        iou_out[o] = temp_iou;
+        iou_out[o] = out_iou;
         // enlarge_box3d (kitti_utils.py:150-160); an ignored row gets negative sizes, which no point is inside
         float pb[7];
         if (st == 0) {
@@ -262,7 +288,8 @@ __device__ __forceinline__ void rt_rotate_box(float *b, float c, float s) {
 
 struct RtCfg {
     int aug, rotation, scaling, flip;
-    float rot_range, flip_prob, reg_fg, cls_fg, cls_bg;
+    int pts_raw_ry;       // the points are rotated by the RoI's ry itself, not by ry mod 2 pi (the in-network layer)
+    float rot_lo, rot_hi, flip_prob, reg_fg, cls_fg, cls_bg;
     uint32_t seed;
 };
 
@@ -281,12 +308,11 @@ __global__ void __launch_bounds__(kRtThreads) rcnn_targets_kernel(
     bool rot = false, scale = false, flip = false;
     if (cf.aug) {
         auto u = [&](int slot) { return rs_u01(rs_key(cf.seed, scene, kSaltAug, r, 0, slot)); };
-        const float lo = -(float)CUDART_PI / cf.rot_range;
         rot = cf.rotation;
         scale = cf.scaling;
         flip = cf.flip && __fsub_rn(1.0f, u(2)) < cf.flip_prob;
         if (rot) {
-            const float angle = __fadd_rn(lo, __fmul_rn(__fmul_rn(lo, -2.0f), u(3)));
+            const float angle = __fadd_rn(cf.rot_lo, __fmul_rn(__fsub_rn(cf.rot_hi, cf.rot_lo), u(3)));   // [lo, hi)
             sincosf(angle, &as, &ac);
             rt_rotate_box(rb, ac, as);
             rt_rotate_box(gb, ac, as);
@@ -306,8 +332,10 @@ __global__ void __launch_bounds__(kRtThreads) rcnn_targets_kernel(
     const float two_pi = (float)(2.0 * CUDART_PI);
     float roi_ry = fmodf(rb[6], two_pi);
     if (roi_ry < 0.f) roi_ry += two_pi;
-    float cc, cs;
+    float cc, cs, pc, ps;
     sincosf(roi_ry, &cs, &cc);
+    if (cf.pts_raw_ry) sincosf(rb[6], &ps, &pc);
+    else { pc = cc; ps = cs; }
     float *p = rows + (size_t)k * S * W;
     for (int i = tid; i < S; i += kRtThreads) {
         float x = p[(size_t)i * W], y = p[(size_t)i * W + 1], z = p[(size_t)i * W + 2];
@@ -315,7 +343,7 @@ __global__ void __launch_bounds__(kRtThreads) rcnn_targets_kernel(
         if (scale) { x *= sc; y *= sc; z *= sc; }
         if (flip) x = -x;
         x -= rb[0]; y -= rb[1]; z -= rb[2];
-        rt_rot(x, z, cc, cs);
+        rt_rot(x, z, pc, ps);
         p[(size_t)i * W] = x; p[(size_t)i * W + 1] = y; p[(size_t)i * W + 2] = z;
     }
     if (tid == 0) {
@@ -345,24 +373,26 @@ __global__ void __launch_bounds__(kRtThreads) rcnn_targets_kernel(
 
 using namespace prb;
 
-extern "C" int prb_rcnn_sample_rois(int b, int m, int g, const float *iou, const float *rois, const int *roi_count, const float *gt_boxes,
-                                    const int *gt_count, int roi_per_image, int fg_per_image, float reg_fg_thresh, float cls_fg_thresh,
-                                    float cls_bg_thresh, float cls_bg_thresh_lo, double hard_bg_ratio, int aug_method, int fg_aug_times,
-                                    float pool_extra_width, unsigned seed, float *rois_out, float *gt_out, float *iou_out,
-                                    float *pool_boxes, int *sel, int *status, void *stream) {
-    PRB_REQUIRE(b > 0 && m >= 0 && g >= 0 && roi_count && gt_count && rois_out && gt_out && iou_out && pool_boxes && sel && status &&
-                    (m == 0 || rois) && (g == 0 || gt_boxes) && (m == 0 || g == 0 || iou),
+extern "C" int prb_rcnn_sample_rois_ex(int b, int m, int g, const float *iou, const float *rois, const int *roi_count,
+                                       const float *gt_boxes, const int *gt_count, int roi_per_image, int fg_per_image,
+                                       float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh, float cls_bg_thresh_lo,
+                                       double hard_bg_ratio, int aug_method, int gt_max_fg, int fg_aug_times, int bg_aug_times,
+                                       int kept_src_iou, float pool_extra_width, unsigned seed, float *rois_out, float *gt_out,
+                                       float *iou_out, float *pool_boxes, int *sel, int *status, void *stream) {
+    PRB_REQUIRE(b > 0 && m >= 0 && g >= 0 && rois_out && gt_out && iou_out && pool_boxes && sel && status && (m == 0 || rois) &&
+                    (g == 0 || gt_boxes) && (m == 0 || g == 0 || iou),
                 "rcnn_sample_rois: bad arguments");
     PRB_REQUIRE(m <= kRsMaxRois, "rcnn_sample_rois: %d proposals per scene > %d", m, kRsMaxRois);
     PRB_REQUIRE(g <= kRsMaxGt, "rcnn_sample_rois: %d GT boxes per scene > %d", g, kRsMaxGt);
     PRB_REQUIRE(roi_per_image > 0 && roi_per_image <= kRsMaxRows, "rcnn_sample_rois: ROI_PER_IMAGE %d not in 1..%d", roi_per_image,
                 kRsMaxRows);
-    PRB_REQUIRE(fg_per_image >= 0 && fg_per_image <= roi_per_image && fg_aug_times >= 1 && fg_aug_times < 64,
-                "rcnn_sample_rois: fg quota %d or fg aug times %d out of range", fg_per_image, fg_aug_times);
+    PRB_REQUIRE(fg_per_image >= 0 && fg_per_image <= roi_per_image && fg_aug_times >= 0 && fg_aug_times < 64 && bg_aug_times >= 0 &&
+                    bg_aug_times < 64,
+                "rcnn_sample_rois: fg quota %d or aug times %d / %d out of range", fg_per_image, fg_aug_times, bg_aug_times);
     PRB_REQUIRE(aug_method >= 0 && aug_method <= 2, "rcnn_sample_rois: REG_AUG_METHOD code %d not in 0..2", aug_method);
     PRB_REQUIRE(hard_bg_ratio >= 0.0 && hard_bg_ratio <= 1.0, "rcnn_sample_rois: HARD_BG_RATIO %g not in [0, 1]", hard_bg_ratio);
-    RsCfg cf{roi_per_image, fg_per_image, aug_method, fg_aug_times, reg_fg_thresh, cls_fg_thresh, cls_bg_thresh, cls_bg_thresh_lo,
-             pool_extra_width, hard_bg_ratio, seed};
+    RsCfg cf{roi_per_image, fg_per_image, aug_method, fg_aug_times, bg_aug_times, gt_max_fg != 0, kept_src_iou != 0, reg_fg_thresh,
+             cls_fg_thresh, cls_bg_thresh, cls_bg_thresh_lo, pool_extra_width, hard_bg_ratio, seed};
     const size_t smem = (size_t)(6 * m + 3 * g) * 4;
     PRB_CUDA(cudaFuncSetAttribute(rcnn_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem > 0 ? smem : 4)));
     rcnn_sample_kernel<<<b, kRsThreads, smem, (cudaStream_t)stream>>>(m, g, cf, iou, rois, roi_count, gt_boxes, gt_count, rois_out,
@@ -370,19 +400,45 @@ extern "C" int prb_rcnn_sample_rois(int b, int m, int g, const float *iou, const
     return check_launch("rcnn_sample_kernel");
 }
 
+// the loader's recipe: GT-max RoIs in the fg list, one try per bg row, the last box's IoU, counts given
+extern "C" int prb_rcnn_sample_rois(int b, int m, int g, const float *iou, const float *rois, const int *roi_count, const float *gt_boxes,
+                                    const int *gt_count, int roi_per_image, int fg_per_image, float reg_fg_thresh, float cls_fg_thresh,
+                                    float cls_bg_thresh, float cls_bg_thresh_lo, double hard_bg_ratio, int aug_method, int fg_aug_times,
+                                    float pool_extra_width, unsigned seed, float *rois_out, float *gt_out, float *iou_out,
+                                    float *pool_boxes, int *sel, int *status, void *stream) {
+    PRB_REQUIRE(roi_count && gt_count && fg_aug_times >= 1, "rcnn_sample_rois: bad arguments");
+    return prb_rcnn_sample_rois_ex(b, m, g, iou, rois, roi_count, gt_boxes, gt_count, roi_per_image, fg_per_image, reg_fg_thresh,
+                                   cls_fg_thresh, cls_bg_thresh, cls_bg_thresh_lo, hard_bg_ratio, aug_method, 1, fg_aug_times, 1, 0,
+                                   pool_extra_width, seed, rois_out, gt_out, iou_out, pool_boxes, sel, status, stream);
+}
+
+extern "C" int prb_rcnn_roi_targets_ex(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
+                                       const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
+                                       int aug_flip, float rot_lo, float rot_hi, float flip_prob, int pts_raw_ry, float reg_fg_thresh,
+                                       float cls_fg_thresh, float cls_bg_thresh, unsigned seed, float *gt_boxes_ct, int *cls_label,
+                                       int *reg_valid_mask, void *stream) {
+    PRB_REQUIRE(b > 0 && roi_per_image > 0 && S > 0 && W >= 3 && rows && rois && gt_boxes && iou && empty_flag && gt_boxes_ct &&
+                    cls_label && reg_valid_mask,
+                "rcnn_roi_targets: bad arguments");
+    PRB_REQUIRE(!aug_data || !aug_rotation || (rot_lo <= rot_hi && isfinite(rot_lo) && isfinite(rot_hi)),
+                "rcnn_roi_targets: rotation interval [%g, %g) is not finite and ordered", rot_lo, rot_hi);
+    PRB_REQUIRE((long)b * roi_per_image <= 0x7fffffffL, "rcnn_roi_targets: too many RoIs");
+    RtCfg cf{aug_data != 0, aug_rotation != 0, aug_scaling != 0, aug_flip != 0, pts_raw_ry != 0, rot_lo, rot_hi, flip_prob,
+             reg_fg_thresh, cls_fg_thresh, cls_bg_thresh, seed};
+    rcnn_targets_kernel<<<b * roi_per_image, kRtThreads, 0, (cudaStream_t)stream>>>(roi_per_image, S, W, cf, rows, rois, gt_boxes, iou,
+                                                                                      empty_flag, gt_boxes_ct, cls_label, reg_valid_mask);
+    return check_launch("rcnn_targets_kernel");
+}
+
+// the loader's recipe: rotation U(-pi / aug_rot_range, pi / aug_rot_range), points and GT box rotated by ry mod 2 pi
 extern "C" int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
                                     const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
                                     int aug_flip, float aug_rot_range, float flip_prob, float reg_fg_thresh, float cls_fg_thresh,
                                     float cls_bg_thresh, unsigned seed, float *gt_boxes_ct, int *cls_label, int *reg_valid_mask,
                                     void *stream) {
-    PRB_REQUIRE(b > 0 && roi_per_image > 0 && S > 0 && W >= 3 && rows && rois && gt_boxes && iou && empty_flag && gt_boxes_ct &&
-                    cls_label && reg_valid_mask,
-                "rcnn_roi_targets: bad arguments");
     PRB_REQUIRE(!aug_data || !aug_rotation || aug_rot_range > 0.f, "rcnn_roi_targets: AUG_ROT_RANGE must be > 0");
-    PRB_REQUIRE((long)b * roi_per_image <= 0x7fffffffL, "rcnn_roi_targets: too many RoIs");
-    RtCfg cf{aug_data != 0, aug_rotation != 0, aug_scaling != 0, aug_flip != 0, aug_rot_range, flip_prob, reg_fg_thresh, cls_fg_thresh,
-             cls_bg_thresh, seed};
-    rcnn_targets_kernel<<<b * roi_per_image, kRtThreads, 0, (cudaStream_t)stream>>>(roi_per_image, S, W, cf, rows, rois, gt_boxes, iou,
-                                                                                      empty_flag, gt_boxes_ct, cls_label, reg_valid_mask);
-    return check_launch("rcnn_targets_kernel");
+    const float lo = aug_data && aug_rotation ? -(float)CUDART_PI / aug_rot_range : 0.f;     // IEEE division, as on the device
+    return prb_rcnn_roi_targets_ex(b, roi_per_image, S, W, rows, rois, gt_boxes, iou, empty_flag, aug_data, aug_rotation, aug_scaling,
+                                   aug_flip, lo, -lo, flip_prob, 0, reg_fg_thresh, cls_fg_thresh, cls_bg_thresh, seed, gt_boxes_ct,
+                                   cls_label, reg_valid_mask, stream);
 }

@@ -11,6 +11,12 @@ synchronisation:
     batch = sampler.prepare_batch(scenes, seed=step)        # dict of CUDA tensors, RoI axis flattened to B * ROI_PER_IMAGE
     loss, terms = trainer.step_offline(batch)
 
+The in-network recipe (ROI_SAMPLE_JIT=True, the shipped default.yaml) reads the same files through
+get_rcnn_sample_jit + collate_batch and samples inside the network; here:
+
+    batch = sampler.prepare_jit_batch(scenes)               # padded input dict of CUDA tensors
+    loss, terms = trainer.step_jit(batch)                   # ProposalTargetLayer inside RCNNStage.forward_train
+
 File IO: `read_rpn_features` / `read_rois` read what the reference reads; `write_rpn_features_batch` writes what
 save_rpn_features writes, for a whole batch.  Differences from the reference (INTEGRATION.md): hashed draws, fp32 IoU,
 the flat RoI layout, the fg-only branch, a status instead of pdb, roipool3d_kernel.cu's inside test.
@@ -101,6 +107,60 @@ def write_rpn_features_batch(feature_dir, sample_ids, seg, rawscore, intensity, 
         np.save(p("_rawscore"), raw)
 
 
+# ------------------------------------------------------------------------------------------------ in-network recipe
+def pack_jit_scenes(scenes):
+    """get_rcnn_sample_jit (kitti_rcnn_dataset.py:1079-1102) + collate_batch (:1104-1137) for numpy scenes, into ONE float32
+    host buffer.  scenes: dicts rpn_xyz (N,3), rpn_features (N,C), rpn_intensity (N,), seg_mask (N,), roi_boxes3d (M,7),
+    gt_boxes3d (G,7).  -> (buffer, dict of views of it): rpn_xyz (B,N,3), rpn_features (B,N,C), rpn_intensity (B,N),
+    seg_mask (B,N), pts_depth (B,N) = ||xyz|| (np.linalg.norm in float32, as get_rcnn_sample_jit), roi_boxes3d (B,M,7) and
+    gt_boxes3d (B,G,7) zero-padded to the batch's longest list (M or G is 0 when every list is empty), roi_count /
+    gt_count (B) int32 (the int32 bits of float32 slots).  collate_batch stacks the point arrays and so needs one N for
+    the batch; a shorter scene is padded here with points at infinity (depth inf), which no box contains."""
+    B = len(scenes)
+    if B == 0:
+        raise ValueError("pack_jit_scenes: empty batch")
+    N = max(len(s["rpn_xyz"]) for s in scenes)
+    Cf = np.shape(scenes[0]["rpn_features"])[1]
+    rb = [_boxes7(np.asarray(s["roi_boxes3d"], np.float32)) for s in scenes]
+    gb = [_boxes7(np.asarray(s["gt_boxes3d"], np.float32)) for s in scenes]
+    M, G = max(len(b) for b in rb), max(len(b) for b in gb)
+    layout = _jit_layout(B, N, Cf, M, G)
+    buf = np.zeros(sum(int(np.prod(shape)) for _, shape in layout), np.float32)
+    v = _jit_views(buf, layout, lambda a: a.view(np.int32))
+    v["rpn_xyz"][:] = FAR
+    v["pts_depth"][:] = FAR
+    for k, s in enumerate(scenes):
+        p = np.asarray(s["rpn_xyz"], np.float32).reshape(-1, 3)
+        n = len(p)
+        if np.shape(s["rpn_features"]) != (n, Cf):
+            raise ValueError("pack_jit_scenes: rpn_features must be (N, C) with one C for the batch")
+        v["rpn_xyz"][k, :n] = p
+        v["rpn_features"][k, :n] = s["rpn_features"]
+        v["rpn_intensity"][k, :n] = np.asarray(s["rpn_intensity"], np.float32).reshape(-1)
+        v["seg_mask"][k, :n] = np.asarray(s["seg_mask"], np.float32).reshape(-1)
+        v["pts_depth"][k, :n] = np.linalg.norm(p, ord=2, axis=1)
+        v["roi_boxes3d"][k, :len(rb[k])] = rb[k]
+        v["gt_boxes3d"][k, :len(gb[k])] = gb[k]
+        v["roi_count"][k], v["gt_count"][k] = len(rb[k]), len(gb[k])
+    return buf, v
+
+
+def _jit_layout(B, N, Cf, M, G):
+    return [("rpn_xyz", (B, N, 3)), ("rpn_features", (B, N, Cf)), ("rpn_intensity", (B, N)), ("seg_mask", (B, N)), ("pts_depth", (B, N)),
+            ("roi_boxes3d", (B, M, 7)), ("gt_boxes3d", (B, G, 7)), ("roi_count", (B,)), ("gt_count", (B,))]
+
+
+def _jit_views(flat, layout, as_int32):
+    """views of a flat float32 array (numpy or torch) in the order of layout; the counts as int32 bits"""
+    out, o = {}, 0
+    for k, shape in layout:
+        n = int(np.prod(shape))
+        a = flat[o:o + n]
+        out[k] = (as_int32(a) if k.endswith("_count") else a).reshape(shape)
+        o += n
+    return out
+
+
 # ------------------------------------------------------------------------------------------------ sampler
 class RCNNOfflineSampler:
     """get_rcnn_training_sample_batch for a batch of scenes on the device.  cfg: the reference's global cfg (or any object
@@ -188,6 +248,32 @@ class RCNNOfflineSampler:
             if shape(s["rpn_features"])[1] != Cf or shape(s["rpn_features"])[0] != shape(s["rpn_xyz"])[0]:
                 raise ValueError("%s: rpn_features must be (N, C) with one C for the batch" % what)
         return B, N, M, G, Cf, (self._pack_device if on_device else self._pack_host)
+
+    def prepare_jit_batch(self, scenes):
+        """get_rcnn_sample_jit + collate_batch for a batch (pack_jit_scenes): the input dict of the in-network recipe, for
+        RCNNTrainer.step_jit (or the reference's rcnn_net under dropin.activate()), whose ProposalTargetLayer samples the
+        RoIs: every row of roi_boxes3d is a candidate there, zero padding included (IoU 0: easy background, as in the
+        reference).  numpy scenes go up in one copy; CUDA scenes are padded with batch-wide torch ops.  -> dict of CUDA
+        tensors rpn_xyz (B,N,3), rpn_features (B,N,C), rpn_intensity (B,N), seg_mask (B,N), pts_depth (B,N), roi_boxes3d
+        (B,M,7), gt_boxes3d (B,G,7), roi_count (B) int32, gt_count (B) int32."""
+        if len(scenes) == 0:
+            raise ValueError("prepare_jit_batch: empty batch")
+        dev = self.device
+        if not all(torch.is_tensor(s["rpn_xyz"]) and s["rpn_xyz"].is_cuda for s in scenes):
+            buf, host = pack_jit_scenes(scenes)
+            layout = [(k, a.shape) for k, a in host.items()]
+            return _jit_views(torch.from_numpy(buf).to(dev), layout, lambda a: a.view(torch.int32))
+        t = lambda v: torch.as_tensor(v, device=dev).float()
+        N = max(s["rpn_xyz"].shape[0] for s in scenes)
+        xyz = _pad([t(s["rpn_xyz"]).reshape(-1, 3) for s in scenes], N, FAR)
+        col = lambda key: _pad([t(s[key]).reshape(-1, 1) for s in scenes], N, 0.0).squeeze(2)
+        rb = [_boxes7(t(s["roi_boxes3d"])) for s in scenes]
+        gb = [_boxes7(t(s["gt_boxes3d"])) for s in scenes]
+        M, G = max(b.shape[0] for b in rb), max(b.shape[0] for b in gb)
+        counts = torch.from_numpy(np.array([[b.shape[0] for b in rb], [b.shape[0] for b in gb]], np.int32)).to(dev, non_blocking=True)
+        return {"rpn_xyz": xyz, "rpn_features": _pad([t(s["rpn_features"]) for s in scenes], N, 0.0), "rpn_intensity": col("rpn_intensity"),
+                "seg_mask": col("seg_mask"), "pts_depth": torch.linalg.vector_norm(xyz, ord=2, dim=2), "roi_boxes3d": _pad(rb, M, 0.0),
+                "gt_boxes3d": _pad(gb, G, 0.0), "roi_count": counts[0], "gt_count": counts[1]}
 
     def prepare_eval_batch(self, scenes):
         """get_proposal_from_file (kitti_rcnn_dataset.py:790-874) for a batch, no sampling and no augmentation: every

@@ -125,17 +125,18 @@ class RCNNStage(nn.Module):
         rcnn_reg = self.reg_layer(l_features[-1]).transpose(1, 2).contiguous().squeeze(dim=1)
         return rcnn_cls, rcnn_reg
 
-    def forward_train(self, input_data, target_layer=None):
+    def forward_train(self, input_data, target_layer=None, target_draw=None):
         """training branch of RCNNNet.forward with cfg.RCNN.ROI_SAMPLE_JIT (rcnn_net.py:119-126, :165-190): the target layer
         (RoI sampling, pooling, augmentation, canonical transform, labels -- no grad) then the network on the sampled RoIs.
-        input_data: the eval keys + gt_boxes3d (B,G,7).  -> the reference's ret_dict: rcnn_cls, rcnn_reg + the target dict
-        (cls_label, reg_valid_mask, gt_of_rois, roi_boxes3d, pts_input, ...)."""
+        input_data: the eval keys + gt_boxes3d (B,G,7).  target_draw: "torch" / "device" for this call (the config switch
+        target_draw, which a layer built with draw=None follows), None leaves the switch as it is.  -> the reference's
+        ret_dict: rcnn_cls, rcnn_reg + the target dict (cls_label, reg_valid_mask, gt_of_rois, roi_boxes3d, pts_input, ...)."""
         if target_layer is None:
             if getattr(self, "proposal_target_layer", None) is None:
                 from ..rpn.proposal_target_layer import ProposalTargetLayer
                 self.proposal_target_layer = ProposalTargetLayer()
             target_layer = self.proposal_target_layer
-        with torch.no_grad():
+        with torch.no_grad(), config.override(**({"target_draw": target_draw} if target_draw is not None else {})):
             target = target_layer(input_data)
             target["pts_input"] = torch.cat((target["sampled_pts"], target["pts_feature"]), dim=2)
         rcnn_cls, rcnn_reg = self.forward_pts(target["pts_input"])

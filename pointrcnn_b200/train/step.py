@@ -64,9 +64,11 @@ class RCNNTrainer:
     """One RCNN training step with the RPN fixed (the reference's second training phase: tools/train_rcnn.py --train_mode rcnn,
     cfg.RPN.FIXED): the RPN stage runs in eval mode without grad on the fused path and hands (rois, point features, mask,
     depth) to the RCNN stage, whose target layer samples 64 RoIs per scene; forward / backward of the RCNN network on the
-    op-by-op path, get_rcnn_loss, bucketed gradient all-reduce, optimizer step."""
+    op-by-op path, get_rcnn_loss, bucketed gradient all-reduce, optimizer step.  target_draw: how the target layer samples
+    ("torch": the reference's random calls, "device": one device pass without host reads; None: the config switch)."""
 
-    def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, rpn_score_thresh=0.3):
+    def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, rpn_score_thresh=0.3,
+                 target_draw=None):
         from ..rcnn.stage import RCNNStage
         torch.manual_seed(seed)
         self.device = torch.device(device)
@@ -79,6 +81,7 @@ class RCNNTrainer:
         self.opt = torch.optim.Adam(self.params, lr=lr, weight_decay=weight_decay, **({"fused": True} if self.device.type == "cuda" else {}))
         self.mean_size = torch.from_numpy(CLS_MEAN_SIZE[0]).to(self.device)
         self.rpn_score_thresh = rpn_score_thresh
+        self.target_draw = target_draw
 
     @torch.no_grad()
     def rpn_outputs(self, pts_input, gt_boxes3d):
@@ -88,7 +91,12 @@ class RCNNTrainer:
                 "pts_depth": torch.norm(xyz, p=2, dim=2), "gt_boxes3d": gt_boxes3d}
 
     def forward_loss(self, pts_input, gt_boxes3d):
-        ret = self.model.forward_train(self.rpn_outputs(pts_input, gt_boxes3d))
+        return self.forward_loss_jit(self.rpn_outputs(pts_input, gt_boxes3d))
+
+    def forward_loss_jit(self, batch):
+        """rcnn_net.forward with ROI_SAMPLE_JIT (:120-126) + get_rcnn_loss on an input dict: the RPN outputs of forward_loss, or
+        a batch of saved features and proposals from datasets.rcnn_offline.RCNNOfflineSampler.prepare_jit_batch"""
+        ret = self.model.forward_train(batch, target_draw=self.target_draw)
         c = self.model.cfg
         return rcnn_loss(ret["rcnn_cls"], ret["rcnn_reg"], ret["cls_label"], ret["reg_valid_mask"], ret["roi_boxes3d"], ret["gt_of_rois"],
                          self.mean_size, loc_scope=c["LOC_SCOPE"], loc_bin_size=c["LOC_BIN_SIZE"], num_head_bin=c["NUM_HEAD_BIN"],
@@ -107,6 +115,11 @@ class RCNNTrainer:
     def step_offline(self, batch, grad_norm_clip=None):
         """one offline-recipe training step (tools/train_rcnn.py --train_mode rcnn_offline) on a prepared batch"""
         return self._step(self.forward_loss_offline, (batch,), grad_norm_clip)
+
+    def step_jit(self, batch, grad_norm_clip=None):
+        """one training step of tools/train_rcnn.py --train_mode rcnn_offline with ROI_SAMPLE_JIT (the target layer inside
+        the network) on a prepare_jit_batch batch"""
+        return self._step(self.forward_loss_jit, (batch,), grad_norm_clip)
 
     def step(self, pts_input, gt_boxes3d, grad_norm_clip=None):
         return self._step(self.forward_loss, (pts_input, gt_boxes3d), grad_norm_clip)
