@@ -225,6 +225,16 @@ def boxes_overlap_bev(a, b):
     return out
 
 
+def box_overlap_pairs(a, b, mutant=0):
+    """aligned pairs (n,5) -> (overlap (n,) f32, polygon vertex count (n,) int32); mutant: see pointops_oracle.c"""
+    a, b = _f32(a), _f32(b)
+    n = a.shape[0]
+    out = np.empty(n, dtype=np.float32)
+    cnt = np.empty(n, dtype=np.int32)
+    lib().orc_box_overlap_pairs(n, _p(a), _p(b), int(mutant), _p(out), _p(cnt))
+    return out, cnt
+
+
 def boxes_iou_bev(a, b):
     a, b = _f32(a), _f32(b)
     out = np.empty((a.shape[0], b.shape[0]), dtype=np.float32)

@@ -15,6 +15,7 @@
  *   orc_pt_in_box3d         lib/utils/roipool3d/src/roipool3d_kernel.cu:14-28
  *   orc_roipool3d           lib/utils/roipool3d/src/roipool3d_kernel.cu:97-194 (== roipool3d.cpp:127-195)
  *   orc_box_overlap         lib/utils/iou3d/src/iou3d_kernel.cu:34-212
+ *   orc_box_overlap_pairs   the same for aligned pairs, with the polygon vertex count and planted mistakes
  *   orc_iou_bev/normal      lib/utils/iou3d/src/iou3d_kernel.cu:214-221, 295-303
  *   orc_nms_mask / orc_nms  lib/utils/iou3d/src/iou3d_kernel.cu:250-348 + iou3d.cpp:100-116
  *
@@ -367,7 +368,13 @@ static inline void rot_center(pt2 c, float ca, float sa, pt2 *p) {
     p->x = nx; p->y = ny;
 }
 
-ORC_API float orc_box_overlap(const float *box_a, const float *box_b) {
+/* The overlap with a planted mistake, for tests that show their error bound catches one (tests/iou_reference.py):
+ * mutant 0 = the reference; 1 = the last corner of box b is never tested; 2 = sin of the heading negated;
+ * 3 = the sort comparison reversed; 4 = the bubble sort stops one pass early.  *cnt: polygon vertex count.  The
+ * reference and the device kernels hold 16 vertices (cp[16], POLY_SLOTS); crossings and corners are counted separately,
+ * so rounding alone does not bound the count by 16 (at most 16 + 8), and cp[24] lets this restatement report a larger
+ * count instead of overflowing.  For every count up to 16 it computes what cp[16] does. */
+static float box_overlap_impl(const float *box_a, const float *box_b, int mutant, int *cnt_out) {
     float a_x1 = box_a[0], a_y1 = box_a[1], a_x2 = box_a[2], a_y2 = box_a[3], a_angle = box_a[4];
     float b_x1 = box_b[0], b_y1 = box_b[1], b_x2 = box_b[2], b_y2 = box_b[3], b_angle = box_b[4];
     pt2 center_a = {(a_x1 + a_x2) / 2, (a_y1 + a_y2) / 2};
@@ -376,13 +383,14 @@ ORC_API float orc_box_overlap(const float *box_a, const float *box_b) {
     pt2 cb[5] = {{b_x1, b_y1}, {b_x2, b_y1}, {b_x2, b_y2}, {b_x1, b_y2}, {0, 0}};
     float a_cos = cosf(a_angle), a_sin = sinf(a_angle);
     float b_cos = cosf(b_angle), b_sin = sinf(b_angle);
+    if (mutant == 2) { a_sin = -a_sin; b_sin = -b_sin; }
     for (int k = 0; k < 4; ++k) {
         rot_center(center_a, a_cos, a_sin, &ca[k]);
         rot_center(center_b, b_cos, b_sin, &cb[k]);
     }
     ca[4] = ca[0];
     cb[4] = cb[0];
-    pt2 cp[16];
+    pt2 cp[24];
     pt2 pc = {0, 0};
     int cnt = 0;
     for (int i = 0; i < 4; ++i)
@@ -392,7 +400,7 @@ ORC_API float orc_box_overlap(const float *box_a, const float *box_b) {
                 ++cnt;
             }
     for (int k = 0; k < 4; ++k) {
-        if (in_box2d(box_a, cb[k])) {
+        if (!(mutant == 1 && k == 3) && in_box2d(box_a, cb[k])) {
             pc.x = pc.x + cb[k].x; pc.y = pc.y + cb[k].y;
             cp[cnt++] = cb[k];
         }
@@ -401,13 +409,16 @@ ORC_API float orc_box_overlap(const float *box_a, const float *box_b) {
             cp[cnt++] = ca[k];
         }
     }
+    if (cnt_out) *cnt_out = cnt;
     pc.x /= cnt;
     pc.y /= cnt;
-    for (int j = 0; j < cnt - 1; ++j)
-        for (int i = 0; i < cnt - j - 1; ++i)
-            if (atan2f(cp[i].y - pc.y, cp[i].x - pc.x) > atan2f(cp[i + 1].y - pc.y, cp[i + 1].x - pc.x)) {
+    for (int j = 0; j < cnt - 1 - (mutant == 4); ++j)
+        for (int i = 0; i < cnt - j - 1; ++i) {
+            float t0 = atan2f(cp[i].y - pc.y, cp[i].x - pc.x), t1 = atan2f(cp[i + 1].y - pc.y, cp[i + 1].x - pc.x);
+            if (mutant == 3 ? t0 < t1 : t0 > t1) {
                 pt2 t = cp[i]; cp[i] = cp[i + 1]; cp[i + 1] = t;
             }
+        }
     float area = 0;
     for (int k = 0; k < cnt - 1; ++k) {
         pt2 u = {cp[k].x - cp[0].x, cp[k].y - cp[0].y};
@@ -415,6 +426,16 @@ ORC_API float orc_box_overlap(const float *box_a, const float *box_b) {
         area += cross2(u, v);
     }
     return (float)(fabsf(area) / 2.0);
+}
+
+ORC_API float orc_box_overlap(const float *box_a, const float *box_b) { return box_overlap_impl(box_a, box_b, 0, NULL); }
+
+/* aligned pairs: out[k] = overlap(a[k], b[k]) (with the planted mistake `mutant`, see above), cnt[k] its polygon
+ * vertex count (cnt may be NULL) */
+ORC_API void orc_box_overlap_pairs(int n, const float *a, const float *b, int mutant, float *out, int *cnt) {
+#pragma omp parallel for schedule(static, 256)
+    for (int k = 0; k < n; ++k)
+        out[k] = box_overlap_impl(a + (size_t)k * 5, b + (size_t)k * 5, mutant, cnt ? cnt + k : NULL);
 }
 
 ORC_API float orc_iou_bev(const float *a, const float *b) {

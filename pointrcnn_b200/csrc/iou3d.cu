@@ -21,7 +21,10 @@ namespace prb {
 // 16 x 16 pairs per CTA; the 32 boxes of the tile are precomputed once (BoxPre: centre, cos/sin, rotated corners), the
 // intersection polygon of each pair lives in a shared-memory column of its thread (no local memory).
 constexpr int PM_T = 16;
-constexpr int POLY_SLOTS = 16;         // an intersection polygon has at most 8 + 8 vertices
+// the reference's cp[16].  The algorithm counts edge crossings and corners separately, so with rounding it can count more
+// than the 8 vertices an exact intersection has: near-parallel and near-duplicate pairs reach exactly 16 in the
+// CPU oracle (tests/test_cpu_iou_geometry.py); none of the generated pairs exceeds it, but no proof bounds the count by 16
+constexpr int POLY_SLOTS = 16;
 template <bool IOU>
 __global__ void __launch_bounds__(PM_T * PM_T) pair_matrix_kernel(int num_a, const float *__restrict__ boxes_a, int num_b,
                                                                   const float *__restrict__ boxes_b, float *__restrict__ out) {

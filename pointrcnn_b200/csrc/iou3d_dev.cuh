@@ -4,6 +4,13 @@
 // The overlap arithmetic IS the spec (keep masks are compared bit-exactly with lib/utils/iou3d/src/iou3d_kernel.cu:
 // 34-221): corners rotated about the box centre, 4x4 edge intersections (bbox reject, straddle test, line solve with
 // an EPS fallback), corners of one box inside the other (MARGIN 1e-5), centroid, bubble sort by atan2f, fan area / 2.0.
+//
+// Measured behaviour (tests/test_cpu_iou_geometry.py, tests/test_gpu_iou_geometry.py): the fixed MARGIN is below a few
+// fp32 ulps at KITTI far range (one ulp is 7.6e-6 at 64 m), so a box's own corners, rotated there and back, can fall
+// outside it: IoU(a, a) < 1, down to 0, for some boxes at z 60-80 m, as in the reference.  Near-parallel and
+// near-duplicate pairs are ill-conditioned the same way, and their polygon can reach 16 vertices (the scratch size).
+// Every consumer inherits this: NMS (matrix, bitmask, proposal), the fused 3D IoU, RoI sampling, recall statistics,
+// GT-paste collisions and the KITTI overlaps.
 #pragma once
 #include "common.cuh"
 
@@ -22,14 +29,20 @@ __device__ __forceinline__ int rect_cross(const P2 &p1, const P2 &p2, const P2 &
     return min(p1.x, p2.x) <= max(q1.x, q2.x) && min(q1.x, q2.x) <= max(p1.x, p2.x) &&
            min(p1.y, p2.y) <= max(q1.y, q2.y) && min(q1.y, q2.y) <= max(p1.y, p2.y);
 }
+// The rotation of in_box2d and rot_center with the contraction the reference's SASS shows (nvcc 12.9 -O2, iou3d_kernel.cu):
+// x' = fma(dx, cos, dy * sin) + c.x and y' = fma(dy, cos, -(dx * sin)) + c.y.  Left to the compiler, the inlined copies
+// here fused the other product of y' in in_box2d_pre, which flips the inside test of near-boundary corners.
+__device__ __forceinline__ P2 rot_about(float dx, float dy, float cx, float cy, float angle_cos, float angle_sin) {
+    return mk(__fadd_rn(__fmaf_rn(dx, angle_cos, __fmul_rn(dy, angle_sin)), cx),
+              __fadd_rn(__fmaf_rn(dy, angle_cos, -__fmul_rn(dx, angle_sin)), cy));
+}
 __device__ __forceinline__ int in_box2d(const float *box, const P2 &p) {
     const float MARGIN = 1e-5;
     float center_x = (box[0] + box[2]) / 2;
     float center_y = (box[1] + box[3]) / 2;
     float angle_cos = cos(-box[4]), angle_sin = sin(-box[4]);
-    float rot_x = (p.x - center_x) * angle_cos + (p.y - center_y) * angle_sin + center_x;
-    float rot_y = -(p.x - center_x) * angle_sin + (p.y - center_y) * angle_cos + center_y;
-    return (rot_x > box[0] - MARGIN && rot_x < box[2] + MARGIN && rot_y > box[1] - MARGIN && rot_y < box[3] + MARGIN);
+    const P2 r = rot_about(__fsub_rn(p.x, center_x), __fsub_rn(p.y, center_y), center_x, center_y, angle_cos, angle_sin);
+    return (r.x > box[0] - MARGIN && r.x < box[2] + MARGIN && r.y > box[1] - MARGIN && r.y < box[3] + MARGIN);
 }
 __device__ __forceinline__ int seg_intersection(const P2 &p1, const P2 &p0, const P2 &q1, const P2 &q0, P2 &ans) {
     const float EPS = 1e-8;
@@ -53,10 +66,7 @@ __device__ __forceinline__ int seg_intersection(const P2 &p1, const P2 &p0, cons
     return 1;
 }
 __device__ __forceinline__ void rot_center(const P2 &c, const float angle_cos, const float angle_sin, P2 &p) {
-    float new_x = (p.x - c.x) * angle_cos + (p.y - c.y) * angle_sin + c.x;
-    float new_y = -(p.x - c.x) * angle_sin + (p.y - c.y) * angle_cos + c.y;
-    p.x = new_x;
-    p.y = new_y;
+    p = rot_about(__fsub_rn(p.x, c.x), __fsub_rn(p.y, c.y), c.x, c.y, angle_cos, angle_sin);
 }
 __device__ __forceinline__ int angle_gt(const P2 &a, const P2 &b, const P2 &c) {
     return atan2(a.y - c.y, a.x - c.x) > atan2(b.y - c.y, b.x - c.x);
@@ -169,10 +179,8 @@ __device__ __forceinline__ void box_pre(const float *box, BoxPre &b) {
 // in_box2d with the box's precomputed centre and cos(-ry) = c, sin(-ry) = -s
 __device__ __forceinline__ int in_box2d_pre(const BoxPre &b, const P2 &p) {
     const float MARGIN = 1e-5;
-    const float angle_cos = b.c, angle_sin = -b.s;
-    float rot_x = (p.x - b.cx) * angle_cos + (p.y - b.cy) * angle_sin + b.cx;
-    float rot_y = -(p.x - b.cx) * angle_sin + (p.y - b.cy) * angle_cos + b.cy;
-    return (rot_x > b.x1 - MARGIN && rot_x < b.x2 + MARGIN && rot_y > b.y1 - MARGIN && rot_y < b.y2 + MARGIN);
+    const P2 r = rot_about(__fsub_rn(p.x, b.cx), __fsub_rn(p.y, b.cy), b.cx, b.cy, b.c, -b.s);
+    return (r.x > b.x1 - MARGIN && r.x < b.x2 + MARGIN && r.y > b.y1 - MARGIN && r.y < b.y2 + MARGIN);
 }
 
 // rotated-rectangle intersection area from two precomputed boxes.  px / py / pa: scratch for up to 16 polygon vertices
@@ -240,6 +248,10 @@ __device__ __forceinline__ float iou_bev_pre(const BoxPre &A, const BoxPre &B, f
 // ---------------------------------------------------------------------------------------------- fused 3D IoU of one pair
 // iou3d_utils.boxes_iou3d_gpu's op sequence for [x,y,z,h,w,l,ry] boxes, every torch op one fp32 rounding (iou3d.cu's
 // iou3d_kernel, rcnn_sample.cu's jitter loop)
+// torch.max / torch.min / torch.clamp propagate a NaN operand, fmaxf / fminf drop it: a NaN height or size must give a
+// NaN IoU, as boxes_iou3d_gpu does, not ov3d / 1e-7
+__device__ __forceinline__ float nan_max(float x, float y) { return x != x ? x : (y != y ? y : fmaxf(x, y)); }
+__device__ __forceinline__ float nan_min(float x, float y) { return x != x ? x : (y != y ? y : fminf(x, y)); }
 __device__ __forceinline__ void box7_to_bev(const float *b, float *bev) {
     const float half_l = __fmul_rn(b[5], 0.5f), half_w = __fmul_rn(b[4], 0.5f);
     bev[0] = __fsub_rn(b[0], half_l); bev[1] = __fsub_rn(b[2], half_w);
@@ -255,10 +267,10 @@ __device__ __forceinline__ float iou3d_pair(const float *a, const float *b, floa
     box_pre(bbev, Bp);
     const float ov_bev = box_overlap_pre(A, Bp, px, py, pa, stride);
     const float a_min = __fsub_rn(a[1], a[3]), b_min = __fsub_rn(b[1], b[3]);       // y - h .. y (y points down)
-    const float ov_h = fmaxf(__fsub_rn(fminf(a[1], b[1]), fmaxf(a_min, b_min)), 0.f);
+    const float ov_h = nan_max(__fsub_rn(nan_min(a[1], b[1]), nan_max(a_min, b_min)), 0.f);
     const float ov3d = __fmul_rn(ov_bev, ov_h);
     const float va = __fmul_rn(__fmul_rn(a[3], a[4]), a[5]), vb = __fmul_rn(__fmul_rn(b[3], b[4]), b[5]);
-    return __fdiv_rn(ov3d, fmaxf(__fsub_rn(__fadd_rn(va, vb), ov3d), 1e-7f));
+    return __fdiv_rn(ov3d, nan_max(__fsub_rn(__fadd_rn(va, vb), ov3d), 1e-7f));
 }
 
 }  // namespace prb
