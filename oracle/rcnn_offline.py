@@ -5,17 +5,29 @@ Follows lib/datasets/kitti_rcnn_dataset.py:876-1077 (get_rcnn_training_sample_ba
 aug_roi_by_noise_batch, random_aug_box3d :746-788, data_augmentation stage 2 :513-570, rotate_box3d_along_y :396-406,
 canonical_transform_batch :685-704) and lib/utils/kitti_utils.py (boxes3d_to_corners3d, rotate_pc_along_y[_torch]).
 
-Two draw sources:
-  "numpy"  the reference's np.random calls in the reference's order (rng = np.random or a RandomState)
+Two recipes (`recipe`), with the values pointrcnn_b200/rcnn/targets.py passes to the device:
+  "loader" get_rcnn_training_sample_batch, above
+  "layer"  the in-network target layer, lib/rpn/proposal_target_layer.py with ROI_SAMPLE_JIT: no GT-max RoIs in the fg
+           list (the layer's :113 is commented out); ROI_FG_AUG_TIMES jitter tries for fg rows (0 allowed), 1 if
+           ROI_FG_AUG_TIMES > 0 else 0 for bg rows, and a row with no try, or whose last try kept the source box, reports
+           the source's max IoU; every row of roi_boxes3d is a candidate (zero padding: IoU 0, easy bg) and trailing
+           all-zero GT rows are trimmed; stage-2 augmentation always rotates, scales and flips: angle U(-pi / AUG_ROT_RANGE,
+           0) (the reference's `rand - 0.5 / 0.5`), flip with p = 0.5; the points' canonical rotation is by the augmented ry
+Three draw sources:
+  "numpy"  the loader's np.random calls in the reference's order (rng = np.random or a RandomState)
+  "ref"    the layer's host random calls in its order: np.random.permutation / rand (fg), torch.randint on the CPU
+           generator (bg), np.random.rand (keep), torch.rand / randint on the CPU (single / multiple jitter); with AUG_DATA
+           off this is the reference layer run on the CPU (its augmentation draws are batch-wide and are not restated)
   "hash"   the device's counter-based keys (csrc/rcnn_sample.cu), restated; the jitter arithmetic in fp32 as the kernel does it
 Two IoU functions:
   "exact"  oracle/gt_paste.py::iou3d, the float64 polygon clip that stands in for shapely
   "fp32"   oracle.boxes_iou3d, prb_boxes_iou3d's op sequence compiled for the host: a few ulp (about 2e-6) from the
            device's IoU, so IoUs are compared within a bound and decisions agree unless an IoU lies that close to a threshold
 and, with them, two pooling predicates: "exact" pools with roipool3d_cpu's mixed float / double test (the reference's
-loader), "fp32" with roipool3d_kernel.cu's (oracle.roipool3d, the device's).  ("numpy", "exact") is the reference's loader;
-("hash", "fp32") is what the device computes.  In "hash" mode the augmentation and the canonical transform are float64
-numpy, which the device matches to fp32 rounding only (sinf / cosf / atan2f).
+loader), "fp32" with roipool3d_kernel.cu's (oracle.roipool3d, the device's).  ("loader", "numpy", "exact") is the
+reference's loader, ("layer", "ref", "fp32") its layer; ("hash", "fp32") is what the device computes.  In "hash" mode the
+augmentation and the canonical transform are float64 numpy, which the device matches to fp32 rounding only (sinf / cosf /
+atan2f).
 """
 import numpy as np
 import torch
@@ -26,8 +38,8 @@ from oracle import oracle as O
 # tools/cfgs/default.yaml
 CFG = dict(AUG_DATA=True, AUG_METHOD_LIST=["rotation", "scaling", "flip"], AUG_METHOD_PROB=[1.0, 1.0, 0.5], AUG_ROT_RANGE=18,
            USE_INTENSITY=False, USE_DEPTH=True, POOL_EXTRA_WIDTH=1.0, NUM_POINTS=512, REG_AUG_METHOD="multiple", CLS_FG_THRESH=0.6,
-           CLS_BG_THRESH=0.45, CLS_BG_THRESH_LO=0.05, REG_FG_THRESH=0.55, FG_RATIO=0.5, ROI_PER_IMAGE=64, HARD_BG_RATIO=0.8)
-FG_AUG_TIMES = 10
+           CLS_BG_THRESH=0.45, CLS_BG_THRESH_LO=0.05, REG_FG_THRESH=0.55, FG_RATIO=0.5, ROI_PER_IMAGE=64, HARD_BG_RATIO=0.8,
+           ROI_FG_AUG_TIMES=10)
 RANGE_CONFIG = [[0.2, 0.1, np.pi / 12, 0.7], [0.3, 0.15, np.pi / 12, 0.6], [0.5, 0.15, np.pi / 9, 0.5], [0.8, 0.15, np.pi / 6, 0.3],
                 [1.0, 0.15, np.pi / 3, 0.2]]
 
@@ -184,11 +196,34 @@ class NumpyDraws:
         return en, angle, scale
 
 
-class HashDraws:
-    """the device's keys; the jitter in fp32 with the kernel's roundings"""
+class RefDraws(NumpyDraws):
+    """the reference layer's host random calls (numpy global state, torch CPU generator)"""
 
-    def __init__(self, seed, scene):
-        self.seed, self.scene = seed & _M, scene
+    def bg(self, rows, size):
+        return torch.randint(low=0, high=size, size=(rows,)).long().numpy()
+
+    def jitter(self, box, method, row, t):
+        b = torch.from_numpy(np.asarray(box, np.float32))
+        if method == "single":
+            pos = torch.rand(3) - 0.5
+            hwl = (torch.rand(3) - 0.5) / (0.5 / 0.15) + 1.0
+            ang = (torch.rand(1) - 0.5) / (0.5 / (np.pi / 12))
+        elif method == "multiple":
+            rc = RANGE_CONFIG[torch.randint(low=0, high=len(RANGE_CONFIG), size=(1,))[0].long()]
+            pos = ((torch.rand(3) - 0.5) / 0.5) * rc[0]
+            hwl = ((torch.rand(3) - 0.5) / 0.5) * rc[1] + 1.0
+            ang = ((torch.rand(1) - 0.5) / 0.5) * rc[2]
+        else:
+            raise NotImplementedError(method)
+        return torch.cat([b[0:3] + pos, b[3:6] * hwl, b[6:7] + ang]).numpy()
+
+
+class HashDraws:
+    """the device's keys; the jitter in fp32 with the kernel's roundings.  rot_hi: the upper end of the rotation interval,
+    whose lower end is -pi / AUG_ROT_RANGE; None: pi / AUG_ROT_RANGE (the loader)"""
+
+    def __init__(self, seed, scene, rot_hi=None):
+        self.seed, self.scene, self.rot_hi = seed & _M, scene, rot_hi
 
     def _u(self, salt, row, t, slot):
         return u01(rs_key(self.seed, self.scene, salt, row, t, slot))
@@ -242,27 +277,53 @@ class HashDraws:
         angle = scale = None
         if "rotation" in cfg["AUG_METHOD_LIST"]:
             lo = f(-f(np.pi) / f(cfg["AUG_ROT_RANGE"]))
-            angle = float(f(lo + f(f(lo * f(-2)) * u(3))))
+            hi = -lo if self.rot_hi is None else f(self.rot_hi)
+            angle = float(f(lo + f(f(hi - lo) * u(3))))
         if "scaling" in cfg["AUG_METHOD_LIST"]:
             scale = float(f(f(0.95) + f(f(0.1) * u(4))))
         return en, angle, scale
 
 
 # ------------------------------------------------------------------------------------------------ one scene
-def sample_scene(scene, cfg=None, draw="numpy", iou="exact", rng=np.random, seed=0, scene_index=0, train=True):
-    """scene: dict rpn_xyz (N,3), rpn_features (N,C), rpn_intensity (N,), seg_mask (N,), roi_boxes3d (M,7), gt_boxes3d (G,7).
-    -> dict: status, sel (R,3) [source RoI, GT, tries], iou (R,), rois / gt_of_rois (R,7) before augmentation,
+def recipe_values(c, which):
+    """the values in which the loader and the layer differ, as pointrcnn_b200/rcnn/targets.py passes them to the device;
+    aug: the stage-2 augmentation's config (AUG_METHOD_LIST, AUG_METHOD_PROB[2] the flip probability, AUG_ROT_RANGE), rot_hi
+    the upper end of the rotation interval (None: symmetric)"""
+    if which == "loader":
+        return dict(gt_max_fg=True, counts=True, fg_aug_times=10, bg_aug_times=1, kept_src_iou=False, aug=c, rot_hi=None, pts_raw_ry=False)
+    if which == "layer":
+        A = c["ROI_FG_AUG_TIMES"]
+        return dict(gt_max_fg=False, counts=False, fg_aug_times=A, bg_aug_times=min(A, 1), kept_src_iou=True,
+                    aug=dict(c, AUG_METHOD_LIST=["rotation", "scaling", "flip"], AUG_METHOD_PROB=[1.0, 1.0, 0.5]), rot_hi=0.0,
+                    pts_raw_ry=True)
+    raise ValueError(which)
+
+
+def trimmed_gt(gt):
+    """the reference layer's `while cur_gt[k].sum() == 0: k -= 1` for rows that are all zero"""
+    nz = np.nonzero(np.any(gt != 0, axis=1))[0]
+    return gt[:nz[-1] + 1] if nz.size else gt[:0]
+
+
+def sample_scene(scene, cfg=None, draw="numpy", iou="exact", rng=np.random, seed=0, scene_index=0, train=True, recipe="loader"):
+    """scene: dict rpn_xyz (N,3), rpn_features (N,C), rpn_intensity (N,), seg_mask (N,), roi_boxes3d (M,7), gt_boxes3d (G,7),
+    and optionally pts_depth (N,) (the layer's input; else the norm of rpn_xyz).
+    -> dict: status, branch, sel (R,3) [source RoI, GT, tries], iou (R,), rois / gt_of_rois (R,7) before augmentation,
     pooled_input / pooled_features / empty (the pool), pts_input / pts_features, cls_label, reg_valid_mask, gt_boxes3d_ct,
     roi_boxes3d, gt_boxes3d (after augmentation and the canonical transform)"""
     c = dict(CFG, **(cfg or {}))
+    rc = recipe_values(c, recipe)
     R, S = c["ROI_PER_IMAGE"], c["NUM_POINTS"]
-    dr = NumpyDraws(rng) if draw == "numpy" else HashDraws(seed, scene_index)
+    dr = {"numpy": NumpyDraws, "ref": RefDraws}[draw](rng) if draw != "hash" else HashDraws(seed, scene_index, rc["rot_hi"])
     rois_all = np.asarray(scene["roi_boxes3d"], np.float32).reshape(-1, 7)
     gts_all = np.asarray(scene["gt_boxes3d"], np.float32).reshape(-1, 7)
+    if not rc["counts"]:
+        gts_all = trimmed_gt(gts_all)
     xyz = np.asarray(scene["rpn_xyz"], np.float32)
     extra = ([np.asarray(scene["rpn_intensity"]).reshape(-1, 1)] if c["USE_INTENSITY"] else []) + [np.asarray(scene["seg_mask"]).reshape(-1, 1)]
     if c["USE_DEPTH"]:
-        extra.append(((np.linalg.norm(xyz, ord=2, axis=1) / 70.0) - 0.5).reshape(-1, 1))
+        depth = scene["pts_depth"] if "pts_depth" in scene else np.linalg.norm(xyz, ord=2, axis=1)
+        extra.append((np.asarray(depth, np.float32) / np.float32(70.0) - np.float32(0.5)).reshape(-1, 1))
     extra = np.concatenate(extra, axis=1)
     E = extra.shape[1]
     feats = np.asarray(scene["rpn_features"], np.float32)
@@ -271,10 +332,11 @@ def sample_scene(scene, cfg=None, draw="numpy", iou="exact", rng=np.random, seed
         return _ignored(out, 2, R, S, E, feats.shape[1])
     iou3d = iou_matrix(rois_all, gts_all, iou)
     max_overlaps, gt_assignment = iou3d.max(axis=1), iou3d.argmax(axis=1)
-    max_iou_of_gt, roi_assignment = iou3d.max(axis=0), iou3d.argmax(axis=0)
-    roi_assignment = roi_assignment[max_iou_of_gt > 0].reshape(-1)
     fg_thresh = min(c["REG_FG_THRESH"], c["CLS_FG_THRESH"])
-    fg_inds = np.concatenate((np.nonzero(max_overlaps >= fg_thresh)[0], roi_assignment), axis=0)
+    fg_inds = np.nonzero(max_overlaps >= fg_thresh)[0]
+    if rc["gt_max_fg"]:
+        max_iou_of_gt, roi_assignment = iou3d.max(axis=0), iou3d.argmax(axis=0)
+        fg_inds = np.concatenate((fg_inds, roi_assignment[max_iou_of_gt > 0].reshape(-1)), axis=0)
     easy = np.nonzero(max_overlaps < c["CLS_BG_THRESH_LO"])[0]
     hard = np.nonzero((max_overlaps < c["CLS_BG_THRESH"]) & (max_overlaps >= c["CLS_BG_THRESH_LO"]))[0]
     fg_num, bg_num = fg_inds.size, hard.size + easy.size
@@ -297,18 +359,20 @@ def sample_scene(scene, cfg=None, draw="numpy", iou="exact", rng=np.random, seed
     else:
         return _ignored(out, 1, R, S, E, feats.shape[1])
     sel = np.concatenate([fg_sel, bg_sel]).astype(np.int64)
-    pos_thresh = fg_thresh
     rois, ious, tries = np.zeros((R, 7), np.float32), np.zeros(R, np.float32), np.zeros(R, np.int64)
     gt_of_rois = gts_all[gt_assignment[sel]]
     for k in range(R):
         src, gt = rois_all[sel[k]].copy(), gt_of_rois[k]
-        times = FG_AUG_TIMES if k < fg_n else 1
-        temp_iou, cnt, box = 0, 0, src
-        while temp_iou < pos_thresh and cnt < times:
-            box = src if dr.keep(k, cnt) else dr.jitter(src, c["REG_AUG_METHOD"], k, cnt)
+        times = rc["fg_aug_times"] if k < fg_n else rc["bg_aug_times"]
+        temp_iou, cnt, box, keep = 0, 0, src, True
+        while temp_iou < fg_thresh and cnt < times:
+            keep = dr.keep(k, cnt)
+            box = src if keep else dr.jitter(src, c["REG_AUG_METHOD"], k, cnt)
             temp_iou = iou_matrix(box.reshape(1, 7), gt.reshape(1, 7), iou)[0][0]
             cnt += 1
-        rois[k], ious[k], tries[k] = box, temp_iou, cnt
+        rois[k], tries[k] = box, cnt
+        # no try, or the layer's kept source box: the source's max IoU
+        ious[k] = max_overlaps[sel[k]] if cnt == 0 or (rc["kept_src_iou"] and keep) else temp_iou
     out.update(sel=np.stack([sel, gt_assignment[sel], tries], 1).astype(np.int32), iou=ious, rois=rois.copy(), gt_of_rois=gt_of_rois.copy())
     # pooling in the original frame
     pool_boxes = enlarge_box3d(rois, c["POOL_EXTRA_WIDTH"])
@@ -329,21 +393,23 @@ def sample_scene(scene, cfg=None, draw="numpy", iou="exact", rng=np.random, seed
     pts_input, pts_features = pooled[:, :, :3 + E].copy(), pooled[:, :, 3 + E:].copy()
     out.update(pooled_input=pts_input.copy(), pooled_features=pts_features, empty=empty)
     if c["AUG_DATA"] and train:
+        if draw == "ref":
+            raise NotImplementedError("the reference layer's augmentation draws are batch-wide on the device generator")
         for k in range(R):
-            en, angle, scale = dr.aug(k, c)
+            en, angle, scale = dr.aug(k, rc["aug"])
             if draw == "numpy":
-                pts_input[k, :, 0:3], rois[k], gt_of_rois[k] = _augment_ref(pts_input[k, :, 0:3].copy(), rois[k], gt_of_rois[k], en, angle, scale, c)
+                pts_input[k, :, 0:3], rois[k], gt_of_rois[k] = _augment_ref(pts_input[k, :, 0:3].copy(), rois[k], gt_of_rois[k], en, angle, scale, rc["aug"])
             else:
-                pts_input[k, :, 0:3], rois[k], gt_of_rois[k] = _augment_f64(pts_input[k, :, 0:3], rois[k], gt_of_rois[k], en, angle, scale, c)
+                pts_input[k, :, 0:3], rois[k], gt_of_rois[k] = _augment_f64(pts_input[k, :, 0:3], rois[k], gt_of_rois[k], en, angle, scale, rc["aug"])
     valid = (empty == 0).astype(np.int32)
     reg_valid_mask = (ious > c["REG_FG_THRESH"]).astype(np.int32) & valid
     cls_label = (ious > c["CLS_FG_THRESH"]).astype(np.int32)
     cls_label[(ious > c["CLS_BG_THRESH"]) & (ious < c["CLS_FG_THRESH"])] = -1
     cls_label[valid == 0] = -1
-    if draw == "numpy":
-        pts_ct, gt_ct = _canonical_ref(pts_input, rois, gt_of_rois)
+    if draw == "hash":
+        pts_ct, gt_ct = _canonical_f64(pts_input, rois, gt_of_rois, rc["pts_raw_ry"])
     else:
-        pts_ct, gt_ct = _canonical_f64(pts_input, rois, gt_of_rois)
+        pts_ct, gt_ct = _canonical_ref(pts_input, rois, gt_of_rois, rc["pts_raw_ry"])
     out.update(pts_input=pts_ct, pts_features=pts_features, cls_label=cls_label, reg_valid_mask=reg_valid_mask, gt_boxes3d_ct=gt_ct,
                roi_boxes3d=rois, gt_boxes3d=gt_of_rois)
     return out
@@ -396,7 +462,9 @@ def _augment_ref(aug_pts, roi, gt, en, angle, scale, c):
     return aug_pts, boxes[0], boxes[1]
 
 
-def _canonical_ref(pts_input, rois, gt_of_rois):
+def _canonical_ref(pts_input, rois, gt_of_rois, raw_ry):
+    """canonical_transform_batch (the loader) and proposal_target_layer.py:45-56 (the layer, raw_ry: the points rotated by
+    the RoI's ry itself) with the reference's operations"""
     roi_ry = rois[:, 6] % (2 * np.pi)
     roi_center = rois[:, 0:3]
     pts_input[:, :, [0, 1, 2]] = pts_input[:, :, [0, 1, 2]] - roi_center.reshape(-1, 1, 3)
@@ -404,7 +472,7 @@ def _canonical_ref(pts_input, rois, gt_of_rois):
     gt_ct[:, 0:3] = gt_ct[:, 0:3] - roi_center
     gt_ct = rotate_pc_along_y_torch(torch.from_numpy(gt_ct.reshape(-1, 1, 7)), torch.from_numpy(roi_ry)).numpy().reshape(-1, 7)
     gt_ct[:, 6] = gt_ct[:, 6] - roi_ry
-    pts = rotate_pc_along_y_torch(torch.from_numpy(pts_input), torch.from_numpy(roi_ry)).numpy()
+    pts = rotate_pc_along_y_torch(torch.from_numpy(pts_input), torch.from_numpy(rois[:, 6].copy() if raw_ry else roi_ry)).numpy()
     return pts, gt_ct
 
 
@@ -438,12 +506,12 @@ def _augment_f64(pts, roi, gt, en, angle, scale, c):
     return p, rb, gb
 
 
-def _canonical_f64(pts_input, rois, gt_of_rois):
+def _canonical_f64(pts_input, rois, gt_of_rois, raw_ry):
     r = rois.astype(np.float64)
     roi_ry = np.mod(r[:, 6], 2 * np.pi)
     p = pts_input.astype(np.float64)
     p[:, :, 0:3] -= r[:, None, 0:3]
-    p[:, :, 0], p[:, :, 2] = _rot64(p[:, :, 0], p[:, :, 2], roi_ry[:, None])
+    p[:, :, 0], p[:, :, 2] = _rot64(p[:, :, 0], p[:, :, 2], (r[:, 6] if raw_ry else roi_ry)[:, None])
     g = gt_of_rois.astype(np.float64)
     g[:, 0:3] -= r[:, 0:3]
     g[:, 0], g[:, 2] = _rot64(g[:, 0], g[:, 2], roi_ry)

@@ -6,9 +6,8 @@
 //            thread per sampled RoI runs the jitter loop with the 3D IoU computed inline (iou3d_dev.cuh's iou3d_pair)
 //   targets  one CTA per sampled RoI: stage-2 data augmentation of the pooled points and both boxes, labels from the
 //            pre-augmentation IoU, canonical transform
-// The _ex entry points take the recipe's choices as values, which also serves the in-network target layer
-// (lib/rpn/proposal_target_layer.py, ROI_SAMPLE_JIT): no GT-max RoIs in the fg list, per-class try counts, the source IoU
-// for a kept box, GT counts from trailing zero rows, an asymmetric rotation interval, points rotated by the raw ry.
+// The entry points take the recipe's choices as values (RsCfg, RtCfg), so the same kernels also serve the in-network
+// target layer (lib/rpn/proposal_target_layer.py, ROI_SAMPLE_JIT); pointrcnn_b200/rcnn/targets.py holds both recipes.
 // Random draws are counter-based hashes keyed by (seed, scene, stage, roi, try, slot): the same distribution as the
 // reference's np.random stream, not the same stream.  oracle/rcnn_offline.py restates the keys, and the jitter arithmetic
 // below uses explicit _rn intrinsics so that an fp32 numpy restatement matches it bit for bit.
@@ -373,12 +372,12 @@ __global__ void __launch_bounds__(kRtThreads) rcnn_targets_kernel(
 
 using namespace prb;
 
-extern "C" int prb_rcnn_sample_rois_ex(int b, int m, int g, const float *iou, const float *rois, const int *roi_count,
-                                       const float *gt_boxes, const int *gt_count, int roi_per_image, int fg_per_image,
-                                       float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh, float cls_bg_thresh_lo,
-                                       double hard_bg_ratio, int aug_method, int gt_max_fg, int fg_aug_times, int bg_aug_times,
-                                       int kept_src_iou, float pool_extra_width, unsigned seed, float *rois_out, float *gt_out,
-                                       float *iou_out, float *pool_boxes, int *sel, int *status, void *stream) {
+extern "C" int prb_rcnn_sample_rois(int b, int m, int g, const float *iou, const float *rois, const int *roi_count,
+                                    const float *gt_boxes, const int *gt_count, int roi_per_image, int fg_per_image,
+                                    float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh, float cls_bg_thresh_lo,
+                                    double hard_bg_ratio, int aug_method, int gt_max_fg, int fg_aug_times, int bg_aug_times,
+                                    int kept_src_iou, float pool_extra_width, unsigned seed, float *rois_out, float *gt_out,
+                                    float *iou_out, float *pool_boxes, int *sel, int *status, void *stream) {
     PRB_REQUIRE(b > 0 && m >= 0 && g >= 0 && rois_out && gt_out && iou_out && pool_boxes && sel && status && (m == 0 || rois) &&
                     (g == 0 || gt_boxes) && (m == 0 || g == 0 || iou),
                 "rcnn_sample_rois: bad arguments");
@@ -400,23 +399,11 @@ extern "C" int prb_rcnn_sample_rois_ex(int b, int m, int g, const float *iou, co
     return check_launch("rcnn_sample_kernel");
 }
 
-// the loader's recipe: GT-max RoIs in the fg list, one try per bg row, the last box's IoU, counts given
-extern "C" int prb_rcnn_sample_rois(int b, int m, int g, const float *iou, const float *rois, const int *roi_count, const float *gt_boxes,
-                                    const int *gt_count, int roi_per_image, int fg_per_image, float reg_fg_thresh, float cls_fg_thresh,
-                                    float cls_bg_thresh, float cls_bg_thresh_lo, double hard_bg_ratio, int aug_method, int fg_aug_times,
-                                    float pool_extra_width, unsigned seed, float *rois_out, float *gt_out, float *iou_out,
-                                    float *pool_boxes, int *sel, int *status, void *stream) {
-    PRB_REQUIRE(roi_count && gt_count && fg_aug_times >= 1, "rcnn_sample_rois: bad arguments");
-    return prb_rcnn_sample_rois_ex(b, m, g, iou, rois, roi_count, gt_boxes, gt_count, roi_per_image, fg_per_image, reg_fg_thresh,
-                                   cls_fg_thresh, cls_bg_thresh, cls_bg_thresh_lo, hard_bg_ratio, aug_method, 1, fg_aug_times, 1, 0,
-                                   pool_extra_width, seed, rois_out, gt_out, iou_out, pool_boxes, sel, status, stream);
-}
-
-extern "C" int prb_rcnn_roi_targets_ex(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
-                                       const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
-                                       int aug_flip, float rot_lo, float rot_hi, float flip_prob, int pts_raw_ry, float reg_fg_thresh,
-                                       float cls_fg_thresh, float cls_bg_thresh, unsigned seed, float *gt_boxes_ct, int *cls_label,
-                                       int *reg_valid_mask, void *stream) {
+extern "C" int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
+                                    const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
+                                    int aug_flip, float rot_lo, float rot_hi, float flip_prob, int pts_raw_ry, float reg_fg_thresh,
+                                    float cls_fg_thresh, float cls_bg_thresh, unsigned seed, float *gt_boxes_ct, int *cls_label,
+                                    int *reg_valid_mask, void *stream) {
     PRB_REQUIRE(b > 0 && roi_per_image > 0 && S > 0 && W >= 3 && rows && rois && gt_boxes && iou && empty_flag && gt_boxes_ct &&
                     cls_label && reg_valid_mask,
                 "rcnn_roi_targets: bad arguments");
@@ -428,17 +415,4 @@ extern "C" int prb_rcnn_roi_targets_ex(int b, int roi_per_image, int S, int W, f
     rcnn_targets_kernel<<<b * roi_per_image, kRtThreads, 0, (cudaStream_t)stream>>>(roi_per_image, S, W, cf, rows, rois, gt_boxes, iou,
                                                                                       empty_flag, gt_boxes_ct, cls_label, reg_valid_mask);
     return check_launch("rcnn_targets_kernel");
-}
-
-// the loader's recipe: rotation U(-pi / aug_rot_range, pi / aug_rot_range), points and GT box rotated by ry mod 2 pi
-extern "C" int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
-                                    const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
-                                    int aug_flip, float aug_rot_range, float flip_prob, float reg_fg_thresh, float cls_fg_thresh,
-                                    float cls_bg_thresh, unsigned seed, float *gt_boxes_ct, int *cls_label, int *reg_valid_mask,
-                                    void *stream) {
-    PRB_REQUIRE(!aug_data || !aug_rotation || aug_rot_range > 0.f, "rcnn_roi_targets: AUG_ROT_RANGE must be > 0");
-    const float lo = aug_data && aug_rotation ? -(float)CUDART_PI / aug_rot_range : 0.f;     // IEEE division, as on the device
-    return prb_rcnn_roi_targets_ex(b, roi_per_image, S, W, rows, rois, gt_boxes, iou, empty_flag, aug_data, aug_rotation, aug_scaling,
-                                   aug_flip, lo, -lo, flip_prob, 0, reg_fg_thresh, cls_fg_thresh, cls_bg_thresh, seed, gt_boxes_ct,
-                                   cls_label, reg_valid_mask, stream);
 }

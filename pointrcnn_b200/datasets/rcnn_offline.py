@@ -22,22 +22,15 @@ save_rpn_features writes, for a whole batch.  Differences from the reference (IN
 the flat RoI layout, the fg-only branch, a status instead of pdb, roipool3d_kernel.cu's inside test.
 """
 import os
-import types
 
 import numpy as np
 import torch
 
 from .. import _cabi as C
+from ..rcnn import targets
+from ..rcnn.targets import AUG_METHODS, DEFAULT_CFG, ns as _ns  # the names this module has always exported
 from .kitti_eval import read_label_anno
 
-# tools/cfgs/default.yaml:6-9, :60-122
-DEFAULT_CFG = dict(AUG_DATA=True, AUG_METHOD_LIST=["rotation", "scaling", "flip"], AUG_METHOD_PROB=[1.0, 1.0, 0.5], AUG_ROT_RANGE=18,
-                   RCNN=dict(USE_INTENSITY=False, USE_DEPTH=True, USE_SEG_SCORE=False, POOL_EXTRA_WIDTH=1.0, NUM_POINTS=512,
-                             REG_AUG_METHOD="multiple", CLS_FG_THRESH=0.6, CLS_BG_THRESH=0.45, CLS_BG_THRESH_LO=0.05,
-                             REG_FG_THRESH=0.55, FG_RATIO=0.5, ROI_PER_IMAGE=64, HARD_BG_RATIO=0.8))
-AUG_METHODS = {"single": 0, "multiple": 1, "normal": 2}
-# aug_roi_by_noise_batch is called with aug_times=10 for the foreground rows (kitti_rcnn_dataset.py:942), not ROI_FG_AUG_TIMES
-FG_AUG_TIMES = 10
 # coordinate of padding points: outside every box (the inside test rejects |dx| > 10), and ignored by the bounds of
 # roipool3d's point grid, which only finite coordinates set
 FAR = float("inf")
@@ -52,10 +45,6 @@ def _pad(ts, n, value):
     """list of (n_k, c) tensors -> (len, n, c), rows n_k.. filled with value"""
     out = torch.nn.utils.rnn.pad_sequence(ts, batch_first=True, padding_value=value)
     return out if out.shape[1] == n else torch.nn.functional.pad(out, (0, 0, 0, n - out.shape[1]), value=value)
-
-
-def _ns(d):
-    return types.SimpleNamespace(**{k: (_ns(v) if isinstance(v, dict) else v) for k, v in d.items()})
 
 
 # ------------------------------------------------------------------------------------------------ files
@@ -314,44 +303,15 @@ class RCNNOfflineSampler:
         rows (K, NUM_POINTS, 3 + extra + C) the pooled buffer; pts_input / pts_features its [xyz | extra] / feature views;
         cls_label (K) int32, reg_valid_mask (K) int32, gt_boxes3d_ct (K,7), roi_boxes3d (K,7), roi_size (K,3), gt_boxes3d
         (K,7), gt_iou (K), sample_status (B) int32, sample_index (K,3) int32 [source RoI, GT, jitter tries]."""
-        cfg, r = self.cfg, self.cfg.RCNN
         B, N, M, G, Cf, pack = self._dims(scenes, "prepare_batch")
-        dev = self.device
-        E, R, S = self.num_extra, int(r.ROI_PER_IMAGE), int(r.NUM_POINTS)
-        with torch.cuda.device(dev):
+        recipe = targets.loader_recipe(self.cfg, mode)
+        E, R = self.num_extra, recipe.roi_per_image
+        with torch.cuda.device(self.device):
             xyz, feat, rois, gt, counts = pack(scenes, B, N, M, G, E, Cf)
-            L, st = C.lib(), C.stream()
-            iou = torch.empty((B, M, G), dtype=torch.float32, device=dev)
-            C.check(L.prb_boxes_iou3d(B, M, C.ptr(rois), G, C.ptr(gt), C.ptr(iou), st), "boxes_iou3d")
-            f = lambda *shp: torch.empty(shp, dtype=torch.float32, device=dev)
-            rois_out, gt_out, iou_out, pool_boxes = f(B, R, 7), f(B, R, 7), f(B, R), f(B, R, 7)
-            sel = torch.empty((B, R, 3), dtype=torch.int32, device=dev)
-            status = torch.empty(B, dtype=torch.int32, device=dev)
-            fg_quota = int(np.round(r.FG_RATIO * R))
-            C.check(L.prb_rcnn_sample_rois(B, M, G, C.ptr(iou), C.ptr(rois), C.ptr(counts[0]), C.ptr(gt), C.ptr(counts[1]), R, fg_quota,
-                                           r.REG_FG_THRESH, r.CLS_FG_THRESH, r.CLS_BG_THRESH, r.CLS_BG_THRESH_LO, r.HARD_BG_RATIO,
-                                           AUG_METHODS[r.REG_AUG_METHOD], FG_AUG_TIMES, r.POOL_EXTRA_WIDTH, seed & 0xffffffff,
-                                           C.ptr(rois_out), C.ptr(gt_out), C.ptr(iou_out), C.ptr(pool_boxes), C.ptr(sel), C.ptr(status),
-                                           st), "rcnn_sample_rois")
-            W = 3 + E + Cf
-            pooled = f(B, R, S, W)
-            empty = torch.zeros((B, R), dtype=torch.int32, device=dev)
-            wsb = L.prb_roipool3d_workspace_bytes(B, N, R, S)
-            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-            C.check(L.prb_roipool3d_ws(B, N, R, E + Cf, S, C.ptr(xyz), C.ptr(pool_boxes), C.ptr(feat), C.ptr(pooled), C.ptr(empty),
-                                       None, 1, C.ptr(ws), C.c_size_t(wsb), st), "roipool3d")
-            aug = bool(cfg.AUG_DATA) and mode == "TRAIN"
-            methods = list(cfg.AUG_METHOD_LIST)
-            gt_ct = f(B * R, 7)
-            cls = torch.empty(B * R, dtype=torch.int32, device=dev)
-            reg = torch.empty(B * R, dtype=torch.int32, device=dev)
-            C.check(L.prb_rcnn_roi_targets(B, R, S, W, C.ptr(pooled), C.ptr(rois_out), C.ptr(gt_out), C.ptr(iou_out), C.ptr(empty),
-                                           int(aug), int("rotation" in methods), int("scaling" in methods), int("flip" in methods),
-                                           float(cfg.AUG_ROT_RANGE), float(cfg.AUG_METHOD_PROB[2]), r.REG_FG_THRESH, r.CLS_FG_THRESH,
-                                           r.CLS_BG_THRESH, seed & 0xffffffff, C.ptr(gt_ct), C.ptr(cls), C.ptr(reg), st), "rcnn_roi_targets")
-        rows = pooled.view(B * R, S, W)
-        rois_flat = rois_out.view(B * R, 7)
-        return {"rows": rows, "pts_input": rows[..., :3 + E], "pts_features": rows[..., 3 + E:], "cls_label": cls,
-                "reg_valid_mask": reg, "gt_boxes3d_ct": gt_ct, "roi_boxes3d": rois_flat, "roi_size": rois_flat[:, 3:6],
-                "gt_boxes3d": gt_out.view(B * R, 7), "gt_iou": iou_out.view(B * R), "sample_status": status,
-                "sample_index": sel.view(B * R, 3), "pooled_empty_flag": empty.view(B * R)}
+            o = targets.run(recipe, xyz, feat, rois, gt, counts, seed)
+        rows = o["pooled"].view(B * R, recipe.num_points, 3 + E + Cf)
+        rois_flat = o["rois"].view(B * R, 7)
+        return {"rows": rows, "pts_input": rows[..., :3 + E], "pts_features": rows[..., 3 + E:], "cls_label": o["cls"],
+                "reg_valid_mask": o["reg"], "gt_boxes3d_ct": o["gt_ct"], "roi_boxes3d": rois_flat, "roi_size": rois_flat[:, 3:6],
+                "gt_boxes3d": o["gts"].view(B * R, 7), "gt_iou": o["iou"].view(B * R), "sample_status": o["status"],
+                "sample_index": o["sel"].view(B * R, 3), "pooled_empty_flag": o["empty"].view(B * R)}

@@ -20,17 +20,13 @@ Here:
     STREAM differs (one batched draw per round instead of per-RoI draws), so augmented boxes are equal in distribution,
     not bit for bit.
 With draw="device" (or draw=None and config switch target_draw = "device") the whole layer runs on the device without a
-host read: prb_boxes_iou3d, csrc/rcnn_sample.cu's sample stage in the layer's recipe (no GT-max RoIs in the fg list,
-ROI_FG_AUG_TIMES tries for fg rows and min(ROI_FG_AUG_TIMES, 1) for bg rows, the source IoU for a kept box, GT count from
-the trailing zero rows), prb_roipool3d_ws and the targets stage (rotation U[-pi / AUG_ROT_RANGE, 0), scaling, flip with
-p = 0.5, the points rotated by the augmented ry, the GT box by ry mod 2 pi).  Random draws are counter-based hashes of
+host read: rcnn/targets.py runs prb_boxes_iou3d, csrc/rcnn_sample.cu's sample stage, prb_roipool3d_ws and the targets
+stage in the layer's recipe (targets.layer_recipe).  Random draws are counter-based hashes of
 (seed, scene, stage, row, try, slot): the reference's distribution, not its stream.  The seed is the layer's call
 counter unless forward(..., seed=) gives one.  Extra output keys: sample_status (B) int32 (0 ok, 1 no fg and no bg RoI --
 the reference stops in pdb --, 2 no GT -- the reference raises; such a scene's rows have cls_label -1 and
 reg_valid_mask 0) and sample_index (B * ROI_PER_IMAGE, 3) int32 [source RoI, GT, jitter tries].
 """
-import types
-
 import numpy as np
 import torch
 import torch.nn as nn
@@ -38,22 +34,13 @@ import torch.nn as nn
 from .. import _cabi as C
 from .. import config, kitti_utils
 from ..ext import iou3d_cuda
+from ..rcnn import targets
+from ..rcnn.targets import AUG_METHODS, DEFAULT_CFG, ns as _ns  # noqa: F401  (the names this module has always exported)
 from ..roipool3d import roipool3d_utils
-
-# tools/cfgs/default.yaml:6-9, :60-122
-DEFAULT_CFG = dict(AUG_DATA=True, AUG_ROT_RANGE=18,
-                   RCNN=dict(USE_INTENSITY=False, USE_DEPTH=True, POOL_EXTRA_WIDTH=1.0, NUM_POINTS=512, REG_AUG_METHOD="multiple",
-                             ROI_FG_AUG_TIMES=10, CLS_FG_THRESH=0.6, CLS_BG_THRESH=0.45, CLS_BG_THRESH_LO=0.05, REG_FG_THRESH=0.55,
-                             FG_RATIO=0.5, ROI_PER_IMAGE=64, HARD_BG_RATIO=0.8))
 
 # REG_AUG_METHOD 'multiple' (proposal_target_layer.py:278-284): [pos_range, hwl_range, angle_range]
 _RANGE_CONFIG = [[0.2, 0.1, np.pi / 12], [0.3, 0.15, np.pi / 12], [0.5, 0.15, np.pi / 9], [0.8, 0.15, np.pi / 6], [1.0, 0.15, np.pi / 3]]
-AUG_METHODS = {"single": 0, "multiple": 1, "normal": 2}
 DRAWS = ("torch", "device")
-
-
-def _ns(d):
-    return types.SimpleNamespace(**{k: (_ns(v) if isinstance(v, dict) else v) for k, v in d.items()})
 
 
 def boxes_iou3d(boxes_a, boxes_b):
@@ -134,52 +121,18 @@ class ProposalTargetLayer(nn.Module):
         """forward() in four device launches and no host read: 3D IoU of every (RoI, GT) pair, the sample stage (selection +
         jitter loop), RoI pooling on the enlarged jittered boxes, the targets stage (augmentation, labels, canonical
         transform).  Same keys and shapes as the torch path, plus sample_status and sample_index."""
-        cfg, r = self.cfg, self.cfg.RCNN
-        if r.REG_AUG_METHOD not in AUG_METHODS:
-            raise NotImplementedError(r.REG_AUG_METHOD)
+        recipe = targets.layer_recipe(self.cfg)
         rois = input_dict['roi_boxes3d'][:, :, 0:7].contiguous().float()
         gts = input_dict['gt_boxes3d'][:, :, 0:7].contiguous().float()
         xyz = input_dict['rpn_xyz'].contiguous().float()
         C.require_cuda(rois, gts, xyz)
-        B, M, G, N = rois.shape[0], rois.shape[1], gts.shape[1], xyz.shape[1]
-        R, S = int(r.ROI_PER_IMAGE), int(r.NUM_POINTS)
-        dev = rois.device
-        with torch.cuda.device(dev):
+        with torch.cuda.device(rois.device):
             feat = self._pts_feature(input_dict).contiguous().float()
-            F_, W = feat.shape[2], 3 + feat.shape[2]
-            L, st = C.lib(), C.stream()
-            f = lambda *shp: torch.empty(shp, dtype=torch.float32, device=dev)
-            iou = f(B, M, G)
-            if M and G:
-                C.check(L.prb_boxes_iou3d(B, M, C.ptr(rois), G, C.ptr(gts), C.ptr(iou), st), "boxes_iou3d")
-            rois_out, gt_out, iou_out, pool_boxes = f(B, R, 7), f(B, R, 7), f(B, R), f(B, R, 7)
-            sel = torch.empty((B, R, 3), dtype=torch.int32, device=dev)
-            status = torch.empty(B, dtype=torch.int32, device=dev)
-            fg_times = int(r.ROI_FG_AUG_TIMES)
-            C.check(L.prb_rcnn_sample_rois_ex(B, M, G, C.ptr(iou), C.ptr(rois), None, C.ptr(gts), None, R, int(np.round(r.FG_RATIO * R)),
-                                              r.REG_FG_THRESH, r.CLS_FG_THRESH, r.CLS_BG_THRESH, r.CLS_BG_THRESH_LO, r.HARD_BG_RATIO,
-                                              AUG_METHODS[r.REG_AUG_METHOD], 0, fg_times, 1 if fg_times > 0 else 0, 1,
-                                              r.POOL_EXTRA_WIDTH, seed & 0xffffffff, C.ptr(rois_out), C.ptr(gt_out), C.ptr(iou_out),
-                                              C.ptr(pool_boxes), C.ptr(sel), C.ptr(status), st), "rcnn_sample_rois_ex")
-            pooled = f(B, R, S, W)
-            empty = torch.zeros((B, R), dtype=torch.int32, device=dev)
-            wsb = L.prb_roipool3d_workspace_bytes(B, N, R, S)
-            ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
-            C.check(L.prb_roipool3d_ws(B, N, R, F_, S, C.ptr(xyz), C.ptr(pool_boxes), C.ptr(feat), C.ptr(pooled), C.ptr(empty), None, 1,
-                                       C.ptr(ws), C.c_size_t(wsb), st), "roipool3d")
-            gt_ct = f(B * R, 7)
-            cls = torch.empty(B * R, dtype=torch.int32, device=dev)
-            reg = torch.empty(B * R, dtype=torch.int32, device=dev)
-            # (rand - 0.5 / 0.5) * (pi / AUG_ROT_RANGE) (:295): operator precedence makes it U(-pi / AUG_ROT_RANGE, 0)
-            lo = float(-np.float32(np.pi) / np.float32(cfg.AUG_ROT_RANGE))
-            C.check(L.prb_rcnn_roi_targets_ex(B, R, S, W, C.ptr(pooled), C.ptr(rois_out), C.ptr(gt_out), C.ptr(iou_out), C.ptr(empty),
-                                              int(bool(cfg.AUG_DATA)), 1, 1, 1, lo, 0.0, 0.5, 1, r.REG_FG_THRESH, r.CLS_FG_THRESH,
-                                              r.CLS_BG_THRESH, seed & 0xffffffff, C.ptr(gt_ct), C.ptr(cls), C.ptr(reg), st),
-                    "rcnn_roi_targets_ex")
-            rows = pooled.view(B * R, S, W)
-            return {'sampled_pts': rows[:, :, 0:3], 'pts_feature': rows[:, :, 3:], 'cls_label': cls.long(), 'reg_valid_mask': reg.long(),
-                    'gt_of_rois': gt_ct, 'gt_iou': iou_out.view(-1), 'roi_boxes3d': rois_out.view(-1, 7), 'sample_status': status,
-                    'sample_index': sel.view(-1, 3)}
+            o = targets.run(recipe, xyz, feat, rois, gts, None, seed)
+        rows = o["pooled"].view(-1, recipe.num_points, o["pooled"].shape[3])
+        return {'sampled_pts': rows[:, :, 0:3], 'pts_feature': rows[:, :, 3:], 'cls_label': o["cls"].long(), 'reg_valid_mask': o["reg"].long(),
+                'gt_of_rois': o["gt_ct"], 'gt_iou': o["iou"].view(-1), 'roi_boxes3d': o["rois"].view(-1, 7), 'sample_status': o["status"],
+                'sample_index': o["sel"].view(-1, 3)}
 
     # ------------------------------------------------------------------ sampling (:78-183)
     def sample_rois_for_rcnn(self, roi_boxes3d, gt_boxes3d):

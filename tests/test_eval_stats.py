@@ -241,10 +241,11 @@ def test_eval_stats_equals_the_golden(cuda, gold, name, batch):
 
 
 def _sampler(cuda, **kw):
-    from pointrcnn_b200.datasets.rcnn_offline import DEFAULT_CFG, RCNNOfflineSampler, _ns
+    from pointrcnn_b200.datasets.rcnn_offline import RCNNOfflineSampler
+    from pointrcnn_b200.rcnn.targets import DEFAULT_CFG, ns
     d = {k: v for k, v in DEFAULT_CFG.items() if k != "RCNN"}
     d["RCNN"] = dict(DEFAULT_CFG["RCNN"], **kw)
-    return RCNNOfflineSampler(cfg=_ns(d), device=cuda)
+    return RCNNOfflineSampler(cfg=ns(d), device=cuda)
 
 
 def _device_scenes(gold, cuda, n_feat=None):

@@ -164,10 +164,10 @@ TARGET_GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden
 
 
 def _target_cfg(aug_times, aug_data):
-    from pointrcnn_b200.rpn import proposal_target_layer as ptl
-    d = dict(ptl.DEFAULT_CFG, AUG_DATA=aug_data)
+    from pointrcnn_b200.rcnn.targets import DEFAULT_CFG, ns
+    d = dict(DEFAULT_CFG, AUG_DATA=aug_data)
     d["RCNN"] = dict(d["RCNN"], ROI_FG_AUG_TIMES=aug_times)
-    return ptl._ns(d)
+    return ns(d)
 
 
 @pytest.mark.gpu

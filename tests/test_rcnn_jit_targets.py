@@ -1,4 +1,4 @@
-"""RCNN targets of the in-network recipe (ROI_SAMPLE_JIT): the CPU restatement (tests/rcnn_jit_oracle.py) against what the
+"""RCNN targets of the in-network recipe (ROI_SAMPLE_JIT): the CPU restatement (oracle/rcnn_offline.py, recipe "layer") against what the
 reference's own ProposalTargetLayer produced (tests/golden/proposal_target_layer.npz), prepare_jit_batch's packing
 against collate_batch; on the GPU ProposalTargetLayer(draw="device") against the restatement with the device's keys,
 seeding, synchronisation, draw statistics and the training steps."""
@@ -9,7 +9,6 @@ import numpy as np
 import pytest
 import torch
 
-import rcnn_jit_oracle as JO
 from oracle import make_golden_proposal_target as MGT
 from oracle import make_golden_rcnn_offline as MG
 from oracle import rcnn_offline as RO
@@ -19,19 +18,27 @@ GOLD = os.path.join(ROOT, "tests", "golden", "proposal_target_layer.npz")
 SMALL = dict(NUM_POINTS=64, ROI_PER_IMAGE=32)
 
 
+def _layer_oracle(scene, cfg, draw, **kw):
+    """the layer's restatement of one scene, with its outputs under the layer's keys: sampled_pts (R,S,3) and pts_feature
+    (R,S,F) after the canonical transform, gt_of_rois_ct (R,7)"""
+    o = RO.sample_scene(scene, cfg, draw=draw, iou="fp32", recipe="layer", **kw)
+    return dict(o, sampled_pts=o["pts_input"][..., 0:3], pts_feature=np.concatenate([o["pooled_input"][..., 3:], o["pooled_features"]], axis=2),
+                gt_of_rois_ct=o["gt_boxes3d_ct"])
+
+
 # ------------------------------------------------------------------------------------------------ CPU
 def test_oracle_reproduces_the_reference_layer():
     g = np.load(GOLD)
     inp = MGT.inputs()
     np.random.seed(MGT.SEED)
     torch.manual_seed(MGT.SEED)
-    outs = [JO.sample_scene({k: v[b] for k, v in inp.items()}, dict(ROI_FG_AUG_TIMES=0, AUG_DATA=False), draw="ref") for b in range(2)]
+    outs = [_layer_oracle({k: v[b] for k, v in inp.items()}, dict(ROI_FG_AUG_TIMES=0, AUG_DATA=False), "ref") for b in range(2)]
     cat = lambda k: np.concatenate([o[k] for o in outs])
     for gk, ok in (("roi_boxes3d", "roi_boxes3d"), ("gt_iou", "iou"), ("gt_of_rois", "gt_of_rois_ct"), ("sampled_pts", "sampled_pts"),
                    ("pts_feature", "pts_feature"), ("cls_label", "cls_label"), ("reg_valid_mask", "reg_valid_mask")):
         np.testing.assert_array_equal(cat(ok).astype(g[gk].dtype), g[gk], err_msg=gk)
     # the fixture's GT lists are zero-padded (7 and 6 of 12 rows): the trimming decides the GT assignment
-    assert [len(JO.trimmed_gt(inp["gt_boxes3d"][b])) for b in range(2)] == [7, 6]
+    assert [len(RO.trimmed_gt(inp["gt_boxes3d"][b])) for b in range(2)] == [7, 6]
     assert (cat("sel")[:, 2] == 0).all() and {o["branch"] for o in outs} == {"fg+bg"}
 
 
@@ -78,11 +85,12 @@ def _scenes():
 
 
 def _layer(cuda, **kw):
-    from pointrcnn_b200.rpn.proposal_target_layer import DEFAULT_CFG, ProposalTargetLayer, _ns
+    from pointrcnn_b200.rcnn.targets import DEFAULT_CFG, ns
+    from pointrcnn_b200.rpn.proposal_target_layer import ProposalTargetLayer
     d = {k: v for k, v in DEFAULT_CFG.items() if k != "RCNN"}
     d["RCNN"] = dict(DEFAULT_CFG["RCNN"], **{k: v for k, v in kw.items() if k not in d})
     d.update({k: v for k, v in kw.items() if k in d})
-    return ProposalTargetLayer(cfg=_ns(d), draw="device")
+    return ProposalTargetLayer(cfg=ns(d), draw="device")
 
 
 def _batch(cuda, scenes):
@@ -116,7 +124,7 @@ def test_device_layer_matches_the_oracle(cuda, method):
     assert out["cls_label"].dtype == np.int64 and out["reg_valid_mask"].dtype == np.int64
     branches, padded = set(), 0
     for b, s in enumerate(scenes):
-        o = JO.sample_scene(_oracle_scene(batch, b, len(s["rpn_xyz"])), dict(REG_AUG_METHOD=method), draw="hash", seed=seed, scene_index=b)
+        o = _layer_oracle(_oracle_scene(batch, b, len(s["rpn_xyz"])), dict(REG_AUG_METHOD=method), "hash", seed=seed, scene_index=b)
         rows = slice(b * R, (b + 1) * R)
         assert out["sample_status"][b] == o["status"]
         branches.add(o["branch"])
@@ -152,8 +160,8 @@ def test_device_jitter_without_augmentation(cuda, method):
         out = _np(_layer(cuda, REG_AUG_METHOD=method, AUG_DATA=False)(batch, seed=8))
     R = 64
     for b, s in enumerate(scenes):
-        o = JO.sample_scene(_oracle_scene(batch, b, len(s["rpn_xyz"])), dict(REG_AUG_METHOD=method, AUG_DATA=False), draw="hash", seed=8,
-                            scene_index=b)
+        o = _layer_oracle(_oracle_scene(batch, b, len(s["rpn_xyz"])), dict(REG_AUG_METHOD=method, AUG_DATA=False), "hash", seed=8,
+                          scene_index=b)
         rows = slice(b * R, (b + 1) * R)
         if method != "normal":
             np.testing.assert_array_equal(out["roi_boxes3d"][rows], o["rois"])          # jittered boxes, bit for bit
@@ -172,8 +180,8 @@ def test_zero_aug_times_keeps_the_sources(cuda):
     R = 64
     rois = batch["roi_boxes3d"].cpu().numpy()
     for b, s in enumerate(scenes):
-        o = JO.sample_scene(_oracle_scene(batch, b, len(s["rpn_xyz"])), dict(ROI_FG_AUG_TIMES=0, AUG_DATA=False), draw="hash", seed=4,
-                            scene_index=b)
+        o = _layer_oracle(_oracle_scene(batch, b, len(s["rpn_xyz"])), dict(ROI_FG_AUG_TIMES=0, AUG_DATA=False), "hash", seed=4,
+                          scene_index=b)
         rows = slice(b * R, (b + 1) * R)
         np.testing.assert_array_equal(out["sample_index"][rows], o["sel"])
         assert (out["sample_index"][rows][:, 2] == 0).all()

@@ -124,10 +124,11 @@ def _scenes():
 
 
 def _sampler(method, cuda, **kw):
-    from pointrcnn_b200.datasets.rcnn_offline import DEFAULT_CFG, RCNNOfflineSampler, _ns
+    from pointrcnn_b200.datasets.rcnn_offline import RCNNOfflineSampler
+    from pointrcnn_b200.rcnn.targets import DEFAULT_CFG, ns
     d = {k: v for k, v in DEFAULT_CFG.items() if k != "RCNN"}
     d["RCNN"] = dict(DEFAULT_CFG["RCNN"], REG_AUG_METHOD=method, **{k: v for k, v in dict(RUN_CFG, **kw).items()})
-    return RCNNOfflineSampler(cfg=_ns(d), device=cuda)
+    return RCNNOfflineSampler(cfg=ns(d), device=cuda)
 
 
 def _np(batch):
@@ -205,6 +206,20 @@ def test_status_one_when_no_roi_is_fg_or_bg(cuda):
     out = _np(_sampler("multiple", cuda, CLS_BG_THRESH=0.0, CLS_BG_THRESH_LO=0.0).prepare_batch(scenes, seed=1))
     assert out["sample_status"].tolist() == [1]
     assert (out["cls_label"] == -1).all() and not out["reg_valid_mask"].any() and not out["rows"].any()
+
+
+@pytest.mark.gpu
+def test_non_positive_rotation_range_is_rejected(cuda):
+    smp = _sampler("multiple", cuda)
+    smp.cfg.AUG_ROT_RANGE = 0           # -pi / 0: the rotation interval is not finite
+    with pytest.raises(RuntimeError, match="rotation interval"):
+        smp.prepare_batch(_scenes()[:1], seed=1)
+
+
+def test_loader_recipe_requires_the_counts():
+    from pointrcnn_b200.rcnn import targets
+    with pytest.raises(ValueError, match="counts"):
+        targets.run(targets.loader_recipe(targets.ns(targets.DEFAULT_CFG), "TRAIN"), None, None, None, None, None, 0)
 
 
 @pytest.mark.gpu
