@@ -480,6 +480,58 @@ PRB_API int prb_eval_seg_iou(int b, int n, const int *pred, const int *label, fl
 PRB_API int prb_eval_cls_acc(int b, int m, const int *box_count, const int *pred_cls, const float *gt_iou, float cls_fg,
                              float cls_bg, float refined_thresh, float *acc, float *acc_refined, void *stream);
 
+/* ------------------------------------------------------------------ stage losses ------
+ * get_rpn_loss / get_rcnn_loss (lib/net/train_functions.py:55-209, lib/utils/loss_utils.py:7-233) and their gradients, for
+ * either stage.  The stage's choices come in a descriptor; [rpn] and [rcnn] name each stage's setting.
+ *
+ * Inputs, `rows` rows: cls (rows, num_class) logits, reg (rows, reg_cols), cls_label (rows) int32 or int64 (label_bytes 4 / 8)
+ * with -1 = ignored, reg_label (rows, 7) [dx, dy, dz, h, w, l, ry]; fg_mask (rows) int32 / int64, a row is foreground when
+ * > 0 [rcnn: reg_valid_mask], or NULL: foreground = cls_label > 0 [rpn].  The sigmoid losses take labels in {-1, 0, 1}.
+ * Size anchor: anchor_boxes (rows, 7), columns 3..5 per row [rcnn SIZE_RES_ON_ROI], or NULL: mean_size (3) on the device.
+ * ce_weight (num_class) on the device or NULL.  reg_cols must equal the width the options imply (get_reg_loss's assert).
+ *
+ * forward: two launches (a row pass writing per-CTA float64 partial sums into the workspace, one CTA summing them in a fixed
+ * order: no float atomics, the same inputs give the same bits).  total (1) = cls * loss_weight_cls + reg * loss_weight_reg;
+ * terms (PRB_SL_TERMS) at the PRB_SL_* slots: the classification term (focal: sum / max(#pos, 1); BCE, CE: sum over the
+ * rows with label >= 0 / max(their count, 1); Dice: 1 - sum min(p, t) / max(sum max(p, t), 1) over the rows with label != -1),
+ * reg = loc + angle + 3 size, every get_reg_loss mean over the foreground rows (exactly 0 without one), the focal sums of the
+ * positive / negative rows over the same normaliser, and the normalisers the backward reads.
+ * backward: one launch.  d_cls (rows, num_class) and d_reg (rows, reg_cols) are written densely (zero rows included, no
+ * memset needed), recomputed from the forward's inputs and its `terms`; grad_total (1) and grad_terms (PRB_SL_TERMS, the
+ * upstream gradient of every term slot) live on the device, either may be NULL (zero).  Neither entry allocates or
+ * synchronises.  The derivatives are torch autograd's for the mirror in pointrcnn_b200/train/losses.py, at its kinks too. */
+enum { PRB_LOSS_FOCAL = 0, PRB_LOSS_BCE = 1, PRB_LOSS_DICE = 2, PRB_LOSS_CE = 3 };
+enum { PRB_SL_CLS = 0, PRB_SL_REG, PRB_SL_X_BIN, PRB_SL_Z_BIN, PRB_SL_X_RES, PRB_SL_Z_RES, PRB_SL_Y_BIN, PRB_SL_Y_RES,
+       PRB_SL_Y_OFFSET, PRB_SL_RY_BIN, PRB_SL_RY_RES, PRB_SL_LOC, PRB_SL_ANGLE, PRB_SL_SIZE, PRB_SL_CLS_POS, PRB_SL_CLS_NEG,
+       PRB_SL_NORM,   /* the classification normaliser (focal: max(#pos, 1); BCE, CE: max(#valid, 1); Dice: max(sum max, 1)) */
+       PRB_SL_NFG,    /* number of foreground rows */
+       PRB_SL_DMIN, PRB_SL_DMAX,   /* Dice: sum min(p, t), sum max(p, t) */
+       PRB_SL_TERMS };
+typedef struct prb_stage_loss_desc {
+    int cls_loss;                /* PRB_LOSS_* [rpn focal / BCE / Dice, rcnn BCE / focal / CE] */
+    int num_class;               /* columns of cls: 1, or 2..16 for PRB_LOSS_CE */
+    double focal_alpha, focal_gamma;
+    double fg_weight;            /* BCE weight of the foreground rows [rpn 15, rcnn 1] */
+    double loss_weight_cls, loss_weight_reg;   /* [rpn RPN.LOSS_WEIGHT, rcnn 1, 1] */
+    double loc_scope, loc_bin_size;            /* x / z bins: int(loc_scope / loc_bin_size) * 2 */
+    int num_head_bin;
+    int xz_fine;                 /* [rpn LOC_XZ_FINE, rcnn 1] */
+    int y_by_bin;                /* [rpn 0, rcnn LOC_Y_BY_BIN] */
+    int ry_fine;                 /* heading folded into [0, pi) [rpn 0, rcnn 1] */
+    double loc_y_scope, loc_y_bin_size;
+} prb_stage_loss_desc;
+PRB_API size_t prb_stage_loss_workspace_bytes(int rows);
+PRB_API int prb_stage_loss_forward(const prb_stage_loss_desc *desc, int rows, int reg_cols, const float *cls, const float *reg,
+                                   const void *cls_label, int label_bytes, const void *fg_mask, int fg_mask_bytes,
+                                   const float *reg_label, const float *mean_size, const float *anchor_boxes,
+                                   const float *ce_weight, float *total, float *terms, void *workspace, size_t workspace_bytes,
+                                   void *stream);
+PRB_API int prb_stage_loss_backward(const prb_stage_loss_desc *desc, int rows, int reg_cols, const float *cls, const float *reg,
+                                    const void *cls_label, int label_bytes, const void *fg_mask, int fg_mask_bytes,
+                                    const float *reg_label, const float *mean_size, const float *anchor_boxes,
+                                    const float *ce_weight, const float *terms, const float *grad_total, const float *grad_terms,
+                                    float *d_cls, float *d_reg, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -21,6 +21,14 @@ class MlpDesc(ctypes.Structure):
                 ("packed_w", c_void_p), ("scale", c_void_p), ("shift", c_void_p), ("flags", c_int)]
 
 
+class StageLossDesc(ctypes.Structure):
+    """struct prb_stage_loss_desc"""
+    _fields_ = [("cls_loss", c_int), ("num_class", c_int), ("focal_alpha", ctypes.c_double), ("focal_gamma", ctypes.c_double),
+                ("fg_weight", ctypes.c_double), ("loss_weight_cls", ctypes.c_double), ("loss_weight_reg", ctypes.c_double),
+                ("loc_scope", ctypes.c_double), ("loc_bin_size", ctypes.c_double), ("num_head_bin", c_int), ("xz_fine", c_int),
+                ("y_by_bin", c_int), ("ry_fine", c_int), ("loc_y_scope", ctypes.c_double), ("loc_y_bin_size", ctypes.c_double)]
+
+
 class Options(ctypes.Structure):
     """struct prb_options (per-thread tuning block)"""
     _fields_ = [(k, c_int) for k in ("fps_cluster", "fps_prune", "fps_threads", "fps_generic", "mlp_gather", "mlp_ng", "mlp_occ",
@@ -60,7 +68,7 @@ def lib():
         for name in ("prb_nms_workspace_bytes", "prb_mlp_packed_bytes", "prb_mlp_packed_bytes_ex",
                      "prb_sa_workspace_bytes", "prb_fp_workspace_bytes", "prb_rows_workspace_bytes", "prb_rows2_workspace_bytes", "prb_grid_workspace_bytes",
                      "prb_fps_workspace_bytes", "prb_fps_ordered_workspace_bytes", "prb_kitti_format_detections", "prb_rpn_proposals_workspace_bytes", "prb_roipool3d_workspace_bytes",
-                     "prb_kitti_eval_workspace_bytes"):
+                     "prb_kitti_eval_workspace_bytes", "prb_stage_loss_workspace_bytes"):
             getattr(L, name).restype = c_size_t
         P, I, F, U = c_void_p, c_int, c_float, ctypes.c_uint
         L.prb_rcnn_sample_rois.argtypes = [I, I, I, P, P, P, P, P, I, I, F, F, F, F, ctypes.c_double, I, I, I, I, I, F, U, P, P, P, P, P, P,
@@ -68,6 +76,9 @@ def lib():
         L.prb_rcnn_roi_targets.argtypes = [I, I, I, I, P, P, P, P, P, I, I, I, I, F, F, F, I, F, F, F, U, P, P, P, P]
         L.prb_eval_box_recall.argtypes = [I, I, P, P, I, P, P, I, ctypes.POINTER(F), P, P, P, P]
         L.prb_eval_cls_acc.argtypes = [I, I, P, P, P, F, F, F, P, P, P]
+        L.prb_stage_loss_workspace_bytes.argtypes = [I]
+        L.prb_stage_loss_forward.argtypes = [P, I, I, P, P, P, I, P, I, P, P, P, P, P, P, P, c_size_t, P]
+        L.prb_stage_loss_backward.argtypes = [P, I, I, P, P, P, I, P, I, P, P, P, P, P, P, P, P, P, P]
         L.prb_options_init.restype = None
         L.prb_get_thread_options.restype = None
         if L.prb_abi_version() != 6:

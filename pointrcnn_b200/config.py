@@ -13,6 +13,8 @@ environment variables ONCE at import; at run time they are changed with `overrid
                     the proven-prefix shortcut of prb_furthest_point_sampling_ordered_ws (same indices), default on
     target_draw     which path ProposalTargetLayer(draw=None) takes: "torch" (the reference's random streams, default) or
                     "device" (csrc/rcnn_sample.cu's hashed draws, no host synchronisation)
+    loss_impl       which path train.losses.rpn_loss / rcnn_loss(impl=None) take: "torch" (the op-by-op mirror, default) or
+                    "device" (csrc/stage_loss.cu: two launches forward, one backward, no host synchronisation)
 """
 import contextlib
 import os
@@ -28,6 +30,7 @@ _DEFAULTS = dict(
     fp_project_min_rows=int(os.environ.get("PRB_FP_PROJECT_MIN_ROWS", "131072")),
     fps_ordered=os.environ.get("PRB_FPS_ORDERED", "1") != "0",
     target_draw=os.environ.get("PRB_TARGET_DRAW", "torch"),
+    loss_impl=os.environ.get("PRB_LOSS_IMPL", "torch"),
 )
 _local = threading.local()
 

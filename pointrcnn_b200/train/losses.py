@@ -1,14 +1,29 @@
 """Losses of the RPN / RCNN training step: mirror of lib/utils/loss_utils.py:7-233 (DiceLoss,
-SigmoidFocalClassificationLoss, get_reg_loss) and of get_rpn_loss in lib/net/train_functions.py:55-120.
+SigmoidFocalClassificationLoss, get_reg_loss) and of get_rpn_loss / get_rcnn_loss in lib/net/train_functions.py:55-209.
 
-Same arithmetic as the reference (the same torch ops in the same order per term); what differs is bookkeeping: the
-reference calls `.item()` on every partial loss (15+ host synchronisations per step, `loss_utils.py:127-128,...`,
-`train_functions.py:77-78,115-118`) -- here every term stays a device tensor and the caller reads what it logs once.
+Two implementations behind one signature, chosen by `impl` ("torch" / "device"; None follows the `loss_impl` switch of
+pointrcnn_b200.config, "torch" unless changed):
+
+- "torch": the same arithmetic as the reference (the same torch ops in the same order per term); what differs is
+  bookkeeping: the reference calls `.item()` on every partial loss (15+ host synchronisations per step,
+  `loss_utils.py:127-128,...`, `train_functions.py:77-78,115-118`) -- here every term stays a device tensor and the caller
+  reads what it logs once.  The foreground rows are still selected with boolean masks, one host synchronisation each.
+- "device": csrc/stage_loss.cu through a torch.autograd.Function: two launches forward, one backward, no host
+  synchronisation, the same (total, terms) keys for the same options (each term a 0-d device tensor), and the gradients
+  torch autograd derives for the mirror.  Values differ from the torch path in the last bits (float64 sums).  Without a
+  foreground row the regression terms are exact zeros here, where the torch path leaves their keys out.  CUDA tensors only.
 """
+import ctypes
+
 import numpy as np
 import torch
 import torch.nn as nn
 import torch.nn.functional as F
+
+from .. import _cabi as C
+from .. import config
+
+IMPLS = ("torch", "device")
 
 
 class DiceLoss(nn.Module):
@@ -111,11 +126,21 @@ def get_reg_loss(pred_reg, reg_label, loc_scope, loc_bin_size, num_head_bin, anc
     return loc_loss, angle_loss, size_loss, terms
 
 
+def _impl(impl):
+    impl = impl or config.get("loss_impl")
+    if impl not in IMPLS:
+        raise ValueError("loss_impl must be one of %s, not %r" % (IMPLS, impl))
+    return impl
+
+
 def rpn_loss(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, mean_size, loss_cls="SigmoidFocalLoss", focal_alpha=0.25, focal_gamma=2.0,
-             fg_weight=15.0, loc_scope=3.0, loc_bin_size=0.5, num_head_bin=12, loc_xz_fine=True, loss_weight=(1.0, 1.0)):
+             fg_weight=15.0, loc_scope=3.0, loc_bin_size=0.5, num_head_bin=12, loc_xz_fine=True, loss_weight=(1.0, 1.0), impl=None):
     """get_rpn_loss (train_functions.py:55-120).  rpn_cls (B,N,1), rpn_reg (B,N,C), rpn_cls_label (B,N) in {-1,0,1},
-    rpn_reg_label (B,N,7) -> total loss, dict of device tensors.  The foreground rows are selected with a boolean mask like
-    the reference (one data-dependent shape, no .item())."""
+    rpn_reg_label (B,N,7) -> total loss, dict of device tensors.  The torch path selects the foreground rows with a boolean
+    mask like the reference (one data-dependent shape, no .item()); impl: see the module docstring."""
+    if _impl(impl) == "device":
+        return _rpn_loss_device(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, mean_size, loss_cls, focal_alpha, focal_gamma, fg_weight,
+                                loc_scope, loc_bin_size, num_head_bin, loc_xz_fine, loss_weight)
     cls_label = rpn_cls_label.view(-1)
     cls_flat = rpn_cls.view(-1)
     fg_mask = cls_label > 0
@@ -150,9 +175,14 @@ def rpn_loss(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, mean_size, loss_cls
 
 def rcnn_loss(rcnn_cls, rcnn_reg, cls_label, reg_valid_mask, roi_boxes3d, gt_of_rois, mean_size, loss_cls="BinaryCrossEntropy",
               focal_alpha=0.25, focal_gamma=2.0, size_res_on_roi=False, loc_scope=1.5, loc_bin_size=0.5, num_head_bin=9,
-              loc_y_by_bin=False, loc_y_scope=0.5, loc_y_bin_size=0.25, ce_weight=None):
+              loc_y_by_bin=False, loc_y_scope=0.5, loc_y_bin_size=0.25, ce_weight=None, impl=None):
     """get_rcnn_loss (train_functions.py:121-209).  rcnn_cls (R,1|K), rcnn_reg (R,C), cls_label (R) in {-1,0,1},
-    reg_valid_mask (R), roi_boxes3d (R,7), gt_of_rois (R,7) canonical -> total loss, dict of device tensors (no .item())."""
+    reg_valid_mask (R), roi_boxes3d (R,7), gt_of_rois (R,7) canonical -> total loss, dict of device tensors (no .item()).
+    impl: see the module docstring."""
+    if _impl(impl) == "device":
+        return _rcnn_loss_device(rcnn_cls, rcnn_reg, cls_label, reg_valid_mask, roi_boxes3d, gt_of_rois, mean_size, loss_cls, focal_alpha,
+                                 focal_gamma, size_res_on_roi, loc_scope, loc_bin_size, num_head_bin, loc_y_by_bin, loc_y_scope,
+                                 loc_y_bin_size, ce_weight)
     R = rcnn_reg.shape[0]
     label = cls_label.float().view(-1)
     terms = {}
@@ -190,4 +220,132 @@ def rcnn_loss(rcnn_cls, rcnn_reg, cls_label, reg_valid_mask, roi_boxes3d, gt_of_
         loss_r = loss_c * 0
     total = loss_c + loss_r
     terms.update(rcnn_loss_cls=loss_c, rcnn_loss_reg=loss_r, rcnn_loss=total)
+    return total, terms
+
+
+# ---------------------------------------------------------------------------------------------- the device path
+# slots of the loss vector (include/pointrcnn_b200.h: PRB_SL_*)
+_SLOT = dict(loss_cls=0, loss_reg=1, loss_x_bin=2, loss_z_bin=3, loss_x_res=4, loss_z_res=5, loss_y_bin=6, loss_y_res=7, loss_y_offset=8,
+             loss_ry_bin=9, loss_ry_res=10, loss_loc=11, loss_angle=12, loss_size=13, cls_pos=14, cls_neg=15)
+_NUM_SLOTS = 20
+_CLS_CODE = {"SigmoidFocalLoss": 0, "BinaryCrossEntropy": 1, "DiceLoss": 2, "CrossEntropy": 3}
+
+
+class _StageLoss(torch.autograd.Function):
+    """(cls, reg) -> (total 0-d, loss vector) through prb_stage_loss_forward; backward through prb_stage_loss_backward, which
+    takes the upstream gradient of the total and of every slot of the vector (either may be absent) on the device"""
+
+    @staticmethod
+    def forward(ctx, cls, reg, desc, label, fg_mask, reg_label, mean_size, anchor_boxes, ce_weight):
+        L = C.lib()
+        rows = reg.shape[0]
+        total = torch.empty((), dtype=torch.float32, device=reg.device)
+        vec = torch.empty(_NUM_SLOTS, dtype=torch.float32, device=reg.device)
+        ws = torch.empty(L.prb_stage_loss_workspace_bytes(rows), dtype=torch.uint8, device=reg.device)
+        with torch.cuda.device(reg.device):
+            C.check(L.prb_stage_loss_forward(ctypes.byref(desc), rows, reg.shape[1], C.ptr(cls), C.ptr(reg), C.ptr(label), label.element_size(),
+                                             C.ptr(fg_mask), 0 if fg_mask is None else fg_mask.element_size(), C.ptr(reg_label),
+                                             C.ptr(mean_size), C.ptr(anchor_boxes), C.ptr(ce_weight), C.ptr(total), C.ptr(vec), C.ptr(ws),
+                                             ws.numel(), C.stream()), "stage_loss_forward")
+        ctx.desc = desc
+        ctx.save_for_backward(cls, reg, label, fg_mask, reg_label, mean_size, anchor_boxes, ce_weight, vec)
+        ctx.set_materialize_grads(False)
+        return total, vec
+
+    @staticmethod
+    def backward(ctx, g_total, g_vec):
+        cls, reg, label, fg_mask, reg_label, mean_size, anchor_boxes, ce_weight, vec = ctx.saved_tensors
+        if g_total is None and g_vec is None:
+            return (None,) * 9
+        g_total = None if g_total is None else g_total.float().contiguous()
+        g_vec = None if g_vec is None else g_vec.float().contiguous()
+        d_cls, d_reg = torch.empty_like(cls), torch.empty_like(reg)
+        with torch.cuda.device(reg.device):
+            C.check(C.lib().prb_stage_loss_backward(ctypes.byref(ctx.desc), reg.shape[0], reg.shape[1], C.ptr(cls), C.ptr(reg), C.ptr(label),
+                                                    label.element_size(), C.ptr(fg_mask), 0 if fg_mask is None else fg_mask.element_size(),
+                                                    C.ptr(reg_label), C.ptr(mean_size), C.ptr(anchor_boxes), C.ptr(ce_weight), C.ptr(vec),
+                                                    C.ptr(g_total), C.ptr(g_vec), C.ptr(d_cls), C.ptr(d_reg), C.stream()),
+                    "stage_loss_backward")
+        return d_cls, d_reg, None, None, None, None, None, None, None
+
+
+def _f32(t, what):
+    C.require_cuda(t)
+    if t.dtype != torch.float32:
+        raise TypeError("device loss: %s must be float32, not %s" % (what, t.dtype))
+    return t.contiguous()
+
+
+def _int_rows(t, n, what):
+    """int32 / int64 rows as they are; another dtype as the mirror reads it (label.float() compared with 0, or mask > 0)"""
+    C.require_cuda(t)
+    t = t.reshape(-1)
+    if t.numel() != n:
+        raise ValueError("device loss: %s has %d rows, the regression input %d" % (what, t.numel(), n))
+    if t.dtype not in (torch.int32, torch.int64):
+        t = t.long() if what == "labels" else (t > 0).to(torch.int32)
+    return t.contiguous()
+
+
+def _reg_keys(xz_fine, y_by_bin):
+    keys = ["loss_x_bin", "loss_z_bin"] + (["loss_x_res", "loss_z_res"] if xz_fine else [])
+    keys += ["loss_y_bin", "loss_y_res"] if y_by_bin else ["loss_y_offset"]
+    return keys + ["loss_ry_bin", "loss_ry_res", "loss_loc", "loss_angle", "loss_size"]
+
+
+def _desc(loss_cls, num_class, focal_alpha, focal_gamma, fg_weight, loss_weight, loc_scope, loc_bin_size, num_head_bin, xz_fine, y_by_bin,
+          ry_fine, loc_y_scope, loc_y_bin_size):
+    if focal_alpha is None:
+        raise NotImplementedError("device loss: focal_alpha=None")
+    return C.StageLossDesc(cls_loss=_CLS_CODE[loss_cls], num_class=num_class, focal_alpha=focal_alpha, focal_gamma=focal_gamma or 0.0,
+                           fg_weight=fg_weight, loss_weight_cls=loss_weight[0], loss_weight_reg=loss_weight[1], loc_scope=loc_scope,
+                           loc_bin_size=loc_bin_size, num_head_bin=num_head_bin, xz_fine=int(bool(xz_fine)), y_by_bin=int(bool(y_by_bin)),
+                           ry_fine=int(bool(ry_fine)), loc_y_scope=loc_y_scope, loc_y_bin_size=loc_y_bin_size)
+
+
+def _mean_size(mean_size, device):
+    return torch.as_tensor(mean_size, dtype=torch.float32, device=device).reshape(3).contiguous()
+
+
+def _rpn_loss_device(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, mean_size, loss_cls, focal_alpha, focal_gamma, fg_weight, loc_scope,
+                     loc_bin_size, num_head_bin, loc_xz_fine, loss_weight):
+    if loss_cls not in ("SigmoidFocalLoss", "DiceLoss", "BinaryCrossEntropy"):
+        raise NotImplementedError(loss_cls)
+    npts = rpn_reg.size(0) * rpn_reg.size(1)
+    reg = _f32(rpn_reg, "rpn_reg").view(npts, -1)
+    cls = _f32(rpn_cls, "rpn_cls").view(npts, 1)
+    label = _int_rows(rpn_cls_label, npts, "labels")
+    reg_label = _f32(rpn_reg_label, "rpn_reg_label").view(npts, 7)
+    desc = _desc(loss_cls, 1, focal_alpha, focal_gamma, fg_weight, loss_weight, loc_scope, loc_bin_size, num_head_bin, loc_xz_fine, False,
+                 False, 0.5, 0.25)
+    total, vec = _StageLoss.apply(cls, reg, desc, label, None, reg_label, _mean_size(mean_size, reg.device), None, None)
+    terms = {k: vec[_SLOT[k]] for k in _reg_keys(loc_xz_fine, False)}
+    terms.update(rpn_loss_cls=vec[_SLOT["loss_cls"]], rpn_loss_reg=vec[_SLOT["loss_reg"]], rpn_loss=total)
+    return total, terms
+
+
+def _rcnn_loss_device(rcnn_cls, rcnn_reg, cls_label, reg_valid_mask, roi_boxes3d, gt_of_rois, mean_size, loss_cls, focal_alpha, focal_gamma,
+                      size_res_on_roi, loc_scope, loc_bin_size, num_head_bin, loc_y_by_bin, loc_y_scope, loc_y_bin_size, ce_weight):
+    if loss_cls not in ("SigmoidFocalLoss", "BinaryCrossEntropy", "CrossEntropy"):
+        raise NotImplementedError(loss_cls)
+    R = rcnn_reg.shape[0]
+    reg = _f32(rcnn_reg, "rcnn_reg").view(R, -1)
+    cls = _f32(rcnn_cls, "rcnn_cls").view(R, -1)
+    if loss_cls != "CrossEntropy" and cls.shape[1] != 1:
+        raise ValueError("device loss: %s takes one logit per RoI, not %d" % (loss_cls, cls.shape[1]))
+    label = _int_rows(cls_label, R, "labels")
+    fg = _int_rows(reg_valid_mask, R, "reg_valid_mask")
+    gt = _f32(gt_of_rois, "gt_of_rois").view(R, 7)
+    anchor = _f32(roi_boxes3d, "roi_boxes3d").view(R, 7) if size_res_on_roi else None
+    w = None if ce_weight is None or loss_cls != "CrossEntropy" else _f32(ce_weight, "ce_weight").view(-1)
+    if w is not None and w.numel() != cls.shape[1]:
+        raise ValueError("device loss: %d class weights for %d classes" % (w.numel(), cls.shape[1]))
+    desc = _desc(loss_cls, cls.shape[1], focal_alpha, focal_gamma, 1.0, (1.0, 1.0), loc_scope, loc_bin_size, num_head_bin, True, loc_y_by_bin,
+                 True, loc_y_scope, loc_y_bin_size)
+    total, vec = _StageLoss.apply(cls, reg, desc, label, fg, gt, _mean_size(mean_size, reg.device), anchor, w)
+    terms = {}
+    if loss_cls == "SigmoidFocalLoss":
+        terms["rpn_loss_cls_pos"], terms["rpn_loss_cls_neg"] = vec[_SLOT["cls_pos"]], vec[_SLOT["cls_neg"]]     # the reference's key names
+    terms.update({k: vec[_SLOT[k]] for k in _reg_keys(True, loc_y_by_bin)})
+    terms.update(rcnn_loss_cls=vec[_SLOT["loss_cls"]], rcnn_loss_reg=vec[_SLOT["loss_reg"]], rcnn_loss=total)
     return total, terms

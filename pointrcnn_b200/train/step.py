@@ -18,7 +18,9 @@ from .losses import rcnn_loss, rpn_loss
 
 
 class RPNTrainer:
-    def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0):
+    """loss_impl: which stage-loss path forward_loss takes ("torch" / "device", see train.losses; None: the config switch)"""
+
+    def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, loss_impl=None):
         torch.manual_seed(seed)                       # identical initial weights on every rank
         self.device = torch.device(device)
         self.model = RPNStage(input_channels=input_channels, mode="TRAIN").to(self.device).train()
@@ -27,13 +29,14 @@ class RPNTrainer:
         fused = self.device.type == "cuda"
         self.opt = torch.optim.Adam(self.params, lr=lr, weight_decay=weight_decay, **({"fused": True} if fused else {}))
         self.mean_size = torch.from_numpy(CLS_MEAN_SIZE[0]).to(self.device)
+        self.loss_impl = loss_impl
 
     def forward_loss(self, pts_input, rpn_cls_label, rpn_reg_label):
         m = self.model
         xyz, feats = m.backbone_net(pts_input)
         rpn_cls = m.rpn_cls_layer(feats).transpose(1, 2).contiguous()       # lib/net/rpn.py:76-77
         rpn_reg = m.rpn_reg_layer(feats).transpose(1, 2).contiguous()
-        return rpn_loss(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, self.mean_size)
+        return rpn_loss(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, self.mean_size, impl=self.loss_impl)
 
     def step(self, pts_input, rpn_cls_label, rpn_reg_label, grad_norm_clip=None):
         self.reducer.reset()
@@ -65,10 +68,11 @@ class RCNNTrainer:
     cfg.RPN.FIXED): the RPN stage runs in eval mode without grad on the fused path and hands (rois, point features, mask,
     depth) to the RCNN stage, whose target layer samples 64 RoIs per scene; forward / backward of the RCNN network on the
     op-by-op path, get_rcnn_loss, bucketed gradient all-reduce, optimizer step.  target_draw: how the target layer samples
-    ("torch": the reference's random calls, "device": one device pass without host reads; None: the config switch)."""
+    ("torch": the reference's random calls, "device": one device pass without host reads; None: the config switch).  loss_impl:
+    which stage-loss path every forward_loss* method takes ("torch" / "device", see train.losses; None: the config switch)."""
 
     def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, rpn_score_thresh=0.3,
-                 target_draw=None):
+                 target_draw=None, loss_impl=None):
         from ..rcnn.stage import RCNNStage
         torch.manual_seed(seed)
         self.device = torch.device(device)
@@ -82,6 +86,7 @@ class RCNNTrainer:
         self.mean_size = torch.from_numpy(CLS_MEAN_SIZE[0]).to(self.device)
         self.rpn_score_thresh = rpn_score_thresh
         self.target_draw = target_draw
+        self.loss_impl = loss_impl
 
     @torch.no_grad()
     def rpn_outputs(self, pts_input, gt_boxes3d):
@@ -100,7 +105,8 @@ class RCNNTrainer:
         c = self.model.cfg
         return rcnn_loss(ret["rcnn_cls"], ret["rcnn_reg"], ret["cls_label"], ret["reg_valid_mask"], ret["roi_boxes3d"], ret["gt_of_rois"],
                          self.mean_size, loc_scope=c["LOC_SCOPE"], loc_bin_size=c["LOC_BIN_SIZE"], num_head_bin=c["NUM_HEAD_BIN"],
-                         loc_y_by_bin=c["LOC_Y_BY_BIN"], loc_y_scope=c["LOC_Y_SCOPE"], loc_y_bin_size=c["LOC_Y_BIN_SIZE"])
+                         loc_y_by_bin=c["LOC_Y_BY_BIN"], loc_y_scope=c["LOC_Y_SCOPE"], loc_y_bin_size=c["LOC_Y_BIN_SIZE"],
+                         impl=self.loss_impl)
 
     def forward_loss_offline(self, batch):
         """the ROI_SAMPLE_JIT=False branch of rcnn_net.forward (:155-163) + get_rcnn_loss on a batch of
@@ -110,7 +116,8 @@ class RCNNTrainer:
         c = self.model.cfg
         return rcnn_loss(rcnn_cls, rcnn_reg, batch["cls_label"], batch["reg_valid_mask"], batch["roi_boxes3d"], batch["gt_boxes3d_ct"],
                          self.mean_size, loc_scope=c["LOC_SCOPE"], loc_bin_size=c["LOC_BIN_SIZE"], num_head_bin=c["NUM_HEAD_BIN"],
-                         loc_y_by_bin=c["LOC_Y_BY_BIN"], loc_y_scope=c["LOC_Y_SCOPE"], loc_y_bin_size=c["LOC_Y_BIN_SIZE"])
+                         loc_y_by_bin=c["LOC_Y_BY_BIN"], loc_y_scope=c["LOC_Y_SCOPE"], loc_y_bin_size=c["LOC_Y_BIN_SIZE"],
+                         impl=self.loss_impl)
 
     def step_offline(self, batch, grad_norm_clip=None):
         """one offline-recipe training step (tools/train_rcnn.py --train_mode rcnn_offline) on a prepared batch"""
