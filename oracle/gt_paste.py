@@ -142,7 +142,8 @@ def paste_in_box(pts, box):
     cx, by, cz, h, w, l, ang = [np.float32(v) for v in box]
     cy = np.float32(np.float64(by) - np.float64(h) / 2.0)
     dx, dz = x - cx, z - cz
-    ok = (np.abs(dx) <= np.float32(10.0)) & (np.abs(y - cy).astype(np.float64) <= np.float64(h) / 2.0) & (np.abs(dz) <= np.float32(10.0))
+    # the source's rejecting form: a NaN difference or height passes these tests and leaves the decision to the rotation
+    ok = ~((np.abs(dx) > np.float32(10.0)) | (np.abs(y - cy).astype(np.float64) > np.float64(h) / 2.0) | (np.abs(dz) > np.float32(10.0)))
     cosa, sina = np.float32(np.cos(np.float64(ang))), np.float32(np.sin(np.float64(ang)))
     x_rot = dx * cosa + dz * (-sina)
     z_rot = dx * sina + dz * cosa

@@ -81,7 +81,9 @@ def in_box(pts, box):
     dx, dy, dz = pts[:, 0] - x, pts[:, 1] - y, pts[:, 2] - z
     c, s = np.float32(np.cos(ry)), np.float32(np.sin(ry))
     xc, zc = dx * c - dz * s, dx * s + dz * c
-    return (dy <= 0) & (dy >= -h) & (np.abs(xc) <= l * np.float32(0.5)) & (np.abs(zc) <= w * np.float32(0.5))
+    # the y tests in the device kernel's rejecting form, so a NaN height leaves the decision to x and z as on the device (the
+    # reference's Delaunay hull has no defined answer for a non-finite box)
+    return ~((dy > 0) | (dy < -h)) & (np.abs(xc) <= l * np.float32(0.5)) & (np.abs(zc) <= w * np.float32(0.5))
 
 
 def rpn_training_labels(pts_rect, gt_boxes3d, extra=0.2):

@@ -42,7 +42,6 @@ def lib():
         _LIB.orc_box_overlap.restype = c_float
         _LIB.orc_iou_bev.restype = c_float
         _LIB.orc_iou_normal.restype = c_float
-        _LIB.orc_pt_in_box3d_margin.restype = c_float
     return _LIB
 
 
@@ -170,16 +169,6 @@ def pts_in_boxes3d(pts, boxes3d):
     flag = np.zeros((M, N), dtype=np.int64)
     lib().orc_pts_in_boxes3d(N, M, _p(pts), _p(boxes3d), _p(flag))
     return flag
-
-
-def pts_in_boxes3d_margin(pts, boxes3d):
-    pts, boxes3d = _f32(pts), _f32(boxes3d)
-    out = np.empty((boxes3d.shape[0], pts.shape[0]), dtype=np.float32)
-    L = lib()
-    for i, b in enumerate(boxes3d):
-        for j, p in enumerate(pts):
-            out[i, j] = L.orc_pt_in_box3d_margin(*(c_float(float(v)) for v in (p[0], p[1], p[2], *b)))
-    return out
 
 
 def roipool3d(xyz, pts_feature, boxes3d, sampled_pt_num=512):

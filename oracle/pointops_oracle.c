@@ -262,23 +262,6 @@ ORC_API int orc_pt_in_box3d(float x, float y, float z, float cx, float bottom_y,
     return (x_rot >= -l / 2.0) & (x_rot <= l / 2.0) & (z_rot >= -w / 2.0) & (z_rot <= w / 2.0);
 }
 
-/* margin (metres) of a point to the nearest decision boundary of the predicate; tests use it
- * to exclude borderline points when comparing host-libm flags with device flags */
-ORC_API float orc_pt_in_box3d_margin(float x, float y, float z, float cx, float bottom_y, float cz,
-                                     float h, float w, float l, float angle) {
-    double cy = bottom_y - h / 2.0;
-    double dx = (double)x - cx, dz = (double)z - cz, dy = (double)y - cy;
-    double ca = cos((double)angle), sa = sin((double)angle);
-    double xr = dx * ca - dz * sa, zr = dx * sa + dz * ca;
-    double mg = fabs(fabs(dx) - 10.0);
-    double t;
-    t = fabs(fabs(dz) - 10.0); if (t < mg) mg = t;
-    t = fabs(fabs(dy) - h / 2.0); if (t < mg) mg = t;
-    t = fabs(fabs(xr) - l / 2.0); if (t < mg) mg = t;
-    t = fabs(fabs(zr) - w / 2.0); if (t < mg) mg = t;
-    return (float)mg;
-}
-
 ORC_API void orc_pts_in_boxes3d(int n, int m, const float *pts, const float *boxes, int64_t *flag) {
 #pragma omp parallel for
     for (int i = 0; i < m; ++i)

@@ -54,8 +54,9 @@ def _in_box_np(pts, box):
     x, y, z = pts[:, 0], pts[:, 1], pts[:, 2]
     cx, by, cz, h, w, l, ang = [np.float32(v) for v in box]
     cy = np.float32(np.float64(by) - np.float64(h) / 2.0)
-    ok = (np.abs(x - cx) <= np.float32(10.0)) & (np.abs(y - cy).astype(np.float64) <= np.float64(h) / 2.0) & \
-         (np.abs(z - cz) <= np.float32(10.0))
+    # the source's rejecting form: a NaN difference or height passes these tests and leaves the decision to the rotation
+    ok = ~((np.abs(x - cx) > np.float32(10.0)) | (np.abs(y - cy).astype(np.float64) > np.float64(h) / 2.0) |
+           (np.abs(z - cz) > np.float32(10.0)))
     cosa, sina = np.float32(np.cos(ang)), np.float32(np.sin(ang))
     x_rot = (x - cx) * cosa + (z - cz) * (-sina)
     z_rot = (x - cx) * sina + (z - cz) * cosa

@@ -84,8 +84,8 @@ def run(recipe, xyz, feat, rois, gts, counts, seed):
     or G is 0), prb_rcnn_sample_rois, prb_roipool3d_ws on the enlarged sampled boxes, prb_rcnn_roi_targets.
     xyz (B,N,3), feat (B,N,F), rois (B,M,7), gts (B,G,7): contiguous float32 CUDA tensors; counts (2,B) int32
     [roi_count; gt_count], required by a recipe with counts and ignored otherwise.  -> dict of the raw outputs, R =
-    ROI_PER_IMAGE, S = NUM_POINTS: pooled (B,R,S,3+F) transformed rows, empty (B,R) int32, rois / gts (B,R,7) after
-    augmentation, iou (B,R) before it, sel (B,R,3) int32, status (B) int32, gt_ct (B*R,7), cls / reg (B*R) int32"""
+    ROI_PER_IMAGE, S = NUM_POINTS: pooled (B,R,S,3+F) transformed rows, empty (B,R) int32, pool_boxes (B,R,7) the boxes the
+    rows were pooled from, rois / gts (B,R,7) after augmentation, iou (B,R) before it, sel (B,R,3) int32, status (B) int32, gt_ct (B*R,7), cls / reg (B*R) int32"""
     if recipe.counts and counts is None:
         raise ValueError("rcnn targets: this recipe takes the RoI and GT counts")
     rc = recipe
@@ -119,4 +119,4 @@ def run(recipe, xyz, feat, rois, gts, counts, seed):
                                    rc.aug_rotation, rc.aug_scaling, rc.aug_flip, rc.rot_lo, rc.rot_hi, rc.flip_prob, rc.pts_raw_ry,
                                    rc.reg_fg_thresh, rc.cls_fg_thresh, rc.cls_bg_thresh, seed, C.ptr(gt_ct), C.ptr(cls), C.ptr(reg), st),
             "rcnn_roi_targets")
-    return dict(pooled=pooled, empty=empty, rois=rois_out, gts=gt_out, iou=iou_out, sel=sel, status=status, gt_ct=gt_ct, cls=cls, reg=reg)
+    return dict(pooled=pooled, empty=empty, pool_boxes=pool_boxes, rois=rois_out, gts=gt_out, iou=iou_out, sel=sel, status=status, gt_ct=gt_ct, cls=cls, reg=reg)

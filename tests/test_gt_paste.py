@@ -7,6 +7,7 @@ import types
 import numpy as np
 import pytest
 
+import inbox_reference as IR
 from oracle import gt_paste as GP
 from oracle import kitti_io as KO
 
@@ -48,11 +49,10 @@ def _gt_database(db=None):
     return GTDatabase.from_reference([dict(e, obj=types.SimpleNamespace(alpha=e["alpha"])) for e in db])
 
 
-def _label_agreement(cls_a, reg_a, cls_b, reg_b, max_frac):
-    diff = cls_a != cls_b
-    assert diff.mean() <= max_frac, "label mismatch fraction %g" % diff.mean()
-    same = ~diff
-    np.testing.assert_allclose(reg_a[same], reg_b[same], rtol=0, atol=1e-6)
+def _labels_in_band(cls, reg, pts, gt, delaunay=False, where=""):
+    """every label agrees with the float64 replay of generate_rpn_training_labels outside the band of its decisions"""
+    gt = np.asarray(gt, np.float32).reshape(-1, 7)
+    IR.check_labels(cls, reg, np.asarray(pts)[:, :3], gt, count=len(gt), delaunay=delaunay, where=where)
 
 
 def _oracle(s, rng):
@@ -69,7 +69,9 @@ def test_oracle_reproduces_the_reference_gt_paste(gold):
         np.testing.assert_allclose(o["pts_input"], gold["train%d_pts_input" % i], rtol=0, atol=2e-5)
         np.testing.assert_allclose(o["gt_boxes3d"], gold["train%d_gt_boxes3d" % i], rtol=0, atol=1e-6)
         assert repr(o["aug_method"]) == str(gold["train%d_aug" % i])
-        _label_agreement(o["rpn_cls_label"], o["rpn_reg_label"], gold["train%d_rpn_cls_label" % i], gold["train%d_rpn_reg_label" % i], 2e-3)
+        _labels_in_band(o["rpn_cls_label"], o["rpn_reg_label"], o["pts_input"], o["gt_boxes3d"], where="oracle %d" % i)
+        _labels_in_band(gold["train%d_rpn_cls_label" % i], gold["train%d_rpn_reg_label" % i], gold["train%d_pts_input" % i], gold["train%d_gt_boxes3d" % i],
+                        delaunay=True, where="reference %d" % i)
         assert o["pasted"] >= 5, "every fixture scene must paste several objects"
         if i == 2:
             assert len(o["pts_all"]) < NPOINTS, "scene 2 must have fewer valid points than npoints after the paste"
@@ -143,8 +145,8 @@ def test_pipeline_with_the_reference_stream_pastes_like_the_reference(cuda, gold
         np.testing.assert_allclose(got[:n], g, rtol=0, atol=1e-6)
         assert not got[n:].any()
         assert repr(out["aug_method"][0]) == str(gold["train%d_aug" % i])
-        _label_agreement(out["rpn_cls_label"][0].cpu().numpy(), out["rpn_reg_label"][0].cpu().numpy(),
-                         gold["train%d_rpn_cls_label" % i], gold["train%d_rpn_reg_label" % i], 2e-3)
+        _labels_in_band(out["rpn_cls_label"][0].cpu().numpy(), out["rpn_reg_label"][0].cpu().numpy(), out["pts_input"][0].cpu().numpy(),
+                        got[:n], where="device %d" % i)
 
 
 def _batch8():
@@ -209,6 +211,11 @@ def test_device_paste_geometry(cuda):
             tall[3] += np.float32(2)
             inside |= GP.paste_in_box(rect, tall)
         assert (inside & (flags & 1).astype(bool)).sum() > 0
+        # against float64 membership: cleared on every valid point certainly inside an accepted box, kept on every valid
+        # point certainly outside all of them
+        _, cin, cout = IR.classify(rect, boxes, "paste")
+        valid, kept = (flags & 1).astype(bool), (flags2[seg] & 1).astype(bool)
+        assert not (valid & cin.any(0) & kept).any() and not (valid & cout.all(0) & ~kept).any()
         expect = (flags & 2) | (((flags & 1).astype(bool) & ~inside).astype(np.uint8))
         np.testing.assert_array_equal(flags2[seg], expect)
         # then the accepted entries' points, moved by their move height, in acceptance order
