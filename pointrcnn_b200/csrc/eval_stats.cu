@@ -13,7 +13,6 @@ namespace prb {
 constexpr int kEsThreads = 128;
 constexpr int kEsMaxBoxes = 512;       // the TRAIN post-NMS proposal count
 constexpr int kEsMaxThresh = 16;
-constexpr int POLY_SLOTS_ES = 16;      // an intersection polygon has at most 8 + 8 vertices
 constexpr int kEsMaxPoints = 16384;    // every count stays exact in fp32
 
 struct EsThresh {
@@ -49,7 +48,7 @@ __global__ void __launch_bounds__(kEsThreads) eval_box_recall_kernel(int m, int 
                                                                      float *__restrict__ box_max_iou) {
     extern __shared__ int s_gt_max[];             // g
     __shared__ int s_row_max[kEsMaxBoxes];
-    __shared__ float s_poly[3 * POLY_SLOTS_ES * kEsThreads];
+    __shared__ float s_poly[3 * POLY_SLOTS * kEsThreads];
     __shared__ int s_hits[kEsMaxThresh];
     const int scene = blockIdx.x, tid = threadIdx.x;
     const int n = box_count ? min(max(box_count[scene], 0), m) : m;
@@ -60,7 +59,7 @@ __global__ void __launch_bounds__(kEsThreads) eval_box_recall_kernel(int m, int 
     if (tid < th.n) s_hits[tid] = 0;
     __syncthreads();
 
-    float *px = s_poly + tid, *py = px + POLY_SLOTS_ES * kEsThreads, *pa = py + POLY_SLOTS_ES * kEsThreads;
+    float *px = s_poly + tid, *py = px + POLY_SLOTS * kEsThreads, *pa = py + POLY_SLOTS * kEsThreads;
     const float *B = boxes + (size_t)scene * m * 7, *G = gt + (size_t)scene * g * 7;
     const int pairs = n * ng;
     for (int p = tid; p < pairs; p += kEsThreads) {
@@ -160,7 +159,7 @@ extern "C" int prb_eval_box_recall(int b, int m, const float *boxes, const int *
     int dev = 0, optin = 0;
     PRB_CUDA(cudaGetDevice(&dev));
     PRB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    const size_t static_smem = sizeof(int) * (kEsMaxBoxes + kEsMaxThresh) + sizeof(float) * 3 * POLY_SLOTS_ES * kEsThreads;
+    const size_t static_smem = sizeof(int) * (kEsMaxBoxes + kEsMaxThresh) + sizeof(float) * 3 * POLY_SLOTS * kEsThreads;
     PRB_REQUIRE(smem + static_smem <= (size_t)optin, "eval_box_recall: %d GT boxes per scene do not fit in shared memory", g);
     if (smem > 48 * 1024 - static_smem)
         PRB_CUDA(cudaFuncSetAttribute(eval_box_recall_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

@@ -26,23 +26,26 @@ constexpr int kSelectThreads = 128;
 // [x-l/2, z-w/2, x+l/2, z+w/2, ry] for box_overlap (the rotation convention of boxes3d_to_corners3d), and the height
 // range [-y, -(y-h)] get_iou3d reads from the corners (y points down)
 struct CollBox {
-    float bev[5];
+    BoxPre bev;
     float lo, hi, vol;
 };
 
 __device__ __forceinline__ void coll_box(const float *__restrict__ q, CollBox &c) {
-    const float x = q[0], y = q[1], z = q[2], h = q[3], w = q[4] + 0.5f, l = q[5] + 0.5f;
-    c.bev[0] = x - l / 2.f; c.bev[1] = z - w / 2.f; c.bev[2] = x + l / 2.f; c.bev[3] = z + w / 2.f; c.bev[4] = q[6];
+    const float y = q[1], h = q[3];
+    const float enlarged[7] = {q[0], y, q[2], h, q[4] + 0.5f, q[5] + 0.5f, q[6]};
+    float bev[5];
+    box7_to_bev(enlarged, bev);
+    box_pre(bev, c.bev);
     c.lo = -y;
     c.hi = -(y - h);
-    c.vol = (c.bev[2] - c.bev[0]) * (c.bev[3] - c.bev[1]) * (c.hi - c.lo);
+    c.vol = (c.bev.x2 - c.bev.x1) * (c.bev.y2 - c.bev.y1) * (c.hi - c.lo);
 }
 
-// 3D IoU >= 1e-8 (kitti_rcnn_dataset.py:479-480)
-__device__ __forceinline__ bool collides(const CollBox &a, const CollBox &b) {
+// 3D IoU >= 1e-8 (kitti_rcnn_dataset.py:479-480); px / py / pa: the thread's polygon scratch column
+__device__ __forceinline__ bool collides(const CollBox &a, const CollBox &b, float *px, float *py, float *pa) {
     const float oh = fminf(a.hi, b.hi) - fmaxf(a.lo, b.lo);
     if (!(oh > 0.f)) return false;
-    const float ov = box_overlap(a.bev, b.bev) * oh;
+    const float ov = box_overlap(a.bev, b.bev, px, py, pa, kSelectThreads) * oh;
     return ov / (a.vol + b.vol - ov) >= 1e-8f;
 }
 
@@ -52,10 +55,12 @@ __global__ void __launch_bounds__(kSelectThreads) gt_paste_select_kernel(
     const float *__restrict__ coll_boxes, const int *__restrict__ coll_count, const float *__restrict__ gt_rows,
     const int *__restrict__ gt_count, const float *__restrict__ cand_rows, int *__restrict__ place, int *__restrict__ stats,
     float *__restrict__ gt_out, int *__restrict__ gt_count_out, int *__restrict__ counts) {
-    extern __shared__ __align__(16) unsigned char s_raw[];
-    CollBox *s_cur = reinterpret_cast<CollBox *>(s_raw);      // m collision boxes + up to k accepted candidates
+    // shared memory: polygon scratch (3 x POLY_SLOTS x kSelectThreads), then m collision boxes + up to k accepted candidates
+    extern __shared__ float s_dyn[];
+    CollBox *s_cur = reinterpret_cast<CollBox *>(s_dyn + 3 * POLY_SLOTS * kSelectThreads);
     __shared__ int s_acc[kPasteMaxCand];                      // candidate index of the r-th accepted one
     const int scene = blockIdx.x, tid = threadIdx.x;
+    float *px = s_dyn + tid, *py = px + POLY_SLOTS * kSelectThreads, *pa = py + POLY_SLOTS * kSelectThreads;
     const int nm = min(coll_count[scene], m), nc = min(cand_count[scene], k);
     for (int q = tid; q < nm; q += kSelectThreads) coll_box(coll_boxes + ((size_t)scene * m + q) * 7, s_cur[q]);
     for (int j = nc + tid; j < k; j += kSelectThreads) place[(size_t)scene * k + j] = -1;
@@ -66,7 +71,7 @@ __global__ void __launch_bounds__(kSelectThreads) gt_paste_select_kernel(
         CollBox cb;
         coll_box(cand_boxes + (size_t)c * 7, cb);
         bool hit = false;
-        for (int q = tid; q < ncur && !hit; q += kSelectThreads) hit = collides(cb, s_cur[q]);
+        for (int q = tid; q < ncur && !hit; q += kSelectThreads) hit = collides(cb, s_cur[q], px, py, pa);
         if (__syncthreads_or(hit)) {
             if (tid == 0) place[c] = -1;
             continue;
@@ -236,8 +241,9 @@ extern "C" int prb_gt_paste_select(int b, int k, int m, int g, const float *cand
     PRB_REQUIRE(!gt_out || (gt_count_out && (g == 0 || gt_rows) && (k == 0 || cand_rows)), "gt_paste_select: label rows need gt_rows, "
                 "cand_rows and gt_count_out");
     PRB_REQUIRE(!gt_out || g + k <= kPasteMaxRows, "gt_paste_select: %d GT + %d candidate rows > %d", g, k, kPasteMaxRows);
-    const size_t smem = (size_t)(m + k) * sizeof(CollBox);
-    if (smem > 48 * 1024) PRB_CUDA(cudaFuncSetAttribute(gt_paste_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    // polygon scratch (24 KB) and 76 bytes per box: m = 1024, k = 128 need 110 KB (above 40 KB: s_acc shares the default 48)
+    const size_t smem = (size_t)3 * POLY_SLOTS * kSelectThreads * sizeof(float) + (size_t)(m + k) * sizeof(CollBox);
+    if (smem > 40 * 1024) PRB_CUDA(cudaFuncSetAttribute(gt_paste_select_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     gt_paste_select_kernel<<<b, kSelectThreads, smem, (cudaStream_t)stream>>>(k, m, g, cand_boxes, cand_count, cand_first, coll_boxes,
                                                                               coll_count, gt_rows, gt_count, cand_rows, place, stats, gt_out,
                                                                               gt_count_out, counts);

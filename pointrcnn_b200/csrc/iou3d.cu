@@ -21,10 +21,6 @@ namespace prb {
 // 16 x 16 pairs per CTA; the 32 boxes of the tile are precomputed once (BoxPre: centre, cos/sin, rotated corners), the
 // intersection polygon of each pair lives in a shared-memory column of its thread (no local memory).
 constexpr int PM_T = 16;
-// the reference's cp[16].  The algorithm counts edge crossings and corners separately, so with rounding it can count more
-// than the 8 vertices an exact intersection has: near-parallel and near-duplicate pairs reach exactly 16 in the
-// CPU oracle (tests/test_cpu_iou_geometry.py); none of the generated pairs exceeds it, but no proof bounds the count by 16
-constexpr int POLY_SLOTS = 16;
 template <bool IOU>
 __global__ void __launch_bounds__(PM_T * PM_T) pair_matrix_kernel(int num_a, const float *__restrict__ boxes_a, int num_b,
                                                                   const float *__restrict__ boxes_b, float *__restrict__ out) {
@@ -42,8 +38,8 @@ __global__ void __launch_bounds__(PM_T * PM_T) pair_matrix_kernel(int num_a, con
     if (ai >= num_a || bi >= num_b) return;
     constexpr int NT = PM_T * PM_T;
     float *px = s_poly + t, *py = px + POLY_SLOTS * NT, *pa = py + POLY_SLOTS * NT;
-    out[(size_t)ai * num_b + bi] = IOU ? iou_bev_pre(sa[threadIdx.y], sb[threadIdx.x], px, py, pa, NT)
-                                       : box_overlap_pre(sa[threadIdx.y], sb[threadIdx.x], px, py, pa, NT);
+    out[(size_t)ai * num_b + bi] = IOU ? iou_bev(sa[threadIdx.y], sb[threadIdx.x], px, py, pa, NT)
+                                       : box_overlap(sa[threadIdx.y], sb[threadIdx.x], px, py, pa, NT);
 }
 
 // ---------------------------------------------------------------- NMS mask (upper-triangle tiles)
@@ -86,7 +82,7 @@ __global__ void __launch_bounds__(NM_THREADS) nms_mask_kernel(int n, float thres
             const int c = lane + 32 * h;
             hit[h] = false;
             if (c >= start && c < col_size) {
-                const float v = NORMAL ? iou_normal(rbx + r * 5, cbx + c * 5) : iou_bev_pre(rpre[r], cpre[c], px, py, pa, NM_THREADS);
+                const float v = NORMAL ? iou_normal(rbx + r * 5, cbx + c * 5) : iou_bev(rpre[r], cpre[c], px, py, pa, NM_THREADS);
                 hit[h] = v > thresh;
             }
         }

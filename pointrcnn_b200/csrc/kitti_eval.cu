@@ -76,7 +76,7 @@ __global__ void __launch_bounds__(128, 4) eval_overlaps_kernel(const double *__r
                                                              const int *__restrict__ dt_count,
                                                              const long long *__restrict__ pair_off, long long n_pairs,
                                                              double *__restrict__ ov) {
-    __shared__ float s_px[16 * 128], s_py[16 * 128], s_pa[16 * 128];
+    __shared__ float s_px[POLY_SLOTS * 128], s_py[POLY_SLOTS * 128], s_pa[POLY_SLOTS * 128];
     const int img = blockIdx.x;
     const int g0 = gt_off[img], ng = gt_off[img + 1] - g0;
     const int d0 = dt_off[img], nd = min(dt_count[img], min(dt_off[img + 1] - d0, kMaxDetPerImage));
@@ -90,7 +90,7 @@ __global__ void __launch_bounds__(128, 4) eval_overlaps_kernel(const double *__r
         float area_a, area_b;
         bev_pre(a, A, area_a);
         bev_pre(b, B, area_b);
-        const float inter = box_overlap_pre(A, B, s_px + threadIdx.x, s_py + threadIdx.x, s_pa + threadIdx.x, 128);
+        const float inter = box_overlap(A, B, s_px + threadIdx.x, s_py + threadIdx.x, s_pa + threadIdx.x, 128);
         // rotate_iou_gpu_eval's fp32 IoU (criterion -1)
         o[n_pairs + at] = (double)__fdiv_rn(inter, __fsub_rn(__fadd_rn(area_b, area_a), inter));
         // d3_box_overlap_kernel (eval.py:120-145): height range [y - h, y] and the volumes l*h*w in double on top of the fp32

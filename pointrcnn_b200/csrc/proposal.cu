@@ -13,8 +13,9 @@
 // EARLIER KEPT box overlaps it by more than the threshold" -- identical to the reference's full N x N bitmask followed
 // by its sequential scan -- so candidates are tested against the <= post_top_n kept boxes only, 32 at a time (8 warps
 // split the kept list; warp 0 resolves the 32 x 32 interactions inside the chunk in order), and the walk stops as
-// soon as post_top_n boxes are kept: ~1e5 IoU evaluations instead of the 2e7 of a 6300 x 6300 mask.  The IoU
-// arithmetic and its argument order (suppressor first) are those of the bitmask kernel (iou3d_dev.cuh).
+// soon as post_top_n boxes are kept: ~1e5 IoU evaluations instead of the 2e7 of a 6300 x 6300 mask.  The IoU is the
+// bitmask kernel's (iou3d_dev.cuh: the kept list and each chunk as BoxPre in shared memory, a polygon scratch column
+// per thread), with its argument order: suppressor first.
 #include "iou3d_dev.cuh"
 
 namespace prb {
@@ -91,26 +92,32 @@ struct ProposalParams {
     int *counts;               // (b, 2)
 };
 
-__device__ __forceinline__ void bev_of(const float *bx, float *bev) {          // kitti_utils.py:134-147
-    const float hl = __fdiv_rn(bx[5], 2.0f), hw = __fdiv_rn(bx[4], 2.0f);
-    bev[0] = __fsub_rn(bx[0], hl); bev[1] = __fsub_rn(bx[2], hw);
-    bev[2] = __fadd_rn(bx[0], hl); bev[3] = __fadd_rn(bx[2], hw);
-    bev[4] = bx[6];
+// IoU of a suppressor (a kept box or an earlier candidate) with a candidate; the axis-aligned one (nms_normal_gpu)
+// reads only the unrotated extent
+__device__ __forceinline__ float nms_iou(bool normal, const BoxPre &s, const BoxPre &c, float *px, float *py, float *pa) {
+    if (normal) {
+        const float a[4] = {s.x1, s.y1, s.x2, s.y2}, b[4] = {c.x1, c.y1, c.x2, c.y2};
+        return iou_normal(a, b);
+    }
+    return iou_bev(s, c, px, py, pa, PL_THREADS);
 }
 
 __global__ void __launch_bounds__(PL_THREADS) proposal_select_nms_kernel(const ProposalParams p) {
-    extern __shared__ int s_dyn[];
+    extern __shared__ float s_dyn[];
+    __shared__ BoxPre s_chunk[32];
     __shared__ int s_wsum[2][PL_WARPS];
     __shared__ unsigned s_sup[PL_WARPS];
     __shared__ int s_nk, s_cnt[2];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int scene = blockIdx.y, area = blockIdx.x;
     const int cap = p.pre[area], post = p.post[area];
-    // shared memory: candidate list (cap), fallback list (area 1 of 2 only: cap), kept indices (post), kept BEV (5 * post)
-    int *cand = s_dyn;
+    // shared memory: polygon scratch (3 x POLY_SLOTS x PL_THREADS), kept boxes (post), candidate list (cap), fallback list
+    // (area 1 of 2 only: cap), kept indices (post)
+    float *px = s_dyn + tid, *py = px + POLY_SLOTS * PL_THREADS, *pa = py + POLY_SLOTS * PL_THREADS;
+    BoxPre *kept_box = reinterpret_cast<BoxPre *>(s_dyn + 3 * POLY_SLOTS * PL_THREADS);
+    int *cand = reinterpret_cast<int *>(kept_box + post);
     int *fall = cand + cap;
     int *kidx = fall + ((p.areas == 2 && area == 1) ? cap : 0);
-    float *kbev = reinterpret_cast<float *>(kidx + post);
     const float *boxes = p.boxes + (size_t)scene * p.n * 7;
     const long long *order = p.order + (size_t)scene * p.n;
 
@@ -160,19 +167,19 @@ __global__ void __launch_bounds__(PL_THREADS) proposal_select_nms_kernel(const P
     for (int c0 = 0; c0 < ncand && nk < post; c0 += 32) {
         const int c = c0 + lane;
         const bool valid = c < ncand;
-        float mine[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-        int my_idx = 0;
-        if (valid) {
-            my_idx = cand[c];
-            bev_of(boxes + (size_t)my_idx * 7, mine);
+        if (warp == 0 && valid) {
+            float bev[5];
+            box7_to_bev(boxes + (size_t)cand[c] * 7, bev);                       // kitti_utils.py:134-147
+            BoxPre &b = s_chunk[lane];
+            if (p.normal) { b.x1 = bev[0]; b.y1 = bev[1]; b.x2 = bev[2]; b.y2 = bev[3]; }     // nms_iou reads the extent only
+            else box_pre(bev, b);
         }
+        __syncthreads();
+        const BoxPre &mine = s_chunk[lane];
         // suppressed by an already kept box?  the 8 warps split the kept list
         bool sup = false;
         if (valid)
-            for (int k = warp; k < nk && !sup; k += PL_WARPS) {
-                const float iou = p.normal ? iou_normal(kbev + k * 5, mine) : iou_bev(kbev + k * 5, mine);
-                sup = iou > p.thresh;
-            }
+            for (int k = warp; k < nk && !sup; k += PL_WARPS) sup = nms_iou(p.normal, kept_box[k], mine, px, py, pa) > p.thresh;
         const unsigned sw = __ballot_sync(0xffffffffu, sup);
         if (lane == 0) s_sup[warp] = sw;
         __syncthreads();
@@ -182,15 +189,9 @@ __global__ void __launch_bounds__(PL_THREADS) proposal_select_nms_kernel(const P
             const unsigned alive = __ballot_sync(0xffffffffu, valid) & ~dead;
             // interactions inside the chunk: bit j of `hit` = candidate j (earlier) overlaps me too much
             unsigned hit = 0;
-            for (int j = 0; j < 31; ++j) {
-                float other[5];
-#pragma unroll
-                for (int t = 0; t < 5; ++t) other[t] = __shfl_sync(0xffffffffu, mine[t], j);
-                if (j < lane && ((alive >> j) & 1u) && ((alive >> lane) & 1u)) {
-                    const float iou = p.normal ? iou_normal(other, mine) : iou_bev(other, mine);
-                    if (iou > p.thresh) hit |= 1u << j;
-                }
-            }
+            if ((alive >> lane) & 1u)
+                for (int j = 0; j < lane; ++j)
+                    if (((alive >> j) & 1u) && nms_iou(p.normal, s_chunk[j], mine, px, py, pa) > p.thresh) hit |= 1u << j;
             unsigned kept = 0, removed = 0;
             for (int j = 0; j < 32; ++j) {
                 const unsigned col = __ballot_sync(0xffffffffu, (hit >> j) & 1u);    // whom does candidate j suppress
@@ -199,9 +200,8 @@ __global__ void __launch_bounds__(PL_THREADS) proposal_select_nms_kernel(const P
             if ((kept >> lane) & 1u) {
                 const int pos = nk + __popc(kept & ((1u << lane) - 1u));
                 if (pos < post) {
-                    kidx[pos] = my_idx;
-#pragma unroll
-                    for (int t = 0; t < 5; ++t) kbev[pos * 5 + t] = mine[t];
+                    kidx[pos] = cand[c];
+                    kept_box[pos] = mine;
                 }
             }
             if (lane == 0) s_nk = min(post, nk + __popc(kept));
@@ -291,13 +291,16 @@ PRB_API int prb_rpn_proposals(int b, int n, const float *boxes, const float *sco
     p.counts = (int *)w;
     p.tmp = (float *)(w + (((size_t)b * 8 + 255) & ~(size_t)255));
     PRB_REQUIRE(workspace_bytes >= (size_t)((char *)(p.tmp + (size_t)b * (p.post[1] > 0 ? p.post[1] : 1) * 8) - (char *)workspace), "rpn_proposals: workspace too small");
+    // shared memory: 4 bytes per candidate (8 in area 1 of 2: the fallback list), 68 per kept box (index + BoxPre) and
+    // 192 per thread (polygon scratch: 48 KB); pre / post top-n of 9000 / 512 in one area need 117 KB
     size_t smem = 0;
     for (int a = 0; a < p.areas; ++a) {
-        const size_t s = ((size_t)p.pre[a] * ((p.areas == 2 && a == 1) ? 2 : 1) + (size_t)p.post[a] * 6) * 4;
+        const size_t s = (size_t)p.pre[a] * ((p.areas == 2 && a == 1) ? 2 : 1) * sizeof(int) + (size_t)p.post[a] * (sizeof(int) + sizeof(BoxPre)) +
+                         (size_t)3 * POLY_SLOTS * PL_THREADS * sizeof(float);
         smem = s > smem ? s : smem;
     }
     PRB_REQUIRE(smem <= 200 * 1024, "rpn_proposals: pre/post top-n of %d/%d need %zu bytes of shared memory", pre_nms_top_n, post_nms_top_n, smem);
-    if (smem > 40 * 1024) PRB_CUDA(cudaFuncSetAttribute(proposal_select_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PRB_CUDA(cudaFuncSetAttribute(proposal_select_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     cudaStream_t st = (cudaStream_t)stream;
     proposal_select_nms_kernel<<<dim3(p.areas, b), PL_THREADS, smem, st>>>(p);
     if (int rc = check_launch("proposal_select_nms_kernel")) return rc;

@@ -23,7 +23,6 @@ constexpr int kRsMaxRois = 4096;       // proposals per scene
 constexpr int kRsMaxGt = 256;          // GT boxes per scene
 constexpr int kRsMaxRows = 1024;       // ROI_PER_IMAGE
 constexpr int kRtThreads = 128;
-constexpr int POLY_SLOTS_RS = 16;    // an intersection polygon has at most 8 + 8 vertices
 constexpr uint32_t kSaltFg = 0x3c6ef372u, kSaltBg = 0xa54ff53au, kSaltJitter = 0x510e527fu, kSaltAug = 0x9b05688cu;
 
 // key of one draw: stage salt, output row (or fg-list position), try, slot
@@ -120,7 +119,7 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
     int *s_roias = s_hard + m;                                // g
     __shared__ int s_src[kRsMaxRows];
     __shared__ int s_wc[kRsThreads / 32];
-    __shared__ float s_poly[3 * POLY_SLOTS_RS * kRsThreads];
+    __shared__ float s_poly[3 * POLY_SLOTS * kRsThreads];
     __shared__ int s_ng;
     const int scene = blockIdx.x, tid = threadIdx.x, R = cf.R;
     const int n = roi_count ? min(roi_count[scene], m) : m;
@@ -209,7 +208,7 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
     }
     // the jitter loop (aug_roi_by_noise_batch), one thread per sampled RoI
     const float pos_thresh = fg_thresh;
-    float *px = s_poly + tid, *py = px + POLY_SLOTS_RS * kRsThreads, *pa = py + POLY_SLOTS_RS * kRsThreads;
+    float *px = s_poly + tid, *py = px + POLY_SLOTS * kRsThreads, *pa = py + POLY_SLOTS * kRsThreads;
     for (int r = tid; r < R; r += kRsThreads) {
         const size_t o = (size_t)scene * R + r;
         float box[7], gt[7];

@@ -5,7 +5,7 @@ The anchor is the overlap / IoU matrix kernel (prb_boxes_overlap_bev / prb_boxes
 well-conditioned pairs, and bit-identical to the reference's own kernel (oracle/_ref) on every pair when that library
 is present.  The consumers must equal the anchor bit for bit on every pair, ill-conditioned and non-finite ones
 included, because a divergence flips NMS keeps and recall counts: the NMS mask, the proposal kernel's NMS, the fused 3D
-IoU (against boxes_iou3d_gpu's torch op sequence on the anchor) and the recall statistics."""
+IoU (against boxes_iou3d_gpu's torch op sequence on the anchor), the recall statistics and the GT-paste collisions."""
 import numpy as np
 import pytest
 import torch
@@ -167,16 +167,18 @@ def test_nms_mask_is_the_anchor_iou_over_the_threshold(cuda, fams, thresh, norma
 def _greedy(iou, thresh):
     kept = []
     for i in range(iou.shape[0]):
-        if all(iou[k, i] <= np.float32(thresh) for k in kept):
+        if all(not (iou[k, i] > np.float32(thresh)) for k in kept):       # the kernel's comparison: a NaN IoU suppresses nothing
             kept.append(i)
     return kept
 
 
 @pytest.mark.parametrize("thresh", [0.1, 0.7, 0.85])
 def test_proposal_nms_keeps_the_greedy_scan_over_the_anchor(cuda, fams, thresh):
-    """the proposal kernel's in-kernel NMS goes through the plain box_overlap (iou_bev), not the precomputed one: its keep
-    list must still be the greedy scan over the anchor IoU, on exact duplicates with distinct scores and near-duplicates"""
-    names = ["identical", "shifted", "rotated", "flipped", "square90", "nested", "generic"]
+    """the proposal kernel's in-kernel NMS (kept boxes and each 32-candidate chunk precomputed in shared memory, the
+    suppressor first): its keep list is the greedy scan over the anchor IoU, on exact duplicates with distinct scores,
+    near-duplicates, touching and degenerate boxes and non-finite fields"""
+    names = ["identical", "shifted", "rotated", "flipped", "square90", "nested", "generic", "shared_edge", "corner", "zero",
+             "nonfinite"]
     scenes = []
     for place in I.PLACES:
         rows = [np.stack([fams[(f, place)][0][:48], fams[(f, place)][1][:48]], 1).reshape(-1, 7) for f in names]
@@ -200,6 +202,48 @@ def test_proposal_nms_keeps_the_greedy_scan_over_the_anchor(cuda, fams, thresh):
         pos = {float(v): k for k, v in enumerate(scores[s][o])}
         got = [pos[float(v)] for v in got_s[s] if v != 0]
         assert got == want, "scene %d: keep list of %d differs from the anchor's greedy scan of %d" % (s, len(got), len(want))
+
+
+# ------------------------------------------------------------------------------------------------ GT-paste collisions
+def _enlarged(b7):
+    e = b7.copy()
+    e[:, 4:6] += np.float32(0.5)                                    # apply_gt_aug_to_one_scene's enlarged w and l
+    return e
+
+
+@pytest.mark.parametrize("shrink", [0.0, 0.5], ids=["rows", "enlarged_rows"])
+@pytest.mark.parametrize("case", CASES, ids=IDS)
+def test_gt_paste_collision_is_the_anchor_overlap_formula(cuda, fams, case, shrink):
+    """one scene per pair (candidate a, collision box b): the candidate is rejected exactly when the fp32 3D IoU of the
+    enlarged boxes, on the anchor overlap of their BEV rows, is >= 1e-8.  Values within a relative 1e-5 of 1e-8 may go
+    either way: nvcc may contract a.vol + b.vol - ov.  The pairs go in as drawn, and with w and l shrunk by 0.5 so that
+    the enlarged boxes are the drawn ones: touching, corner-to-corner and zero-width pairs reach the clip"""
+    a7, b7 = (x.copy() for x in fams[case])
+    for x in (a7, b7):
+        x[:, 4:6] -= np.float32(shrink)
+    ea, eb = _enlarged(a7), _enlarged(b7)
+    A, B = I.to_bev(ea), I.to_bev(eb)
+    ov_bev = anchor_overlap(T(A, cuda), T(B, cuda)).diagonal().cpu().numpy()
+    with np.errstate(all="ignore"):
+        lo_a, hi_a, lo_b, hi_b = -a7[:, 1], -(a7[:, 1] - a7[:, 3]), -b7[:, 1], -(b7[:, 1] - b7[:, 3])
+        vol_a = (A[:, 2] - A[:, 0]) * (A[:, 3] - A[:, 1]) * (hi_a - lo_a)
+        vol_b = (B[:, 2] - B[:, 0]) * (B[:, 3] - B[:, 1]) * (hi_b - lo_b)
+        oh = np.fmin(hi_a, hi_b) - np.fmax(lo_a, lo_b)             # fminf / fmaxf: a NaN operand is dropped
+        ov = ov_bev * oh
+        ratio = ov / (vol_a + vol_b - ov)
+        want = (oh > 0) & (ratio >= np.float32(1e-8))
+        either = (oh > 0) & (np.abs(ratio.astype(np.float64) - 1e-8) <= 1e-5 * 1e-8)
+    n = len(a7)
+    ta, tb = T(a7, cuda), T(b7, cuda)
+    ones, zeros = torch.ones(n, dtype=torch.int32, device=cuda), torch.zeros(n + 1, dtype=torch.int32, device=cuda)
+    place = torch.empty(n, dtype=torch.int32, device=cuda)
+    stats = torch.empty((n, 2), dtype=torch.int32, device=cuda)
+    C.check(C.lib().prb_gt_paste_select(n, 1, 1, 0, C.ptr(ta), C.ptr(ones), C.ptr(zeros), C.ptr(tb), C.ptr(ones),
+                                        None, None, None, C.ptr(place), C.ptr(stats), None, None, None, C.stream()), "gt_paste_select")
+    got = place.cpu().numpy() == -1
+    bad = (got != want) & ~either
+    assert not bad.any(), "%d of %d decisions differ from the anchor formula (%d pairs within 1e-5 of 1e-8 not asserted)" % (
+        bad.sum(), n, either.sum())
 
 
 # ------------------------------------------------------------------------------------------------ recall statistics
