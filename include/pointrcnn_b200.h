@@ -532,6 +532,44 @@ PRB_API int prb_stage_loss_backward(const prb_stage_loss_desc *desc, int rows, i
                                     const float *ce_weight, const float *terms, const float *grad_total, const float *grad_terms,
                                     float *d_cls, float *d_reg, void *stream);
 
+/* --- training-mode SA scale (csrc/sa_train.cu): the grouped SharedMLP + max-pool of one PointnetSAModule(MSG) scale,
+ * forward and backward for autograd, with batch-statistics BatchNorm2d (or conv bias without BN) and ReLU after every
+ * 1x1 conv.  The geometry arguments are those of prb_sa_group_mlp_max_ws (GroupAll: npoint 1, zero centres, idx 0..n-1).
+ * Parameters are read in torch's layout on every call.  rows = b * npoint * nsample.
+ * forward:  z[l] (rows, c_out[l]) receives the pre-activation A_l W_l^T (bias excluded); stats (num_layers, 4, 512)
+ *           receives per channel mean, invstd, a, b with y_l = relu(a * z + b) (no BN: 0, 1, 1, bias); chosen
+ *           (b * npoint, c_out[last]) uint8 the sample each output took; out (b, out_stride_c, npoint) and optionally
+ *           out_pm (b, npoint, out_stride_c) the pooled features at channel out_c_off.  With BN the running statistics
+ *           and num_batches_tracked are updated in place as BatchNorm2d.train() does (unbiased running variance).
+ * backward: from grad_out (b, out_stride_c, npoint) and the forward's z / stats / chosen: grad_weight[l]
+ *           (c_out, c_in_l) written, grad_bias[l] (no BN) or grad_gamma[l] / grad_beta[l] (BN) written where non-NULL,
+ *           and grad_feats (b, c_feat, n), when non-NULL, ACCUMULATED with atomics (the caller zeroes it).
+ * Neither entry allocates or synchronises; all sums except the feature scatter are in a fixed order. */
+typedef struct prb_sa_train_desc {
+    int num_layers;                             /* 1..3 */
+    int c_in;                                   /* 3 + c_feat */
+    int c_out[3];                               /* 1..512 each */
+    int bn;                                     /* 1: BatchNorm2d in training mode after every conv; 0: conv bias */
+    double eps, momentum;                       /* BatchNorm2d's (bn) */
+    const float *weight[3];                     /* (c_out, c_in_l, 1, 1) */
+    const float *bias[3];                       /* conv bias (no bn; NULL: none) */
+    const float *gamma[3], *beta[3];            /* BN affine (bn; NULL: 1 / 0) */
+    float *running_mean[3], *running_var[3];    /* updated by the forward (bn; NULL: not tracked) */
+    long long *num_batches_tracked[3];          /* incremented by the forward (bn; NULL: not tracked) */
+} prb_sa_train_desc;
+/* device scratch of prb_sa_train_forward (backward 0: the BN statistics partials) or prb_sa_train_backward (backward 1: also
+ * the weight-gradient partials and two rows x inner-width gradient buffers); 0 for a descriptor the entries refuse */
+PRB_API size_t prb_sa_train_workspace_bytes(int b, int npoint, int nsample, int c_feat, const prb_sa_train_desc *desc, int backward);
+PRB_API int prb_sa_train_forward(const prb_sa_train_desc *desc, int b, int n, int npoint, int nsample, int c_feat, const float *xyz,
+                                 const float *new_xyz, const float *feats_pm, const int *idx, float *const *z, float *stats,
+                                 unsigned char *chosen, float *out, float *out_pm, int out_stride_c, int out_c_off, void *workspace,
+                                 size_t workspace_bytes, void *stream);
+PRB_API int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n, int npoint, int nsample, int c_feat, const float *xyz,
+                                  const float *new_xyz, const float *feats_pm, const int *idx, const float *const *z,
+                                  const float *stats, const unsigned char *chosen, const float *grad_out, int out_stride_c,
+                                  int out_c_off, float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma,
+                                  float *const *grad_beta, float *grad_feats, void *workspace, size_t workspace_bytes, void *stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -29,6 +29,13 @@ class StageLossDesc(ctypes.Structure):
                 ("y_by_bin", c_int), ("ry_fine", c_int), ("loc_y_scope", ctypes.c_double), ("loc_y_bin_size", ctypes.c_double)]
 
 
+class SATrainDesc(ctypes.Structure):
+    """struct prb_sa_train_desc"""
+    _fields_ = [("num_layers", c_int), ("c_in", c_int), ("c_out", c_int * 3), ("bn", c_int), ("eps", ctypes.c_double),
+                ("momentum", ctypes.c_double)] + [(k, c_void_p * 3) for k in ("weight", "bias", "gamma", "beta", "running_mean",
+                                                                             "running_var", "num_batches_tracked")]
+
+
 class Options(ctypes.Structure):
     """struct prb_options (per-thread tuning block)"""
     _fields_ = [(k, c_int) for k in ("fps_cluster", "fps_prune", "fps_threads", "fps_generic", "mlp_gather", "mlp_ng", "mlp_occ",
@@ -68,7 +75,7 @@ def lib():
         for name in ("prb_nms_workspace_bytes", "prb_mlp_packed_bytes", "prb_mlp_packed_bytes_ex",
                      "prb_sa_workspace_bytes", "prb_fp_workspace_bytes", "prb_rows_workspace_bytes", "prb_rows2_workspace_bytes", "prb_grid_workspace_bytes",
                      "prb_fps_workspace_bytes", "prb_fps_ordered_workspace_bytes", "prb_kitti_format_detections", "prb_rpn_proposals_workspace_bytes", "prb_roipool3d_workspace_bytes",
-                     "prb_kitti_eval_workspace_bytes", "prb_stage_loss_workspace_bytes"):
+                     "prb_kitti_eval_workspace_bytes", "prb_stage_loss_workspace_bytes", "prb_sa_train_workspace_bytes"):
             getattr(L, name).restype = c_size_t
         P, I, F, U = c_void_p, c_int, c_float, ctypes.c_uint
         L.prb_rcnn_sample_rois.argtypes = [I, I, I, P, P, P, P, P, I, I, F, F, F, F, ctypes.c_double, I, I, I, I, I, F, U, P, P, P, P, P, P,
@@ -79,6 +86,9 @@ def lib():
         L.prb_stage_loss_workspace_bytes.argtypes = [I]
         L.prb_stage_loss_forward.argtypes = [P, I, I, P, P, P, I, P, I, P, P, P, P, P, P, P, c_size_t, P]
         L.prb_stage_loss_backward.argtypes = [P, I, I, P, P, P, I, P, I, P, P, P, P, P, P, P, P, P, P]
+        L.prb_sa_train_workspace_bytes.argtypes = [I, I, I, I, P, I]
+        L.prb_sa_train_forward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, I, I, P, c_size_t, P]
+        L.prb_sa_train_backward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, I, I, P, P, P, P, P, P, c_size_t, P]
         L.prb_options_init.restype = None
         L.prb_get_thread_options.restype = None
         if L.prb_abi_version() != 6:

@@ -15,6 +15,8 @@ environment variables ONCE at import; at run time they are changed with `overrid
                     "device" (csrc/rcnn_sample.cu's hashed draws, no host synchronisation)
     loss_impl       which path train.losses.rpn_loss / rcnn_loss(impl=None) take: "torch" (the op-by-op mirror, default) or
                     "device" (csrc/stage_loss.cu: two launches forward, one backward, no host synchronisation)
+    sa_train        which path SA modules take when they need an autograd graph: "torch" (the op-by-op mirror, default) or
+                    "device" (csrc/sa_train.cu through pointnet2/sa_train.py, where its rule holds)
 """
 import contextlib
 import os
@@ -31,6 +33,7 @@ _DEFAULTS = dict(
     fps_ordered=os.environ.get("PRB_FPS_ORDERED", "1") != "0",
     target_draw=os.environ.get("PRB_TARGET_DRAW", "torch"),
     loss_impl=os.environ.get("PRB_LOSS_IMPL", "torch"),
+    sa_train=os.environ.get("PRB_SA_TRAIN", "torch"),
 )
 _local = threading.local()
 

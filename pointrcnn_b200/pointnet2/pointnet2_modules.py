@@ -7,6 +7,9 @@ Two execution paths per module, chosen per call:
            FPS(+new_xyz) -> [one ball-query scan for both radii] -> per scale ONE tensor-core kernel that
            gathers the neighbourhood, runs the whole SharedMLP and max-pools (csrc/mlp_tc.cu).  FP modules:
            three_nn(+weights) -> ONE kernel that interpolates, concatenates the skip features and runs the MLP.
+  train    (SA modules, opt-in with config.sa_train="device", autograd graph needed, batch-statistics BN or none, every
+           layer at most sa_train.FAST_MAX_WIDTH wide):
+           the fused path's sampling and ball query, then sa_train.py's autograd Function (csrc/sa_train.cu).
   unfused  (training / anything else): the reference's op-by-op sequence on the H100 natives with
            torch.nn convolutions, full autograd support.
 `config.override(disable_fused=True)` forces the unfused path (used by tests to cross-check the two).
@@ -21,6 +24,7 @@ from .. import config
 from .. import mlp_chain
 from . import pointnet2_utils
 from . import pytorch_utils as pt_utils
+from . import sa_train
 
 
 class _FusedMLP:
@@ -211,6 +215,15 @@ class _PointnetSAModuleBase(nn.Module):
         ret_xyz, centres, idxs, nss = self.fused_geometry(xyz, new_xyz)
         return ret_xyz, self.fused_mlp(xyz, features, centres, idxs, nss)
 
+    # ------------------------------------------------------------------ training path (config.sa_train == "device")
+    def _forward_train(self, xyz, features, new_xyz):
+        """the fused path's sampling and neighbour search, then sa_train's autograd Function over all scales"""
+        xyz = xyz.contiguous()
+        ret_xyz, centres, idxs, nss = self.fused_geometry(xyz, new_xyz)
+        feats_pm = _point_major(features) if features is not None else None
+        out, out_pm = sa_train.forward(self, xyz, features, feats_pm, centres, idxs, nss)
+        return ret_xyz, _attach_pm(out, out_pm)
+
     # ------------------------------------------------------------------ reference-shaped path
     def forward(self, xyz: torch.Tensor, features: torch.Tensor = None, new_xyz=None) -> (torch.Tensor, torch.Tensor):
         """
@@ -221,6 +234,9 @@ class _PointnetSAModuleBase(nn.Module):
         """
         if self._can_fuse(xyz, features, new_xyz):
             return self._forward_fused(xyz, features, new_xyz)
+        if (config.get("sa_train") == "device" and _needs_graph(self, xyz, features, new_xyz)
+                and sa_train.supported(self, xyz, features, new_xyz) and sa_train.faster_on_device(self)):
+            return self._forward_train(xyz, features, new_xyz)
 
         new_features_list = []
         if new_xyz is None and self.npoint is not None:

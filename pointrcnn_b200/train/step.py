@@ -5,22 +5,38 @@ backward, gradient all-reduce over the data-parallel ranks, optimizer step.
 Forward / backward use the reference-shaped op-by-op path of the mirror modules: this repo's sampling / neighbour / grouping
 / interpolation natives with their scatter backward kernels (gather_points_grad, group_points_grad,
 three_interpolate_grad), the shared MLPs through cuDNN / cuBLAS with torch autograd.  (The fused tensor-core chain is an
-eval-mode kernel: batch-statistics BatchNorm couples all tiles of a launch.)  What this module adds over the reference's
+eval-mode kernel: batch-statistics BatchNorm couples all tiles of a launch.  sa_train="device" runs the SA modules it
+supports through csrc/sa_train.cu instead, see pointnet2/sa_train.py.)  What this module adds over the reference's
 loop: no `.item()` inside the loss, per-rank processes instead of nn.DataParallel's per-step replicate / scatter / gather,
 and the bucketed all-reduce of `parallel_utils.GradBucketReducer` overlapped with backward.
 """
+import contextlib
+
 import numpy as np
 import torch
 
+from .. import config
 from ..parallel_utils import GradBucketReducer
 from ..rpn.stage import CLS_MEAN_SIZE, RPNStage
 from .losses import rcnn_loss, rpn_loss
 
 
-class RPNTrainer:
-    """loss_impl: which stage-loss path forward_loss takes ("torch" / "device", see train.losses; None: the config switch)"""
+def _sa_switch(sa_train):
+    """the config.sa_train override of a trainer's forward (None: leave the switch as it is)"""
+    if sa_train is None:
+        return contextlib.nullcontext()
+    if sa_train not in ("torch", "device"):
+        raise ValueError("sa_train must be 'torch', 'device' or None, not %r" % (sa_train,))
+    return config.override(sa_train=sa_train)
 
-    def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, loss_impl=None):
+
+class RPNTrainer:
+    """loss_impl: which stage-loss path forward_loss takes ("torch" / "device", see train.losses; None: the config switch).
+    sa_train: which path the SA modules take in training ("torch" / "device", see pointnet2/sa_train.py; None: the config
+    switch)"""
+
+    def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, loss_impl=None,
+                 sa_train=None):
         torch.manual_seed(seed)                       # identical initial weights on every rank
         self.device = torch.device(device)
         self.model = RPNStage(input_channels=input_channels, mode="TRAIN").to(self.device).train()
@@ -30,10 +46,13 @@ class RPNTrainer:
         self.opt = torch.optim.Adam(self.params, lr=lr, weight_decay=weight_decay, **({"fused": True} if fused else {}))
         self.mean_size = torch.from_numpy(CLS_MEAN_SIZE[0]).to(self.device)
         self.loss_impl = loss_impl
+        self.sa_train = sa_train
+        _sa_switch(sa_train)
 
     def forward_loss(self, pts_input, rpn_cls_label, rpn_reg_label):
         m = self.model
-        xyz, feats = m.backbone_net(pts_input)
+        with _sa_switch(self.sa_train):
+            xyz, feats = m.backbone_net(pts_input)
         rpn_cls = m.rpn_cls_layer(feats).transpose(1, 2).contiguous()       # lib/net/rpn.py:76-77
         rpn_reg = m.rpn_reg_layer(feats).transpose(1, 2).contiguous()
         return rpn_loss(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, self.mean_size, impl=self.loss_impl)
@@ -69,10 +88,12 @@ class RCNNTrainer:
     depth) to the RCNN stage, whose target layer samples 64 RoIs per scene; forward / backward of the RCNN network on the
     op-by-op path, get_rcnn_loss, bucketed gradient all-reduce, optimizer step.  target_draw: how the target layer samples
     ("torch": the reference's random calls, "device": one device pass without host reads; None: the config switch).  loss_impl:
-    which stage-loss path every forward_loss* method takes ("torch" / "device", see train.losses; None: the config switch)."""
+    which stage-loss path every forward_loss* method takes ("torch" / "device", see train.losses; None: the config switch).
+    sa_train: which path the RCNN network's SA modules take ("torch" / "device", see pointnet2/sa_train.py; None: the config
+    switch)."""
 
     def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, rpn_score_thresh=0.3,
-                 target_draw=None, loss_impl=None):
+                 target_draw=None, loss_impl=None, sa_train=None):
         from ..rcnn.stage import RCNNStage
         torch.manual_seed(seed)
         self.device = torch.device(device)
@@ -87,6 +108,8 @@ class RCNNTrainer:
         self.rpn_score_thresh = rpn_score_thresh
         self.target_draw = target_draw
         self.loss_impl = loss_impl
+        self.sa_train = sa_train
+        _sa_switch(sa_train)
 
     @torch.no_grad()
     def rpn_outputs(self, pts_input, gt_boxes3d):
@@ -101,7 +124,8 @@ class RCNNTrainer:
     def forward_loss_jit(self, batch):
         """rcnn_net.forward with ROI_SAMPLE_JIT (:120-126) + get_rcnn_loss on an input dict: the RPN outputs of forward_loss, or
         a batch of saved features and proposals from datasets.rcnn_offline.RCNNOfflineSampler.prepare_jit_batch"""
-        ret = self.model.forward_train(batch, target_draw=self.target_draw)
+        with _sa_switch(self.sa_train):
+            ret = self.model.forward_train(batch, target_draw=self.target_draw)
         c = self.model.cfg
         return rcnn_loss(ret["rcnn_cls"], ret["rcnn_reg"], ret["cls_label"], ret["reg_valid_mask"], ret["roi_boxes3d"], ret["gt_of_rois"],
                          self.mean_size, loc_scope=c["LOC_SCOPE"], loc_bin_size=c["LOC_BIN_SIZE"], num_head_bin=c["NUM_HEAD_BIN"],
@@ -112,7 +136,8 @@ class RCNNTrainer:
         """the ROI_SAMPLE_JIT=False branch of rcnn_net.forward (:155-163) + get_rcnn_loss on a batch of
         datasets.rcnn_offline.RCNNOfflineSampler.prepare_batch: the network reads the pooled rows as they are (no
         torch.cat of pts_input and pts_features), the targets are the batch's labels and canonical GT boxes"""
-        rcnn_cls, rcnn_reg = self.model.forward_pts(batch["rows"])
+        with _sa_switch(self.sa_train):
+            rcnn_cls, rcnn_reg = self.model.forward_pts(batch["rows"])
         c = self.model.cfg
         return rcnn_loss(rcnn_cls, rcnn_reg, batch["cls_label"], batch["reg_valid_mask"], batch["roi_boxes3d"], batch["gt_boxes3d_ct"],
                          self.mean_size, loc_scope=c["LOC_SCOPE"], loc_bin_size=c["LOC_BIN_SIZE"], num_head_bin=c["NUM_HEAD_BIN"],
