@@ -14,7 +14,8 @@ constexpr int NB_MAX = 4;            // weight ring depth upper bound (runtime d
 constexpr int MAX_LAYERS = 3;
 constexpr int MAX_NP = 512;
 constexpr int NSUB_MAX = 8;          // 32-column subtiles per warpgroup (2 warpgroups x 8 x 32 = MAX_NP; wgmma N <= 256)
-constexpr int POOL_STRIDE = 33;      // floats per row of a warpgroup's 64 x 32 max-pool staging tile (conflict-free columns)
+constexpr int RED_STRIDE = MAX_NP;   // SA pool: floats per warp of the per-warp maxima of a centre spanning several warps
+static_assert(4 * RED_STRIDE * 4 <= A_STAGE_BYTES, "the per-warp pool maxima fit in the smallest work region");
 constexpr int CHAIN_THREADS = 2 * 128 + 32;       // two MMA / epilogue warpgroups + one weight-producer warp
 constexpr int RES_NP_MAX = 128;      // resident kernel: widest layer (one warpgroup covers it: <= 64 accumulator registers)
 constexpr int RES_WG_MAX = 5;        // resident kernel: warpgroups per CTA, at most
@@ -35,7 +36,7 @@ struct ChainParams {
     // resources (sized per launch)
     int nb;                          // weight ring depth
     int b_stage_bytes;               // weight stage = one K chunk of the widest layer: max np * 128 bytes
-    int work_bytes;                  // layer-0 A ring / resident activations / pool staging (aliased, see the kernel)
+    int work_bytes;                  // layer-0 A ring / resident activations / pool maxima (aliased, see the kernel)
     // layer-0 K segments (each padded to a multiple of KC)
     int nseg, seg_chunks[2], seg_width[2];
     long total_rows;

@@ -19,10 +19,13 @@
 // loads the segment's whole packed image with cp.async.bulk on one mbarrier, which every warpgroup waits on once.  Each
 // warpgroup then runs its own 64-row tiles (strided over the grid; the tiles of a pooled SA centre stay together)
 // through every layer at full width -- one m64n(np)k8 instruction per K=8 step -- in a private work region (layer-0 A
-// slots -> activations -> pool staging, as below), synchronising only on its own named barrier, so one warpgroup's
-// gather and epilogues overlap another's MMAs.  The B operand of chunk kc of layer l is the image at the layer's offset
+// slots -> activations -> per-warp pool maxima), synchronising only on its own named barrier, so one warpgroup's
+// gather and epilogues overlap another's MMAs.  Where every layer is at most 64 wide, a warpgroup runs tiles 2u and
+// 2u + 1 together: two row tables and work regions, two MMAs on the same B descriptor per K step in one commit group,
+// and one drain, barrier and epilogue pass per layer for the 128 rows -- the serial steps of a narrow tile are short, so
+// the pair halves their count per row.  The B operand of chunk kc of layer l is the image at the layer's offset
 // + kc * np * 128 bytes.  Warpgroups per CTA and CTAs per SM are the pair the occupancy calculator allows the most
-// warpgroups per SM for (registers: 96 for 32-wide chains, 128 otherwise).
+// warpgroups per SM for (registers: 128 for 32-wide pairs and single tiles, 168 for 64-wide pairs).
 //
 // Streaming kernel (mlp_chain_kernel; persistent CTAs over 64-row tiles; rows = (centre, sample) pairs or points):
 //   warpgroups 0, 1  gather layer 0's A operand chunk by chunk (32 K-columns = one 128-byte swizzle row) into a
@@ -58,41 +61,45 @@ __device__ __forceinline__ T per_layer(const T (&a)[MAX_LAYERS], int l) {
     return l == 0 ? a[0] : l == 1 ? a[1] : a[2];
 }
 
-// The MMAs of one K chunk over a warpgroup's nsub * 32 output columns: one m64n(32*NSUB)k8 instruction per K=8 step,
-// KSTEPS steps in K order, straight-line.  nsub and ksteps are warp-uniform and select the sequence before the first
-// wgmma, so no predicate sits between wgmma_fence and wgmma_commit (a divergent one makes ptxas serialise every
-// wgmma behind its own arrive / wait).
-template <int NSUB, int KSTEPS, int NS>
-__device__ __forceinline__ void mma_steps(float (&acc)[16 * NS], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+// The MMAs of one K chunk over a warpgroup's nsub * 32 output columns, for T 64-row tiles that share the B operand: per
+// K=8 step, one m64n(32*NSUB)k8 instruction per tile, KSTEPS steps in K order, straight-line.  nsub and ksteps are
+// warp-uniform and select the sequence before the first wgmma, so no predicate sits between wgmma_fence and wgmma_commit
+// (a divergent one makes ptxas serialise every wgmma behind its own arrive / wait).
+template <int NSUB, int KSTEPS, int NS, int T>
+__device__ __forceinline__ void mma_steps(float (&acc)[T][16 * NS], const uint64_t (&adesc)[T], uint64_t bdesc,
+                                          uint32_t accumulate) {
 #pragma unroll
     for (int ks = 0; ks < KSTEPS; ++ks)
-        wgmma_tf32<NSUB, NS>(acc, adesc + (uint64_t)(2 * ks), bdesc + (uint64_t)(2 * ks), ks > 0 ? 1u : accumulate);
+#pragma unroll
+        for (int s = 0; s < T; ++s)
+            wgmma_tf32<NSUB, NS>(acc[s], adesc[s] + (uint64_t)(2 * ks), bdesc + (uint64_t)(2 * ks), ks > 0 ? 1u : accumulate);
 }
-template <int NSUB, int NS>
-__device__ __forceinline__ void mma_chunk_n(float (&acc)[16 * NS], int ksteps, uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+template <int NSUB, int NS, int T>
+__device__ __forceinline__ void mma_chunk_n(float (&acc)[T][16 * NS], int ksteps, const uint64_t (&adesc)[T], uint64_t bdesc,
+                                            uint32_t accumulate) {
     static_assert(KC / 8 == 4, "mma_chunk_n: one case per K=8 step of a chunk");
     switch (ksteps) {   // fewer than 4 only for the last chunk of a layer-0 segment (the rest of the chunk is padding)
-        case 1: mma_steps<NSUB, 1, NS>(acc, adesc, bdesc, accumulate); break;
-        case 2: mma_steps<NSUB, 2, NS>(acc, adesc, bdesc, accumulate); break;
-        case 3: mma_steps<NSUB, 3, NS>(acc, adesc, bdesc, accumulate); break;
-        default: mma_steps<NSUB, 4, NS>(acc, adesc, bdesc, accumulate); break;
+        case 1: mma_steps<NSUB, 1, NS, T>(acc, adesc, bdesc, accumulate); break;
+        case 2: mma_steps<NSUB, 2, NS, T>(acc, adesc, bdesc, accumulate); break;
+        case 3: mma_steps<NSUB, 3, NS, T>(acc, adesc, bdesc, accumulate); break;
+        default: mma_steps<NSUB, 4, NS, T>(acc, adesc, bdesc, accumulate); break;
     }
 }
-template <int NS>
-__device__ __forceinline__ void mma_chunk(float (&acc)[16 * NS], int nsub, int ksteps, uint64_t adesc, uint64_t bdesc,
-                                          uint32_t accumulate) {
+template <int NS, int T>
+__device__ __forceinline__ void mma_chunk(float (&acc)[T][16 * NS], int nsub, int ksteps, const uint64_t (&adesc)[T],
+                                          uint64_t bdesc, uint32_t accumulate) {
     // both are warp-uniform already; the broadcast keeps ptxas from losing track of that under register pressure
     nsub = __shfl_sync(0xffffffffu, nsub, 0);
     ksteps = __shfl_sync(0xffffffffu, ksteps, 0);
     switch (nsub) {
-        case 1: mma_chunk_n<1, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
-        case 2: if constexpr (NS >= 2) mma_chunk_n<2, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
-        case 3: if constexpr (NS >= 3) mma_chunk_n<3, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
-        case 4: if constexpr (NS >= 4) mma_chunk_n<4, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
-        case 5: if constexpr (NS >= 5) mma_chunk_n<5, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
-        case 6: if constexpr (NS >= 6) mma_chunk_n<6, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
-        case 7: if constexpr (NS >= 7) mma_chunk_n<7, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
-        case 8: if constexpr (NS >= 8) mma_chunk_n<8, NS>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 1: mma_chunk_n<1, NS, T>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 2: if constexpr (NS >= 2) mma_chunk_n<2, NS, T>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 3: if constexpr (NS >= 3) mma_chunk_n<3, NS, T>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 4: if constexpr (NS >= 4) mma_chunk_n<4, NS, T>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 5: if constexpr (NS >= 5) mma_chunk_n<5, NS, T>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 6: if constexpr (NS >= 6) mma_chunk_n<6, NS, T>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 7: if constexpr (NS >= 7) mma_chunk_n<7, NS, T>(acc, ksteps, adesc, bdesc, accumulate); break;
+        case 8: if constexpr (NS >= 8) mma_chunk_n<8, NS, T>(acc, ksteps, adesc, bdesc, accumulate); break;
         default: break;   // the warpgroup owns no columns of this layer (np = 32: all of them go to warpgroup 0)
     }
 }
@@ -293,13 +300,15 @@ __device__ __forceinline__ void store_activations(const ChainParams &p, const fl
     }
 }
 
-// Last layer: SA max-pool, FP (channel-major + optional point-major copy) or rows.  The SA pool goes through the
-// warpgroup's 64 x 32 staging tile `stg` one 32-column subtile at a time (named barrier bar_id over the warpgroup's
-// 128 threads, tw = thread inside the warpgroup); a centre spanning several tiles keeps its partial maxima in s_carry
-// (indexed by column).
+// Last layer: SA max-pool, FP (channel-major + optional point-major copy) or rows.  The SA pool reduces the fragment in
+// registers: a centre's nse = min(ns, 64) rows are nse consecutive rows of the tile, so a centre of 4 or 8 rows lies in
+// the lanes of one warp that differ in g (and one row half h), one of 16 rows in both row halves of one warp, and one of
+// 32 or 64 rows in 2 or 4 warps, whose per-warp maxima meet in `red` (4 x np floats of the warpgroup's free work region)
+// behind one named barrier bar_id over the warpgroup's 128 threads (tw = thread inside the warpgroup).  A centre spanning
+// several tiles keeps its partial maxima in s_carry (indexed by column).
 template <int NS>
-__device__ __forceinline__ void final_epilogue(const ChainParams &p, const float (&acc)[16 * NS], int nsub, int col0, int wq,
-                                               int g, int t4, int tw, int tile, const float *sc, const float *sh, float *stg,
+__device__ __forceinline__ void final_epilogue(const ChainParams &p, float (&acc)[16 * NS], int nsub, int col0, int wq,
+                                               int g, int t4, int tw, int tile, const float *sc, const float *sh, float *red,
                                                float *s_carry, int bar_id) {
     const float lo = p.linear_last ? -CUDART_INF_F : 0.f;   // ReLU = max(., 0); a linear last layer keeps the sign
     const bool pool_raw = p.unit_scale && p.mode_out == OUT_SA_MAX;
@@ -310,38 +319,95 @@ __device__ __forceinline__ void final_epilogue(const ChainParams &p, const float
     };
     if (p.mode_out == OUT_SA_MAX) {
         const int nse = p.ns < TM ? p.ns : TM, per = p.ns > TM ? p.ns / TM : 1;
-        const int sub = tile % per, ncent = TM / nse;
+        const bool halves = nse >= 16;              // a centre covers both row halves of the thread
+        const int gspan = nse < 8 ? nse : 8;        // lanes (4 g + t4) of a centre that differ in g
+        // the maxima of subtile j over the centre's rows of this warp, in place in acc[16 j + 4 i + e] (and in
+        // acc[16 j + 4 i + 2 + e] for the second row half when it is another centre): in the thread, then over the lanes
+        // that differ in g (2 steps for a centre of 4 rows, 3 for 8 rows and more); every lane of the centre ends with them
+        auto warp_max = [&](int j) {
+            float *v = acc + 16 * j;
 #pragma unroll
-        for (int j = 0; j < NS; ++j) {
-            if (j >= nsub) continue;
+            for (int q = 0; q < 16; ++q) v[q] = value(v[q], col0 + 32 * j + 8 * (q >> 2) + 2 * t4 + (q & 1));
+            if (halves) {
 #pragma unroll
-            for (int i = 0; i < 4; ++i)
+                for (int q = 0; q < 16; ++q)
+                    if (!(q & 2)) v[q] = fmaxf(v[q], v[q + 2]);
+            }
+            for (int m = 4; m < 4 * gspan; m <<= 1) {
 #pragma unroll
-                for (int h = 0; h < 2; ++h)
+                for (int q = 0; q < 16; ++q)
+                    if (!(halves && (q & 2))) v[q] = fmaxf(v[q], __shfl_xor_sync(0xffffffffu, v[q], m));
+            }
+        };
+        // the first element of centre ci in `out` (channel stride npoint) and in out_pm (channel stride 1), or nullptr
+        // for a centre past the last row (a partial last tile holds whole centres)
+        auto centre_out = [&](int ci, float *&o, float *&o2) {
+            const long Rg = (long)tile * TM + ci * nse;
+            o = nullptr;
+            o2 = nullptr;
+            if (Rg >= p.total_rows) return;
+            const int pr = (int)(Rg >> p.log_ns);   // rows < 2^31
+            const int scene = pr / p.npoint, pp = pr - scene * p.npoint;
+            o = p.out + ((size_t)scene * p.out_stride_c + p.out_c_off) * p.npoint + pp;
+            if (p.out_pm) o2 = p.out_pm + (size_t)pr * p.out_stride_c + p.out_c_off;
+        };
+        auto store = [&](float x, int c, float *o, float *o2) {
+            if (pool_raw) x = fmaxf(x + sh[c], lo);
+            if (o && c < Cl) {
+                o[(size_t)c * p.npoint] = x;
+                if (o2) o2[c] = x;
+            }
+        };
+        if (nse <= 16) {
+            // a centre inside one warp: the lanes with g % gspan == 0 write it
 #pragma unroll
-                    for (int e = 0; e < 2; ++e) {
-                        const int cs = 8 * i + 2 * t4 + e;
-                        stg[(16 * wq + g + 8 * h) * POOL_STRIDE + cs] = value(acc[16 * j + 4 * i + 2 * h + e], col0 + 32 * j + cs);
+            for (int j = 0; j < NS; ++j)
+                if (j < nsub) warp_max(j);
+            if ((g & (gspan - 1)) == 0) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (halves && h) continue;
+                    float *o, *o2;
+                    centre_out((16 * wq + g + 8 * h) / nse, o, o2);
+#pragma unroll
+                    for (int j = 0; j < NS; ++j) {
+                        if (j >= nsub) continue;
+#pragma unroll
+                        for (int i = 0; i < 4; ++i)
+#pragma unroll
+                            for (int e = 0; e < 2; ++e)
+                                store(acc[16 * j + 4 * i + 2 * h + e], col0 + 32 * j + 8 * i + 2 * t4 + e, o, o2);
                     }
+                }
+            }
+        } else {
+            // a centre of 2 or 4 warps: each warp's maxima to red[wq][c], one barrier, then one thread per (centre,
+            // column) takes the max over the centre's warps; a centre spanning several tiles carries it in s_carry
+#pragma unroll
+            for (int j = 0; j < NS; ++j) {
+                if (j >= nsub) continue;
+                warp_max(j);
+                if (g == 0) {
+#pragma unroll
+                    for (int q = 0; q < 16; ++q)
+                        if (!(q & 2)) red[wq * RED_STRIDE + col0 + 32 * j + 8 * (q >> 2) + 2 * t4 + (q & 1)] = acc[16 * j + q];
+                }
+            }
             bar_wg_id(bar_id);
-            for (int o = tw; o < ncent * 32; o += 128) {
-                const int ci = o >> 5, cs = o & 31, c = col0 + 32 * j + cs;
-                float x = stg[(ci * nse) * POOL_STRIDE + cs];
-                for (int r = 1; r < nse; ++r) x = fmaxf(x, stg[(ci * nse + r) * POOL_STRIDE + cs]);
+            const int np_w = 32 * nsub, wpc = nse >> 4, ncent = TM / nse;   // columns, warps per centre, centres per tile
+            const int sub = tile % per;
+            for (int o = tw; o < ncent * np_w; o += 128) {
+                const int ci = o / np_w, c = col0 + o - ci * np_w;
+                float x = red[(ci * wpc) * RED_STRIDE + c];
+                for (int w = 1; w < wpc; ++w) x = fmaxf(x, red[(ci * wpc + w) * RED_STRIDE + c]);
                 if (per > 1) {
                     if (sub > 0) x = fmaxf(x, s_carry[c]);
                     if (sub < per - 1) { s_carry[c] = x; continue; }
                 }
-                if (pool_raw) x = fmaxf(x + sh[c], lo);
-                const long Rg = (long)tile * TM + ci * nse;    // a row of the centre (whole centres per tile)
-                if (Rg < p.total_rows && c < Cl) {
-                    const long pr = Rg >> p.log_ns;
-                    const int scene = (int)(pr / p.npoint), pp = (int)(pr - (long)scene * p.npoint);
-                    p.out[((size_t)scene * p.out_stride_c + p.out_c_off + c) * p.npoint + pp] = x;
-                    if (p.out_pm) p.out_pm[((size_t)scene * p.npoint + pp) * p.out_stride_c + p.out_c_off + c] = x;
-                }
+                float *op, *op2;
+                centre_out(ci, op, op2);
+                store(x, c, op, op2);
             }
-            bar_wg_id(bar_id);
         }
     } else {
 #pragma unroll
@@ -401,7 +467,7 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
     int np_total = 0;
 #pragma unroll
     for (int l = 0; l < MAX_LAYERS; ++l) np_total += l < L ? p.np[l] : 0;
-    // work region, by phase of a tile: layer-0 A slots -> resident activations (layers >= 1) -> pool staging
+    // work region, by phase of a tile: layer-0 A slots -> resident activations (layers >= 1) -> per-warp pool maxima
     uint8_t *sW = base;
     uint8_t *sB = sW + p.work_bytes;
     float *s_scale = reinterpret_cast<float *>(sB + (size_t)p.nb * p.b_stage_bytes);
@@ -447,13 +513,14 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
     const int tw = tid & 127;                    // thread inside the warpgroup
     RingPos rb = {0, 0};
     int aslot = 0;
-    float acc[16 * NS];                          // subtile j (32 columns) = registers 16 j .. 16 j + 15
+    float accs[1][16 * NS];
+    float (&acc)[16 * NS] = accs[0];             // subtile j (32 columns) = registers 16 j .. 16 j + 15
 
     for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
         for (int s = 0; s < p.tiles_per_item; ++s) {
             const int tile = item * p.tiles_per_item + s;
             if (tile >= p.num_tiles) break;
-            bar_mma();   // the previous tile's readers of S.rows and of the pool staging are done
+            bar_mma();   // the previous tile's readers of S.rows and of the pool maxima are done
             load_tile_rows(p, tile, tid, S.rows);
             bar_mma();
 
@@ -483,7 +550,8 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                     mbar_wait(s2u(&S.b_full[rb.stage]), rb.phase);
                     const uint32_t b_addr = s2u(sB + (size_t)rb.stage * p.b_stage_bytes) + (uint32_t)col0 * (KC * 4);
                     wgmma_fence();
-                    mma_chunk<NS>(acc, nsub, ksteps, make_desc(a_addr), make_desc(b_addr), kc > 0 ? 1u : 0u);
+                    const uint64_t adesc[1] = {make_desc(a_addr)};
+                    mma_chunk<NS, 1>(accs, nsub, ksteps, adesc, make_desc(b_addr), kc > 0 ? 1u : 0u);
                     wgmma_commit();
                     wgmma_wait<1>();     // the previous chunk's MMAs are done: release its weight stage
                     if (prev_stage >= 0 && lane == 0) mbar_arrive(s2u(&S.b_empty[prev_stage]));
@@ -503,19 +571,21 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                     bar_mma();   // the next layer's A operand is complete
                     continue;
                 }
-                final_epilogue<NS>(p, acc, nsub, col0, wq, g, t4, tw, tile, sc, sh,
-                                   reinterpret_cast<float *>(sW) + wg * (TM * POOL_STRIDE), s_carry, 2 + wg);
+                final_epilogue<NS>(p, acc, nsub, col0, wq, g, t4, tw, tile, sc, sh, reinterpret_cast<float *>(sW), s_carry, 2 + wg);
             }
         }
     }
 }
 
 // ------------------------------------------------------------------------------------------------ resident kernel
-// NS: 32-column subtiles of the widest layer, all of them in one warpgroup (np <= RES_NP_MAX).  blockDim.x = 128 * nwg.
-template <int NS, int NWG, int MINB>
+// NS: 32-column subtiles of the widest layer, all of them in one warpgroup (np <= RES_NP_MAX).  T: 64-row tiles a
+// warpgroup runs together (2: tiles 2u and 2u + 1 share every B operand, drain, barrier and epilogue pass).
+// blockDim.x = 128 * nwg.
+template <int NS, int NWG, int MINB, int T>
 __global__ void __launch_bounds__(NWG * 128, MINB) mlp_resident_kernel(const ChainParams p) {
     static_assert(NWG <= RES_WG_MAX, "mlp_resident_kernel: one named barrier per warpgroup");
     static_assert(NS * 32 <= RES_NP_MAX, "mlp_resident_kernel: one warpgroup covers the widest layer");
+    static_assert(T == 1 || T == 2, "mlp_resident_kernel: one or two tiles per warpgroup");
     extern __shared__ uint8_t smem_raw[];
     __shared__ uint64_t w_full;
     uint8_t *base = smem_raw + ((1024u - (s2u(smem_raw) & 1023u)) & 1023u);
@@ -527,10 +597,10 @@ __global__ void __launch_bounds__(NWG * 128, MINB) mlp_resident_kernel(const Cha
         w_bytes += l < L ? p.nchunks[l] * p.np[l] * KC * 4 : 0;
     }
     const int np_last = per_layer(p.np, L - 1);
-    // [weight image of every layer | nwg work regions | scale | shift | nwg pool carries | nwg tile-row tables]
+    // [weight image of every layer | nwg x T work regions | scale | shift | nwg pool carries | nwg x T tile-row tables]
     uint8_t *sWt = base;
     uint8_t *sWork = sWt + w_bytes;
-    float *s_scale = reinterpret_cast<float *>(sWork + (size_t)nwg * p.work_bytes);
+    float *s_scale = reinterpret_cast<float *>(sWork + (size_t)nwg * T * p.work_bytes);
     float *s_shift = s_scale + np_total;
     float *s_carry_all = s_shift + np_total;
     TileRows *rows_all = reinterpret_cast<TileRows *>(s_carry_all + nwg * np_last);
@@ -560,20 +630,27 @@ __global__ void __launch_bounds__(NWG * 128, MINB) mlp_resident_kernel(const Cha
     const int g = lane >> 2, t4 = lane & 3;
     const int tw = tid & 127;
     const int bar_id = 1 + wg;
-    uint8_t *W = sWork + (size_t)wg * p.work_bytes;   // this warpgroup's A slots / activations / pool staging
+    // tile s of the warpgroup's unit: work region (A slots / activations / pool maxima) W + s * work_bytes, row table
+    // M[s]; its stages run on thread index tw ^ 64 s, so the half-warpgroup stages (row table, xyz gather) of the two
+    // tiles run on different warps
+    uint8_t *W = sWork + (size_t)wg * T * p.work_bytes;
     float *s_carry = s_carry_all + wg * np_last;
-    TileRows &M = rows_all[wg];
+    TileRows *M = rows_all + wg * T;
     const int nslots = p.nchunks[0] < A_SLOTS ? p.nchunks[0] : A_SLOTS;
     bool w_ready = false;
-    float acc[16 * NS];
+    float acc[T][16 * NS];
 
-    // warpgroups take items in a strided order over the whole grid; an item's tiles stay with one warpgroup
-    for (int item = blockIdx.x * nwg + wg; item < p.num_items; item += gridDim.x * nwg) {
-        for (int s = 0; s < p.tiles_per_item; ++s) {
-            const int tile = item * p.tiles_per_item + s;
-            if (tile >= p.num_tiles) break;
-            bar_wg_id(bar_id);   // the previous tile's readers of M and of the pool staging are done
-            load_tile_rows(p, tile, tw, M);
+    // a unit is an item's tiles one after another (T = 1), or tiles 2u and 2u + 1 together (T = 2: two items of at most
+    // one tile, or the two tiles of one item); warpgroups take units in a strided order over the whole grid
+    const int num_units = T == 1 ? p.num_items : (p.num_tiles + 1) >> 1;
+    const int steps = T == 1 ? p.tiles_per_item : 1;
+    for (int unit = blockIdx.x * nwg + wg; unit < num_units; unit += gridDim.x * nwg) {
+        for (int st = 0; st < steps; ++st) {
+            const int tile0 = T == 1 ? unit * p.tiles_per_item + st : 2 * unit;   // tile 2u + 1 may lie past the last
+            if (tile0 >= p.num_tiles) break;                                         // one: no valid rows, nothing written
+            bar_wg_id(bar_id);   // the previous unit's readers of M and of the pool maxima are done
+#pragma unroll
+            for (int s = 0; s < T; ++s) load_tile_rows(p, tile0 + s, tw ^ (64 * s), M[s]);
             bar_wg_id(bar_id);
 
             int sc_base = 0;
@@ -583,40 +660,51 @@ __global__ void __launch_bounds__(NWG * 128, MINB) mlp_resident_kernel(const Cha
                 const int nch = per_layer(p.nchunks, l);
                 int aslot = 0;
                 for (int kc = 0; kc < nch; ++kc) {
-                    uint32_t a_addr;
+                    uint64_t adesc[T];
                     int ksteps = KC / 8;
                     if (l == 0) {
-                        uint8_t *A = W + (size_t)aslot * A_STAGE_BYTES;
-                        ksteps = gather_chunk<128>(p, tile, kc, tw, M, A);
+#pragma unroll
+                        for (int s = 0; s < T; ++s) {
+                            uint8_t *A = W + (size_t)s * p.work_bytes + (size_t)aslot * A_STAGE_BYTES;
+                            ksteps = gather_chunk<128>(p, tile0 + s, kc, tw ^ (64 * s), M[s], A);
+                            adesc[s] = make_desc(s2u(A));
+                        }
                         fence_async_smem();
                         // slot `aslot` was last read by the MMAs of chunk kc-3, which every warp of the warpgroup
                         // retired (wgmma_wait<1> of chunk kc-2) before the barrier of chunk kc-1
                         bar_wg_id(bar_id);
-                        a_addr = s2u(A);
                         aslot = aslot == nslots - 1 ? 0 : aslot + 1;
                     } else {
-                        a_addr = s2u(W + (size_t)kc * A_STAGE_BYTES);
+#pragma unroll
+                        for (int s = 0; s < T; ++s)
+                            adesc[s] = make_desc(s2u(W + (size_t)s * p.work_bytes + (size_t)kc * A_STAGE_BYTES));
                     }
                     if (!w_ready) { mbar_wait(s2u(&w_full), 0); w_ready = true; }
                     const uint32_t b_addr = s2u(sWt) + w_off + (uint32_t)kc * np_l * (KC * 4);
                     wgmma_fence();
-                    mma_chunk<NS>(acc, nsub, ksteps, make_desc(a_addr), make_desc(b_addr), kc > 0 ? 1u : 0u);
+                    mma_chunk<NS, T>(acc, nsub, ksteps, adesc, make_desc(b_addr), kc > 0 ? 1u : 0u);
                     wgmma_commit();
                     wgmma_wait<1>();
                 }
                 w_off += (uint32_t)nch * np_l * (KC * 4);
                 wgmma_wait<0>();
-                reg_fence(acc);
-                bar_wg_id(bar_id);   // the warpgroup's MMAs of layer l have read their A operand: the work region is free
+#pragma unroll
+                for (int s = 0; s < T; ++s) reg_fence(acc[s]);
+                bar_wg_id(bar_id);   // the warpgroup's MMAs of layer l have read their A operands: the work regions are free
                 const float *sc = s_scale + sc_base, *sh = s_shift + sc_base;
                 sc_base += np_l;
                 if (l + 1 < L) {
-                    store_activations<NS>(p, acc, nsub, 0, wq, g, t4, sc, sh, W);
+#pragma unroll
+                    for (int s = 0; s < T; ++s)
+                        store_activations<NS>(p, acc[s], nsub, 0, wq, g, t4, sc, sh, W + (size_t)s * p.work_bytes);
                     fence_async_smem();
-                    bar_wg_id(bar_id);   // the next layer's A operand is complete
+                    bar_wg_id(bar_id);   // the next layer's A operands are complete
                     continue;
                 }
-                final_epilogue<NS>(p, acc, nsub, 0, wq, g, t4, tw, tile, sc, sh, reinterpret_cast<float *>(W), s_carry, bar_id);
+#pragma unroll
+                for (int s = 0; s < T; ++s)
+                    final_epilogue<NS>(p, acc[s], nsub, 0, wq, g, t4, tw, tile0 + s, sc, sh,
+                                       reinterpret_cast<float *>(W + (size_t)s * p.work_bytes), s_carry, bar_id);
             }
         }
     }
@@ -754,7 +842,7 @@ static size_t segment_smem(const int *np, int n, int nb, int *work_bytes, int *b
         np_max = np[i] > np_max ? np[i] : np_max;
         if (i + 1 < n && np[i] > mid_max) mid_max = np[i];
     }
-    int work = A_SLOTS * A_STAGE_BYTES;                                    // >= the pool staging of both warpgroups
+    int work = A_SLOTS * A_STAGE_BYTES;
     if (TM * mid_max * 4 > work) work = TM * mid_max * 4;
     if (work_bytes) *work_bytes = work;
     if (b_stage_bytes) *b_stage_bytes = np_max * KC * 4;
@@ -785,16 +873,18 @@ static bool launch_resident(ChainParams &p, int max_optin, cudaStream_t st, int 
     // Measured on an H100 80GB HBM3 (600 W limit): the two larger images of the RPN backbone -- the FP0 chain, 144 KB
     // (2 warpgroups per SM), and its projection, 128 KB (3) -- ran 1.33x and 1.16x slower resident than streamed.
     if (2 * w_bytes > (size_t)max_optin) return false;
-    // a warpgroup's work region: its layer-0 A slots, the activations of the widest inner layer, its pool staging
+    // two 64-row tiles per warpgroup where every layer is at most 64 wide: a tile's serial steps (row table, gather, MMA,
+    // drain, barrier, epilogue per layer, pool) are short there, and the pair halves their count per row
+    const int T = np_max <= 64 ? 2 : 1;
+    // a tile's work region: its layer-0 A slots, the activations of the widest inner layer (the pool maxima fit in either)
     const int slots = p.nchunks[0] < A_SLOTS ? p.nchunks[0] : A_SLOTS;
     int work = slots * A_STAGE_BYTES;
     if (TM * mid_max * 4 > work) work = TM * mid_max * 4;
-    if (TM * POOL_STRIDE * 4 > work) work = TM * POOL_STRIDE * 4;
     work = round_up(work, 1024);
     const int np_last = p.np[L - 1];
     auto smem_for = [&](int nwg) -> size_t {
         return 1024 /*alignment slack*/ + w_bytes + 2 * (size_t)np_total * sizeof(float) +
-               (size_t)nwg * (work + np_last * sizeof(float) + sizeof(TileRows));
+               (size_t)nwg * (T * (work + sizeof(TileRows)) + np_last * sizeof(float));
     };
     if (smem_for(1) + 64 /*static: the weight mbarrier*/ > (size_t)max_optin) return false;
     p.work_bytes = work;
@@ -813,15 +903,17 @@ static bool launch_resident(ChainParams &p, int max_optin, cudaStream_t st, int 
         }
         int sms = num_sms();
         if (const int v = opts().mlp_sms; v >= 1 && v < sms) sms = v;
-        const int ctas = (p.num_items + best_nwg - 1) / best_nwg;   // every CTA has an item for its warpgroup 0
+        const int units = T == 2 ? (p.num_tiles + 1) / 2 : p.num_items;
+        const int ctas = (units + best_nwg - 1) / best_nwg;   // every CTA has a unit for its warpgroup 0
         const int grid = ctas < sms * best_occ ? ctas : sms * best_occ;
         kern<<<grid, best_nwg * 128, smem_for(best_nwg), st>>>(p);
         return check_launch("mlp_resident_kernel");
     };
-    const int ns = np_max >> 5;
-    // register bounds without spills: <1, 5> 96 (five warpgroups per SM), <4, 4> 128 (four); a 64-wide chain takes the
-    // <4, 4> build, whose m64n64 path needs no more registers than the <2, *> builds that were tried and spilled
-    *rc = ns <= 1 ? go(mlp_resident_kernel<1, 5, 1>, 5) : go(mlp_resident_kernel<4, 4, 1>, 4);
+    // register bounds without spills: <1, 4, 1, 2> and <4, 4, 1, 1> 128 (four warpgroups per SM), <2, 3, 1, 2> 168 (three);
+    // the pairs spilled at 96 and 128
+    if (np_max <= 32) *rc = go(mlp_resident_kernel<1, 4, 1, 2>, 4);
+    else if (np_max <= 64) *rc = go(mlp_resident_kernel<2, 3, 1, 2>, 3);
+    else *rc = go(mlp_resident_kernel<4, 4, 1, 1>, 4);
     return true;
 }
 
