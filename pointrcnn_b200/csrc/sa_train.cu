@@ -63,9 +63,12 @@ __device__ __forceinline__ float st_a0(const StGeom &G, int r, int k) {
     return G.feats_pm[src * G.c_feat + (k - 3)];
 }
 
+// ReLU that passes NaN through, as torch.relu does (fmaxf alone returns 0 for NaN); finite results keep fmaxf's bits
+__device__ __forceinline__ float st_relu(float x) { return isnan(x) ? x : fmaxf(x, 0.f); }
+
 __device__ __forceinline__ float st_act(const StGeom &G, const StLayer &P, int r, int k) {
     if (r >= G.rows || k >= P.c) return 0.f;
-    return fmaxf(fmaf(P.st[ST_A * kStMaxC + k], P.z[(size_t)r * P.c + k], P.st[ST_B * kStMaxC + k]), 0.f);
+    return st_relu(fmaf(P.st[ST_A * kStMaxC + k], P.z[(size_t)r * P.c + k], P.st[ST_B * kStMaxC + k]));
 }
 
 __device__ __forceinline__ float st_dz(const StGeom &G, const StGrad &L, int r, int c) {
@@ -256,7 +259,9 @@ __global__ void __launch_bounds__(kStThreads) sa_train_bn_finalise(int T, const 
     }
     if (threadIdx.x == 0) {
         const double mean = s[0][0] / n;
-        const double var = fmax(s[1][0] / n - mean * mean, 0.0);
+        // clamp the cancellation below zero only: a NaN variance stays NaN, as in torch
+        double var = s[1][0] / n - mean * mean;
+        if (var < 0.0) var = 0.0;
         const double invstd = 1.0 / sqrt(var + eps);
         const double ga = gamma ? gamma[c] : 1.0, be = beta ? beta[c] : 0.0;
         st[ST_MEAN * kStMaxC + c] = (float)mean;
@@ -270,7 +275,8 @@ __global__ void __launch_bounds__(kStThreads) sa_train_bn_finalise(int T, const 
 }
 
 // y = relu(max_s (a z + b)) per (group, channel) -> out (b, out_stride_c, npoint) and out_pm (b, npoint, out_stride_c) at
-// out_c_off; the first maximal sample is recorded
+// out_c_off; the first maximal sample is recorded.  A NaN sample wins, as in ATen's max-pool (the last NaN is recorded);
+// the backward's "a z + b > 0" test then drops its gradient, as torch's ReLU backward does.
 __global__ void __launch_bounds__(kStThreads) sa_train_pool(StGeom G, StLayer L, float *out, float *out_pm, int out_stride_c, int out_c_off,
                                                             unsigned char *chosen) {
     const long e = (long)blockIdx.x * kStThreads + threadIdx.x;
@@ -283,12 +289,12 @@ __global__ void __launch_bounds__(kStThreads) sa_train_pool(StGeom G, StLayer L,
     int arg = 0;
     for (int s = 1; s < G.ns; ++s) {
         const float v = fmaf(a, z[(size_t)s * L.c], b);
-        if (v > best) {
+        if (v > best || isnan(v)) {
             best = v;
             arg = s;
         }
     }
-    const float y = fmaxf(best, 0.f);
+    const float y = st_relu(best);
     const int bb = grp / G.npoint, p = grp - bb * G.npoint;
     out[((size_t)bb * out_stride_c + out_c_off + c) * G.npoint + p] = y;
     if (out_pm) out_pm[(size_t)grp * out_stride_c + out_c_off + c] = y;

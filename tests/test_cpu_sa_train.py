@@ -1,5 +1,6 @@
 """CPU side of the device SA training path: the C ABI exports and descriptor layout, CPU tensors refused, the dispatch rule,
-and the float64 reference's tolerances shown to catch each of the mistakes they guard against."""
+the float64 reference's tolerances shown to catch each of the mistakes they guard against, and the integer-valued cases
+of the exact GPU tests: the generator's cases pass the exactness check, which refuses an operand or a sum too large."""
 import copy
 import ctypes
 
@@ -152,11 +153,20 @@ def test_each_mutant_of_the_reference_exceeds_a_tolerance(mutant):
     assert max(R.all_ratios(R.scale(xyz, centres, feats, idx, layers, gout), ref).values()) == 0.0
 
 
-def test_reference_matches_the_torch_module_in_float64():
-    """the float64 reference is the torch module's own math: grouping, conv, train-mode BN, ReLU, max-pool, autograd"""
-    m, xyz, centres, feats, idx, gout = _case()
-    layers = R.layer_params(m.mlps[0])
-    ref = R.scale(xyz, centres, feats, idx, layers, gout)
+def _integer_bias_case():
+    """an integer-valued bias-only chain (sa_train_reference.integer_case) as a torch module and its inputs"""
+    B, N, P, ns, c_feat, widths = 2, 96, 16, 8, 2, [16, 16, 24]
+    case = R.integer_case(B, N, P, ns, c_feat, widths, seed=4)
+    m = PointnetSAModule(npoint=P, radius=1.0, nsample=ns, mlp=[c_feat] + widths, bn=False).train()
+    with torch.no_grad():
+        for layer, lay in zip(m.mlps[0].children(), case["layers"]):
+            layer.conv.weight.copy_(lay["w"].view_as(layer.conv.weight))
+            layer.conv.bias.copy_(lay["b"])
+    return m, case["xyz"], case["centres"], case["feats"], case["idx"].long(), case["grad_out"]
+
+
+def _torch_module_run(m, xyz, centres, feats, idx, gout):
+    """the torch module itself in float64 on the same grouping, with autograd -> (out, feature gradient, module)"""
     md = copy.deepcopy(m).double()
     f = feats.double().requires_grad_(True)
     bi = torch.arange(xyz.shape[0])[:, None, None]
@@ -165,11 +175,89 @@ def test_reference_matches_the_torch_module_in_float64():
     y = md.mlps[0](grouped)
     out = nn.functional.max_pool2d(y, kernel_size=[1, y.size(3)]).squeeze(-1)
     out.backward(gout.double())
+    return out, f.grad, md
+
+
+def test_reference_matches_the_torch_module_in_float64():
+    """the float64 reference is the torch module's own math: grouping, conv, train-mode BN, ReLU, max-pool, autograd"""
+    m, xyz, centres, feats, idx, gout = _case()
+    layers = R.layer_params(m.mlps[0])
+    ref = R.scale(xyz, centres, feats, idx, layers, gout)
+    out, f_grad, md = _torch_module_run(m, xyz, centres, feats, idx, gout)
     assert torch.allclose(out, ref["out"], rtol=1e-10, atol=1e-12)
-    assert torch.allclose(f.grad, ref["feats"], rtol=1e-8, atol=1e-10)
+    assert torch.allclose(f_grad, ref["feats"], rtol=1e-8, atol=1e-10)
     for l, layer in enumerate(md.mlps[0].children()):
         assert torch.allclose(layer.conv.weight.grad.flatten(1), ref["w"][l], rtol=1e-8, atol=1e-10)
         bn = layer.bn.bn
         assert torch.allclose(bn.weight.grad, ref["gamma"][l], rtol=1e-8, atol=1e-10)
         assert torch.allclose(bn.running_var, ref["running"][l][1], rtol=1e-10)
         assert int(bn.num_batches_tracked) == ref["running"][l][2]
+
+
+def test_reference_equals_the_torch_module_on_an_integer_bias_chain():
+    """on an integer-valued bias-only chain both the reference and the torch module are exact: they agree exactly"""
+    m, xyz, centres, feats, idx, gout = _integer_bias_case()
+    layers = R.layer_params(m.mlps[0])
+    ref = R.scale(xyz, centres, feats, idx, layers, gout)
+    R.check_exact(dict(xyz=xyz, centres=centres, feats=feats, idx=idx, layers=layers), ref)
+    out, f_grad, md = _torch_module_run(m, xyz, centres, feats, idx, gout)
+    assert torch.equal(out, ref["out"]) and torch.equal(f_grad, ref["feats"])
+    assert f_grad.abs().max() > 0
+    for l, layer in enumerate(md.mlps[0].children()):
+        assert torch.equal(layer.conv.weight.grad.flatten(1), ref["w"][l]), l
+        assert torch.equal(layer.conv.bias.grad, ref["b"][l]), l
+
+
+# ---------------------------------------------------------------------------------------------- exact integer cases
+EXACT_CASES = [
+    # B, N, npoint, ns, c_feat, widths, bn, group_all
+    (1, 40, 3, 4, 0, [1], False, False),
+    (2, 300, 37, 8, 29, [40, 63, 64], False, False),
+    (2, 200, 9, 64, 62, [196], False, False),
+    (1, 600, 6, 16, 509, [512, 1, 24], False, False),
+    (2, 100, 11, 4, 128, [64, 65, 40], False, False),
+    (3, 500, 41, 32, 1, [32, 32, 64], True, False),
+    (4, 32, 1, 32, 256, [256, 256, 512], False, True),
+]
+
+
+def _exact_case(B, N, npoint, ns, c_feat, widths, bn, group_all):
+    case = R.integer_case(B, N, npoint, ns, c_feat, widths, seed=B * 7 + ns + c_feat, bn=bn, group_all=group_all)
+    ref = R.scale(case["xyz"], case["centres"], case["feats"], case["idx"], case["layers"], None if bn else case["grad_out"])
+    return case, ref
+
+
+@pytest.mark.parametrize("B,N,npoint,ns,c_feat,widths,bn,group_all", EXACT_CASES)
+def test_exactness_check_accepts_the_generated_cases(B, N, npoint, ns, c_feat, widths, bn, group_all):
+    case, ref = _exact_case(B, N, npoint, ns, c_feat, widths, bn, group_all)
+    R.check_exact(case, ref, layers_exact=1 if bn else None)
+    idx = case["idx"].long()
+    assert (idx[:, :, 1:] == idx[:, :, :1]).any() or group_all, "no ball-query padding"
+    assert int(idx[-1, -1].max()) == N - 1
+    if not bn:
+        assert all(int((dz != 0).any(1).sum()) > 0 for dz in ref["dz"]), "a layer without gradient"
+    w0 = case["layers"][0]["w"]
+    assert (w0 != 0).any(0).all(), "an input column no weight reads"
+
+
+def test_exactness_check_rejects_a_tf32_operand_of_2049():
+    case, _ = _exact_case(2, 300, 37, 8, 29, [40, 63, 64], False, False)
+    case["feats"][0, 5, case["idx"][0, 0, 0]] = 2049.0
+    ref = R.scale(case["xyz"], case["centres"], case["feats"], case["idx"], case["layers"], case["grad_out"])
+    with pytest.raises(AssertionError, match="layer 0 input reaches 2049"):
+        R.check_exact(case, ref)
+
+
+def test_exactness_check_rejects_an_absolute_sum_of_2_to_the_24():
+    """four products of 2048 x 2048 in one row of |A| |W|^T: every operand is allowed, their sum is not"""
+    case, _ = _exact_case(2, 300, 37, 8, 4, [8], False, False)
+    case["feats"][0, :, case["idx"][0, 0, 0]] = 2048.0
+    w = case["layers"][0]["w"]
+    w[0, 3:7] = 2048.0
+    ref = R.scale(case["xyz"], case["centres"], case["feats"], case["idx"], case["layers"], case["grad_out"])
+    with pytest.raises(AssertionError, match="layer 0 forward"):
+        R.check_exact(case, ref)
+    w[0, 6] = 2047.0                                    # one below: 2^24 - 2^11 plus the other columns still passes
+    w[0, :3] = 0.0
+    ref = R.scale(case["xyz"], case["centres"], case["feats"], case["idx"], case["layers"], case["grad_out"])
+    R.check_exact(case, ref)

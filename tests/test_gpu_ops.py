@@ -371,6 +371,80 @@ def test_three_interpolate_and_grad(cuda):
         assert torch.equal(got, R.three_interpolate(f, i, ww))
 
 
+# ------------------------------------------------------------------------------------------------ scatter backwards, exact
+# The atomic scatters of group_points_grad, gather_points_grad and three_interpolate_grad, bit for bit: on integer
+# gradients in [-8, 8] and weights in {0, 1/4, 1/2, 1} every product and partial sum is a multiple of 1/4 far below 2^22,
+# so fp32 is exact in any order of the atomics and a float64 index_add is the one right answer.  The shapes are those
+# of RPN training at B = 16, and ones whose grid-stride loop wraps: group_points_grad caps its grid at 1024 CTAs of 256
+# threads (262144 (centre, sample) pairs per pass), three_interpolate_grad at 64 (16384 unknown points per pass).
+def _int_grad(shape, g):
+    return torch.randint(-8, 9, shape, generator=g).float()
+
+
+def _scatter_idx(B, rows, n, g):
+    """random points in [0, n) with repeats, point n - 1 included"""
+    idx = torch.randint(0, n, (B, rows), generator=g, dtype=torch.int32)
+    idx[:, -1] = n - 1
+    return idx
+
+
+def _scatter_ref(gout, idx, n):
+    """(B, C, rows) gradients scattered by idx (B, rows) into (B, C, n), in float64"""
+    B, C, rows = gout.shape
+    out = torch.zeros(B, C, n, dtype=torch.float64, device=gout.device)
+    return out.scatter_add_(2, idx.long()[:, None, :].expand(B, C, rows), gout.double())
+
+
+@pytest.mark.parametrize("B,C,N,npoint,ns", [
+    (16, 1, 16384, 4096, 32),         # RPN SA1 features
+    (16, 96, 4096, 1024, 32),         # RPN SA2
+    (16, 256, 1024, 256, 32),         # RPN SA3
+    (2, 9, 40000, 16384, 32),         # 524288 pairs per scene: the grid-stride loop runs twice
+    (1, 3, 300000, 100000, 3),        # 300000 pairs: the loop wraps once; n > 16384
+])
+def test_group_points_grad_bits(cuda, B, C, N, npoint, ns):
+    g = torch.Generator().manual_seed(B * C + ns)
+    idx = _scatter_idx(B, npoint * ns, N, g).view(B, npoint, ns).to(cuda)
+    go = _int_grad((B, C, npoint, ns), g).to(cuda)
+    f = torch.zeros(B, C, N, device=cuda, requires_grad=True)
+    pu.grouping_operation(f, idx).backward(go)
+    want = _scatter_ref(go.view(B, C, -1), idx.view(B, -1), N)
+    assert want.abs().max() < 2 ** 22
+    assert torch.equal(f.grad.double(), want), int((f.grad.double() != want).sum())
+
+
+@pytest.mark.parametrize("B,C,N,npoint", [
+    (16, 3, 16384, 4096),             # the sampled centres of RPN SA1
+    (16, 96, 4096, 1024),
+    (2, 5, 300000, 280000),           # 280000 centres: the grid-stride loop wraps
+])
+def test_gather_points_grad_bits(cuda, B, C, N, npoint):
+    g = torch.Generator().manual_seed(B * C + npoint)
+    idx = _scatter_idx(B, npoint, N, g).to(cuda)
+    go = _int_grad((B, C, npoint), g).to(cuda)
+    f = torch.zeros(B, C, N, device=cuda, requires_grad=True)
+    pu.gather_operation(f, idx).backward(go)
+    assert torch.equal(f.grad.double(), _scatter_ref(go, idx, N))
+
+
+@pytest.mark.parametrize("B,C,n,m", [
+    (16, 128, 16384, 4096),           # RPN FP to the input points: exactly 64 CTAs of 256, no wrap
+    (16, 256, 4096, 1024),
+    (2, 13, 40000, 5000),             # n > 16384: the grid-stride loop wraps twice
+])
+def test_three_interpolate_grad_bits(cuda, B, C, n, m):
+    g = torch.Generator().manual_seed(B * C + n)
+    idx = _scatter_idx(B, n * 3, m, g).view(B, n, 3).to(cuda)
+    w = (torch.tensor([0.0, 0.25, 0.5, 1.0])[torch.randint(0, 4, (B, n, 3), generator=g)]).to(cuda)
+    go = _int_grad((B, C, n), g).to(cuda)
+    f = torch.zeros(B, C, m, device=cuda, requires_grad=True)
+    pu.three_interpolate(f, idx, w).backward(go)
+    contrib = (go.double()[:, :, :, None] * w.double()[:, None, :, :]).reshape(B, C, n * 3)
+    want = _scatter_ref(contrib, idx.view(B, -1), m)
+    assert want.abs().max() < 2 ** 22
+    assert torch.equal(f.grad.double(), want), int((f.grad.double() != want).sum())
+
+
 # ------------------------------------------------------------------------------------------------ roipool3d
 def _roi_scene(B, N, M, C, seed):
     rng = np.random.default_rng(seed)
