@@ -570,6 +570,29 @@ PRB_API int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n, i
                                   int out_c_off, float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma,
                                   float *const *grad_beta, float *grad_feats, void *workspace, size_t workspace_bytes, void *stream);
 
+/* --- training-mode FP module (csrc/sa_train.cu): three_interpolate + cat(skip) + SharedMLP of one PointnetFPModule,
+ * forward and backward for autograd, with the layers of a prb_sa_train_desc (c_in = c_interp + c_skip, at most 2048;
+ * layer-0 weight columns [interpolated | skip]).  rows = b * n; idx / weight (b, n, 3) are the three taps of every
+ * unknown point (prb three_nn_weights), known_pm (b, m, c_interp) the known features point-major, skip (b, c_skip, n)
+ * channel-major (c_skip 0: none).
+ * forward:  project 0 interpolates the known features on load; project 1 computes P = known Wi^T over the b * m known
+ *           rows first and interpolates P (the same Z up to rounding).  z[l] (rows, c_out[l]) and stats as in
+ *           prb_sa_train_forward; out (b, c_last, n) and, when non-NULL, out_pm (b, n, c_last) receive relu(a z + b).
+ * backward: from grad_out (b, c_last, n): grad_weight[l] written (layer 0: both column blocks), grad_bias / grad_gamma /
+ *           grad_beta as in prb_sa_train_backward, grad_known (b, c_interp, m) and grad_skip (b, c_skip, n) WRITTEN where
+ *           non-NULL.  The interpolation's transpose runs through a reverse index of the taps: no float atomics, every
+ *           result is the same bits on every call.
+ * Neither entry allocates or synchronises. */
+PRB_API size_t prb_fp_train_workspace_bytes(int b, int n, int m, int c_interp, int c_skip, const prb_sa_train_desc *desc, int backward);
+PRB_API int prb_fp_train_forward(const prb_sa_train_desc *desc, int b, int n, int m, int c_interp, int c_skip, int project, const int *idx,
+                                 const float *weight, const float *known_pm, const float *skip, float *const *z, float *stats, float *out,
+                                 float *out_pm, void *workspace, size_t workspace_bytes, void *stream);
+PRB_API int prb_fp_train_backward(const prb_sa_train_desc *desc, int b, int n, int m, int c_interp, int c_skip, const int *idx,
+                                  const float *weight, const float *known_pm, const float *skip, const float *const *z, const float *stats,
+                                  const float *grad_out, float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma,
+                                  float *const *grad_beta, float *grad_known, float *grad_skip, void *workspace, size_t workspace_bytes,
+                                  void *stream);
+
 #ifdef __cplusplus
 }
 #endif

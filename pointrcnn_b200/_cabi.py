@@ -75,7 +75,8 @@ def lib():
         for name in ("prb_nms_workspace_bytes", "prb_mlp_packed_bytes", "prb_mlp_packed_bytes_ex",
                      "prb_sa_workspace_bytes", "prb_fp_workspace_bytes", "prb_rows_workspace_bytes", "prb_rows2_workspace_bytes", "prb_grid_workspace_bytes",
                      "prb_fps_workspace_bytes", "prb_fps_ordered_workspace_bytes", "prb_kitti_format_detections", "prb_rpn_proposals_workspace_bytes", "prb_roipool3d_workspace_bytes",
-                     "prb_kitti_eval_workspace_bytes", "prb_stage_loss_workspace_bytes", "prb_sa_train_workspace_bytes"):
+                     "prb_kitti_eval_workspace_bytes", "prb_stage_loss_workspace_bytes", "prb_sa_train_workspace_bytes",
+                     "prb_fp_train_workspace_bytes"):
             getattr(L, name).restype = c_size_t
         P, I, F, U = c_void_p, c_int, c_float, ctypes.c_uint
         L.prb_rcnn_sample_rois.argtypes = [I, I, I, P, P, P, P, P, I, I, F, F, F, F, ctypes.c_double, I, I, I, I, I, F, U, P, P, P, P, P, P,
@@ -89,6 +90,9 @@ def lib():
         L.prb_sa_train_workspace_bytes.argtypes = [I, I, I, I, P, I]
         L.prb_sa_train_forward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, I, I, P, c_size_t, P]
         L.prb_sa_train_backward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, I, I, P, P, P, P, P, P, c_size_t, P]
+        L.prb_fp_train_workspace_bytes.argtypes = [I, I, I, I, I, P, I]
+        L.prb_fp_train_forward.argtypes = [P, I, I, I, I, I, I, P, P, P, P, P, P, P, P, P, c_size_t, P]
+        L.prb_fp_train_backward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P, P, c_size_t, P]
         L.prb_options_init.restype = None
         L.prb_get_thread_options.restype = None
         if L.prb_abi_version() != 6:

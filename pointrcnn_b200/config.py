@@ -17,6 +17,9 @@ environment variables ONCE at import; at run time they are changed with `overrid
                     "device" (csrc/stage_loss.cu: two launches forward, one backward, no host synchronisation)
     sa_train        which path SA modules take when they need an autograd graph: "torch" (the op-by-op mirror, default) or
                     "device" (csrc/sa_train.cu through pointnet2/sa_train.py, where its rule holds)
+    fp_train        which path FP modules take when they need an autograd graph: "torch" (the op-by-op mirror, default) or
+                    "device" (prb_fp_train_* in csrc/sa_train.cu through pointnet2/fp_train.py, on the levels its rule
+                    selects); independent of sa_train
 """
 import contextlib
 import os
@@ -34,6 +37,7 @@ _DEFAULTS = dict(
     target_draw=os.environ.get("PRB_TARGET_DRAW", "torch"),
     loss_impl=os.environ.get("PRB_LOSS_IMPL", "torch"),
     sa_train=os.environ.get("PRB_SA_TRAIN", "torch"),
+    fp_train=os.environ.get("PRB_FP_TRAIN", "torch"),
 )
 _local = threading.local()
 

@@ -66,9 +66,16 @@ __device__ __forceinline__ float st_a0(const StGeom &G, int r, int k) {
 // ReLU that passes NaN through, as torch.relu does (fmaxf alone returns 0 for NaN); finite results keep fmaxf's bits
 __device__ __forceinline__ float st_relu(float x) { return isnan(x) ? x : fmaxf(x, 0.f); }
 
-__device__ __forceinline__ float st_act(const StGeom &G, const StLayer &P, int r, int k) {
-    if (r >= G.rows || k >= P.c) return 0.f;
+__device__ __forceinline__ float st_act(int rows, const StLayer &P, int r, int k) {
+    if (r >= rows || k >= P.c) return 0.f;
     return st_relu(fmaf(P.st[ST_A * kStMaxC + k], P.z[(size_t)r * P.c + k], P.st[ST_B * kStMaxC + k]));
+}
+
+// dZ from g (the upstream gradient of y, ReLU mask applied) and the pre-activation z
+__device__ __forceinline__ float st_dz_bn(const StGrad &L, int c, float z, float g) {
+    if (!L.bn) return g;
+    const float xhat = (z - L.st[ST_MEAN * kStMaxC + c]) * L.st[ST_INVSTD * kStMaxC + c];
+    return L.st[ST_A * kStMaxC + c] * (g - L.mg[c] - xhat * L.mg[kStMaxC + c]);
 }
 
 __device__ __forceinline__ float st_dz(const StGeom &G, const StGrad &L, int r, int c) {
@@ -86,10 +93,86 @@ __device__ __forceinline__ float st_dz(const StGeom &G, const StGrad &L, int r, 
             g = L.gout[((size_t)bb * L.out_stride_c + L.out_c_off + c) * G.npoint + p];
         }
     }
-    if (!L.bn) return g;
-    const float xhat = (z - L.st[ST_MEAN * kStMaxC + c]) * L.st[ST_INVSTD * kStMaxC + c];
-    return L.st[ST_A * kStMaxC + c] * (g - L.mg[c] - xhat * L.mg[kStMaxC + c]);
+    return st_dz_bn(L, c, z, g);
 }
+
+// ------------------------------------------------------------------------------------------------ row sources
+// The GEMM kernels stage their row operands through one of these: s(r, k) is row r, column k, and 0 outside the operand.
+struct SaA0Src {      // SA layer 0: the grouped row
+    StGeom G;
+    __device__ float operator()(int r, int k) const { return st_a0(G, r, k); }
+};
+struct ActSrc {       // relu(a Z + b) of a layer
+    int rows;
+    StLayer P;
+    __device__ float operator()(int r, int k) const { return st_act(rows, P, r, k); }
+};
+struct SaDzSrc {      // SA dZ; the last layer's g comes through the pooled choice
+    StGeom G;
+    StGrad L;
+    __device__ float operator()(int r, int c) const { return st_dz(G, L, r, c); }
+};
+struct DzSrc {        // dZ of a layer whose g is materialised (rows, c)
+    int rows;
+    StGrad L;
+    __device__ float operator()(int r, int c) const {
+        if (r >= rows || c >= L.c) return 0.f;
+        const size_t e = (size_t)r * L.c + c;
+        return st_dz_bn(L, c, L.z[e], L.g[e]);
+    }
+};
+struct MatSrc {       // a dense row-major matrix
+    int rows, cols, ld;
+    const float *p;
+    __device__ float operator()(int r, int k) const { return (r < rows && k < cols) ? p[(size_t)r * ld + k] : 0.f; }
+};
+
+// FP module: unknown row r = b * n + i takes three taps idx[r][t] (known points of its scene) with weights w[r][t]
+struct FpGeom {
+    int rows, n, m, ci, cs;
+    const int *idx;
+    const float *w;
+    const float *known_pm;    // (b, m, ci)
+    const float *skip;        // (b, cs, n)
+};
+
+// sum_t w_t x[b * m + idx_t][k] for row-major x of width ld, in three_interpolate's order
+__device__ __forceinline__ float fp_taps(const FpGeom &F, int r, const float *x, int ld, int k) {
+    const int *id = F.idx + (size_t)r * 3;
+    const float *w = F.w + (size_t)r * 3;
+    const float *base = x + (size_t)(r / F.n) * F.m * ld + k;
+    return fmaf(w[2], base[(size_t)id[2] * ld], fmaf(w[0], base[(size_t)id[0] * ld], w[1] * base[(size_t)id[1] * ld]));
+}
+
+__device__ __forceinline__ float fp_skip(const FpGeom &F, int r, int k) {
+    const int b = r / F.n;
+    return F.skip[((size_t)b * F.cs + k) * F.n + (r - b * F.n)];
+}
+
+struct FpA0Src {      // FP layer 0, plain: [interpolated known features | skip]
+    FpGeom F;
+    __device__ float operator()(int r, int k) const {
+        if (r >= F.rows || k >= F.ci + F.cs) return 0.f;
+        return k < F.ci ? fp_taps(F, r, F.known_pm, F.ci, k) : fp_skip(F, r, k - F.ci);
+    }
+};
+struct FpSkipSrc {    // FP skip columns alone
+    FpGeom F;
+    __device__ float operator()(int r, int k) const { return (r < F.rows && k < F.cs) ? fp_skip(F, r, k) : 0.f; }
+};
+
+// what the forward GEMM adds to its accumulator before storing Z
+struct NoAdd {
+    static constexpr bool kOn = false;
+    __device__ float operator()(int, int) const { return 0.f; }
+};
+struct FpTapAdd {     // projected FP layer 0: the three-tap sum of the projected known rows (b * m, c1)
+    static constexpr bool kOn = true;
+    FpGeom F;
+    const float *proj;
+    int c1;
+    __device__ float operator()(int r, int c) const { return fp_taps(F, r, proj, c1, c); }
+};
 
 // ------------------------------------------------------------------------------------------------ tensor-core tile
 // BM x BN outputs per CTA, 8 warps of 32 x (BN / WN).  Operands live in shared memory in the orientation they are read
@@ -192,10 +275,11 @@ using StRowsTile = StTile<kStRowTile, kStColTile, false, false>;   // forward: A
 using StDaTile = StTile<kStRowTile, kStColTile, false, true>;      // dA: A = dZ [row][k], B = W [k][n]
 using StDwTile = StTile<64, 64, true, true>;                       // dW: A = dZ [row][m], B = A_l [row][n]
 
-// Z_l = A_l W_l^T; with BN also the column sums of z and z^2 of this row tile
-template <bool L0>
-__global__ void __launch_bounds__(kStThreads) sa_train_fwd_gemm(StGeom G, StLayer P, const float *__restrict__ W, int cin, int cout,
-                                                                float *__restrict__ z, int bn, int T, double *p1, double *p2) {
+// Z_l = A_l W_l^T (+ add(r, c)); with BN also the column sums of z and z^2 of this row tile.  W is (cout, cin) with row
+// pitch ldw (a column block of a wider weight).
+template <class Src, class Add>
+__global__ void __launch_bounds__(kStThreads) sa_train_fwd_gemm(Src A, Add add, int rows, const float *__restrict__ W, int ldw, int cin,
+                                                                int cout, float *__restrict__ z, int bn, int T, double *p1, double *p2) {
     using Tl = StRowsTile;
     __shared__ __align__(16) float sA[Tl::A_FLOATS];
     __shared__ __align__(16) float sB[Tl::B_FLOATS];
@@ -203,9 +287,9 @@ __global__ void __launch_bounds__(kStThreads) sa_train_fwd_gemm(StGeom G, StLaye
     const int r0 = blockIdx.x * kStRowTile, n0 = blockIdx.y * kStColTile;
     float acc[2][Tl::NI][4] = {};
     for (int k0 = 0; k0 < cin; k0 += kStBK) {
-        st_fill<kStRowTile, kStBK>(sA, Tl::SA, [&](int r, int k) { return L0 ? st_a0(G, r0 + r, k0 + k) : st_act(G, P, r0 + r, k0 + k); });
+        st_fill<kStRowTile, kStBK>(sA, Tl::SA, [&](int r, int k) { return A(r0 + r, k0 + k); });
         st_fill<kStColTile, kStBK>(sB, Tl::SB, [&](int n, int k) {
-            return (n0 + n < cout && k0 + k < cin) ? W[(size_t)(n0 + n) * cin + k0 + k] : 0.f;
+            return (n0 + n < cout && k0 + k < cin) ? W[(size_t)(n0 + n) * ldw + k0 + k] : 0.f;
         });
         __syncthreads();
         Tl::mma(sA, sB, acc);
@@ -219,8 +303,11 @@ __global__ void __launch_bounds__(kStThreads) sa_train_fwd_gemm(StGeom G, StLaye
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const int r = r0 + Tl::row(mi, e), c = n0 + Tl::col(ni, e);
-                const float v = acc[mi][ni][e];          // rows past the end read zeros: v == 0
-                if (r < G.rows && c < cout) z[(size_t)r * cout + c] = v;
+                float v = acc[mi][ni][e];                // rows past the end read zeros: v == 0
+                if constexpr (Add::kOn) {
+                    if (r < rows && c < cout) v += add(r, c);
+                }
+                if (r < rows && c < cout) z[(size_t)r * cout + c] = v;
                 s1[ni][e & 1] += (double)v;
                 s2[ni][e & 1] += (double)v * (double)v;
             }
@@ -356,21 +443,53 @@ __global__ void __launch_bounds__(kStThreads) sa_train_grad_finalise(int T, cons
     }
 }
 
-// dA_l = dZ_l W_l.  TO_FEATS (layer 0): the feature columns are scattered into grad_feats (b, c_feat, n).  Otherwise the
-// result is masked by the previous layer's ReLU and stored as its g, with that layer's BN sums of g and g xhat.
-template <bool TO_FEATS>
-__global__ void __launch_bounds__(kStThreads) sa_train_da_gemm(StGeom G, StGrad L, const float *__restrict__ W, int cin, StLayer P,
-                                                               float *__restrict__ gprev, int T, double *p1, double *p2, float *grad_feats) {
+// what the dA GEMM does with each output element (r, c) = v
+struct DaScatterFeats {     // SA layer 0: the feature columns are scattered into grad_feats (b, c_feat, n)
+    static constexpr bool kSums = false;
+    StGeom G;
+    float *grad_feats;
+    __device__ void operator()(int r, int c, float v, float &, float &) const {
+        if (c >= 3) {
+            const int bb = (r >> G.log_ns) / G.npoint;
+            atomicAdd(grad_feats + ((size_t)bb * G.c_feat + (c - 3)) * G.n + G.idx[r], v);
+        }
+    }
+};
+struct DaMasked {           // inner layer: masked by the previous layer's ReLU, stored as its g; g and xhat feed its BN sums
+    static constexpr bool kSums = true;
+    StLayer P;
+    float *gprev;
+    __device__ void operator()(int r, int c, float v, float &g, float &xhat) const {
+        const float zp = P.z[(size_t)r * P.c + c];
+        g = fmaf(P.st[ST_A * kStMaxC + c], zp, P.st[ST_B * kStMaxC + c]) > 0.f ? v : 0.f;
+        gprev[(size_t)r * P.c + c] = g;
+        xhat = (zp - P.st[ST_MEAN * kStMaxC + c]) * P.st[ST_INVSTD * kStMaxC + c];
+    }
+};
+struct DaChannelMajor {     // FP input gradients: row r = b * n + i of a (b, c, n) tensor
+    static constexpr bool kSums = false;
+    float *out;
+    int n, c;
+    __device__ void operator()(int r, int k, float v, float &, float &) const {
+        const int b = r / n;
+        out[((size_t)b * c + k) * n + (r - b * n)] = v;
+    }
+};
+
+// dA = dZ W for dZ (rows, K) staged through A and W (K, cin) with row pitch ldw; epi consumes the result
+template <class Src, class Epi>
+__global__ void __launch_bounds__(kStThreads) sa_train_da_gemm(Src A, Epi epi, int rows, int K, const float *__restrict__ W, int ldw, int cin,
+                                                               int T, double *p1, double *p2) {
     using Tl = StDaTile;
     __shared__ __align__(16) float sA[Tl::A_FLOATS];
     __shared__ __align__(16) float sB[Tl::B_FLOATS];
     __shared__ double red[Tl::WM][2][64];
     const int r0 = blockIdx.x * kStRowTile, n0 = blockIdx.y * kStColTile;
     float acc[2][Tl::NI][4] = {};
-    for (int k0 = 0; k0 < L.c; k0 += kStBK) {
-        st_fill<kStRowTile, kStBK>(sA, Tl::SA, [&](int r, int k) { return st_dz(G, L, r0 + r, k0 + k); });
+    for (int k0 = 0; k0 < K; k0 += kStBK) {
+        st_fill<kStRowTile, kStBK>(sA, Tl::SA, [&](int r, int k) { return A(r0 + r, k0 + k); });
         st_fill<kStBK, kStColTile>(sB, Tl::SB, [&](int k, int n) {
-            return (k0 + k < L.c && n0 + n < cin) ? W[(size_t)(k0 + k) * cin + n0 + n] : 0.f;
+            return (k0 + k < K && n0 + n < cin) ? W[(size_t)(k0 + k) * ldw + n0 + n] : 0.f;
         });
         __syncthreads();
         Tl::mma(sA, sB, acc);
@@ -384,44 +503,36 @@ __global__ void __launch_bounds__(kStThreads) sa_train_da_gemm(StGeom G, StGrad 
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const int r = r0 + Tl::row(mi, e), c = n0 + Tl::col(ni, e);
-                if (r >= G.rows || c >= cin) continue;
-                const float v = acc[mi][ni][e];
-                if (TO_FEATS) {
-                    if (c >= 3) {
-                        const int bb = (r >> G.log_ns) / G.npoint;
-                        atomicAdd(grad_feats + ((size_t)bb * G.c_feat + (c - 3)) * G.n + G.idx[r], v);
-                    }
-                } else {
-                    const float zp = P.z[(size_t)r * cin + c];
-                    const float g = fmaf(P.st[ST_A * kStMaxC + c], zp, P.st[ST_B * kStMaxC + c]) > 0.f ? v : 0.f;
-                    gprev[(size_t)r * cin + c] = g;
+                if (r >= rows || c >= cin) continue;
+                float g, xhat;
+                epi(r, c, acc[mi][ni][e], g, xhat);
+                if constexpr (Epi::kSums) {
                     s1[ni][e & 1] += (double)g;
-                    s2[ni][e & 1] += (double)g * (double)((zp - P.st[ST_MEAN * kStMaxC + c]) * P.st[ST_INVSTD * kStMaxC + c]);
+                    s2[ni][e & 1] += (double)g * (double)xhat;
                 }
             }
-    if (!TO_FEATS) st_col_sums<Tl>(s1, s2, red, n0, cin, T, blockIdx.x, p1, p2);
+    if constexpr (Epi::kSums) st_col_sums<Tl>(s1, s2, red, n0, cin, T, blockIdx.x, p1, p2);
 }
 
-// partial dW_l = dZ_l^T A_l over the rows [blockIdx.z * chunk, +chunk) -> part[blockIdx.z][cout][cin]
-template <bool L0>
-__global__ void __launch_bounds__(kStThreads) sa_train_dw_gemm(StGeom G, StGrad L, StLayer P, int cin, int chunk, float *__restrict__ part) {
+// partial dW = dZ^T A over the rows [blockIdx.z * chunk, +chunk) -> part[blockIdx.z][cout][cin]; dZ (rows, cout) staged
+// through D, A (rows, cin) through S
+template <class SrcD, class SrcA>
+__global__ void __launch_bounds__(kStThreads) sa_train_dw_gemm(SrcD D, SrcA S, int rows, int cout, int cin, int chunk,
+                                                               float *__restrict__ part) {
     using Tl = StDwTile;
     __shared__ __align__(16) float sA[Tl::A_FLOATS];
     __shared__ __align__(16) float sB[Tl::B_FLOATS];
     const int m0 = blockIdx.x * 64, n0 = blockIdx.y * 64;
-    const int q0 = blockIdx.z * chunk, q1 = min(G.rows, q0 + chunk);
+    const int q0 = blockIdx.z * chunk, q1 = min(rows, q0 + chunk);
     float acc[2][Tl::NI][4] = {};
     for (int k0 = q0; k0 < q1; k0 += kStBK) {
-        st_fill<kStBK, 64>(sA, Tl::SA, [&](int k, int m) { return k0 + k < q1 ? st_dz(G, L, k0 + k, m0 + m) : 0.f; });
-        st_fill<kStBK, 64>(sB, Tl::SB, [&](int k, int n) {
-            if (k0 + k >= q1) return 0.f;
-            return L0 ? st_a0(G, k0 + k, n0 + n) : st_act(G, P, k0 + k, n0 + n);
-        });
+        st_fill<kStBK, 64>(sA, Tl::SA, [&](int k, int m) { return k0 + k < q1 ? D(k0 + k, m0 + m) : 0.f; });
+        st_fill<kStBK, 64>(sB, Tl::SB, [&](int k, int n) { return k0 + k < q1 ? S(k0 + k, n0 + n) : 0.f; });
         __syncthreads();
         Tl::mma(sA, sB, acc);
         __syncthreads();
     }
-    float *o = part + (size_t)blockIdx.z * L.c * cin;
+    float *o = part + (size_t)blockIdx.z * cout * cin;
 #pragma unroll
     for (int mi = 0; mi < 2; ++mi)
 #pragma unroll
@@ -429,19 +540,224 @@ __global__ void __launch_bounds__(kStThreads) sa_train_dw_gemm(StGeom G, StGrad 
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const int m = m0 + Tl::row(mi, e), n = n0 + Tl::col(ni, e);
-                if (m < L.c && n < cin) o[(size_t)m * cin + n] = acc[mi][ni][e];
+                if (m < cout && n < cin) o[(size_t)m * cin + n] = acc[mi][ni][e];
             }
 }
 
-__global__ void __launch_bounds__(kStThreads) sa_train_dw_reduce(int parts, int count, const float *part, float *dw) {
+// dw[m * ld + n] = the partials [parts][cout][ncol] summed in part order (count = cout * ncol)
+__global__ void __launch_bounds__(kStThreads) sa_train_dw_reduce(int parts, int count, int ncol, int ld, const float *part, float *dw) {
     const int e = blockIdx.x * kStThreads + threadIdx.x;
     if (e >= count) return;
     double s = 0.0;
     for (int p = 0; p < parts; ++p) s += part[(size_t)p * count + e];
-    dw[e] = (float)s;
+    dw[(size_t)(e / ncol) * ld + e % ncol] = (float)s;
+}
+
+// ------------------------------------------------------------------------------------------------ FP module
+// Training-mode forward and backward of one PointnetFPModule's three_interpolate + cat + SharedMLP (no pool), rows
+// r = b * n + i.  The inner layers are the SA kernels above with the row sources ActSrc / DzSrc.  Layer 0 reads
+// [I F | S] with I the (rows x b m) three-tap interpolation, F the known features (point-major), S the skip features
+// (channel-major); W_0 = [Wi | Ws].
+//   forward  plain: one GEMM whose A operand interpolates on load; projected: P = F Wi^T over the b m known rows, then
+//            Z_0 = S Ws^T + (three-tap sum of P) in one GEMM that also writes the BN column sums
+//   backward G = I^T dZ_0 from a reverse index of the taps (no float atomics), then dWi = G^T F, dF = G Wi,
+//            dWs = dZ_0^T S, dS = dZ_0 Ws
+// y_L = relu(a Z_L + b) -> out (b, c, n) and optionally its point-major twin (b, n, c), through a 32 x 32 tile
+__global__ void __launch_bounds__(kStThreads) fp_train_out(int rows, int n, StLayer L, float *out, float *out_pm) {
+    __shared__ float t[32][33];
+    const int r0 = blockIdx.x * 32, c0 = blockIdx.y * 32, tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
+    for (int i = ty; i < 32; i += kStThreads / 32) {
+        const int r = r0 + i, c = c0 + tx;
+        if (r < rows && c < L.c) {
+            const float y = st_act(rows, L, r, c);
+            t[i][tx] = y;
+            if (out_pm) out_pm[(size_t)r * L.c + c] = y;
+        }
+    }
+    __syncthreads();
+    for (int i = ty; i < 32; i += kStThreads / 32) {
+        const int c = c0 + i, r = r0 + tx;
+        if (r < rows && c < L.c) {
+            const int b = r / n;
+            out[((size_t)b * L.c + c) * n + (r - b * n)] = t[tx][i];
+        }
+    }
+}
+
+// the last layer: g = grad_out (b, c, n) where a z + b > 0, stored (rows, c) for the GEMMs, and the BN sums of g and
+// g xhat over each 128-row tile, in row order -> part[c * gridDim.x + blockIdx.x]
+__global__ void __launch_bounds__(kStThreads) fp_train_last_grad(int rows, int n, StGrad L, float *g, double *p1, double *p2) {
+    __shared__ float sg[32][kStRowTile + 1], sx[32][kStRowTile + 1];
+    const int r0 = blockIdx.x * kStRowTile, c0 = blockIdx.y * 32;
+    for (int e = threadIdx.x; e < 32 * kStRowTile; e += kStThreads) {
+        const int cl = e / kStRowTile, rl = e % kStRowTile, r = r0 + rl, c = c0 + cl;
+        float v = 0.f;
+        if (r < rows && c < L.c) {
+            const int b = r / n;
+            v = L.gout[((size_t)b * L.c + c) * n + (r - b * n)];
+        }
+        sg[cl][rl] = v;
+    }
+    __syncthreads();
+    for (int e = threadIdx.x; e < 32 * kStRowTile; e += kStThreads) {
+        const int rl = e / 32, cl = e % 32, r = r0 + rl, c = c0 + cl;
+        float v = 0.f, xhat = 0.f;
+        if (r < rows && c < L.c) {
+            const float z = L.z[(size_t)r * L.c + c];
+            v = fmaf(L.st[ST_A * kStMaxC + c], z, L.st[ST_B * kStMaxC + c]) > 0.f ? sg[cl][rl] : 0.f;
+            xhat = (z - L.st[ST_MEAN * kStMaxC + c]) * L.st[ST_INVSTD * kStMaxC + c];
+            g[(size_t)r * L.c + c] = v;
+        }
+        sg[cl][rl] = v;
+        sx[cl][rl] = xhat;
+    }
+    __syncthreads();
+    const int c = c0 + (int)threadIdx.x;
+    if (threadIdx.x < 32 && c < L.c) {
+        double s1 = 0.0, s2 = 0.0;
+        for (int rl = 0; rl < kStRowTile; ++rl) {
+            s1 += (double)sg[threadIdx.x][rl];
+            s2 += (double)sg[threadIdx.x][rl] * (double)sx[threadIdx.x][rl];
+        }
+        p1[(size_t)c * gridDim.x + blockIdx.x] = s1;
+        p2[(size_t)c * gridDim.x + blockIdx.x] = s2;
+    }
+}
+
+// Reverse index of the taps: the references q = 3 r + t of known point j = b * m + idx[q] end up in list[off[j] ..
+// off[j + 1]) in increasing q.  Counts and slots use integer atomics; the per-point sort fixes the order.
+__global__ void __launch_bounds__(kStThreads) fp_rev_count(FpGeom F, int *cnt) {
+    const int q = blockIdx.x * kStThreads + threadIdx.x;
+    if (q < 3 * F.rows) atomicAdd(cnt + (q / 3 / F.n) * F.m + F.idx[q], 1);
+}
+
+constexpr int kScanItems = 4 * kStThreads;   // counts per block of the offset scan
+
+// exclusive prefix of v over the block; total receives the block's sum
+__device__ __forceinline__ int st_block_scan(int v, int &total) {
+    __shared__ int ws[kStThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    int x = v;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const int y = __shfl_up_sync(0xffffffffu, x, o);
+        if (lane >= o) x += y;
+    }
+    if (lane == 31) ws[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+        int w = lane < kStThreads / 32 ? ws[lane] : 0;
+#pragma unroll
+        for (int o = 1; o < kStThreads / 32; o <<= 1) {
+            const int y = __shfl_up_sync(0xffffffffu, w, o);
+            if (lane >= o) w += y;
+        }
+        if (lane < kStThreads / 32) ws[lane] = w;
+    }
+    __syncthreads();
+    const int before = warp ? ws[warp - 1] : 0;
+    total = ws[kStThreads / 32 - 1];
+    __syncthreads();
+    return before + x - v;
+}
+
+// off[i] = the prefix of cnt within its block of kScanItems; tot[block] = the block's sum
+__global__ void __launch_bounds__(kStThreads) fp_scan_local(int K, const int *cnt, int *off, int *tot) {
+    const int base = blockIdx.x * kScanItems + threadIdx.x * 4;
+    int v[4], s = 0;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        v[i] = base + i < K ? cnt[base + i] : 0;
+        s += v[i];
+    }
+    int total;
+    int x = st_block_scan(s, total);
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+        if (base + i < K) off[base + i] = x;
+        x += v[i];
+    }
+    if (threadIdx.x == 0) tot[blockIdx.x] = total;
+}
+
+// one block: tot -> its exclusive prefix; off[K] = the sum of all counts
+__global__ void __launch_bounds__(kStThreads) fp_scan_blocks(int nb, int *tot, int *off_end) {
+    int carry = 0;
+    for (int b0 = 0; b0 < nb; b0 += kStThreads) {
+        const int i = b0 + (int)threadIdx.x;
+        const int v = i < nb ? tot[i] : 0;
+        int total;
+        const int x = st_block_scan(v, total);
+        if (i < nb) tot[i] = carry + x;
+        carry += total;
+    }
+    if (threadIdx.x == 0) *off_end = carry;
+}
+
+__global__ void __launch_bounds__(kStThreads) fp_scan_add(int K, const int *tot, int *off) {
+    const int i = blockIdx.x * kStThreads + threadIdx.x;
+    if (i < K) off[i] += tot[i / kScanItems];
+}
+
+// each reference into a free slot of its point (cnt counts down to 0)
+__global__ void __launch_bounds__(kStThreads) fp_rev_fill(FpGeom F, const int *off, int *cnt, int *list) {
+    const int q = blockIdx.x * kStThreads + threadIdx.x;
+    if (q >= 3 * F.rows) return;
+    const int j = (q / 3 / F.n) * F.m + F.idx[q];
+    list[off[j] + atomicSub(cnt + j, 1) - 1] = q;
+}
+
+// every point's references in increasing order (heapsort: bounded work however many rows share a known point)
+__global__ void __launch_bounds__(kStThreads) fp_rev_sort(int K, const int *off, int *list) {
+    const int j = blockIdx.x * kStThreads + threadIdx.x;
+    if (j >= K) return;
+    int *a = list + off[j];
+    const int len = off[j + 1] - off[j];
+    auto sift = [a](int root, int end) {
+        for (;;) {
+            int ch = 2 * root + 1;
+            if (ch >= end) return;
+            if (ch + 1 < end && a[ch + 1] > a[ch]) ++ch;
+            if (a[root] >= a[ch]) return;
+            const int t = a[root];
+            a[root] = a[ch];
+            a[ch] = t;
+            root = ch;
+        }
+    };
+    for (int i = len / 2 - 1; i >= 0; --i) sift(i, len);
+    for (int e = len - 1; e > 0; --e) {
+        const int t = a[0];
+        a[0] = a[e];
+        a[e] = t;
+        sift(0, e);
+    }
+}
+
+// G = I^T dZ_0 (b m, c1): per known point the sum over its references in list order, one warp per point
+__global__ void __launch_bounds__(kStThreads) fp_train_gather_g(int K, const int *off, const int *list, const float *w, DzSrc D, float *G) {
+    const int j = blockIdx.x * (kStThreads / 32) + (threadIdx.x >> 5);
+    if (j >= K) return;
+    const int e0 = off[j], e1 = off[j + 1];
+    for (int c = threadIdx.x & 31; c < D.L.c; c += 32) {
+        float acc = 0.f;
+        for (int e = e0; e < e1; ++e) {
+            const int q = list[e];
+            acc = fmaf(w[q], D(q / 3, c), acc);
+        }
+        G[(size_t)j * D.L.c + c] = acc;
+    }
 }
 
 // ------------------------------------------------------------------------------------------------ host side
+// row split of a weight-gradient GEMM over `rows` rows: about kStWCtas CTAs, chunks a multiple of kStBK
+inline void st_wsplit(int rows, int cout, int cin, int &chunk, int &parts) {
+    const int tiles = ceil_div(cout, 64) * ceil_div(cin, 64);
+    parts = max(min(ceil_div(kStWCtas, tiles), ceil_div(rows, 256)), 1);
+    chunk = ceil_div(ceil_div(rows, parts), kStBK) * kStBK;
+    parts = ceil_div(rows, chunk);
+}
+
 struct StPlan {
     int L, cin[3], cout[3];
     long rows;
@@ -479,11 +795,7 @@ int st_plan(const prb_sa_train_desc *d, int b, int npoint, int ns, int c_feat, S
     p.P = ceil_div(groups, p.gpp);
     size_t wpart = 0;
     for (int l = 0; l < p.L; ++l) {
-        const int tiles = ceil_div(p.cout[l], 64) * ceil_div(p.cin[l], 64);
-        int parts = min(ceil_div(kStWCtas, tiles), ceil_div((int)rows, 256));
-        parts = max(parts, 1);
-        p.wchunk[l] = ceil_div(ceil_div((int)rows, parts), kStBK) * kStBK;
-        p.wparts[l] = ceil_div((int)rows, p.wchunk[l]);
+        st_wsplit((int)rows, p.cout[l], p.cin[l], p.wchunk[l], p.wparts[l]);
         wpart = std::max(wpart, (size_t)p.wparts[l] * p.cout[l] * p.cin[l]);
     }
     const size_t nparts = (size_t)cmax * max(p.T, p.P);
@@ -538,9 +850,11 @@ extern "C" int prb_sa_train_forward(const prb_sa_train_desc *desc, int b, int n,
         PRB_REQUIRE(z[l] && desc->weight[l], "sa_train_forward: layer %d: no Z buffer or weight", l);
         const dim3 grid(p.T, ceil_div(p.cout[l], kStColTile));
         if (l == 0)
-            sa_train_fwd_gemm<true><<<grid, kStThreads, 0, s>>>(G, prev, desc->weight[l], p.cin[l], p.cout[l], z[l], desc->bn, p.T, p1, p2);
+            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(SaA0Src{G}, NoAdd{}, G.rows, desc->weight[l], p.cin[l], p.cin[l], p.cout[l], z[l],
+                                                          desc->bn, p.T, p1, p2);
         else
-            sa_train_fwd_gemm<false><<<grid, kStThreads, 0, s>>>(G, prev, desc->weight[l], p.cin[l], p.cout[l], z[l], desc->bn, p.T, p1, p2);
+            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(ActSrc{G.rows, prev}, NoAdd{}, G.rows, desc->weight[l], p.cin[l], p.cin[l], p.cout[l],
+                                                          z[l], desc->bn, p.T, p1, p2);
         if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
         float *st = stats + (size_t)l * ST_ROWS * kStMaxC;
         sa_train_bn_finalise<<<p.cout[l], kStThreads, 0, s>>>(p.T, p1, p2, p.rows, desc->bn, desc->eps, desc->momentum, desc->gamma[l],
@@ -588,24 +902,241 @@ extern "C" int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n
         const StLayer prev = l ? StLayer{p.cout[l - 1], z[l - 1], stats + (size_t)(l - 1) * ST_ROWS * kStMaxC} : StLayer{0, nullptr, nullptr};
         const dim3 wgrid(ceil_div(p.cout[l], 64), ceil_div(p.cin[l], 64), p.wparts[l]);
         if (l == 0)
-            sa_train_dw_gemm<true><<<wgrid, kStThreads, 0, s>>>(G, Lg, prev, p.cin[l], p.wchunk[l], wpart);
+            sa_train_dw_gemm<<<wgrid, kStThreads, 0, s>>>(SaDzSrc{G, Lg}, SaA0Src{G}, G.rows, p.cout[l], p.cin[l], p.wchunk[l], wpart);
         else
-            sa_train_dw_gemm<false><<<wgrid, kStThreads, 0, s>>>(G, Lg, prev, p.cin[l], p.wchunk[l], wpart);
+            sa_train_dw_gemm<<<wgrid, kStThreads, 0, s>>>(SaDzSrc{G, Lg}, ActSrc{G.rows, prev}, G.rows, p.cout[l], p.cin[l], p.wchunk[l], wpart);
         if (int rc = check_launch("sa_train_dw_gemm")) return rc;
         PRB_REQUIRE(grad_weight[l], "sa_train_backward: layer %d: no weight gradient", l);
         const int count = p.cout[l] * p.cin[l];
-        sa_train_dw_reduce<<<ceil_div(count, kStThreads), kStThreads, 0, s>>>(p.wparts[l], count, wpart, grad_weight[l]);
+        sa_train_dw_reduce<<<ceil_div(count, kStThreads), kStThreads, 0, s>>>(p.wparts[l], count, p.cin[l], p.cin[l], wpart, grad_weight[l]);
         if (int rc = check_launch("sa_train_dw_reduce")) return rc;
         const dim3 agrid(p.T, ceil_div(p.cin[l], kStColTile));
         if (l > 0) {
             float *g_out = gbuf[(l - 1) & 1];
-            sa_train_da_gemm<false><<<agrid, kStThreads, 0, s>>>(G, Lg, desc->weight[l], p.cin[l], prev, g_out, p.T, p1, p2, nullptr);
+            sa_train_da_gemm<<<agrid, kStThreads, 0, s>>>(SaDzSrc{G, Lg}, DaMasked{prev, g_out}, G.rows, p.cout[l], desc->weight[l], p.cin[l],
+                                                          p.cin[l], p.T, p1, p2);
             if (int rc = check_launch("sa_train_da_gemm")) return rc;
             g_in = g_out;
             nparts = p.T;
         } else if (grad_feats && c_feat > 0) {
-            sa_train_da_gemm<true><<<agrid, kStThreads, 0, s>>>(G, Lg, desc->weight[0], p.cin[0], prev, nullptr, p.T, nullptr, nullptr,
-                                                                 grad_feats);
+            sa_train_da_gemm<<<agrid, kStThreads, 0, s>>>(SaDzSrc{G, Lg}, DaScatterFeats{G, grad_feats}, G.rows, p.cout[0], desc->weight[0],
+                                                          p.cin[0], p.cin[0], p.T, nullptr, nullptr);
+            if (int rc = check_launch("sa_train_da_gemm")) return rc;
+        }
+    }
+    return 0;
+}
+
+// ------------------------------------------------------------------------------------------------ FP module, host side
+namespace prb {
+
+constexpr int kFpMaxIn = 2048;     // widest layer-0 input (interpolated + skip channels)
+
+struct FpPlan {
+    int L, cin[3], cout[3], ci, cs;
+    int rows, krows;        // b n unknown rows, b m known rows
+    int T, KT;              // row tiles of the unknown / known rows
+    int wparts[3], wchunk[3];   // dW of layers 1.. and of Ws (index 0, over the unknown rows)
+    int wparts_i, wchunk_i;     // dWi over the known rows
+    int scan_blocks;
+    size_t off_p1, off_p2, off_proj, off_mg, off_wpart, off_g0, off_g1, off_cnt, off_off, off_tot, off_list;
+    size_t fwd_total, total;
+};
+
+int fp_plan(const prb_sa_train_desc *d, int b, int n, int m, int ci, int cs, FpPlan &p) {
+    PRB_REQUIRE(d, "fp_train: NULL descriptor");
+    PRB_REQUIRE(d->num_layers >= 1 && d->num_layers <= 3, "fp_train: %d layers (1..3)", d->num_layers);
+    PRB_REQUIRE(b >= 1 && n >= 1 && m >= 1, "fp_train: b %d, n %d, m %d", b, n, m);
+    PRB_REQUIRE(ci >= 1 && cs >= 0 && d->c_in == ci + cs && d->c_in <= kFpMaxIn, "fp_train: layer 0 reads %d channels, not %d + %d (at most %d)",
+                d->c_in, ci, cs, kFpMaxIn);
+    PRB_REQUIRE(3L * b * n < (1L << 30) && (long)b * m < (1L << 30), "fp_train: %d x %d rows", b, n);
+    p.L = d->num_layers;
+    p.ci = ci;
+    p.cs = cs;
+    p.rows = b * n;
+    p.krows = b * m;
+    int cmax = 0;
+    for (int l = 0; l < p.L; ++l) {
+        p.cin[l] = l ? d->c_out[l - 1] : d->c_in;
+        p.cout[l] = d->c_out[l];
+        PRB_REQUIRE(p.cout[l] >= 1 && p.cout[l] <= kStMaxC, "fp_train: layer %d has %d channels (1..%d)", l, p.cout[l], kStMaxC);
+        cmax = max(cmax, p.cout[l]);
+    }
+    p.T = ceil_div(p.rows, kStRowTile);
+    p.KT = ceil_div(p.krows, kStRowTile);
+    size_t wpart = 0;
+    for (int l = 1; l < p.L; ++l) {
+        st_wsplit(p.rows, p.cout[l], p.cin[l], p.wchunk[l], p.wparts[l]);
+        wpart = std::max(wpart, (size_t)p.wparts[l] * p.cout[l] * p.cin[l]);
+    }
+    st_wsplit(p.rows, p.cout[0], max(cs, 1), p.wchunk[0], p.wparts[0]);
+    wpart = std::max(wpart, (size_t)p.wparts[0] * p.cout[0] * cs);
+    st_wsplit(p.krows, p.cout[0], ci, p.wchunk_i, p.wparts_i);
+    wpart = std::max(wpart, (size_t)p.wparts_i * p.cout[0] * ci);
+    p.scan_blocks = ceil_div(p.krows, kScanItems);
+    const size_t nparts = (size_t)cmax * p.T;
+    p.off_p1 = 0;
+    p.off_p2 = st_align(p.off_p1 + nparts * sizeof(double));
+    p.off_proj = st_align(p.off_p2 + nparts * sizeof(double));     // forward: P = F Wi^T; backward: G = I^T dZ_0
+    p.fwd_total = st_align(p.off_proj + (size_t)p.krows * p.cout[0] * sizeof(float));
+    p.off_mg = p.fwd_total;
+    p.off_wpart = st_align(p.off_mg + 2 * kStMaxC * sizeof(float));
+    p.off_g0 = st_align(p.off_wpart + wpart * sizeof(float));
+    p.off_g1 = st_align(p.off_g0 + (size_t)p.rows * cmax * sizeof(float));
+    p.off_cnt = st_align(p.off_g1 + (size_t)p.rows * cmax * sizeof(float));
+    p.off_off = st_align(p.off_cnt + (size_t)p.krows * sizeof(int));
+    p.off_tot = st_align(p.off_off + (size_t)(p.krows + 1) * sizeof(int));
+    p.off_list = st_align(p.off_tot + (size_t)p.scan_blocks * sizeof(int));
+    p.total = st_align(p.off_list + (size_t)3 * p.rows * sizeof(int));
+    return 0;
+}
+
+}  // namespace prb
+
+extern "C" size_t prb_fp_train_workspace_bytes(int b, int n, int m, int c_interp, int c_skip, const prb_sa_train_desc *desc, int backward) {
+    FpPlan p;
+    if (fp_plan(desc, b, n, m, c_interp, c_skip, p)) return 0;
+    return backward ? p.total : p.fwd_total;
+}
+
+extern "C" int prb_fp_train_forward(const prb_sa_train_desc *desc, int b, int n, int m, int c_interp, int c_skip, int project, const int *idx,
+                                    const float *weight, const float *known_pm, const float *skip, float *const *z, float *stats, float *out,
+                                    float *out_pm, void *workspace, size_t workspace_bytes, void *stream) {
+    FpPlan p;
+    if (int rc = fp_plan(desc, b, n, m, c_interp, c_skip, p)) return rc;
+    PRB_REQUIRE(idx && weight && known_pm && (c_skip == 0 || skip) && z && stats && out && workspace, "fp_train_forward: bad arguments");
+    PRB_REQUIRE(workspace_bytes >= p.fwd_total, "fp_train_forward: workspace of %zu bytes < %zu", workspace_bytes, p.fwd_total);
+    PRB_REQUIRE(!desc->bn || p.rows > 1, "fp_train_forward: batch statistics need more than one value per channel");
+    const cudaStream_t s = (cudaStream_t)stream;
+    char *ws = reinterpret_cast<char *>(workspace);
+    double *p1 = reinterpret_cast<double *>(ws + p.off_p1), *p2 = reinterpret_cast<double *>(ws + p.off_p2);
+    const FpGeom F{p.rows, n, m, c_interp, c_skip, idx, weight, known_pm, skip};
+    StLayer prev{0, nullptr, nullptr};
+    for (int l = 0; l < p.L; ++l) {
+        PRB_REQUIRE(z[l] && desc->weight[l], "fp_train_forward: layer %d: no Z buffer or weight", l);
+        const float *W = desc->weight[l];
+        const dim3 grid(p.T, ceil_div(p.cout[l], kStColTile));
+        if (l > 0) {
+            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(ActSrc{p.rows, prev}, NoAdd{}, p.rows, W, p.cin[l], p.cin[l], p.cout[l], z[l], desc->bn,
+                                                          p.T, p1, p2);
+        } else if (project) {
+            float *proj = reinterpret_cast<float *>(ws + p.off_proj);
+            sa_train_fwd_gemm<<<dim3(p.KT, grid.y), kStThreads, 0, s>>>(MatSrc{p.krows, c_interp, c_interp, known_pm}, NoAdd{}, p.krows, W,
+                                                                        p.cin[0], c_interp, p.cout[0], proj, 0, 0, nullptr, nullptr);
+            if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
+            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(FpSkipSrc{F}, FpTapAdd{F, proj, p.cout[0]}, p.rows, W + c_interp, p.cin[0], c_skip,
+                                                          p.cout[0], z[0], desc->bn, p.T, p1, p2);
+        } else {
+            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(FpA0Src{F}, NoAdd{}, p.rows, W, p.cin[0], p.cin[0], p.cout[0], z[0], desc->bn, p.T,
+                                                          p1, p2);
+        }
+        if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
+        float *st = stats + (size_t)l * ST_ROWS * kStMaxC;
+        sa_train_bn_finalise<<<p.cout[l], kStThreads, 0, s>>>(p.T, p1, p2, p.rows, desc->bn, desc->eps, desc->momentum, desc->gamma[l],
+                                                              desc->beta[l], desc->bias[l], desc->running_mean[l], desc->running_var[l],
+                                                              desc->num_batches_tracked[l], st);
+        if (int rc = check_launch("sa_train_bn_finalise")) return rc;
+        prev = StLayer{p.cout[l], z[l], st};
+    }
+    fp_train_out<<<dim3(ceil_div(p.rows, 32), ceil_div(prev.c, 32)), kStThreads, 0, s>>>(p.rows, n, prev, out, out_pm);
+    return check_launch("fp_train_out");
+}
+
+extern "C" int prb_fp_train_backward(const prb_sa_train_desc *desc, int b, int n, int m, int c_interp, int c_skip, const int *idx,
+                                     const float *weight, const float *known_pm, const float *skip, const float *const *z, const float *stats,
+                                     const float *grad_out, float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma,
+                                     float *const *grad_beta, float *grad_known, float *grad_skip, void *workspace, size_t workspace_bytes,
+                                     void *stream) {
+    FpPlan p;
+    if (int rc = fp_plan(desc, b, n, m, c_interp, c_skip, p)) return rc;
+    PRB_REQUIRE(idx && weight && known_pm && (c_skip == 0 || skip) && z && stats && grad_out && grad_weight && workspace,
+                "fp_train_backward: bad arguments");
+    PRB_REQUIRE(workspace_bytes >= p.total, "fp_train_backward: workspace of %zu bytes < %zu", workspace_bytes, p.total);
+    for (int l = 0; l < p.L; ++l) PRB_REQUIRE(z[l] && desc->weight[l] && grad_weight[l], "fp_train_backward: layer %d: no Z, weight or gradient", l);
+    const cudaStream_t s = (cudaStream_t)stream;
+    char *ws = reinterpret_cast<char *>(workspace);
+    double *p1 = reinterpret_cast<double *>(ws + p.off_p1), *p2 = reinterpret_cast<double *>(ws + p.off_p2);
+    float *mg = reinterpret_cast<float *>(ws + p.off_mg), *wpart = reinterpret_cast<float *>(ws + p.off_wpart);
+    float *gbuf[2] = {reinterpret_cast<float *>(ws + p.off_g0), reinterpret_cast<float *>(ws + p.off_g1)};
+    float *G = reinterpret_cast<float *>(ws + p.off_proj);
+    int *cnt = reinterpret_cast<int *>(ws + p.off_cnt), *off = reinterpret_cast<int *>(ws + p.off_off);
+    int *tot = reinterpret_cast<int *>(ws + p.off_tot), *list = reinterpret_cast<int *>(ws + p.off_list);
+    const FpGeom F{p.rows, n, m, c_interp, c_skip, idx, weight, known_pm, skip};
+    const int last = p.L - 1;
+
+    // the reverse index depends only on the taps: build it first
+    if (cudaMemsetAsync(cnt, 0, (size_t)p.krows * sizeof(int), s) != cudaSuccess) return check_launch("fp_train_backward: memset");
+    const int qblocks = ceil_div(3 * p.rows, kStThreads);
+    fp_rev_count<<<qblocks, kStThreads, 0, s>>>(F, cnt);
+    if (int rc = check_launch("fp_rev_count")) return rc;
+    fp_scan_local<<<p.scan_blocks, kStThreads, 0, s>>>(p.krows, cnt, off, tot);
+    if (int rc = check_launch("fp_scan_local")) return rc;
+    fp_scan_blocks<<<1, kStThreads, 0, s>>>(p.scan_blocks, tot, off + p.krows);
+    if (int rc = check_launch("fp_scan_blocks")) return rc;
+    fp_scan_add<<<ceil_div(p.krows, kStThreads), kStThreads, 0, s>>>(p.krows, tot, off);
+    if (int rc = check_launch("fp_scan_add")) return rc;
+    fp_rev_fill<<<qblocks, kStThreads, 0, s>>>(F, off, cnt, list);
+    if (int rc = check_launch("fp_rev_fill")) return rc;
+    fp_rev_sort<<<ceil_div(p.krows, kStThreads), kStThreads, 0, s>>>(p.krows, off, list);
+    if (int rc = check_launch("fp_rev_sort")) return rc;
+
+    StGrad Lg{p.cout[last], desc->bn, z[last], stats + (size_t)last * ST_ROWS * kStMaxC, nullptr, grad_out, nullptr, p.cout[last], 0, mg};
+    const float *g_in = gbuf[last & 1];
+    fp_train_last_grad<<<dim3(p.T, ceil_div(p.cout[last], 32)), kStThreads, 0, s>>>(p.rows, n, Lg, gbuf[last & 1], p1, p2);
+    if (int rc = check_launch("fp_train_last_grad")) return rc;
+    for (int l = last; l >= 0; --l) {
+        Lg = StGrad{p.cout[l], desc->bn, z[l], stats + (size_t)l * ST_ROWS * kStMaxC, g_in, nullptr, nullptr, p.cout[l], 0, mg};
+        sa_train_grad_finalise<<<p.cout[l], kStThreads, 0, s>>>(p.T, p1, p2, p.rows, desc->bn, grad_gamma ? grad_gamma[l] : nullptr,
+                                                                grad_beta ? grad_beta[l] : nullptr, grad_bias ? grad_bias[l] : nullptr, mg);
+        if (int rc = check_launch("sa_train_grad_finalise")) return rc;
+        const DzSrc D{p.rows, Lg};
+        if (l > 0) {
+            // dW first: it reads this layer's g, which the dA launch below does not overwrite (it writes the other buffer)
+            const StLayer prev{p.cout[l - 1], z[l - 1], stats + (size_t)(l - 1) * ST_ROWS * kStMaxC};
+            sa_train_dw_gemm<<<dim3(ceil_div(p.cout[l], 64), ceil_div(p.cin[l], 64), p.wparts[l]), kStThreads, 0, s>>>(
+                D, ActSrc{p.rows, prev}, p.rows, p.cout[l], p.cin[l], p.wchunk[l], wpart);
+            if (int rc = check_launch("sa_train_dw_gemm")) return rc;
+            const int count = p.cout[l] * p.cin[l];
+            sa_train_dw_reduce<<<ceil_div(count, kStThreads), kStThreads, 0, s>>>(p.wparts[l], count, p.cin[l], p.cin[l], wpart, grad_weight[l]);
+            if (int rc = check_launch("sa_train_dw_reduce")) return rc;
+            float *g_out = gbuf[(l - 1) & 1];
+            sa_train_da_gemm<<<dim3(p.T, ceil_div(p.cin[l], kStColTile)), kStThreads, 0, s>>>(D, DaMasked{prev, g_out}, p.rows, p.cout[l],
+                                                                                              desc->weight[l], p.cin[l], p.cin[l], p.T, p1, p2);
+            if (int rc = check_launch("sa_train_da_gemm")) return rc;
+            g_in = g_out;
+            continue;
+        }
+        const int c1 = p.cout[0], cin0 = p.cin[0];
+        const float *W0 = desc->weight[0];
+        fp_train_gather_g<<<ceil_div(p.krows, kStThreads / 32), kStThreads, 0, s>>>(p.krows, off, list, weight, D, G);
+        if (int rc = check_launch("fp_train_gather_g")) return rc;
+        const MatSrc Gs{p.krows, c1, c1, G};
+        // dWi = G^T F
+        sa_train_dw_gemm<<<dim3(ceil_div(c1, 64), ceil_div(c_interp, 64), p.wparts_i), kStThreads, 0, s>>>(
+            Gs, MatSrc{p.krows, c_interp, c_interp, known_pm}, p.krows, c1, c_interp, p.wchunk_i, wpart);
+        if (int rc = check_launch("sa_train_dw_gemm")) return rc;
+        sa_train_dw_reduce<<<ceil_div(c1 * c_interp, kStThreads), kStThreads, 0, s>>>(p.wparts_i, c1 * c_interp, c_interp, cin0, wpart,
+                                                                                      grad_weight[0]);
+        if (int rc = check_launch("sa_train_dw_reduce")) return rc;
+        if (c_skip > 0) {
+            // dWs = dZ_0^T S
+            sa_train_dw_gemm<<<dim3(ceil_div(c1, 64), ceil_div(c_skip, 64), p.wparts[0]), kStThreads, 0, s>>>(D, FpSkipSrc{F}, p.rows, c1, c_skip,
+                                                                                                           p.wchunk[0], wpart);
+            if (int rc = check_launch("sa_train_dw_gemm")) return rc;
+            sa_train_dw_reduce<<<ceil_div(c1 * c_skip, kStThreads), kStThreads, 0, s>>>(p.wparts[0], c1 * c_skip, c_skip, cin0, wpart,
+                                                                                        grad_weight[0] + c_interp);
+            if (int rc = check_launch("sa_train_dw_reduce")) return rc;
+        }
+        if (grad_known) {
+            // dF = G Wi -> (b, c_interp, m)
+            sa_train_da_gemm<<<dim3(p.KT, ceil_div(c_interp, kStColTile)), kStThreads, 0, s>>>(Gs, DaChannelMajor{grad_known, m, c_interp}, p.krows,
+                                                                                               c1, W0, cin0, c_interp, 0, nullptr, nullptr);
+            if (int rc = check_launch("sa_train_da_gemm")) return rc;
+        }
+        if (grad_skip && c_skip > 0) {
+            // dS = dZ_0 Ws -> (b, c_skip, n)
+            sa_train_da_gemm<<<dim3(p.T, ceil_div(c_skip, kStColTile)), kStThreads, 0, s>>>(D, DaChannelMajor{grad_skip, n, c_skip}, p.rows, c1,
+                                                                                            W0 + c_interp, cin0, c_skip, 0, nullptr, nullptr);
             if (int rc = check_launch("sa_train_da_gemm")) return rc;
         }
     }

@@ -10,6 +10,8 @@ Two execution paths per module, chosen per call:
   train    (SA modules, opt-in with config.sa_train="device", autograd graph needed, batch-statistics BN or none, every
            layer at most sa_train.FAST_MAX_WIDTH wide):
            the fused path's sampling and ball query, then sa_train.py's autograd Function (csrc/sa_train.cu).
+           FP modules (opt-in with config.fp_train="device", levels fp_train.FAST_LEVELS selects): the fused path's
+           3-NN, then fp_train.py's autograd Function (csrc/sa_train.cu).
   unfused  (training / anything else): the reference's op-by-op sequence on the H100 natives with
            torch.nn convolutions, full autograd support.
 `config.override(disable_fused=True)` forces the unfused path (used by tests to cross-check the two).
@@ -23,6 +25,7 @@ import torch.nn.functional as F
 from .. import config
 from .. import mlp_chain
 from . import pointnet2_utils
+from . import fp_train
 from . import pytorch_utils as pt_utils
 from . import sa_train
 
@@ -343,6 +346,21 @@ class PointnetFPModule(nn.Module):
         idx, weight = self.fused_geometry(unknown, known)
         return self.fused_mlp(unknown.size(1), idx, weight, unknow_feats, known_feats)
 
+    def _train_projection(self, unknown, known, unknow_feats, known_feats):
+        """None: the device training path does not apply; else whether its layer 0 runs projected (fp_train's rule)"""
+        if config.get("fp_train") != "device" or not _needs_graph(self, unknown, known, unknow_feats, known_feats):
+            return None
+        if not fp_train.supported(self, unknown, known, unknow_feats, known_feats):
+            return None
+        return fp_train.projection(self, known_feats.size(1), 0 if unknow_feats is None else unknow_feats.size(1))
+
+    def _forward_train(self, unknown, known, unknow_feats, known_feats, project):
+        """the fused path's 3-NN, then fp_train's autograd Function"""
+        idx, weight = self.fused_geometry(unknown, known)
+        skip = unknow_feats.contiguous() if unknow_feats is not None else None
+        out, out_pm = fp_train.forward(self, idx, weight, _point_major(known_feats), known_feats, skip, project, self.emit_point_major)
+        return _attach_pm(out, out_pm) if out_pm is not None else out
+
     def forward(self, unknown: torch.Tensor, known: torch.Tensor, unknow_feats: torch.Tensor,
                 known_feats: torch.Tensor) -> torch.Tensor:
         """
@@ -354,6 +372,9 @@ class PointnetFPModule(nn.Module):
         """
         if self._can_fuse(unknown, known, unknow_feats, known_feats):
             return self._forward_fused(unknown, known, unknow_feats, known_feats)
+        project = self._train_projection(unknown, known, unknow_feats, known_feats)
+        if project is not None:
+            return self._forward_train(unknown, known, unknow_feats, known_feats, project)
 
         if known is not None:
             dist, idx = pointnet2_utils.three_nn(unknown, known)

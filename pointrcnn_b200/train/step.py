@@ -21,22 +21,25 @@ from ..rpn.stage import CLS_MEAN_SIZE, RPNStage
 from .losses import rcnn_loss, rpn_loss
 
 
-def _sa_switch(sa_train):
-    """the config.sa_train override of a trainer's forward (None: leave the switch as it is)"""
-    if sa_train is None:
-        return contextlib.nullcontext()
-    if sa_train not in ("torch", "device"):
-        raise ValueError("sa_train must be 'torch', 'device' or None, not %r" % (sa_train,))
-    return config.override(sa_train=sa_train)
+def _sa_switch(sa_train, fp_train=None):
+    """the config.sa_train / config.fp_train override of a trainer's forward (None: leave that switch as it is)"""
+    kw = {}
+    for name, value in (("sa_train", sa_train), ("fp_train", fp_train)):
+        if value is None:
+            continue
+        if value not in ("torch", "device"):
+            raise ValueError("%s must be 'torch', 'device' or None, not %r" % (name, value))
+        kw[name] = value
+    return config.override(**kw) if kw else contextlib.nullcontext()
 
 
 class RPNTrainer:
     """loss_impl: which stage-loss path forward_loss takes ("torch" / "device", see train.losses; None: the config switch).
     sa_train: which path the SA modules take in training ("torch" / "device", see pointnet2/sa_train.py; None: the config
-    switch)"""
+    switch).  fp_train: the same for the FP modules (see pointnet2/fp_train.py)"""
 
     def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, loss_impl=None,
-                 sa_train=None):
+                 sa_train=None, fp_train=None):
         torch.manual_seed(seed)                       # identical initial weights on every rank
         self.device = torch.device(device)
         self.model = RPNStage(input_channels=input_channels, mode="TRAIN").to(self.device).train()
@@ -47,11 +50,12 @@ class RPNTrainer:
         self.mean_size = torch.from_numpy(CLS_MEAN_SIZE[0]).to(self.device)
         self.loss_impl = loss_impl
         self.sa_train = sa_train
-        _sa_switch(sa_train)
+        self.fp_train = fp_train
+        _sa_switch(sa_train, fp_train)
 
     def forward_loss(self, pts_input, rpn_cls_label, rpn_reg_label):
         m = self.model
-        with _sa_switch(self.sa_train):
+        with _sa_switch(self.sa_train, self.fp_train):
             xyz, feats = m.backbone_net(pts_input)
         rpn_cls = m.rpn_cls_layer(feats).transpose(1, 2).contiguous()       # lib/net/rpn.py:76-77
         rpn_reg = m.rpn_reg_layer(feats).transpose(1, 2).contiguous()
