@@ -17,6 +17,12 @@ constexpr int NSUB_MAX = 8;          // 32-column subtiles per warpgroup (2 warp
 constexpr int RED_STRIDE = MAX_NP;   // SA pool: floats per warp of the per-warp maxima of a centre spanning several warps
 static_assert(4 * RED_STRIDE * 4 <= A_STAGE_BYTES, "the per-warp pool maxima fit in the smallest work region");
 constexpr int CHAIN_THREADS = 2 * 128 + 32;       // two MMA / epilogue warpgroups + one weight-producer warp
+// Threads of the streaming kernel with NS column subtiles per warpgroup and T tiles per CTA.  9 warps put 3 on one SM
+// sub-partition (16384 registers), so no thread gets more than 168 registers; a pair of 128-wide column halves needs 128
+// accumulators and more.  There the producer is a whole warpgroup that gives its registers to the MMA warpgroups with
+// setmaxnreg: 40 + 2 x 232 per sub-partition.
+constexpr int chain_threads(int ns, int t) { return t == 2 && ns > 2 ? 3 * 128 : CHAIN_THREADS; }
+constexpr int PRODUCER_REGS = 40, MMA_REGS = 232;
 constexpr int RES_NP_MAX = 128;      // resident kernel: widest layer (one warpgroup covers it: <= 64 accumulator registers)
 constexpr int RES_WG_MAX = 5;        // resident kernel: warpgroups per CTA, at most
 
@@ -92,6 +98,12 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void *src, uint32_t
 }
 // generic-proxy shared-memory stores become visible to the async proxy (wgmma operand reads)
 __device__ __forceinline__ void fence_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// per-thread register budget of the executing warpgroup (every thread of it runs the instruction)
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
@@ -200,8 +212,10 @@ struct TileRows {
     int valid[TM];
 };
 
+// static shared memory of the streaming kernel: the row tables of its T tiles and the weight ring's mbarriers
+template <int T>
 struct SmemFixed {
-    TileRows rows;
+    TileRows rows[T];
     uint64_t b_full[NB_MAX], b_empty[NB_MAX];
 };
 

@@ -40,6 +40,13 @@
 //                    next chunk while the current one runs.  The whole layer is drained before its epilogue.
 //   warp 8           weight producer: one thread streams pre-packed weight chunks (already in the K-major
 //                    SWIZZLE_128B image, see prb_mlp_pack_weights) with cp.async.bulk + mbarrier transaction counts.
+// Where the widest layer is 129-256 wide and a three-stage weight ring still fits beside two work regions (the SA3
+// chains of the RPN), a CTA runs tiles 2u and 2u + 1 together (T = 2): warpgroup s gathers tile s's row table and layer-0
+// chunks (all of a chunk's loads in flight at once), then each warpgroup issues two MMAs on the same B descriptor per K step for its column half of both tiles, and
+// the two tiles share every drain, barrier and epilogue pass.  The producer streams each chunk once per pair, so the L2
+// weight traffic halves.  The 128 accumulators per thread need more than the 168 registers 9 warps allow, so there the
+// producer is a whole warpgroup that hands its registers to the MMA warpgroups (setmaxnreg).  launch_chain holds the
+// per-launch timings the rule follows.
 // Chains whose activation buffer and weight stages do not fit in shared memory are split into several launches by
 // the host wrapper (rows materialised in between).
 // Precision: operands are rounded to TF32 (cvt.rn), products accumulate in fp32 -- the same contract as the
@@ -137,8 +144,9 @@ __device__ __forceinline__ void load_tile_rows(const ChainParams &p, int tile, i
 }
 
 // gather K chunk kc of the tile's layer-0 input rows, rounded to tf32, into the A chunk at A; returns the K=8 steps that
-// hold data (the rest of the chunk is padding)
-template <int NT>
+// hold data (the rest of the chunk is padding).  STEPS: row steps of a point-major segment whose loads are in flight
+// together (TM / (STEPS * NT / 8) dependent batches per chunk)
+template <int NT, int STEPS = 2>
 __device__ __forceinline__ int gather_chunk(const ChainParams &p, int tile, int kc, int t, const TileRows &M, uint8_t *A) {
     static_assert(NT == 128 || NT == 256, "gather_chunk: one or two warpgroups");
     int c = kc, seg = 0;
@@ -149,8 +157,9 @@ __device__ __forceinline__ int gather_chunk(const ChainParams &p, int tile, int 
     const bool rows_seg = (p.mode_in == IN_DIRECT) || (p.mode_in == IN_SA && seg == 0 && p.c_feat > 5) ||
                           (p.mode_in == IN_FP && seg == 0);
     if (rows_seg) {
-        // point-major sources: 8 threads cover one row's 128 bytes, NT threads NT/8 rows per step, two steps in flight
-        constexpr int RS = NT / 8, STEPS = 2;
+        // point-major sources: 8 threads cover one row's 128 bytes, NT threads NT/8 rows per step, STEPS steps in flight
+        constexpr int RS = NT / 8;
+        static_assert(TM % (STEPS * RS) == 0, "gather_chunk: whole batches of rows");
         const int j8 = t & 7, kk = k0 + 4 * j8;
 #pragma unroll 1
         for (int r0 = 0; r0 < TM; r0 += STEPS * RS) {
@@ -245,7 +254,7 @@ __device__ __forceinline__ int gather_chunk(const ChainParams &p, int tile, int 
         // along consecutive points
         const int r = t & (TM - 1);
         const long R = (long)tile * TM + r;
-#pragma unroll 1
+#pragma unroll(STEPS > 2 ? 256 / NT : 1)
         for (int i = 0; i < 256 / NT; ++i) {
             const int q8 = (t >> 6) + i * (NT / 64);
             float o[8];
@@ -457,19 +466,23 @@ __device__ __forceinline__ void load_scale_shift(const ChainParams &p, float *s_
 }
 
 // ------------------------------------------------------------------------------------------------ streaming kernel
-// NS: 32-column subtiles per warpgroup of the widest layer (accumulator registers: 16 * NS per thread)
-template <int NS, int MINB>
-__global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const ChainParams p) {
+// NS: 32-column subtiles per warpgroup of the widest layer.  T: 64-row tiles a CTA runs together (2: tiles 2u and 2u + 1
+// share every weight chunk, drain, barrier and epilogue pass).  Accumulator registers: 16 * NS * T per thread.
+template <int NS, int MINB, int T>
+__global__ void __launch_bounds__(chain_threads(NS, T), MINB) mlp_chain_kernel(const ChainParams p) {
+    static_assert(T == 1 || T == 2, "mlp_chain_kernel: one or two tiles per CTA");
+    constexpr int NTHR = chain_threads(NS, T);
     extern __shared__ uint8_t smem_raw[];
-    __shared__ SmemFixed S;
+    __shared__ SmemFixed<T> S;
     uint8_t *base = smem_raw + ((1024u - (s2u(smem_raw) & 1023u)) & 1023u);
     const int L = p.num_layers;
     int np_total = 0;
 #pragma unroll
     for (int l = 0; l < MAX_LAYERS; ++l) np_total += l < L ? p.np[l] : 0;
-    // work region, by phase of a tile: layer-0 A slots -> resident activations (layers >= 1) -> per-warp pool maxima
+    // T work regions of work_bytes, tile s at sW + s * work_bytes; by phase of a tile: layer-0 A slots -> resident
+    // activations (layers >= 1) -> per-warp pool maxima
     uint8_t *sW = base;
-    uint8_t *sB = sW + p.work_bytes;
+    uint8_t *sB = sW + (size_t)T * p.work_bytes;
     float *s_scale = reinterpret_cast<float *>(sB + (size_t)p.nb * p.b_stage_bytes);
     float *s_shift = s_scale + np_total;
     float *s_carry = s_shift + np_total;     // SA max over several tiles: partial maxima of the last layer
@@ -480,17 +493,23 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
         for (int i = 0; i < NB; ++i) { mbar_init(s2u(&S.b_full[i]), 1); mbar_init(s2u(&S.b_empty[i]), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    load_scale_shift(p, s_scale, s_shift, tid, CHAIN_THREADS);
+    load_scale_shift(p, s_scale, s_shift, tid, NTHR);
     __syncthreads();
+
+    // a unit is an item's tiles one after another (T = 1), or tiles 2u and 2u + 1 together (T = 2: two items of at most
+    // one tile, or the two tiles of one item); CTAs take units in a strided order
+    const int num_units = T == 1 ? p.num_items : (p.num_tiles + 1) >> 1;
+    const int steps = T == 1 ? p.tiles_per_item : 1;
 
     // the broadcast tells the compiler that wg -- and with it every column range and MMA width -- is warp-uniform
     const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
     if (wg == 2) {
-        // ===================================================== weight producer
-        if (lane == 0) {
+        // ===================================================== weight producer: every chunk once per step of a unit
+        if constexpr (NTHR == 3 * 128) setmaxnreg_dec<PRODUCER_REGS>();
+        if (tid == 2 * 128) {
             RingPos rb = {0, 0};
-            for (int item = blockIdx.x; item < p.num_items; item += gridDim.x)
-                for (int s = 0; s < p.tiles_per_item && item * p.tiles_per_item + s < p.num_tiles; ++s)
+            for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x)
+                for (int st = 0; st < steps && (T == 1 ? unit * p.tiles_per_item + st : 2 * unit) < p.num_tiles; ++st)
                     for (int l = 0; l < L; ++l) {
                         const int np_l = per_layer(p.np, l), nch = per_layer(p.nchunks, l);
                         const float *w = per_layer(p.w, l);
@@ -508,20 +527,27 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
     }
 
     // ===================================================== MMA / epilogue warpgroups
+    if constexpr (NTHR == 3 * 128) setmaxnreg_inc<MMA_REGS>();
     const int wq = warp & 3;
     const int g = lane >> 2, t4 = lane & 3;      // accumulator fragment: rows 16 wq + g (+8), columns 2 t4 (+1) of each 8
     const int tw = tid & 127;                    // thread inside the warpgroup
     RingPos rb = {0, 0};
     int aslot = 0;
-    float accs[1][16 * NS];
-    float (&acc)[16 * NS] = accs[0];             // subtile j (32 columns) = registers 16 j .. 16 j + 15
+    float acc[T][16 * NS];                       // tile s, subtile j (32 columns) = registers acc[s][16 j .. 16 j + 15]
+    // the row table and layer-0 gather of a tile: T = 1, both warpgroups (NT = 256 threads); T = 2, warpgroup wg alone runs
+    // tile wg of the unit (NT = 128) with twice the row steps in flight, so a pair's chunk costs one dependent batch of
+    // loads per thread, as a single tile's does: the gathers are latency-bound.  Every warpgroup's MMAs read both tiles'
+    // slots after the barrier that follows.
+    constexpr int NT = 256 / T;
+    const int my = T == 1 ? 0 : wg;              // this thread's tile of the unit for those stages
+    const int ti = T == 1 ? tid : tw;            // ... and its index among their NT threads
 
-    for (int item = blockIdx.x; item < p.num_items; item += gridDim.x) {
-        for (int s = 0; s < p.tiles_per_item; ++s) {
-            const int tile = item * p.tiles_per_item + s;
-            if (tile >= p.num_tiles) break;
-            bar_mma();   // the previous tile's readers of S.rows and of the pool maxima are done
-            load_tile_rows(p, tile, tid, S.rows);
+    for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+        for (int st = 0; st < steps; ++st) {
+            const int tile0 = T == 1 ? unit * p.tiles_per_item + st : 2 * unit;   // tile 2u + 1 may lie past the last
+            if (tile0 >= p.num_tiles) break;                                         // one: no valid rows, nothing written
+            bar_mma();   // the previous unit's readers of S.rows and of the pool maxima are done
+            load_tile_rows(p, tile0 + my, ti, S.rows[my]);
             bar_mma();
 
             int sc_base = 0;   // layer l's scale / shift in s_scale / s_shift
@@ -533,25 +559,28 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                 const int nch = per_layer(p.nchunks, l);
                 int prev_stage = -1;
                 for (int kc = 0; kc < nch; ++kc) {
-                    uint32_t a_addr;
+                    uint64_t adesc[T];
                     int ksteps = KC / 8;
                     if (l == 0) {
-                        uint8_t *A = sW + (size_t)aslot * A_STAGE_BYTES;
-                        ksteps = gather_chunk<2 * 128>(p, tile, kc, tid, S.rows, A);
+                        uint8_t *A = sW + (size_t)my * p.work_bytes + (size_t)aslot * A_STAGE_BYTES;
+                        ksteps = gather_chunk<NT, 2 * T>(p, tile0 + my, kc, ti, S.rows[my], A);
                         fence_async_smem();
-                        // slot `aslot` is complete.  It was last read by the MMAs of chunk kc-3, which both warpgroups
-                        // retired (wgmma_wait<1> of chunk kc-2) before the barrier of chunk kc-1.
+                        // slot `aslot` of every tile is complete.  It was last read by the MMAs of chunk kc-3, which both
+                        // warpgroups retired (wgmma_wait<1> of chunk kc-2) before the barrier of chunk kc-1.
                         bar_mma();
-                        a_addr = s2u(A);
+#pragma unroll
+                        for (int s = 0; s < T; ++s)
+                            adesc[s] = make_desc(s2u(sW + (size_t)s * p.work_bytes + (size_t)aslot * A_STAGE_BYTES));
                         aslot = aslot == A_SLOTS - 1 ? 0 : aslot + 1;
                     } else {
-                        a_addr = s2u(sW + (size_t)kc * A_STAGE_BYTES);
+#pragma unroll
+                        for (int s = 0; s < T; ++s)
+                            adesc[s] = make_desc(s2u(sW + (size_t)s * p.work_bytes + (size_t)kc * A_STAGE_BYTES));
                     }
                     mbar_wait(s2u(&S.b_full[rb.stage]), rb.phase);
                     const uint32_t b_addr = s2u(sB + (size_t)rb.stage * p.b_stage_bytes) + (uint32_t)col0 * (KC * 4);
                     wgmma_fence();
-                    const uint64_t adesc[1] = {make_desc(a_addr)};
-                    mma_chunk<NS, 1>(accs, nsub, ksteps, adesc, make_desc(b_addr), kc > 0 ? 1u : 0u);
+                    mma_chunk<NS, T>(acc, nsub, ksteps, adesc, make_desc(b_addr), kc > 0 ? 1u : 0u);
                     wgmma_commit();
                     wgmma_wait<1>();     // the previous chunk's MMAs are done: release its weight stage
                     if (prev_stage >= 0 && lane == 0) mbar_arrive(s2u(&S.b_empty[prev_stage]));
@@ -559,19 +588,27 @@ __global__ void __launch_bounds__(CHAIN_THREADS, MINB) mlp_chain_kernel(const Ch
                     rb.advance(NB);
                 }
                 wgmma_wait<0>();
-                reg_fence(acc);
+#pragma unroll
+                for (int s = 0; s < T; ++s) reg_fence(acc[s]);
                 if (lane == 0) mbar_arrive(s2u(&S.b_empty[prev_stage]));
-                bar_mma();   // both warpgroups' MMAs of layer l have read their A operand: the work region is free
+                bar_mma();   // both warpgroups' MMAs of layer l have read their A operands: the work regions are free
                 const float *sc = s_scale + sc_base, *sh = s_shift + sc_base;
                 sc_base += np_l;
 
                 if (l + 1 < L) {
-                    store_activations<NS>(p, acc, nsub, col0, wq, g, t4, sc, sh, sW);
+#pragma unroll
+                    for (int s = 0; s < T; ++s)
+                        store_activations<NS>(p, acc[s], nsub, col0, wq, g, t4, sc, sh, sW + (size_t)s * p.work_bytes);
                     fence_async_smem();
-                    bar_mma();   // the next layer's A operand is complete
+                    bar_mma();   // the next layer's A operands are complete
                     continue;
                 }
-                final_epilogue<NS>(p, acc, nsub, col0, wq, g, t4, tw, tile, sc, sh, reinterpret_cast<float *>(sW), s_carry, 2 + wg);
+                // an SA centre of two tiles (T = 2) carries its partial maxima from tile 0 to tile 1 in s_carry: the
+                // same thread writes and reads column c
+#pragma unroll
+                for (int s = 0; s < T; ++s)
+                    final_epilogue<NS>(p, acc[s], nsub, col0, wq, g, t4, tw, tile0 + s, sc, sh,
+                                       reinterpret_cast<float *>(sW + (size_t)s * p.work_bytes), s_carry, 2 + wg);
             }
         }
     }
@@ -834,19 +871,21 @@ int prb_mlp_pack_weights(int num_layers, int c_in, const int *c_out, const float
 
 namespace prb {
 
-// dynamic shared memory of a fused segment [l0, l1) with an nb-deep weight ring
-static size_t segment_smem(const int *np, int n, int nb, int *work_bytes, int *b_stage_bytes) {
+// shared memory of a fused segment [l0, l1) in the streaming kernel with t tiles per CTA and an nb-deep weight ring:
+// dynamic (returned) and static (*fixed); *work_bytes is one tile's work region
+static size_t segment_smem(const int *np, int n, int nb, int t, int *work_bytes, int *b_stage_bytes, size_t *fixed) {
     int np_total = 0, np_max = 0, mid_max = 0;
     for (int i = 0; i < n; ++i) {
         np_total += np[i];
         np_max = np[i] > np_max ? np[i] : np_max;
         if (i + 1 < n && np[i] > mid_max) mid_max = np[i];
     }
-    int work = A_SLOTS * A_STAGE_BYTES;
+    int work = A_SLOTS * A_STAGE_BYTES;   // a multiple of 8 KB, so every tile's region stays 1024-byte aligned
     if (TM * mid_max * 4 > work) work = TM * mid_max * 4;
     if (work_bytes) *work_bytes = work;
     if (b_stage_bytes) *b_stage_bytes = np_max * KC * 4;
-    return chain_smem_bytes(work, nb, np_max * KC * 4, np_total, np[n - 1]) + sizeof(SmemFixed);
+    if (fixed) *fixed = t == 2 ? sizeof(SmemFixed<2>) : sizeof(SmemFixed<1>);
+    return chain_smem_bytes(t * work, nb, np_max * KC * 4, np_total, np[n - 1]);
 }
 
 // Resident variant of one launch, if it applies: every layer at most RES_NP_MAX wide, one of the three plain mode pairs,
@@ -935,38 +974,51 @@ static int launch_chain(ChainParams &p, cudaStream_t st) {
         const int nsub0 = ((p.np[l] >> 5) + 1) >> 1;
         ns_max = nsub0 > ns_max ? nsub0 : ns_max;
     }
+    // A tile pair where the widest layer is 129-256 wide and the pair still has a weight ring of three stages: each
+    // warpgroup holds its column half of both tiles in 128 accumulator registers, and every weight chunk leaves L2 once
+    // per 128 rows instead of once per 64.  Single tile against pair, ms per launch of the RPN backbone at B = 16 (H100
+    // 80GB HBM3, 700 W limit):
+    //   SA3 [259]->128,196,256, ns 16 / 32 (pair ring 3)   0.156 / 0.299 -> 0.130 / 0.232
+    //   FP1 [512+96]->256,256 (pair ring 2, single 4)       0.367 -> 0.368
+    //   128 wide, FP0 chain / projection (pair 1 CTA per SM, single 2)   0.231 / 0.065 -> 0.316 / 0.079
+    size_t smem = 0, fixed = 0;
+    const int T = ns_max > 2 && ns_max <= 4 &&
+                  segment_smem(p.np, L, 3, 2, nullptr, nullptr, &fixed) + fixed <= (size_t)max_optin ? 2 : 1;
     // deepest weight ring that fits (a stage is one K chunk of the widest layer)
-    size_t smem = 0;
     for (p.nb = NB_MAX; p.nb >= 2; --p.nb) {
-        smem = segment_smem(p.np, L, p.nb, &p.work_bytes, &p.b_stage_bytes) - sizeof(SmemFixed);
-        if (smem + sizeof(SmemFixed) <= (size_t)max_optin) break;
+        smem = segment_smem(p.np, L, p.nb, T, &p.work_bytes, &p.b_stage_bytes, &fixed);
+        if (smem + fixed <= (size_t)max_optin) break;
     }
-    PRB_REQUIRE(p.nb >= 2, "mlp: %zu bytes of shared memory needed, %d available", smem + sizeof(SmemFixed), max_optin);
+    PRB_REQUIRE(p.nb >= 2, "mlp: %zu bytes of shared memory needed, %d available", smem + fixed, max_optin);
     // the accumulators of the widest layer set the register budget, and with it how many CTAs share an SM: several
     // CTAs of a narrow chain overlap one another's latency-bound gathers
-    auto go = [&](auto kern) -> int {
+    auto go = [&](auto kern, int threads) -> int {
         PRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         int occ = 0;
-        PRB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, CHAIN_THREADS, smem));
+        PRB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
         if (occ < 1) occ = 1;
         if (const int o = opts().mlp_occ; o >= 1 && o < occ) occ = o;
         int sms = num_sms();
         if (const int v = opts().mlp_sms; v >= 1 && v < sms) sms = v;
-        const int grid = p.num_items < sms * occ ? p.num_items : sms * occ;
-        kern<<<grid, CHAIN_THREADS, smem, st>>>(p);
+        const int units = T == 2 ? (p.num_tiles + 1) / 2 : p.num_items;
+        const int grid = units < sms * occ ? units : sms * occ;
+        kern<<<grid, threads, smem, st>>>(p);
         return check_launch("mlp_chain_kernel");
     };
-    // register bounds without spills: <2,2> 96, <4,1> 168 (the weight ring of a 256-wide chain leaves room for one CTA)
-    if (ns_max <= 2) return go(mlp_chain_kernel<2, 2>);
-    if (ns_max <= 4) return go(mlp_chain_kernel<4, 1>);
-    return go(mlp_chain_kernel<8, 1>);
+    // registers without spills: <2,2,1> 96 (two CTAs per SM), <4,1,1> 152; <4,1,2> 168 at launch, the MMA warpgroups
+    // raised to 232 by setmaxnreg
+    if (T == 2) return go(mlp_chain_kernel<4, 1, 2>, chain_threads(4, 2));
+    if (ns_max <= 2) return go(mlp_chain_kernel<2, 2, 1>, chain_threads(2, 1));
+    if (ns_max <= 4) return go(mlp_chain_kernel<4, 1, 1>, chain_threads(4, 1));
+    return go(mlp_chain_kernel<8, 1, 1>, chain_threads(8, 1));
 }
 
 // can layers [l0, l1) run as one launch: the activations of the widest inner layer and two weight stages in shared memory
 static bool fits(const LayerGeom *g, int l0, int l1) {
     int np[MAX_LAYERS];
     for (int l = l0; l < l1; ++l) np[l - l0] = g[l].np;
-    return segment_smem(np, l1 - l0, 2, nullptr, nullptr) <= 227 * 1024;
+    size_t fixed = 0;
+    return segment_smem(np, l1 - l0, 2, 1, nullptr, nullptr, &fixed) + fixed <= 227 * 1024;
 }
 
 struct ChainIO {
