@@ -43,8 +43,8 @@ def projection(module, c_known, c_skip):
 
 def supported(module, unknown, known, unknow_feats, known_feats):
     """the whole rule but the switch, the need for an autograd graph and the shape rule: known points given, fp32 CUDA
-    inputs and contiguous fp32 CUDA parameters, coordinates without grad, and a SharedMLP as sa_train._mlp_ok describes
-    for c_known + c_skip (at most MAX_IN) input channels"""
+    inputs and contiguous fp32 CUDA parameters (sa_train._params_ok), coordinates without grad, and a SharedMLP as
+    sa_train._mlp_ok describes for c_known + c_skip (at most MAX_IN) input channels"""
     if known is None or known_feats is None:
         return False
     for t in (unknown, known):
@@ -53,8 +53,7 @@ def supported(module, unknown, known, unknow_feats, known_feats):
     for t in (known_feats, unknow_feats):
         if t is not None and (not t.is_cuda or t.dtype != torch.float32):
             return False
-    if any(not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()
-           for t in list(module.mlp.parameters()) + list(module.mlp.buffers()) if t.is_floating_point()):
+    if not sa_train._params_ok(module.mlp):
         return False
     c_in = known_feats.size(1) + (0 if unknow_feats is None else unknow_feats.size(1))
     return c_in <= MAX_IN and sa_train._mlp_ok(module.mlp, c_in)
@@ -72,9 +71,7 @@ class _FPTrain(torch.autograd.Function):
         c_skip = 0 if skip is None else skip.size(1)
         dev = known_pm.device
         rows = B * n
-        if scale.bn and rows == 1:
-            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
-                             % (torch.Size([B, scale.c_out[0], n, 1]),))
+        sa_train._check_batch(scale, [B, scale.c_out[0], n, 1])
         d = scale.desc(c_known + c_skip, params)
         c_last = scale.c_out[-1]
         out = torch.empty((B, c_last, n), dtype=torch.float32, device=dev)
@@ -83,10 +80,9 @@ class _FPTrain(torch.autograd.Function):
         stats = torch.empty((len(scale.c_out), sa_train.STAT_ROWS, sa_train.MAX_WIDTH), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
             ws = torch.empty(L.prb_fp_train_workspace_bytes(B, n, m, c_known, c_skip, ctypes.byref(d), 0), dtype=torch.uint8, device=dev)
-            zp = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in z])
             C.check(L.prb_fp_train_forward(ctypes.byref(d), B, n, m, c_known, c_skip, int(project), C.ptr(idx), C.ptr(weight), C.ptr(known_pm),
-                                           C.ptr(skip), zp, C.ptr(stats), C.ptr(out), C.ptr(out_pm), C.ptr(ws), ws.numel(), C.stream()),
-                    "fp_train_forward")
+                                           C.ptr(skip), sa_train._ptrs(z), C.ptr(stats), C.ptr(out), C.ptr(out_pm), C.ptr(ws), ws.numel(),
+                                           C.stream()), "fp_train_forward")
         ctx.scale, ctx.desc = scale, d
         ctx.save_for_backward(idx, weight, known_pm, skip, *params, *z, stats)
         if out_pm is not None:
@@ -111,25 +107,14 @@ class _FPTrain(torch.autograd.Function):
         g_out = g_out.contiguous()
         g_known = torch.empty((B, c_known, m), dtype=torch.float32, device=dev) if ctx.needs_input_grad[3] else None
         g_skip = torch.empty((B, c_skip, n), dtype=torch.float32, device=dev) if ctx.needs_input_grad[4] and c_skip > 0 else None
-        gw = [torch.empty_like(w) for w in params[0::4][:nl]]
-        gb = [torch.empty_like(b) if b is not None else None for b in params[1::4][:nl]]
-        gg = [torch.empty_like(g) if g is not None else None for g in params[2::4][:nl]]
-        gbe = [torch.empty_like(b) if b is not None else None for b in params[3::4][:nl]]
-
-        def arr(ts):
-            return (ctypes.c_void_p * 3)(*[x.data_ptr() if x is not None else None for x in ts])
-
+        bufs = sa_train._grad_buffers(params, nl)
         d = ctx.desc
         with torch.cuda.device(dev):
             ws = torch.empty(L.prb_fp_train_workspace_bytes(B, n, m, c_known, c_skip, ctypes.byref(d), 1), dtype=torch.uint8, device=dev)
             C.check(L.prb_fp_train_backward(ctypes.byref(d), B, n, m, c_known, c_skip, C.ptr(idx), C.ptr(weight), C.ptr(known_pm), C.ptr(skip),
-                                            arr(z), C.ptr(stats), C.ptr(g_out), arr(gw), arr(gb), arr(gg), arr(gbe), C.ptr(g_known),
-                                            C.ptr(g_skip), C.ptr(ws), ws.numel(), C.stream()), "fp_train_backward")
-        grads = [None] * len(params)
-        for l in range(nl):
-            grads[4 * l:4 * l + 4] = [gw[l], gb[l], gg[l], gbe[l]]
-        grads = [g if ctx.needs_input_grad[5 + i] else None for i, g in enumerate(grads)]
-        return (None, None, None, g_known, g_skip) + tuple(grads)
+                                            sa_train._ptrs(z), C.ptr(stats), C.ptr(g_out), *[sa_train._ptrs(b) for b in bufs],
+                                            C.ptr(g_known), C.ptr(g_skip), C.ptr(ws), ws.numel(), C.stream()), "fp_train_backward")
+        return (None, None, None, g_known, g_skip) + tuple(sa_train._slot_grads(bufs, ctx.needs_input_grad[5:]))
 
 
 def forward(module, idx, weight, known_pm, known_feats, skip, project, emit_pm):
@@ -138,15 +123,8 @@ def forward(module, idx, weight, known_pm, known_feats, skip, project, emit_pm):
     skip (B, c_skip, n) contiguous or None"""
     C.require_cuda(idx, weight, known_pm, known_feats, skip)
     scale = sa_train._Scale(module.mlp)
-    p = scale.params()
-    params = p + [None] * (12 - len(p))
-    out, out_pm = _FPTrain.apply(scale, (idx, weight, project, emit_pm), known_pm.detach(), known_feats, skip, *params)
-    # the kernel wrote the running statistics in place: bump their versions as torch's in-place update would (see
-    # sa_train.forward)
-    if scale.bn:
-        for layer in scale.layers:
-            bn = layer.bn.bn
-            torch.autograd.graph.increment_version([bn.running_mean, bn.running_var, bn.num_batches_tracked])
+    out, out_pm = _FPTrain.apply(scale, (idx, weight, project, emit_pm), known_pm.detach(), known_feats, skip, *scale.params())
+    sa_train._bump_running_stats(scale)
     return out, out_pm
 
 

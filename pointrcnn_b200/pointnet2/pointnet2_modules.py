@@ -30,6 +30,60 @@ from . import pytorch_utils as pt_utils
 from . import sa_train
 
 
+_BLOCK_LAYOUTS = {("conv",), ("conv", "bn"), ("conv", "activation"), ("conv", "bn", "activation")}
+
+
+def read_block(block):
+    """(conv, bn or None, relu) of a pt_utils Conv1d / Conv2d block that is a plain 1x1 convolution, else None: children
+    exactly conv [, bn] [, activation] in that order, the activation an nn.ReLU, and a Conv1d / Conv2d whose every kernel,
+    stride and dilation entry is 1, with no padding and one group.  `bn` is the inner BatchNorm module.  This is what every
+    device path computes for a block; anything else (instance norm, pre-activation order, strided or grouped convolutions)
+    must take the torch path."""
+    children = block._modules      # read once: the eval path evaluates this on every call, named_children() costs more
+    if tuple(children) not in _BLOCK_LAYOUTS:
+        return None
+    conv, act = children["conv"], children.get("activation")
+    if not isinstance(conv, (nn.Conv1d, nn.Conv2d)):
+        return None
+    ones = (1,) * len(conv.kernel_size)
+    if not conv.kernel_size == conv.stride == conv.dilation == ones or conv.padding != (0,) * len(ones) or conv.groups != 1:
+        return None
+    if act is not None and not isinstance(act, nn.ReLU):
+        return None
+    bn = getattr(children["bn"], "bn", None) if "bn" in children else None
+    if "bn" in children and bn is None:
+        return None
+    return conv, bn, act is not None
+
+
+def read_mlp(mlp):
+    """[(conv, bn or None, True)] of a SharedMLP of 1-3 plain blocks (read_block), each with ReLU, whose channels chain (the
+    input width of block l is the output width of block l - 1), else None"""
+    blocks = [read_block(layer) for layer in mlp.children()]
+    if not 1 <= len(blocks) <= 3 or any(b is None or not b[2] for b in blocks):
+        return None
+    if any(b[0].in_channels != a[0].out_channels for a, b in zip(blocks, blocks[1:])):
+        return None
+    return blocks
+
+
+def grouping_ok(module, n_points):
+    """the grouping every device path of an SA module computes: max-pool over QueryAndGroup / GroupAll groups with use_xyz
+    and a power-of-two sample count in 4..128 (GroupAll: the n_points of the input)"""
+    if module.pool_method != "max_pool":
+        return False
+    for g in module.groupers:
+        if isinstance(g, pointnet2_utils.QueryAndGroup):
+            ns = g.nsample
+        elif isinstance(g, pointnet2_utils.GroupAll):
+            ns = n_points
+        else:
+            return False
+        if not g.use_xyz or not 4 <= ns <= 128 or ns & (ns - 1):
+            return False
+    return True
+
+
 class _FusedMLP:
     """The mlp_chain.Chain of one SharedMLP (folded BN, packed weights on the device), rebuilt whenever a parameter / buffer
     version changes (optimizer step, load_state_dict, .to())."""
@@ -41,21 +95,9 @@ class _FusedMLP:
 
     @staticmethod
     def supported(mlp: nn.Sequential):
-        layers = list(mlp.children())
-        if not 1 <= len(layers) <= 3:
-            return False
-        for layer in layers:
-            names = [k for k, _ in layer.named_children()]
-            if names not in (["conv", "bn", "activation"], ["conv", "activation"]):
-                return False
-            if not isinstance(layer.activation, nn.ReLU):
-                return False
-            conv = layer.conv
-            if tuple(conv.kernel_size) not in ((1, 1), (1,)) or conv.out_channels > 512:
-                return False
-            if "bn" in names and layer.bn.bn.training:
-                return False
-        return True
+        """read_mlp's SharedMLP, at most 512 wide, with no BatchNorm in training mode"""
+        blocks = read_mlp(mlp)
+        return blocks is not None and all(conv.out_channels <= 512 and (bn is None or not bn.training) for conv, bn, _ in blocks)
 
     def get(self, mlp: nn.Sequential, kind: int, split: int, device, project_known: bool = False):
         """-> the chain of `mlp`, packed as (kind, split) on `device`.
@@ -154,26 +196,13 @@ class _PointnetSAModuleBase(nn.Module):
 
     # ------------------------------------------------------------------ fused (tensor-core) path
     def _can_fuse(self, xyz, features, new_xyz):
-        if not _fused_enabled() or not xyz.is_cuda or self.pool_method != 'max_pool':
+        if not _fused_enabled() or not xyz.is_cuda:
             return False
         if _needs_graph(self, xyz, features, new_xyz):
             return False
         if xyz.dtype != torch.float32 or (features is not None and features.dtype != torch.float32):
             return False
-        for g, mlp in zip(self.groupers, self.mlps):
-            if not _FusedMLP.supported(mlp):
-                return False
-            if isinstance(g, pointnet2_utils.QueryAndGroup):
-                ns = g.nsample
-                if not g.use_xyz or ns < 4 or ns > 128 or (ns & (ns - 1)):
-                    return False
-            elif isinstance(g, pointnet2_utils.GroupAll):
-                n = xyz.size(1)
-                if not g.use_xyz or n < 4 or n > 128 or (n & (n - 1)):
-                    return False
-            else:
-                return False
-        return True
+        return grouping_ok(self, xyz.size(1)) and all(_FusedMLP.supported(mlp) for mlp in self.mlps)
 
     def fused_geometry(self, xyz, new_xyz=None):
         """sampling + neighbour search of the fused path (depends on coordinates only, so a caller may run it on a side

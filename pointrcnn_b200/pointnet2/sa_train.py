@@ -14,7 +14,7 @@ import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
 from .. import _cabi as C
-from . import pointnet2_utils
+from . import pointnet2_modules as pm     # imports this module in turn: read its attributes at call time only
 
 MAX_WIDTH = 512
 # Dispatch rule: the device path is taken only for modules whose every layer is at most this wide.  Measured on an H100
@@ -26,59 +26,39 @@ STAT_ROWS = 4          # mean, invstd, a, b (y = relu(a * z + b)) per channel, M
 
 
 def _mlp_ok(mlp, c_in):
-    """1-3 layers of 1x1 Conv2d + [BatchNorm2d in training mode with tracked statistics | conv bias] + ReLU, at most
-    MAX_WIDTH wide, all with or all without BN (one eps / momentum: the descriptor holds one)"""
-    layers = list(mlp.children())
-    if not 1 <= len(layers) <= 3:
+    """a SharedMLP as pointnet2_modules.read_mlp reads it, of Conv2d blocks, reading c_in channels, at most MAX_WIDTH wide,
+    each with [BatchNorm2d in training mode with tracked statistics | conv bias], all with or all without BN (one eps /
+    momentum: the descriptor holds one)"""
+    blocks = pm.read_mlp(mlp)
+    if blocks is None or blocks[0][0].in_channels != c_in:
         return False
     kinds = set()
-    for layer in layers:
-        names = [k for k, _ in layer.named_children()]
-        if names not in (["conv", "bn", "activation"], ["conv", "activation"]) or not isinstance(layer.activation, nn.ReLU):
+    for conv, bn, _ in blocks:
+        if not isinstance(conv, nn.Conv2d) or conv.out_channels > MAX_WIDTH:
             return False
-        conv = layer.conv
-        if (not isinstance(conv, nn.Conv2d) or tuple(conv.kernel_size) != (1, 1) or tuple(conv.stride) != (1, 1)
-                or tuple(conv.padding) != (0, 0) or tuple(conv.dilation) != (1, 1) or conv.groups != 1
-                or conv.in_channels != c_in or conv.out_channels > MAX_WIDTH):
+        if bn is not None and (not isinstance(bn, nn.BatchNorm2d) or not bn.training or not bn.track_running_stats
+                               or bn.momentum is None or not bn.affine or conv.bias is not None):
             return False
-        if "bn" in names:
-            bn = layer.bn.bn
-            if (not isinstance(bn, nn.BatchNorm2d) or not bn.training or not bn.track_running_stats or bn.momentum is None
-                    or not bn.affine or conv.bias is not None):
-                return False
-            kinds.add((float(bn.eps), float(bn.momentum)))
-        else:
-            kinds.add(None)
-        c_in = conv.out_channels
+        kinds.add(None if bn is None else (float(bn.eps), float(bn.momentum)))
     return len(kinds) == 1
 
 
-def _nsample_ok(ns):
-    return 4 <= ns <= 128 and ns & (ns - 1) == 0
-
-
 def layout_ok(module, c_feat, n_points):
-    """the module half of the rule: max-pool, QueryAndGroup / GroupAll with use_xyz and a power-of-two sample count in
-    4..128 (GroupAll: the n_points of the input), and every SharedMLP as _mlp_ok describes for 3 + c_feat input channels"""
-    if module.pool_method != "max_pool":
-        return False
-    for g, mlp in zip(module.groupers, module.mlps):
-        if isinstance(g, pointnet2_utils.QueryAndGroup):
-            if not g.use_xyz or not _nsample_ok(g.nsample):
-                return False
-        elif isinstance(g, pointnet2_utils.GroupAll):
-            if not g.use_xyz or not _nsample_ok(n_points):
-                return False
-        else:
-            return False
-        if not _mlp_ok(mlp, 3 + c_feat):
-            return False
-    return True
+    """the module half of the rule: pointnet2_modules.grouping_ok, and every SharedMLP as _mlp_ok describes for 3 + c_feat
+    input channels"""
+    return pm.grouping_ok(module, n_points) and all(_mlp_ok(mlp, 3 + c_feat) for mlp in module.mlps)
 
 
 def faster_on_device(module):
     """the fixed shape rule of the dispatch (see FAST_MAX_WIDTH)"""
     return all(layer.conv.out_channels <= FAST_MAX_WIDTH for mlp in module.mlps for layer in mlp.children())
+
+
+def _params_ok(module):
+    """every floating parameter and buffer of `module` is contiguous fp32 CUDA: the kernels read the parameters and write
+    their gradients as dense (c_out, c_in) rows"""
+    return all(t.is_cuda and t.dtype == torch.float32 and t.is_contiguous()
+               for t in list(module.parameters()) + list(module.buffers()) if t.is_floating_point())
 
 
 def supported(module, xyz, features, new_xyz):
@@ -90,9 +70,7 @@ def supported(module, xyz, features, new_xyz):
         return False
     if features is not None and (not features.is_cuda or features.dtype != torch.float32):
         return False
-    # the kernels read the parameters and write their gradients as dense (c_out, c_in) rows
-    if any(not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()
-           for m in module.mlps for t in list(m.parameters()) + list(m.buffers()) if t.is_floating_point()):
+    if not _params_ok(module.mlps):
         return False
     return layout_ok(module, 0 if features is None else features.size(1), xyz.size(1))
 
@@ -106,12 +84,13 @@ class _Scale:
         self.c_out = [layer.conv.out_channels for layer in self.layers]
 
     def params(self):
-        """weight, bias, gamma, beta per layer (None where absent): the Function's differentiable inputs"""
+        """weight, bias, gamma, beta per layer (None where absent), in the 12 slots of three layers: the Function's
+        differentiable inputs"""
         out = []
         for layer in self.layers:
             bn = layer.bn.bn if self.bn else None
             out += [layer.conv.weight, layer.conv.bias, bn.weight if bn is not None else None, bn.bias if bn is not None else None]
-        return out
+        return out + [None] * (12 - len(out))
 
     def desc(self, c_in, params):
         d = C.SATrainDesc()
@@ -132,6 +111,40 @@ class _Scale:
         return d
 
 
+def _check_batch(scale, size):
+    """BatchNorm2d's refusal of a training batch with one value per channel; size: (B, C, H, W) of layer 0's output"""
+    if scale.bn and size[0] * size[2] * size[3] == 1:
+        raise ValueError("Expected more than 1 value per channel when training, got input size %s" % (torch.Size(size),))
+
+
+def _ptrs(ts):
+    """the C ABI's per-layer pointer array of up to three tensors (None where absent)"""
+    return (ctypes.c_void_p * 3)(*[t.data_ptr() if t is not None else None for t in ts])
+
+
+def _grad_buffers(params, nl):
+    """[weight, bias, gamma, beta] gradient buffers of one scale's nl layers, each a list of uninitialised tensors shaped as
+    the parameter slots of `params` (None where a slot is empty)"""
+    return [[torch.empty_like(t) if t is not None else None for t in params[j::4][:nl]] for j in range(4)]
+
+
+def _slot_grads(bufs, needs):
+    """the gradients of one scale's 12 parameter slots from its _grad_buffers, None where `needs` (the scale's entries of
+    ctx.needs_input_grad) is False"""
+    nl = len(bufs[0])
+    grads = [bufs[j][l] for l in range(nl) for j in range(4)] + [None] * (12 - 4 * nl)
+    return [g if need else None for g, need in zip(grads, needs)]
+
+
+def _bump_running_stats(scale):
+    """the kernel wrote the running statistics in place: bump their versions as torch's in-place update would, so caches
+    keyed on them (the eval chain's folded weights) see the change"""
+    if scale.bn:
+        for layer in scale.layers:
+            bn = layer.bn.bn
+            torch.autograd.graph.increment_version([bn.running_mean, bn.running_var, bn.num_batches_tracked])
+
+
 class _SATrain(torch.autograd.Function):
     """(features, *params) -> (out (B, sum C_last, npoint), out_pm (B, npoint, sum C_last)) of one SA module"""
 
@@ -150,18 +163,15 @@ class _SATrain(torch.autograd.Function):
         with torch.cuda.device(dev):
             for k, (s, idx, ns) in enumerate(zip(scales, idxs, nss)):
                 rows = B * npoint * ns
-                if s.bn and rows == 1:
-                    raise ValueError("Expected more than 1 value per channel when training, got input size %s"
-                                     % (torch.Size([B, s.c_out[0], npoint, ns]),))
+                _check_batch(s, [B, s.c_out[0], npoint, ns])
                 p = params[k * 12:(k + 1) * 12]
                 d = s.desc(3 + c_feat, p)
                 z = [torch.empty((rows, c), dtype=torch.float32, device=dev) for c in s.c_out]
                 stats = torch.empty((len(s.c_out), STAT_ROWS, MAX_WIDTH), dtype=torch.float32, device=dev)
                 chosen = torch.empty((B * npoint, s.c_out[-1]), dtype=torch.uint8, device=dev)
                 ws = torch.empty(L.prb_sa_train_workspace_bytes(B, npoint, ns, c_feat, ctypes.byref(d), 0), dtype=torch.uint8, device=dev)
-                zp = (ctypes.c_void_p * 3)(*[t.data_ptr() for t in z])
                 C.check(L.prb_sa_train_forward(ctypes.byref(d), B, N, npoint, ns, c_feat, C.ptr(xyz), C.ptr(centres), C.ptr(feats_pm),
-                                               C.ptr(idx), zp, C.ptr(stats), C.ptr(chosen), C.ptr(out), C.ptr(out_pm), c_total, off,
+                                               C.ptr(idx), _ptrs(z), C.ptr(stats), C.ptr(chosen), C.ptr(out), C.ptr(out_pm), c_total, off,
                                                C.ptr(ws), ws.numel(), C.stream()), "sa_train_forward")
                 saved += z + [stats, chosen]
                 descs.append(d)
@@ -179,10 +189,9 @@ class _SATrain(torch.autograd.Function):
         idxs = t[3:3 + ctx.n_idx]
         params = t[3 + ctx.n_idx:3 + ctx.n_idx + 12 * len(ctx.scales)]
         rest = list(t[3 + ctx.n_idx + 12 * len(ctx.scales):])
-        grads = [None] * len(params)
         g_feats = None
         if g_out is None:
-            return (None, None, None, None) + tuple(grads)
+            return (None,) * (4 + len(params))
         L = C.lib()
         B, N, _ = xyz.shape
         npoint = centres.size(1)
@@ -192,30 +201,20 @@ class _SATrain(torch.autograd.Function):
         c_total = g_out.size(1)
         if ctx.needs_input_grad[3] and c_feat > 0:
             g_feats = torch.zeros((B, c_feat, N), dtype=torch.float32, device=dev)
-        off = 0
+        grads, off = [], 0
         with torch.cuda.device(dev):
             for k, (s, idx, ns, d) in enumerate(zip(ctx.scales, idxs, ctx.nss, ctx.descs)):
                 nl = len(s.c_out)
                 z, stats, chosen = rest[:nl], rest[nl], rest[nl + 1]
                 rest = rest[nl + 2:]
-                p = params[k * 12:(k + 1) * 12]
-                gw = [torch.empty_like(w) for w in p[0::4][:nl]]
-                gb = [torch.empty_like(b) if b is not None else None for b in p[1::4][:nl]]
-                gg = [torch.empty_like(g) if g is not None else None for g in p[2::4][:nl]]
-                gbe = [torch.empty_like(b) if b is not None else None for b in p[3::4][:nl]]
-
-                def arr(ts):
-                    return (ctypes.c_void_p * 3)(*[x.data_ptr() if x is not None else None for x in ts])
-
+                bufs = _grad_buffers(params[k * 12:(k + 1) * 12], nl)
                 ws = torch.empty(L.prb_sa_train_workspace_bytes(B, npoint, ns, c_feat, ctypes.byref(d), 1), dtype=torch.uint8, device=dev)
                 C.check(L.prb_sa_train_backward(ctypes.byref(d), B, N, npoint, ns, c_feat, C.ptr(xyz), C.ptr(centres), C.ptr(feats_pm),
-                                                C.ptr(idx), arr(z), C.ptr(stats), C.ptr(chosen), C.ptr(g_out), c_total, off, arr(gw),
-                                                arr(gb), arr(gg), arr(gbe), C.ptr(g_feats), C.ptr(ws), ws.numel(), C.stream()),
+                                                C.ptr(idx), _ptrs(z), C.ptr(stats), C.ptr(chosen), C.ptr(g_out), c_total, off,
+                                                *[_ptrs(b) for b in bufs], C.ptr(g_feats), C.ptr(ws), ws.numel(), C.stream()),
                         "sa_train_backward")
-                for l in range(nl):
-                    grads[k * 12 + 4 * l:k * 12 + 4 * l + 4] = [gw[l], gb[l], gg[l], gbe[l]]
+                grads += _slot_grads(bufs, ctx.needs_input_grad[4 + k * 12:4 + (k + 1) * 12])
                 off += s.c_out[-1]
-        grads = [g if ctx.needs_input_grad[4 + i] else None for i, g in enumerate(grads)]
         return (None, None, None, g_feats) + tuple(grads)
 
 
@@ -223,18 +222,10 @@ def forward(module, xyz, features, feats_pm, centres, idxs, nss):
     """the pooled features (B, sum C_last, npoint) of `module` through the device path, and their point-major twin"""
     C.require_cuda(xyz, centres, features, *idxs)
     scales = [_Scale(mlp) for mlp in module.mlps]
-    params = []
-    for s in scales:
-        p = s.params()
-        params += p + [None] * (12 - len(p))
+    params = [p for s in scales for p in s.params()]
     out, out_pm = _SATrain.apply(scales, (xyz, centres, idxs, nss), feats_pm, features, *params)
-    # the kernel wrote the running statistics in place: bump their versions as torch's in-place update would, so caches
-    # keyed on them (the eval chain's folded weights) see the change
     for s in scales:
-        if s.bn:
-            for layer in s.layers:
-                bn = layer.bn.bn
-                torch.autograd.graph.increment_version([bn.running_mean, bn.running_var, bn.num_batches_tracked])
+        _bump_running_stats(s)
     return out, out_pm
 
 

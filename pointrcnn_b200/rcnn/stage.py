@@ -79,7 +79,7 @@ class RCNNStage(nn.Module):
     def _rows_fusable(self, pts_input):
         if config.get("disable_fused") or not pts_input.is_cuda or pts_input.dtype != torch.float32 or not pts_input.is_contiguous():
             return False
-        if torch.is_grad_enabled() and (pts_input.requires_grad or any(p.requires_grad for p in self.parameters())):
+        if pn2._needs_graph(self, pts_input):
             return False
         return pn2._FusedMLP.supported(self.xyz_up_layer) and pn2._FusedMLP.supported(self.merge_down_layer)
 

@@ -16,14 +16,10 @@ from ..pointnet2 import pointnet2_modules as pm
 
 
 def _layers(seq):
-    """[(conv, bn or None, has_relu)] of a reference head stack; Dropout is the identity in eval mode"""
-    out = []
-    for layer in seq.children():
-        if isinstance(layer, nn.Dropout):
-            continue
-        names = [k for k, _ in layer.named_children()]
-        out.append((layer.conv, layer.bn.bn if "bn" in names else None, "activation" in names))
-    return out
+    """[(conv, bn or None, relu)] of a reference head stack, Dropout skipped (the identity in eval mode); None unless every
+    other child is a plain conv block (pointnet2_modules.read_block)"""
+    out = [pm.read_block(layer) for layer in seq.children() if not isinstance(layer, nn.Dropout)]
+    return None if any(b is None for b in out) else out
 
 
 class FusedRPNHeads:
@@ -36,14 +32,12 @@ class FusedRPNHeads:
 
     @staticmethod
     def supported(cls_seq, reg_seq):
-        try:
-            a, b = _layers(cls_seq), _layers(reg_seq)
-        except AttributeError:
+        a, b = _layers(cls_seq), _layers(reg_seq)
+        if a is None or b is None:
             return False
         ok = len(a) == 2 and len(b) == 2 and a[0][2] and b[0][2] and not a[1][2] and not b[1][2]
         ok = ok and a[0][0].in_channels == b[0][0].in_channels and a[0][0].out_channels + b[0][0].out_channels <= 512
-        ok = ok and all(bn is None or not bn.training for _, bn, _ in a + b)
-        return ok and all(tuple(c.kernel_size) in ((1,), (1, 1)) for c, _, _ in a + b)
+        return ok and all(bn is None or not bn.training for _, bn, _ in a + b)
 
     @staticmethod
     def _build(cls_seq, reg_seq, device):

@@ -308,6 +308,24 @@ def test_sa_module_group_all_and_no_bn(cuda):
     assert (out - ref).abs().max().item() <= TOL * ref.abs().max().item()
 
 
+@pytest.mark.parametrize("conv", [dict(stride=(1, 2)), dict(groups=2)])
+def test_sa_module_with_a_block_the_kernel_cannot_compute_matches_unfused(cuda, conv):
+    """a strided or grouped 1x1 convolution in the SharedMLP: the module computes what the op-by-op path computes (the fused
+    kernel would pool every sample / read every input channel, or refuse the grouped weight)"""
+    torch.manual_seed(6)
+    mod = pm.PointnetSAModuleMSG(npoint=64, radii=[0.3], nsamples=[16], mlps=[[8, 16, 32]], bn=True)
+    mod.mlps[0].layer1.conv = torch.nn.Conv2d(16, 32, kernel_size=1, bias=False, **conv)
+    mod = mod.to(cuda).eval()
+    _randomise_bn(mod, 2)
+    x = torch.from_numpy(synth.u_cube(2, 512, 21)).to(cuda)
+    f = torch.randn(2, 8, 512, device=cuda)
+    with torch.no_grad():
+        out = mod(x, f)[1]
+        ref = _unfused(lambda: mod(x, f))[1]
+    assert out.shape == ref.shape == (2, 32, 64)
+    assert (out - ref).abs().max().item() <= TOL * ref.abs().max().item()
+
+
 FP_CASES = [
     (256, 64, 1024, 512, [512, 512]),     # FP3 (split: N=512 twice)
     (1024, 256, 512, 256, [512, 512]),    # FP2
