@@ -29,10 +29,11 @@
 extern "C" {
 #endif
 
-#define PRB_ABI_VERSION 6   /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
+#define PRB_ABI_VERSION 7   /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
                              * 5: ordered FPS, input pipeline / KITTI output group, prb_options.roipool_fused;
                              * 6: prb_rcnn_sample_rois / prb_rcnn_roi_targets take the recipe as values (the signatures of
-                             *    the former _ex entries, which are gone) */
+                             *    the former _ex entries, which are gone);
+                             * 7: prb_fp_train_forward loses its `project` argument (layer 0 always runs projected) */
 #if defined(__GNUC__)
 #define PRB_API __attribute__((visibility("default")))
 #else
@@ -575,16 +576,17 @@ PRB_API int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n, i
  * layer-0 weight columns [interpolated | skip]).  rows = b * n; idx / weight (b, n, 3) are the three taps of every
  * unknown point (prb three_nn_weights), known_pm (b, m, c_interp) the known features point-major, skip (b, c_skip, n)
  * channel-major (c_skip 0: none).
- * forward:  project 0 interpolates the known features on load; project 1 computes P = known Wi^T over the b * m known
- *           rows first and interpolates P (the same Z up to rounding).  z[l] (rows, c_out[l]) and stats as in
- *           prb_sa_train_forward; out (b, c_last, n) and, when non-NULL, out_pm (b, n, c_last) receive relu(a z + b).
+ * forward:  layer 0 computes P = known Wi^T over the b * m known rows first and interpolates P, so Z_0 = skip Ws^T +
+ *           interp(P) (interpolation commutes with the linear layer; the same Z as interpolating first, up to rounding).
+ *           z[l] (rows, c_out[l]) and stats as in prb_sa_train_forward; out (b, c_last, n) and, when non-NULL, out_pm
+ *           (b, n, c_last) receive relu(a z + b).
  * backward: from grad_out (b, c_last, n): grad_weight[l] written (layer 0: both column blocks), grad_bias / grad_gamma /
  *           grad_beta as in prb_sa_train_backward, grad_known (b, c_interp, m) and grad_skip (b, c_skip, n) WRITTEN where
  *           non-NULL.  The interpolation's transpose runs through a reverse index of the taps: no float atomics, every
  *           result is the same bits on every call.
  * Neither entry allocates or synchronises. */
 PRB_API size_t prb_fp_train_workspace_bytes(int b, int n, int m, int c_interp, int c_skip, const prb_sa_train_desc *desc, int backward);
-PRB_API int prb_fp_train_forward(const prb_sa_train_desc *desc, int b, int n, int m, int c_interp, int c_skip, int project, const int *idx,
+PRB_API int prb_fp_train_forward(const prb_sa_train_desc *desc, int b, int n, int m, int c_interp, int c_skip, const int *idx,
                                  const float *weight, const float *known_pm, const float *skip, float *const *z, float *stats, float *out,
                                  float *out_pm, void *workspace, size_t workspace_bytes, void *stream);
 PRB_API int prb_fp_train_backward(const prb_sa_train_desc *desc, int b, int n, int m, int c_interp, int c_skip, const int *idx,

@@ -91,11 +91,11 @@ def lib():
         L.prb_sa_train_forward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, I, I, P, c_size_t, P]
         L.prb_sa_train_backward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, I, I, P, P, P, P, P, P, c_size_t, P]
         L.prb_fp_train_workspace_bytes.argtypes = [I, I, I, I, I, P, I]
-        L.prb_fp_train_forward.argtypes = [P, I, I, I, I, I, I, P, P, P, P, P, P, P, P, P, c_size_t, P]
+        L.prb_fp_train_forward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, c_size_t, P]
         L.prb_fp_train_backward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P, P, c_size_t, P]
         L.prb_options_init.restype = None
         L.prb_get_thread_options.restype = None
-        if L.prb_abi_version() != 6:
+        if L.prb_abi_version() != 7:
             raise RuntimeError("pointrcnn_b200: ABI version mismatch")
         _lib = L
     return _lib

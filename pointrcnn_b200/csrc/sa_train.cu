@@ -149,13 +149,6 @@ __device__ __forceinline__ float fp_skip(const FpGeom &F, int r, int k) {
     return F.skip[((size_t)b * F.cs + k) * F.n + (r - b * F.n)];
 }
 
-struct FpA0Src {      // FP layer 0, plain: [interpolated known features | skip]
-    FpGeom F;
-    __device__ float operator()(int r, int k) const {
-        if (r >= F.rows || k >= F.ci + F.cs) return 0.f;
-        return k < F.ci ? fp_taps(F, r, F.known_pm, F.ci, k) : fp_skip(F, r, k - F.ci);
-    }
-};
 struct FpSkipSrc {    // FP skip columns alone
     FpGeom F;
     __device__ float operator()(int r, int k) const { return (r < F.rows && k < F.cs) ? fp_skip(F, r, k) : 0.f; }
@@ -166,7 +159,7 @@ struct NoAdd {
     static constexpr bool kOn = false;
     __device__ float operator()(int, int) const { return 0.f; }
 };
-struct FpTapAdd {     // projected FP layer 0: the three-tap sum of the projected known rows (b * m, c1)
+struct FpTapAdd {     // FP layer 0: the three-tap sum of the projected known rows (b * m, c1)
     static constexpr bool kOn = true;
     FpGeom F;
     const float *proj;
@@ -558,8 +551,8 @@ __global__ void __launch_bounds__(kStThreads) sa_train_dw_reduce(int parts, int 
 // r = b * n + i.  The inner layers are the SA kernels above with the row sources ActSrc / DzSrc.  Layer 0 reads
 // [I F | S] with I the (rows x b m) three-tap interpolation, F the known features (point-major), S the skip features
 // (channel-major); W_0 = [Wi | Ws].
-//   forward  plain: one GEMM whose A operand interpolates on load; projected: P = F Wi^T over the b m known rows, then
-//            Z_0 = S Ws^T + (three-tap sum of P) in one GEMM that also writes the BN column sums
+//   forward  P = F Wi^T over the b m known rows, then Z_0 = S Ws^T + (three-tap sum of P) in one GEMM that also writes the
+//            BN column sums
 //   backward G = I^T dZ_0 from a reverse index of the taps (no float atomics), then dWi = G^T F, dF = G Wi,
 //            dWs = dZ_0^T S, dS = dZ_0 Ws
 // y_L = relu(a Z_L + b) -> out (b, c, n) and optionally its point-major twin (b, n, c), through a 32 x 32 tile
@@ -758,62 +751,152 @@ inline void st_wsplit(int rows, int cout, int cin, int &chunk, int &parts) {
     parts = ceil_div(rows, chunk);
 }
 
-struct StPlan {
+// the offset of `bytes` placed at `at`; `at` moves past them to the next 256-byte boundary
+inline size_t st_take(size_t &at, size_t bytes) {
+    const size_t off = at;
+    at = (at + bytes + 255) & ~(size_t)255;
+    return off;
+}
+
+template <class T>
+T *st_at(void *ws, size_t off) { return reinterpret_cast<T *>(static_cast<char *>(ws) + off); }
+
+// The layer stack of an SA scale or an FP module: its widths, the row tiles and weight-gradient row splits of the layer
+// GEMMs, and the workspace both modules lay out.  The forward reads only the statistics partials and the module's own
+// forward scratch after them (fwd_total); the backward the whole layout.
+struct StackPlan {
     int L, cin[3], cout[3];
-    long rows;
-    int T;                 // row tiles of the row-parallel GEMMs
-    int P, gpp;            // parts / groups per part of the last layer's statistics pass
-    int wparts[3], wchunk[3];
+    int rows, T;                  // rows of the layer GEMMs, their row tiles
+    int wparts[3], wchunk[3];     // dW row splits over those rows (FP: index 0 is Ws's)
     size_t off_p1, off_p2, off_mg, off_wpart, off_g0, off_g1;
-    size_t fwd_total, total;   // the forward reads only the statistics partials; the backward the whole layout
+    size_t fwd_total, total;
+    // the gradient buffer g of layer l (every layer but SA's last)
+    float *g(void *ws, int l) const { return st_at<float>(ws, l & 1 ? off_g1 : off_g0); }
 };
 
-inline size_t st_align(size_t x) { return (x + 255) & ~(size_t)255; }
-
-int st_plan(const prb_sa_train_desc *d, int b, int npoint, int ns, int c_feat, StPlan &p) {
-    PRB_REQUIRE(d, "sa_train: NULL descriptor");
-    PRB_REQUIRE(d->num_layers >= 1 && d->num_layers <= 3, "sa_train: %d layers (1..3)", d->num_layers);
-    PRB_REQUIRE(b >= 1 && npoint >= 1 && ns >= 1 && ns <= 128 && (ns & (ns - 1)) == 0, "sa_train: nsample %d must be a power of two <= 128", ns);
-    PRB_REQUIRE(c_feat >= 0 && d->c_in == 3 + c_feat, "sa_train: layer 0 reads %d channels, the rows have 3 + %d", d->c_in, c_feat);
-    const long rows = (long)b * npoint * ns;
-    PRB_REQUIRE(rows < (1L << 30), "sa_train: %ld rows", rows);
+// The descriptor checks both modules share (1..3 layers, each 1..kStMaxC channels), the widths, and the row tiles and
+// dW row splits of layers 1.. over `rows` rows; layer 0's split is the module's.
+int st_stack(const prb_sa_train_desc *d, const char *who, int rows, StackPlan &p) {
+    PRB_REQUIRE(d, "%s: NULL descriptor", who);
+    PRB_REQUIRE(d->num_layers >= 1 && d->num_layers <= 3, "%s: %d layers (1..3)", who, d->num_layers);
     p.L = d->num_layers;
     p.rows = rows;
-    int cmax = 0, cinner = 0;
+    p.T = ceil_div(rows, kStRowTile);
     for (int l = 0; l < p.L; ++l) {
         p.cin[l] = l ? d->c_out[l - 1] : d->c_in;
         p.cout[l] = d->c_out[l];
-        PRB_REQUIRE(p.cout[l] >= 1 && p.cout[l] <= kStMaxC, "sa_train: layer %d has %d channels (1..%d)", l, p.cout[l], kStMaxC);
-        PRB_REQUIRE(p.cin[l] <= kStMaxC + 3, "sa_train: layer %d reads %d channels", l, p.cin[l]);
-        cmax = max(cmax, p.cout[l]);
-        if (l + 1 < p.L) cinner = max(cinner, p.cout[l]);
+        PRB_REQUIRE(p.cout[l] >= 1 && p.cout[l] <= kStMaxC, "%s: layer %d has %d channels (1..%d)", who, l, p.cout[l], kStMaxC);
+        if (l) st_wsplit(rows, p.cout[l], p.cin[l], p.wchunk[l], p.wparts[l]);
     }
-    p.T = ceil_div((int)rows, kStRowTile);
+    return 0;
+}
+
+// The shared layout: the statistics partials p1 / p2 (nparts float64 each), then `fwd_extra` bytes of the module's forward
+// scratch at the returned offset; for the backward mg, the dW partials (the largest of layer 0's wpart0 floats and those of
+// layers 1..) and the gradient buffers g0 / g1 of rows x gw floats each.
+size_t st_layout(StackPlan &p, size_t nparts, size_t fwd_extra, size_t wpart0, int gw) {
+    size_t wpart = wpart0;
+    for (int l = 1; l < p.L; ++l) wpart = std::max(wpart, (size_t)p.wparts[l] * p.cout[l] * p.cin[l]);
+    size_t at = 0;
+    p.off_p1 = st_take(at, nparts * sizeof(double));
+    p.off_p2 = st_take(at, nparts * sizeof(double));
+    const size_t off_extra = st_take(at, fwd_extra);
+    p.fwd_total = at;
+    p.off_mg = st_take(at, 2 * kStMaxC * sizeof(float));
+    p.off_wpart = st_take(at, wpart * sizeof(float));
+    p.off_g0 = st_take(at, (size_t)p.rows * gw * sizeof(float));
+    p.off_g1 = st_take(at, (size_t)p.rows * gw * sizeof(float));
+    p.total = at;
+    return off_extra;
+}
+
+// every layer's Z buffer and weight, and with grad_weight its weight gradient, before an entry launches anything
+int st_check_layers(const StackPlan &p, const prb_sa_train_desc *d, const char *who, const float *const *z, float *const *grad_weight) {
+    for (int l = 0; l < p.L; ++l) {
+        PRB_REQUIRE(z[l] && d->weight[l], "%s: layer %d: no Z buffer or weight", who, l);
+        PRB_REQUIRE(!grad_weight || grad_weight[l], "%s: layer %d: no weight gradient", who, l);
+    }
+    return 0;
+}
+
+// The forward's layer loop, once the module's layer-0 GEMM has stored Z_0 and its statistics partials: every layer has its
+// statistics finalised, and layers 1.. run the GEMM over relu(a Z + b) of the layer before.  `top` receives the last layer.
+int st_forward(const StackPlan &p, const prb_sa_train_desc *d, float *const *z, float *stats, void *ws, cudaStream_t s, StLayer &top) {
+    double *p1 = st_at<double>(ws, p.off_p1), *p2 = st_at<double>(ws, p.off_p2);
+    for (int l = 0; l < p.L; ++l) {
+        if (l > 0) {
+            sa_train_fwd_gemm<<<dim3(p.T, ceil_div(p.cout[l], kStColTile)), kStThreads, 0, s>>>(ActSrc{p.rows, top}, NoAdd{}, p.rows, d->weight[l],
+                                                                                               p.cin[l], p.cin[l], p.cout[l], z[l], d->bn, p.T, p1, p2);
+            if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
+        }
+        float *st = stats + (size_t)l * ST_ROWS * kStMaxC;
+        sa_train_bn_finalise<<<p.cout[l], kStThreads, 0, s>>>(p.T, p1, p2, p.rows, d->bn, d->eps, d->momentum, d->gamma[l], d->beta[l], d->bias[l],
+                                                              d->running_mean[l], d->running_var[l], d->num_batches_tracked[l], st);
+        if (int rc = check_launch("sa_train_bn_finalise")) return rc;
+        top = StLayer{p.cout[l], z[l], st};
+    }
+    return 0;
+}
+
+// The backward's layer loop, last layer to first, once the module has written the last layer's statistics partials
+// (nparts_last per channel; T for every other layer).  dz(l) stages layer l's dZ.  Every layer has dgamma / dbeta or dbias
+// finalised; layers 1.. then run dW = dZ^T A over the layer before's relu(a Z + b), and dA = dZ W masked by that layer's
+// ReLU into its g buffer, with its BN sums.  Layer 0's weight and input gradients are the module's.
+template <class Dz>
+int st_backward(const StackPlan &p, const prb_sa_train_desc *d, Dz dz, int nparts_last, const float *const *z, const float *stats,
+                float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma, float *const *grad_beta, void *ws,
+                cudaStream_t s) {
+    double *p1 = st_at<double>(ws, p.off_p1), *p2 = st_at<double>(ws, p.off_p2);
+    float *mg = st_at<float>(ws, p.off_mg), *wpart = st_at<float>(ws, p.off_wpart);
+    for (int l = p.L - 1; l >= 0; --l) {
+        sa_train_grad_finalise<<<p.cout[l], kStThreads, 0, s>>>(l == p.L - 1 ? nparts_last : p.T, p1, p2, p.rows, d->bn,
+                                                                grad_gamma ? grad_gamma[l] : nullptr, grad_beta ? grad_beta[l] : nullptr,
+                                                                grad_bias ? grad_bias[l] : nullptr, mg);
+        if (int rc = check_launch("sa_train_grad_finalise")) return rc;
+        if (l == 0) break;
+        // dW first: it reads this layer's g, which the dA launch below does not overwrite (it writes the other buffer)
+        const auto D = dz(l);
+        const StLayer prev{p.cout[l - 1], z[l - 1], stats + (size_t)(l - 1) * ST_ROWS * kStMaxC};
+        sa_train_dw_gemm<<<dim3(ceil_div(p.cout[l], 64), ceil_div(p.cin[l], 64), p.wparts[l]), kStThreads, 0, s>>>(
+            D, ActSrc{p.rows, prev}, p.rows, p.cout[l], p.cin[l], p.wchunk[l], wpart);
+        if (int rc = check_launch("sa_train_dw_gemm")) return rc;
+        const int count = p.cout[l] * p.cin[l];
+        sa_train_dw_reduce<<<ceil_div(count, kStThreads), kStThreads, 0, s>>>(p.wparts[l], count, p.cin[l], p.cin[l], wpart, grad_weight[l]);
+        if (int rc = check_launch("sa_train_dw_reduce")) return rc;
+        sa_train_da_gemm<<<dim3(p.T, ceil_div(p.cin[l], kStColTile)), kStThreads, 0, s>>>(D, DaMasked{prev, p.g(ws, l - 1)}, p.rows, p.cout[l],
+                                                                                          d->weight[l], p.cin[l], p.cin[l], p.T, p1, p2);
+        if (int rc = check_launch("sa_train_da_gemm")) return rc;
+    }
+    return 0;
+}
+
+struct StPlan : StackPlan {
+    int P, gpp;            // parts / groups per part of the last layer's statistics pass
+};
+
+int st_plan(const prb_sa_train_desc *d, int b, int npoint, int ns, int c_feat, StPlan &p) {
+    PRB_REQUIRE(b >= 1 && npoint >= 1 && ns >= 1 && ns <= 128 && (ns & (ns - 1)) == 0, "sa_train: nsample %d must be a power of two <= 128", ns);
+    const long rows = (long)b * npoint * ns;
+    PRB_REQUIRE(rows < (1L << 30), "sa_train: %ld rows", rows);
+    if (int rc = st_stack(d, "sa_train", (int)rows, p)) return rc;
+    PRB_REQUIRE(c_feat >= 0 && d->c_in == 3 + c_feat, "sa_train: layer 0 reads %d channels, the rows have 3 + %d", d->c_in, c_feat);
+    PRB_REQUIRE(d->c_in <= kStMaxC + 3, "sa_train: layer 0 reads %d channels", d->c_in);
+    st_wsplit(p.rows, p.cout[0], p.cin[0], p.wchunk[0], p.wparts[0]);
     const int groups = b * npoint;
     p.P = min(max(ceil_div(groups, 32), 1), kStMaxParts);
     p.gpp = ceil_div(groups, p.P);
     p.P = ceil_div(groups, p.gpp);
-    size_t wpart = 0;
-    for (int l = 0; l < p.L; ++l) {
-        st_wsplit((int)rows, p.cout[l], p.cin[l], p.wchunk[l], p.wparts[l]);
-        wpart = std::max(wpart, (size_t)p.wparts[l] * p.cout[l] * p.cin[l]);
-    }
-    const size_t nparts = (size_t)cmax * max(p.T, p.P);
-    p.off_p1 = 0;
-    p.off_p2 = st_align(p.off_p1 + nparts * sizeof(double));
-    p.off_mg = st_align(p.off_p2 + nparts * sizeof(double));
-    p.fwd_total = p.off_mg;
-    p.off_wpart = st_align(p.off_mg + 2 * kStMaxC * sizeof(float));
-    p.off_g0 = st_align(p.off_wpart + wpart * sizeof(float));
-    p.off_g1 = st_align(p.off_g0 + (size_t)rows * cinner * sizeof(float));
-    p.total = st_align(p.off_g1 + (size_t)rows * cinner * sizeof(float));
+    // the partials serve the last layer's statistics pass too; the g buffers only the inner layers
+    const int cmax = *std::max_element(p.cout, p.cout + p.L);
+    const int cinner = p.L > 1 ? *std::max_element(p.cout, p.cout + p.L - 1) : 0;
+    st_layout(p, (size_t)cmax * max(p.T, p.P), 0, (size_t)p.wparts[0] * p.cout[0] * p.cin[0], cinner);
     return 0;
 }
 
-StGeom st_geom(int b, int n, int npoint, int ns, int c_feat, long rows, const float *xyz, const float *new_xyz, const float *feats_pm,
+StGeom st_geom(int b, int n, int npoint, int ns, int c_feat, int rows, const float *xyz, const float *new_xyz, const float *feats_pm,
                const int *idx) {
     StGeom G;
-    G.b = b; G.n = n; G.npoint = npoint; G.ns = ns; G.c_feat = c_feat; G.rows = (int)rows;
+    G.b = b; G.n = n; G.npoint = npoint; G.ns = ns; G.c_feat = c_feat; G.rows = rows;
     G.log_ns = 0;
     while ((1 << G.log_ns) < ns) ++G.log_ns;
     G.xyz = xyz; G.centres = new_xyz; G.feats_pm = feats_pm; G.idx = idx;
@@ -841,30 +924,17 @@ extern "C" int prb_sa_train_forward(const prb_sa_train_desc *desc, int b, int n,
     PRB_REQUIRE(out_c_off >= 0 && out_c_off + p.cout[p.L - 1] <= out_stride_c, "sa_train_forward: channels %d..%d outside %d", out_c_off,
                 out_c_off + p.cout[p.L - 1], out_stride_c);
     PRB_REQUIRE(!desc->bn || p.rows > 1, "sa_train_forward: batch statistics need more than one value per channel");
+    if (int rc = st_check_layers(p, desc, "sa_train_forward", z, nullptr)) return rc;
     const cudaStream_t s = (cudaStream_t)stream;
-    char *ws = reinterpret_cast<char *>(workspace);
-    double *p1 = reinterpret_cast<double *>(ws + p.off_p1), *p2 = reinterpret_cast<double *>(ws + p.off_p2);
+    double *p1 = st_at<double>(workspace, p.off_p1), *p2 = st_at<double>(workspace, p.off_p2);
     const StGeom G = st_geom(b, n, npoint, nsample, c_feat, p.rows, xyz, new_xyz, feats_pm, idx);
-    StLayer prev{0, nullptr, nullptr};
-    for (int l = 0; l < p.L; ++l) {
-        PRB_REQUIRE(z[l] && desc->weight[l], "sa_train_forward: layer %d: no Z buffer or weight", l);
-        const dim3 grid(p.T, ceil_div(p.cout[l], kStColTile));
-        if (l == 0)
-            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(SaA0Src{G}, NoAdd{}, G.rows, desc->weight[l], p.cin[l], p.cin[l], p.cout[l], z[l],
-                                                          desc->bn, p.T, p1, p2);
-        else
-            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(ActSrc{G.rows, prev}, NoAdd{}, G.rows, desc->weight[l], p.cin[l], p.cin[l], p.cout[l],
-                                                          z[l], desc->bn, p.T, p1, p2);
-        if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
-        float *st = stats + (size_t)l * ST_ROWS * kStMaxC;
-        sa_train_bn_finalise<<<p.cout[l], kStThreads, 0, s>>>(p.T, p1, p2, p.rows, desc->bn, desc->eps, desc->momentum, desc->gamma[l],
-                                                              desc->beta[l], desc->bias[l], desc->running_mean[l], desc->running_var[l],
-                                                              desc->num_batches_tracked[l], st);
-        if (int rc = check_launch("sa_train_bn_finalise")) return rc;
-        prev = StLayer{p.cout[l], z[l], st};
-    }
-    const long items = (long)b * npoint * prev.c;
-    sa_train_pool<<<(unsigned)((items + kStThreads - 1) / kStThreads), kStThreads, 0, s>>>(G, prev, out, out_pm, out_stride_c, out_c_off, chosen);
+    sa_train_fwd_gemm<<<dim3(p.T, ceil_div(p.cout[0], kStColTile)), kStThreads, 0, s>>>(SaA0Src{G}, NoAdd{}, p.rows, desc->weight[0], p.cin[0],
+                                                                                       p.cin[0], p.cout[0], z[0], desc->bn, p.T, p1, p2);
+    if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
+    StLayer top{};
+    if (int rc = st_forward(p, desc, z, stats, workspace, s, top)) return rc;
+    const long items = (long)b * npoint * top.c;
+    sa_train_pool<<<(unsigned)((items + kStThreads - 1) / kStThreads), kStThreads, 0, s>>>(G, top, out, out_pm, out_stride_c, out_c_off, chosen);
     return check_launch("sa_train_pool");
 }
 
@@ -880,51 +950,30 @@ extern "C" int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n
     PRB_REQUIRE(workspace_bytes >= p.total, "sa_train_backward: workspace of %zu bytes < %zu", workspace_bytes, p.total);
     PRB_REQUIRE(out_c_off >= 0 && out_c_off + p.cout[p.L - 1] <= out_stride_c, "sa_train_backward: channels %d..%d outside %d", out_c_off,
                 out_c_off + p.cout[p.L - 1], out_stride_c);
+    if (int rc = st_check_layers(p, desc, "sa_train_backward", z, grad_weight)) return rc;
     const cudaStream_t s = (cudaStream_t)stream;
-    char *ws = reinterpret_cast<char *>(workspace);
-    double *p1 = reinterpret_cast<double *>(ws + p.off_p1), *p2 = reinterpret_cast<double *>(ws + p.off_p2);
-    float *mg = reinterpret_cast<float *>(ws + p.off_mg), *wpart = reinterpret_cast<float *>(ws + p.off_wpart);
-    float *gbuf[2] = {reinterpret_cast<float *>(ws + p.off_g0), reinterpret_cast<float *>(ws + p.off_g1)};
+    double *p1 = st_at<double>(workspace, p.off_p1), *p2 = st_at<double>(workspace, p.off_p2);
+    float *mg = st_at<float>(workspace, p.off_mg), *wpart = st_at<float>(workspace, p.off_wpart);
     const StGeom G = st_geom(b, n, npoint, nsample, c_feat, p.rows, xyz, new_xyz, feats_pm, idx);
-    const float *g_in = nullptr;      // g of the current layer (nullptr: the last layer, from grad_out)
-    int nparts = p.P;                 // partial rows of the current layer's statistics
-    for (int l = p.L - 1; l >= 0; --l) {
-        const float *st = stats + (size_t)l * ST_ROWS * kStMaxC;
-        const StGrad Lg{p.cout[l], desc->bn, z[l], st, g_in, grad_out, chosen, out_stride_c, out_c_off, mg};
-        if (l == p.L - 1) {
-            sa_train_last_stats<<<p.P, kStThreads, 0, s>>>(G, Lg, p.gpp, p1, p2);
-            if (int rc = check_launch("sa_train_last_stats")) return rc;
-        }
-        sa_train_grad_finalise<<<p.cout[l], kStThreads, 0, s>>>(nparts, p1, p2, p.rows, desc->bn, grad_gamma ? grad_gamma[l] : nullptr,
-                                                                grad_beta ? grad_beta[l] : nullptr, grad_bias ? grad_bias[l] : nullptr, mg);
-        if (int rc = check_launch("sa_train_grad_finalise")) return rc;
-        // dW first: it reads this layer's g, which the dA launch below does not overwrite (it writes the other buffer)
-        const StLayer prev = l ? StLayer{p.cout[l - 1], z[l - 1], stats + (size_t)(l - 1) * ST_ROWS * kStMaxC} : StLayer{0, nullptr, nullptr};
-        const dim3 wgrid(ceil_div(p.cout[l], 64), ceil_div(p.cin[l], 64), p.wparts[l]);
-        if (l == 0)
-            sa_train_dw_gemm<<<wgrid, kStThreads, 0, s>>>(SaDzSrc{G, Lg}, SaA0Src{G}, G.rows, p.cout[l], p.cin[l], p.wchunk[l], wpart);
-        else
-            sa_train_dw_gemm<<<wgrid, kStThreads, 0, s>>>(SaDzSrc{G, Lg}, ActSrc{G.rows, prev}, G.rows, p.cout[l], p.cin[l], p.wchunk[l], wpart);
-        if (int rc = check_launch("sa_train_dw_gemm")) return rc;
-        PRB_REQUIRE(grad_weight[l], "sa_train_backward: layer %d: no weight gradient", l);
-        const int count = p.cout[l] * p.cin[l];
-        sa_train_dw_reduce<<<ceil_div(count, kStThreads), kStThreads, 0, s>>>(p.wparts[l], count, p.cin[l], p.cin[l], wpart, grad_weight[l]);
-        if (int rc = check_launch("sa_train_dw_reduce")) return rc;
-        const dim3 agrid(p.T, ceil_div(p.cin[l], kStColTile));
-        if (l > 0) {
-            float *g_out = gbuf[(l - 1) & 1];
-            sa_train_da_gemm<<<agrid, kStThreads, 0, s>>>(SaDzSrc{G, Lg}, DaMasked{prev, g_out}, G.rows, p.cout[l], desc->weight[l], p.cin[l],
-                                                          p.cin[l], p.T, p1, p2);
-            if (int rc = check_launch("sa_train_da_gemm")) return rc;
-            g_in = g_out;
-            nparts = p.T;
-        } else if (grad_feats && c_feat > 0) {
-            sa_train_da_gemm<<<agrid, kStThreads, 0, s>>>(SaDzSrc{G, Lg}, DaScatterFeats{G, grad_feats}, G.rows, p.cout[0], desc->weight[0],
-                                                          p.cin[0], p.cin[0], p.T, nullptr, nullptr);
-            if (int rc = check_launch("sa_train_da_gemm")) return rc;
-        }
-    }
-    return 0;
+    // the last layer's g comes from grad_out through the pooled choice
+    auto dz = [&](int l) {
+        return SaDzSrc{G, StGrad{p.cout[l], desc->bn, z[l], stats + (size_t)l * ST_ROWS * kStMaxC, l == p.L - 1 ? nullptr : p.g(workspace, l),
+                                 grad_out, chosen, out_stride_c, out_c_off, mg}};
+    };
+    sa_train_last_stats<<<p.P, kStThreads, 0, s>>>(G, dz(p.L - 1).L, p.gpp, p1, p2);
+    if (int rc = check_launch("sa_train_last_stats")) return rc;
+    if (int rc = st_backward(p, desc, dz, p.P, z, stats, grad_weight, grad_bias, grad_gamma, grad_beta, workspace, s)) return rc;
+    // layer 0: dW over the grouped rows; dA only for the feature columns, scattered into grad_feats
+    sa_train_dw_gemm<<<dim3(ceil_div(p.cout[0], 64), ceil_div(p.cin[0], 64), p.wparts[0]), kStThreads, 0, s>>>(dz(0), SaA0Src{G}, p.rows, p.cout[0],
+                                                                                                            p.cin[0], p.wchunk[0], wpart);
+    if (int rc = check_launch("sa_train_dw_gemm")) return rc;
+    const int count = p.cout[0] * p.cin[0];
+    sa_train_dw_reduce<<<ceil_div(count, kStThreads), kStThreads, 0, s>>>(p.wparts[0], count, p.cin[0], p.cin[0], wpart, grad_weight[0]);
+    if (int rc = check_launch("sa_train_dw_reduce")) return rc;
+    if (!grad_feats || c_feat == 0) return 0;
+    sa_train_da_gemm<<<dim3(p.T, ceil_div(p.cin[0], kStColTile)), kStThreads, 0, s>>>(dz(0), DaScatterFeats{G, grad_feats}, p.rows, p.cout[0],
+                                                                                      desc->weight[0], p.cin[0], p.cin[0], p.T, nullptr, nullptr);
+    return check_launch("sa_train_da_gemm");
 }
 
 // ------------------------------------------------------------------------------------------------ FP module, host side
@@ -932,62 +981,34 @@ namespace prb {
 
 constexpr int kFpMaxIn = 2048;     // widest layer-0 input (interpolated + skip channels)
 
-struct FpPlan {
-    int L, cin[3], cout[3], ci, cs;
-    int rows, krows;        // b n unknown rows, b m known rows
-    int T, KT;              // row tiles of the unknown / known rows
-    int wparts[3], wchunk[3];   // dW of layers 1.. and of Ws (index 0, over the unknown rows)
+struct FpPlan : StackPlan {
+    int krows, KT;              // b m known rows, their row tiles
     int wparts_i, wchunk_i;     // dWi over the known rows
     int scan_blocks;
-    size_t off_p1, off_p2, off_proj, off_mg, off_wpart, off_g0, off_g1, off_cnt, off_off, off_tot, off_list;
-    size_t fwd_total, total;
+    size_t off_proj, off_cnt, off_off, off_tot, off_list;
 };
 
 int fp_plan(const prb_sa_train_desc *d, int b, int n, int m, int ci, int cs, FpPlan &p) {
-    PRB_REQUIRE(d, "fp_train: NULL descriptor");
-    PRB_REQUIRE(d->num_layers >= 1 && d->num_layers <= 3, "fp_train: %d layers (1..3)", d->num_layers);
     PRB_REQUIRE(b >= 1 && n >= 1 && m >= 1, "fp_train: b %d, n %d, m %d", b, n, m);
+    PRB_REQUIRE(3L * b * n < (1L << 30) && (long)b * m < (1L << 30), "fp_train: %d x %d rows", b, n);
+    if (int rc = st_stack(d, "fp_train", b * n, p)) return rc;
     PRB_REQUIRE(ci >= 1 && cs >= 0 && d->c_in == ci + cs && d->c_in <= kFpMaxIn, "fp_train: layer 0 reads %d channels, not %d + %d (at most %d)",
                 d->c_in, ci, cs, kFpMaxIn);
-    PRB_REQUIRE(3L * b * n < (1L << 30) && (long)b * m < (1L << 30), "fp_train: %d x %d rows", b, n);
-    p.L = d->num_layers;
-    p.ci = ci;
-    p.cs = cs;
-    p.rows = b * n;
     p.krows = b * m;
-    int cmax = 0;
-    for (int l = 0; l < p.L; ++l) {
-        p.cin[l] = l ? d->c_out[l - 1] : d->c_in;
-        p.cout[l] = d->c_out[l];
-        PRB_REQUIRE(p.cout[l] >= 1 && p.cout[l] <= kStMaxC, "fp_train: layer %d has %d channels (1..%d)", l, p.cout[l], kStMaxC);
-        cmax = max(cmax, p.cout[l]);
-    }
-    p.T = ceil_div(p.rows, kStRowTile);
     p.KT = ceil_div(p.krows, kStRowTile);
-    size_t wpart = 0;
-    for (int l = 1; l < p.L; ++l) {
-        st_wsplit(p.rows, p.cout[l], p.cin[l], p.wchunk[l], p.wparts[l]);
-        wpart = std::max(wpart, (size_t)p.wparts[l] * p.cout[l] * p.cin[l]);
-    }
     st_wsplit(p.rows, p.cout[0], max(cs, 1), p.wchunk[0], p.wparts[0]);
-    wpart = std::max(wpart, (size_t)p.wparts[0] * p.cout[0] * cs);
     st_wsplit(p.krows, p.cout[0], ci, p.wchunk_i, p.wparts_i);
-    wpart = std::max(wpart, (size_t)p.wparts_i * p.cout[0] * ci);
     p.scan_blocks = ceil_div(p.krows, kScanItems);
-    const size_t nparts = (size_t)cmax * p.T;
-    p.off_p1 = 0;
-    p.off_p2 = st_align(p.off_p1 + nparts * sizeof(double));
-    p.off_proj = st_align(p.off_p2 + nparts * sizeof(double));     // forward: P = F Wi^T; backward: G = I^T dZ_0
-    p.fwd_total = st_align(p.off_proj + (size_t)p.krows * p.cout[0] * sizeof(float));
-    p.off_mg = p.fwd_total;
-    p.off_wpart = st_align(p.off_mg + 2 * kStMaxC * sizeof(float));
-    p.off_g0 = st_align(p.off_wpart + wpart * sizeof(float));
-    p.off_g1 = st_align(p.off_g0 + (size_t)p.rows * cmax * sizeof(float));
-    p.off_cnt = st_align(p.off_g1 + (size_t)p.rows * cmax * sizeof(float));
-    p.off_off = st_align(p.off_cnt + (size_t)p.krows * sizeof(int));
-    p.off_tot = st_align(p.off_off + (size_t)(p.krows + 1) * sizeof(int));
-    p.off_list = st_align(p.off_tot + (size_t)p.scan_blocks * sizeof(int));
-    p.total = st_align(p.off_list + (size_t)3 * p.rows * sizeof(int));
+    const int cmax = *std::max_element(p.cout, p.cout + p.L);
+    const size_t wpart0 = std::max((size_t)p.wparts[0] * p.cout[0] * cs, (size_t)p.wparts_i * p.cout[0] * ci);
+    // proj: the forward's P = F Wi^T, the backward's G = I^T dZ_0
+    p.off_proj = st_layout(p, (size_t)cmax * p.T, (size_t)p.krows * p.cout[0] * sizeof(float), wpart0, cmax);
+    size_t at = p.total;
+    p.off_cnt = st_take(at, (size_t)p.krows * sizeof(int));
+    p.off_off = st_take(at, (size_t)(p.krows + 1) * sizeof(int));
+    p.off_tot = st_take(at, (size_t)p.scan_blocks * sizeof(int));
+    p.off_list = st_take(at, (size_t)3 * p.rows * sizeof(int));
+    p.total = at;
     return 0;
 }
 
@@ -999,7 +1020,7 @@ extern "C" size_t prb_fp_train_workspace_bytes(int b, int n, int m, int c_interp
     return backward ? p.total : p.fwd_total;
 }
 
-extern "C" int prb_fp_train_forward(const prb_sa_train_desc *desc, int b, int n, int m, int c_interp, int c_skip, int project, const int *idx,
+extern "C" int prb_fp_train_forward(const prb_sa_train_desc *desc, int b, int n, int m, int c_interp, int c_skip, const int *idx,
                                     const float *weight, const float *known_pm, const float *skip, float *const *z, float *stats, float *out,
                                     float *out_pm, void *workspace, size_t workspace_bytes, void *stream) {
     FpPlan p;
@@ -1007,38 +1028,22 @@ extern "C" int prb_fp_train_forward(const prb_sa_train_desc *desc, int b, int n,
     PRB_REQUIRE(idx && weight && known_pm && (c_skip == 0 || skip) && z && stats && out && workspace, "fp_train_forward: bad arguments");
     PRB_REQUIRE(workspace_bytes >= p.fwd_total, "fp_train_forward: workspace of %zu bytes < %zu", workspace_bytes, p.fwd_total);
     PRB_REQUIRE(!desc->bn || p.rows > 1, "fp_train_forward: batch statistics need more than one value per channel");
+    if (int rc = st_check_layers(p, desc, "fp_train_forward", z, nullptr)) return rc;
     const cudaStream_t s = (cudaStream_t)stream;
-    char *ws = reinterpret_cast<char *>(workspace);
-    double *p1 = reinterpret_cast<double *>(ws + p.off_p1), *p2 = reinterpret_cast<double *>(ws + p.off_p2);
+    double *p1 = st_at<double>(workspace, p.off_p1), *p2 = st_at<double>(workspace, p.off_p2);
+    float *proj = st_at<float>(workspace, p.off_proj);
     const FpGeom F{p.rows, n, m, c_interp, c_skip, idx, weight, known_pm, skip};
-    StLayer prev{0, nullptr, nullptr};
-    for (int l = 0; l < p.L; ++l) {
-        PRB_REQUIRE(z[l] && desc->weight[l], "fp_train_forward: layer %d: no Z buffer or weight", l);
-        const float *W = desc->weight[l];
-        const dim3 grid(p.T, ceil_div(p.cout[l], kStColTile));
-        if (l > 0) {
-            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(ActSrc{p.rows, prev}, NoAdd{}, p.rows, W, p.cin[l], p.cin[l], p.cout[l], z[l], desc->bn,
-                                                          p.T, p1, p2);
-        } else if (project) {
-            float *proj = reinterpret_cast<float *>(ws + p.off_proj);
-            sa_train_fwd_gemm<<<dim3(p.KT, grid.y), kStThreads, 0, s>>>(MatSrc{p.krows, c_interp, c_interp, known_pm}, NoAdd{}, p.krows, W,
-                                                                        p.cin[0], c_interp, p.cout[0], proj, 0, 0, nullptr, nullptr);
-            if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
-            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(FpSkipSrc{F}, FpTapAdd{F, proj, p.cout[0]}, p.rows, W + c_interp, p.cin[0], c_skip,
-                                                          p.cout[0], z[0], desc->bn, p.T, p1, p2);
-        } else {
-            sa_train_fwd_gemm<<<grid, kStThreads, 0, s>>>(FpA0Src{F}, NoAdd{}, p.rows, W, p.cin[0], p.cin[0], p.cout[0], z[0], desc->bn, p.T,
-                                                          p1, p2);
-        }
-        if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
-        float *st = stats + (size_t)l * ST_ROWS * kStMaxC;
-        sa_train_bn_finalise<<<p.cout[l], kStThreads, 0, s>>>(p.T, p1, p2, p.rows, desc->bn, desc->eps, desc->momentum, desc->gamma[l],
-                                                              desc->beta[l], desc->bias[l], desc->running_mean[l], desc->running_var[l],
-                                                              desc->num_batches_tracked[l], st);
-        if (int rc = check_launch("sa_train_bn_finalise")) return rc;
-        prev = StLayer{p.cout[l], z[l], st};
-    }
-    fp_train_out<<<dim3(ceil_div(p.rows, 32), ceil_div(prev.c, 32)), kStThreads, 0, s>>>(p.rows, n, prev, out, out_pm);
+    const float *W = desc->weight[0];
+    const int cols = ceil_div(p.cout[0], kStColTile);
+    sa_train_fwd_gemm<<<dim3(p.KT, cols), kStThreads, 0, s>>>(MatSrc{p.krows, c_interp, c_interp, known_pm}, NoAdd{}, p.krows, W, p.cin[0], c_interp,
+                                                              p.cout[0], proj, 0, 0, nullptr, nullptr);
+    if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
+    sa_train_fwd_gemm<<<dim3(p.T, cols), kStThreads, 0, s>>>(FpSkipSrc{F}, FpTapAdd{F, proj, p.cout[0]}, p.rows, W + c_interp, p.cin[0], c_skip,
+                                                             p.cout[0], z[0], desc->bn, p.T, p1, p2);
+    if (int rc = check_launch("sa_train_fwd_gemm")) return rc;
+    StLayer top{};
+    if (int rc = st_forward(p, desc, z, stats, workspace, s, top)) return rc;
+    fp_train_out<<<dim3(ceil_div(p.rows, 32), ceil_div(top.c, 32)), kStThreads, 0, s>>>(p.rows, n, top, out, out_pm);
     return check_launch("fp_train_out");
 }
 
@@ -1052,15 +1057,13 @@ extern "C" int prb_fp_train_backward(const prb_sa_train_desc *desc, int b, int n
     PRB_REQUIRE(idx && weight && known_pm && (c_skip == 0 || skip) && z && stats && grad_out && grad_weight && workspace,
                 "fp_train_backward: bad arguments");
     PRB_REQUIRE(workspace_bytes >= p.total, "fp_train_backward: workspace of %zu bytes < %zu", workspace_bytes, p.total);
-    for (int l = 0; l < p.L; ++l) PRB_REQUIRE(z[l] && desc->weight[l] && grad_weight[l], "fp_train_backward: layer %d: no Z, weight or gradient", l);
+    if (int rc = st_check_layers(p, desc, "fp_train_backward", z, grad_weight)) return rc;
     const cudaStream_t s = (cudaStream_t)stream;
-    char *ws = reinterpret_cast<char *>(workspace);
-    double *p1 = reinterpret_cast<double *>(ws + p.off_p1), *p2 = reinterpret_cast<double *>(ws + p.off_p2);
-    float *mg = reinterpret_cast<float *>(ws + p.off_mg), *wpart = reinterpret_cast<float *>(ws + p.off_wpart);
-    float *gbuf[2] = {reinterpret_cast<float *>(ws + p.off_g0), reinterpret_cast<float *>(ws + p.off_g1)};
-    float *G = reinterpret_cast<float *>(ws + p.off_proj);
-    int *cnt = reinterpret_cast<int *>(ws + p.off_cnt), *off = reinterpret_cast<int *>(ws + p.off_off);
-    int *tot = reinterpret_cast<int *>(ws + p.off_tot), *list = reinterpret_cast<int *>(ws + p.off_list);
+    double *p1 = st_at<double>(workspace, p.off_p1), *p2 = st_at<double>(workspace, p.off_p2);
+    float *mg = st_at<float>(workspace, p.off_mg), *wpart = st_at<float>(workspace, p.off_wpart);
+    float *G = st_at<float>(workspace, p.off_proj);
+    int *cnt = st_at<int>(workspace, p.off_cnt), *off = st_at<int>(workspace, p.off_off);
+    int *tot = st_at<int>(workspace, p.off_tot), *list = st_at<int>(workspace, p.off_list);
     const FpGeom F{p.rows, n, m, c_interp, c_skip, idx, weight, known_pm, skip};
     const int last = p.L - 1;
 
@@ -1080,65 +1083,48 @@ extern "C" int prb_fp_train_backward(const prb_sa_train_desc *desc, int b, int n
     fp_rev_sort<<<ceil_div(p.krows, kStThreads), kStThreads, 0, s>>>(p.krows, off, list);
     if (int rc = check_launch("fp_rev_sort")) return rc;
 
-    StGrad Lg{p.cout[last], desc->bn, z[last], stats + (size_t)last * ST_ROWS * kStMaxC, nullptr, grad_out, nullptr, p.cout[last], 0, mg};
-    const float *g_in = gbuf[last & 1];
-    fp_train_last_grad<<<dim3(p.T, ceil_div(p.cout[last], 32)), kStThreads, 0, s>>>(p.rows, n, Lg, gbuf[last & 1], p1, p2);
+    const StGrad Lg{p.cout[last], desc->bn, z[last], stats + (size_t)last * ST_ROWS * kStMaxC, nullptr, grad_out, nullptr, p.cout[last], 0, mg};
+    fp_train_last_grad<<<dim3(p.T, ceil_div(p.cout[last], 32)), kStThreads, 0, s>>>(p.rows, n, Lg, p.g(workspace, last), p1, p2);
     if (int rc = check_launch("fp_train_last_grad")) return rc;
-    for (int l = last; l >= 0; --l) {
-        Lg = StGrad{p.cout[l], desc->bn, z[l], stats + (size_t)l * ST_ROWS * kStMaxC, g_in, nullptr, nullptr, p.cout[l], 0, mg};
-        sa_train_grad_finalise<<<p.cout[l], kStThreads, 0, s>>>(p.T, p1, p2, p.rows, desc->bn, grad_gamma ? grad_gamma[l] : nullptr,
-                                                                grad_beta ? grad_beta[l] : nullptr, grad_bias ? grad_bias[l] : nullptr, mg);
-        if (int rc = check_launch("sa_train_grad_finalise")) return rc;
-        const DzSrc D{p.rows, Lg};
-        if (l > 0) {
-            // dW first: it reads this layer's g, which the dA launch below does not overwrite (it writes the other buffer)
-            const StLayer prev{p.cout[l - 1], z[l - 1], stats + (size_t)(l - 1) * ST_ROWS * kStMaxC};
-            sa_train_dw_gemm<<<dim3(ceil_div(p.cout[l], 64), ceil_div(p.cin[l], 64), p.wparts[l]), kStThreads, 0, s>>>(
-                D, ActSrc{p.rows, prev}, p.rows, p.cout[l], p.cin[l], p.wchunk[l], wpart);
-            if (int rc = check_launch("sa_train_dw_gemm")) return rc;
-            const int count = p.cout[l] * p.cin[l];
-            sa_train_dw_reduce<<<ceil_div(count, kStThreads), kStThreads, 0, s>>>(p.wparts[l], count, p.cin[l], p.cin[l], wpart, grad_weight[l]);
-            if (int rc = check_launch("sa_train_dw_reduce")) return rc;
-            float *g_out = gbuf[(l - 1) & 1];
-            sa_train_da_gemm<<<dim3(p.T, ceil_div(p.cin[l], kStColTile)), kStThreads, 0, s>>>(D, DaMasked{prev, g_out}, p.rows, p.cout[l],
-                                                                                              desc->weight[l], p.cin[l], p.cin[l], p.T, p1, p2);
-            if (int rc = check_launch("sa_train_da_gemm")) return rc;
-            g_in = g_out;
-            continue;
-        }
-        const int c1 = p.cout[0], cin0 = p.cin[0];
-        const float *W0 = desc->weight[0];
-        fp_train_gather_g<<<ceil_div(p.krows, kStThreads / 32), kStThreads, 0, s>>>(p.krows, off, list, weight, D, G);
-        if (int rc = check_launch("fp_train_gather_g")) return rc;
-        const MatSrc Gs{p.krows, c1, c1, G};
-        // dWi = G^T F
-        sa_train_dw_gemm<<<dim3(ceil_div(c1, 64), ceil_div(c_interp, 64), p.wparts_i), kStThreads, 0, s>>>(
-            Gs, MatSrc{p.krows, c_interp, c_interp, known_pm}, p.krows, c1, c_interp, p.wchunk_i, wpart);
+    auto dz = [&](int l) {
+        return DzSrc{p.rows, StGrad{p.cout[l], desc->bn, z[l], stats + (size_t)l * ST_ROWS * kStMaxC, p.g(workspace, l), nullptr, nullptr, p.cout[l],
+                                    0, mg}};
+    };
+    if (int rc = st_backward(p, desc, dz, p.T, z, stats, grad_weight, grad_bias, grad_gamma, grad_beta, workspace, s)) return rc;
+
+    const int c1 = p.cout[0], cin0 = p.cin[0];
+    const float *W0 = desc->weight[0];
+    const DzSrc D = dz(0);
+    fp_train_gather_g<<<ceil_div(p.krows, kStThreads / 32), kStThreads, 0, s>>>(p.krows, off, list, weight, D, G);
+    if (int rc = check_launch("fp_train_gather_g")) return rc;
+    const MatSrc Gs{p.krows, c1, c1, G};
+    // dWi = G^T F
+    sa_train_dw_gemm<<<dim3(ceil_div(c1, 64), ceil_div(c_interp, 64), p.wparts_i), kStThreads, 0, s>>>(
+        Gs, MatSrc{p.krows, c_interp, c_interp, known_pm}, p.krows, c1, c_interp, p.wchunk_i, wpart);
+    if (int rc = check_launch("sa_train_dw_gemm")) return rc;
+    sa_train_dw_reduce<<<ceil_div(c1 * c_interp, kStThreads), kStThreads, 0, s>>>(p.wparts_i, c1 * c_interp, c_interp, cin0, wpart,
+                                                                                  grad_weight[0]);
+    if (int rc = check_launch("sa_train_dw_reduce")) return rc;
+    if (c_skip > 0) {
+        // dWs = dZ_0^T S
+        sa_train_dw_gemm<<<dim3(ceil_div(c1, 64), ceil_div(c_skip, 64), p.wparts[0]), kStThreads, 0, s>>>(D, FpSkipSrc{F}, p.rows, c1, c_skip,
+                                                                                                       p.wchunk[0], wpart);
         if (int rc = check_launch("sa_train_dw_gemm")) return rc;
-        sa_train_dw_reduce<<<ceil_div(c1 * c_interp, kStThreads), kStThreads, 0, s>>>(p.wparts_i, c1 * c_interp, c_interp, cin0, wpart,
-                                                                                      grad_weight[0]);
+        sa_train_dw_reduce<<<ceil_div(c1 * c_skip, kStThreads), kStThreads, 0, s>>>(p.wparts[0], c1 * c_skip, c_skip, cin0, wpart,
+                                                                                    grad_weight[0] + c_interp);
         if (int rc = check_launch("sa_train_dw_reduce")) return rc;
-        if (c_skip > 0) {
-            // dWs = dZ_0^T S
-            sa_train_dw_gemm<<<dim3(ceil_div(c1, 64), ceil_div(c_skip, 64), p.wparts[0]), kStThreads, 0, s>>>(D, FpSkipSrc{F}, p.rows, c1, c_skip,
-                                                                                                           p.wchunk[0], wpart);
-            if (int rc = check_launch("sa_train_dw_gemm")) return rc;
-            sa_train_dw_reduce<<<ceil_div(c1 * c_skip, kStThreads), kStThreads, 0, s>>>(p.wparts[0], c1 * c_skip, c_skip, cin0, wpart,
-                                                                                        grad_weight[0] + c_interp);
-            if (int rc = check_launch("sa_train_dw_reduce")) return rc;
-        }
-        if (grad_known) {
-            // dF = G Wi -> (b, c_interp, m)
-            sa_train_da_gemm<<<dim3(p.KT, ceil_div(c_interp, kStColTile)), kStThreads, 0, s>>>(Gs, DaChannelMajor{grad_known, m, c_interp}, p.krows,
-                                                                                               c1, W0, cin0, c_interp, 0, nullptr, nullptr);
-            if (int rc = check_launch("sa_train_da_gemm")) return rc;
-        }
-        if (grad_skip && c_skip > 0) {
-            // dS = dZ_0 Ws -> (b, c_skip, n)
-            sa_train_da_gemm<<<dim3(p.T, ceil_div(c_skip, kStColTile)), kStThreads, 0, s>>>(D, DaChannelMajor{grad_skip, n, c_skip}, p.rows, c1,
-                                                                                            W0 + c_interp, cin0, c_skip, 0, nullptr, nullptr);
-            if (int rc = check_launch("sa_train_da_gemm")) return rc;
-        }
+    }
+    if (grad_known) {
+        // dF = G Wi -> (b, c_interp, m)
+        sa_train_da_gemm<<<dim3(p.KT, ceil_div(c_interp, kStColTile)), kStThreads, 0, s>>>(Gs, DaChannelMajor{grad_known, m, c_interp}, p.krows,
+                                                                                           c1, W0, cin0, c_interp, 0, nullptr, nullptr);
+        if (int rc = check_launch("sa_train_da_gemm")) return rc;
+    }
+    if (grad_skip && c_skip > 0) {
+        // dS = dZ_0 Ws -> (b, c_skip, n)
+        sa_train_da_gemm<<<dim3(p.T, ceil_div(c_skip, kStColTile)), kStThreads, 0, s>>>(D, DaChannelMajor{grad_skip, n, c_skip}, p.rows, c1,
+                                                                                        W0 + c_interp, cin0, c_skip, 0, nullptr, nullptr);
+        if (int rc = check_launch("sa_train_da_gemm")) return rc;
     }
     return 0;
 }

@@ -1,15 +1,14 @@
 """The device training path of a PointnetFPModule's three_interpolate + cat(skip) + SharedMLP (csrc/sa_train.cu,
 prb_fp_train_*), taken when the switch `config.fp_train` is "device", `supported` holds and the dispatch rule
-(`projection`) selects the level; everything else keeps the op-by-op torch path.
+(`faster_on_device`) selects the level; everything else keeps the op-by-op torch path.
 
 One autograd Function per module.  Its inputs are the known features, the skip features and every conv weight / bias and
 BN weight / bias, so autograd accumulates their .grad as for the torch path; the BN running statistics and
 num_batches_tracked are updated in place by the forward, as BatchNorm2d does in training mode.  The interpolation taps
 come from three_nn_weights (the fused path's 3-NN).  Saved for backward: the taps, the point-major known features, the
 skip features, the pre-activations Z of every layer and the per-channel statistics.
-Layer 0 runs in one of two orders, chosen per level by the rule: plain (interpolate the known features, then the GEMM) or
-projected (project the m known points through the interpolated columns of layer 0, then interpolate; n = 4 m at every
-RPN level, so this removes three quarters of that part of layer 0).  The backward always takes the projected order.
+Layer 0 runs projected: the m known points go through the interpolated columns of layer 0 first, then the result is
+interpolated (n = 4 m at every RPN level, so this removes three quarters of that part of layer 0).
 Precision: TF32 tensor-core GEMMs with fp32 accumulation, the BN statistics summed in float64.
 """
 import ctypes
@@ -22,23 +21,19 @@ from . import sa_train
 
 MAX_IN = 2048          # widest layer-0 input (interpolated + skip channels)
 
-# Dispatch rule: (c_known, c_skip, widths) of the levels the device path is faster on, forward + backward, and whether
-# that level projects.  Measured on an H100 SXM (80 GB, 700 W) with scripts/bench_fp_train.py at B = 16 (see
-# INTEGRATION.md); every other level keeps the torch path.
+# Dispatch rule: (c_known, c_skip, widths) of the levels the device path is faster on, forward + backward.  Measured on an
+# H100 SXM (80 GB, 700 W) with scripts/bench_fp_train.py at B = 16 (see INTEGRATION.md); every other level keeps the
+# torch path.
 FAST_LEVELS = {
-    (256, 1, (128, 128)): True,       # RPN FP0: 5.7-5.8 ms projected vs 6.8-7.0 ms torch (plain 7.4 ms)
-    (1024, 512, (512, 512)): True,    # RPN FP3: 1.7-2.6 ms projected vs 2.7-4.6 ms torch (plain 2.3-3.7 ms)
+    (256, 1, (128, 128)),       # RPN FP0: 5.7-5.8 ms device vs 6.8-7.0 ms torch
+    (1024, 512, (512, 512)),    # RPN FP3: 1.7-2.6 ms device vs 2.7-4.6 ms torch
 }
-# RPN FP1 (5.2-5.3 ms projected vs 4.1-4.7 ms torch) and FP2 (4.3-4.4 vs 2.9-3.5 ms) lose in their backward GEMMs.
+# RPN FP1 (5.2-5.3 ms device vs 4.1-4.7 ms torch) and FP2 (4.3-4.4 vs 2.9-3.5 ms) lose in their backward GEMMs.
 
 
-def _key(module, c_known, c_skip):
-    return (c_known, c_skip, tuple(layer.conv.out_channels for layer in module.mlp.children()))
-
-
-def projection(module, c_known, c_skip):
-    """the fixed shape rule of the dispatch: None (torch path), or whether layer 0 runs projected"""
-    return FAST_LEVELS.get(_key(module, c_known, c_skip))
+def faster_on_device(module, c_known, c_skip):
+    """the fixed shape rule of the dispatch (see FAST_LEVELS)"""
+    return (c_known, c_skip, tuple(layer.conv.out_channels for layer in module.mlp.children())) in FAST_LEVELS
 
 
 def supported(module, unknown, known, unknow_feats, known_feats):
@@ -64,7 +59,7 @@ class _FPTrain(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, scale, geom, known_pm, known_feats, skip, *params):
-        idx, weight, project, emit_pm = geom
+        idx, weight, emit_pm = geom
         L = C.lib()
         B, n, _ = idx.shape
         m, c_known = known_pm.size(1), known_pm.size(2)
@@ -80,9 +75,9 @@ class _FPTrain(torch.autograd.Function):
         stats = torch.empty((len(scale.c_out), sa_train.STAT_ROWS, sa_train.MAX_WIDTH), dtype=torch.float32, device=dev)
         with torch.cuda.device(dev):
             ws = torch.empty(L.prb_fp_train_workspace_bytes(B, n, m, c_known, c_skip, ctypes.byref(d), 0), dtype=torch.uint8, device=dev)
-            C.check(L.prb_fp_train_forward(ctypes.byref(d), B, n, m, c_known, c_skip, int(project), C.ptr(idx), C.ptr(weight), C.ptr(known_pm),
-                                           C.ptr(skip), sa_train._ptrs(z), C.ptr(stats), C.ptr(out), C.ptr(out_pm), C.ptr(ws), ws.numel(),
-                                           C.stream()), "fp_train_forward")
+            C.check(L.prb_fp_train_forward(ctypes.byref(d), B, n, m, c_known, c_skip, C.ptr(idx), C.ptr(weight), C.ptr(known_pm), C.ptr(skip),
+                                           sa_train._ptrs(z), C.ptr(stats), C.ptr(out), C.ptr(out_pm), C.ptr(ws), ws.numel(), C.stream()),
+                    "fp_train_forward")
         ctx.scale, ctx.desc = scale, d
         ctx.save_for_backward(idx, weight, known_pm, skip, *params, *z, stats)
         if out_pm is not None:
@@ -117,13 +112,13 @@ class _FPTrain(torch.autograd.Function):
         return (None, None, None, g_known, g_skip) + tuple(sa_train._slot_grads(bufs, ctx.needs_input_grad[5:]))
 
 
-def forward(module, idx, weight, known_pm, known_feats, skip, project, emit_pm):
+def forward(module, idx, weight, known_pm, known_feats, skip, emit_pm):
     """the features (B, C_last, n) of FP module `module` through the device path, and their point-major twin (None unless
     emit_pm).  idx / weight (B, n, 3): three_nn_weights' taps; known_pm (B, m, c_known): known_feats point-major;
     skip (B, c_skip, n) contiguous or None"""
     C.require_cuda(idx, weight, known_pm, known_feats, skip)
     scale = sa_train._Scale(module.mlp)
-    out, out_pm = _FPTrain.apply(scale, (idx, weight, project, emit_pm), known_pm.detach(), known_feats, skip, *scale.params())
+    out, out_pm = _FPTrain.apply(scale, (idx, weight, emit_pm), known_pm.detach(), known_feats, skip, *scale.params())
     sa_train._bump_running_stats(scale)
     return out, out_pm
 

@@ -375,19 +375,11 @@ class PointnetFPModule(nn.Module):
         idx, weight = self.fused_geometry(unknown, known)
         return self.fused_mlp(unknown.size(1), idx, weight, unknow_feats, known_feats)
 
-    def _train_projection(self, unknown, known, unknow_feats, known_feats):
-        """None: the device training path does not apply; else whether its layer 0 runs projected (fp_train's rule)"""
-        if config.get("fp_train") != "device" or not _needs_graph(self, unknown, known, unknow_feats, known_feats):
-            return None
-        if not fp_train.supported(self, unknown, known, unknow_feats, known_feats):
-            return None
-        return fp_train.projection(self, known_feats.size(1), 0 if unknow_feats is None else unknow_feats.size(1))
-
-    def _forward_train(self, unknown, known, unknow_feats, known_feats, project):
+    def _forward_train(self, unknown, known, unknow_feats, known_feats):
         """the fused path's 3-NN, then fp_train's autograd Function"""
         idx, weight = self.fused_geometry(unknown, known)
         skip = unknow_feats.contiguous() if unknow_feats is not None else None
-        out, out_pm = fp_train.forward(self, idx, weight, _point_major(known_feats), known_feats, skip, project, self.emit_point_major)
+        out, out_pm = fp_train.forward(self, idx, weight, _point_major(known_feats), known_feats, skip, self.emit_point_major)
         return _attach_pm(out, out_pm) if out_pm is not None else out
 
     def forward(self, unknown: torch.Tensor, known: torch.Tensor, unknow_feats: torch.Tensor,
@@ -401,9 +393,10 @@ class PointnetFPModule(nn.Module):
         """
         if self._can_fuse(unknown, known, unknow_feats, known_feats):
             return self._forward_fused(unknown, known, unknow_feats, known_feats)
-        project = self._train_projection(unknown, known, unknow_feats, known_feats)
-        if project is not None:
-            return self._forward_train(unknown, known, unknow_feats, known_feats, project)
+        if (config.get("fp_train") == "device" and _needs_graph(self, unknown, known, unknow_feats, known_feats)
+                and fp_train.supported(self, unknown, known, unknow_feats, known_feats)
+                and fp_train.faster_on_device(self, known_feats.size(1), 0 if unknow_feats is None else unknow_feats.size(1))):
+            return self._forward_train(unknown, known, unknow_feats, known_feats)
 
         if known is not None:
             dist, idx = pointnet2_utils.three_nn(unknown, known)

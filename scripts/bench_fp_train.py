@@ -1,11 +1,11 @@
 """FP modules in training mode: the torch path (config.fp_train="torch") against the device path (prb_fp_train_* in
-csrc/sa_train.cu), plain and projected, per level forward / backward time, launches, host syncs and peak memory, and whole
-RPNTrainer steps with the switch off and on.
+csrc/sa_train.cu), per level forward / backward time, launches, host syncs and peak memory, and whole RPNTrainer steps with
+the switch off and on.
 
     python scripts/bench_fp_train.py [--steps 10] [--warmup 3] [--repeats 3] [--batch 16]
 
 Levels: the RPN backbone's FP3-FP0 on B x 16384 points, each fed what the training step gives it (one forward without
-grad, captured at the module).  Every time is measured --repeats times, the three variants alternating, and reported as
+grad, captured at the module).  Every time is measured --repeats times, the two variants alternating, and reported as
 the list of repeats.  The "split" line puts the torch path's FP levels (forward + backward, each measured alone) next to
 the whole torch RPNTrainer.step.  Prints one JSON line per measurement with the card name and power limit.
 """
@@ -78,8 +78,7 @@ def bench_levels(backbone, inputs, steps, warmup, repeats, name):
         sk = skip.detach().requires_grad_(k > 0) if skip is not None else None
         variants = {
             "torch": lambda: m(unknown, known, sk, kf),
-            "device": lambda: m._forward_train(unknown, known, sk, kf, False),
-            "device_proj": lambda: m._forward_train(unknown, known, sk, kf, True),
+            "device": lambda: m._forward_train(unknown, known, sk, kf),
         }
         res = {v: [] for v in variants}
         for _ in range(repeats):

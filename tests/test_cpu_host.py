@@ -102,7 +102,7 @@ def test_cabi_library_exports_every_declared_symbol():
     assert len(names) >= 25
     for n in names:
         assert hasattr(lib, n), "libpointrcnn_b200.so does not export %s" % n
-    assert lib.prb_abi_version() == 6
+    assert lib.prb_abi_version() == 7
     assert lib.prb_launch_count() == 0
     # and the other way round: nothing is exported that the header does not declare
     import subprocess

@@ -53,12 +53,12 @@ def _layers(mod, bn):
     return out
 
 
-def _device(mod, unknown, known, kf, skip, project, gout=None):
+def _device(mod, unknown, known, kf, skip, gout=None):
     mod.zero_grad(set_to_none=True)
     kf.grad = None
     if skip is not None:
         skip.grad = None
-    out = mod._forward_train(unknown, known, skip, kf, project)
+    out = mod._forward_train(unknown, known, skip, kf)
     if gout is None:
         gout = torch.randn(out.shape, device=DEV, generator=torch.Generator(device=DEV).manual_seed(5))
     out.backward(gout)
@@ -71,16 +71,16 @@ def _device_masks(out):
     return [(s[2, :z.size(1)].double() * z.double() + s[3, :z.size(1)].double()) > 0 for z, s in zip(dec["z"], dec["stats"])]
 
 
-def _check_against_reference(mod, unknown, known, kf, skip, project, bn):
+def _check_against_reference(mod, unknown, known, kf, skip, bn):
     _, idx, w = pointnet2_utils.three_nn_weights(unknown.contiguous(), known.contiguous())
     mod.zero_grad(set_to_none=True)
-    out = mod._forward_train(unknown, known, skip, kf, project)
+    out = mod._forward_train(unknown, known, skip, kf)
     gout = torch.randn(out.shape, device=DEV, generator=torch.Generator(device=DEV).manual_seed(5))
     masks = _device_masks(out)
     out.backward(gout)
     out = out.detach()
     ref_out, cache = R.forward(kf.detach().cpu(), skip.detach().cpu() if skip is not None else None, idx.cpu(), w.cpu(), _layers(mod, bn), bn,
-                               order="projected" if project else "plain")
+                               order="projected")
     ref = R.backward(cache, gout.cpu(), masks=masks)
     bad = []
     ok, msg = R.compare(ref_out, out, "fwd")
@@ -105,16 +105,14 @@ def _check_against_reference(mod, unknown, known, kf, skip, project, bn):
     assert not bad, bad
 
 
-@pytest.mark.parametrize("project", [False, True])
 @pytest.mark.parametrize("level", sorted(RPN_LEVELS))
-def test_rpn_levels_match_the_reference(level, project):
+def test_rpn_levels_match_the_reference(level):
     c_known, c_skip, widths, n, m = RPN_LEVELS[level]
     mod = _module(c_known, c_skip, widths)
     unknown, known, kf, skip, _ = _inputs(2, n, m, c_known, c_skip, skip_grad=level != "fp0")
-    _check_against_reference(mod, unknown, known, kf, skip, project, True)
+    _check_against_reference(mod, unknown, known, kf, skip, True)
 
 
-@pytest.mark.parametrize("project", [False, True])
 @pytest.mark.parametrize("c_skip,widths,bn,B,n,m", [
     (0, (32,), True, 2, 200, 50),               # no skip, one layer
     (7, (48, 24, 16), True, 2, 300, 75),        # three layers
@@ -122,14 +120,13 @@ def test_rpn_levels_match_the_reference(level, project):
     (3, (40, 70), False, 1, 50, 13),            # fewer rows than one row tile
     (5, (64, 64), True, 1, 90, 3),              # three known points
 ])
-def test_shapes_match_the_reference(c_skip, widths, bn, B, n, m, project):
+def test_shapes_match_the_reference(c_skip, widths, bn, B, n, m):
     mod = _module(20, c_skip, widths, bn=bn)
     unknown, known, kf, skip, _ = _inputs(B, n, m, 20, c_skip)
-    _check_against_reference(mod, unknown, known, kf, skip, project, bn)
+    _check_against_reference(mod, unknown, known, kf, skip, bn)
 
 
-@pytest.mark.parametrize("project", [False, True])
-def test_two_calls_are_the_same_bits(project):
+def test_two_calls_are_the_same_bits():
     c_known, c_skip, widths, n, m = RPN_LEVELS["fp1"]
     mod = _module(c_known, c_skip, widths)
     unknown, known, kf, skip, _ = _inputs(2, n, m, c_known, c_skip)
@@ -137,7 +134,7 @@ def test_two_calls_are_the_same_bits(project):
     for _ in range(2):
         bns = [layer.bn.bn for layer in mod.mlp.children()]
         saved = [(b.running_mean.clone(), b.running_var.clone()) for b in bns]
-        out, _ = _device(mod, unknown, known, kf, skip, project)
+        out, _ = _device(mod, unknown, known, kf, skip)
         stats = [(b.running_mean.clone(), b.running_var.clone()) for b in bns]
         for b, (rm, rv) in zip(bns, saved):
             b.running_mean.copy_(rm)
@@ -151,12 +148,11 @@ def test_no_host_synchronisation():
     c_known, c_skip, widths, n, m = RPN_LEVELS["fp0"]
     mod = _module(c_known, c_skip, widths)
     unknown, known, kf, skip, _ = _inputs(2, n, m, c_known, c_skip, skip_grad=False)
-    _device(mod, unknown, known, kf, skip, True)
+    _device(mod, unknown, known, kf, skip)
     torch.cuda.synchronize()
     torch.cuda.set_sync_debug_mode("error")
     try:
-        _device(mod, unknown, known, kf, skip, True)
-        _device(mod, unknown, known, kf, skip, False)
+        _device(mod, unknown, known, kf, skip)
     finally:
         torch.cuda.set_sync_debug_mode(0)
 
@@ -167,7 +163,7 @@ def test_nan_in_known_features_propagates_as_on_the_torch_path():
     unknown, known, kf, skip, _ = _inputs(2, n, m, c_known, c_skip)
     with torch.no_grad():
         kf[0, 3, 5] = float("nan")
-    out, _ = _device(mod, unknown, known, kf, skip, True)
+    out, _ = _device(mod, unknown, known, kf, skip)
     with config.override(fp_train="torch"):
         ref = mod(unknown, known, skip, kf)
     assert torch.equal(torch.isnan(out), torch.isnan(ref.detach()))
@@ -202,13 +198,12 @@ def test_the_rule_selects_the_measured_levels():
     chosen = {}
     for k, mod in enumerate(bb.FP_modules):
         c_in = mod.mlp[0].conv.in_channels
-        chosen["fp%d" % k] = fp_train.projection(mod, c_in - skips[k], skips[k])
-    assert chosen == {"fp0": True, "fp1": None, "fp2": None, "fp3": True}
+        chosen["fp%d" % k] = fp_train.faster_on_device(mod, c_in - skips[k], skips[k])
+    assert chosen == {"fp0": True, "fp1": False, "fp2": False, "fp3": True}
 
 
-@pytest.mark.parametrize("B,level,taps,project", [(2, "fp1", "onehot", True), (2, "fp3", "onehot", False), (16, "fp0", "onehot", True),
-                                                  (16, "fp0", "half", False)])
-def test_integer_cases_are_bit_exact(B, level, taps, project):
+@pytest.mark.parametrize("B,level,taps", [(2, "fp1", "onehot"), (2, "fp3", "onehot"), (16, "fp0", "onehot"), (16, "fp0", "half")])
+def test_integer_cases_are_bit_exact(B, level, taps):
     c_known, c_skip, widths, n, m = RPN_LEVELS[level]
     if taps == "half":
         widths = widths[:1]
@@ -224,7 +219,7 @@ def test_integer_cases_are_bit_exact(B, level, taps, project):
     kf = c["known"].to(DEV).requires_grad_(True)
     skip = c["skip"].to(DEV).requires_grad_(True)
     known_pm = kf.detach().transpose(1, 2).contiguous()
-    out, _ = fp_train.forward(mod, c["idx"].to(DEV), c["w"].to(DEV), known_pm, kf, skip, project, False)
+    out, _ = fp_train.forward(mod, c["idx"].to(DEV), c["w"].to(DEV), known_pm, kf, skip, False)
     out.backward(c["gout"].to(DEV))
     assert torch.equal(out.detach().cpu().double(), out_ref)
     assert torch.equal(kf.grad.cpu().double(), ref["known"])
