@@ -120,6 +120,10 @@ PRB_API int prb_gather_points(int b, int c, int n, int npoints, const float *poi
                       float *out, void *stream);
 PRB_API int prb_gather_points_grad(int b, int c, int n, int npoints, const float *grad_out, const int *idx,
                            float *grad_points, void *stream);
+/* ordered form of prb_gather_points_grad: prb_group_points_grad_ws with nsample 1 */
+PRB_API size_t prb_gather_points_grad_workspace_bytes(int b, int n, int npoints);
+PRB_API int prb_gather_points_grad_ws(int b, int c, int n, int npoints, const float *grad_out, const int *idx,
+                                      float *grad_points, void *workspace, size_t workspace_bytes, void *stream);
 
 /* ball_query_wrapper_fast, ball_query.cpp:14-25 -> ball_query_gpu.cu:9-67.
  * argument order is the reference's positional order (b,n,m,radius,nsample,new_xyz,xyz,idx). */
@@ -136,6 +140,23 @@ PRB_API int prb_group_points(int b, int c, int n, int npoints, int nsample, cons
 PRB_API int prb_group_points_grad(int b, int c, int n, int npoints, int nsample, const float *grad_out,
                           const int *idx, float *grad_points, void *stream);
 
+/* Ordered (deterministic) forms of the three gradient scatters above, for torch.use_deterministic_algorithms: the same
+ * arguments and the same contract (the caller zeroes grad_points, the entry ACCUMULATES into it), plus caller scratch
+ * of *_workspace_bytes bytes (0: nothing to do for those sizes).  The plain entries scatter with float atomics, so their
+ * sums come in any order; these give the same bits on every call.
+ * Summation order: the references of one scene are numbered q = 0 .. L-1 in idx's flat order (grouping: L = npoints *
+ * nsample, q = j * nsample + k; interpolation: L = 3 n, q = 3 i + t).  For every source point p and channel ch:
+ *     acc = +0.0f;  for each q with idx[q] == p, in increasing q:  acc = acc + v_q   (fp32 add, rounded to nearest);
+ *     grad_points[b, ch, p] = grad_points[b, ch, p] + acc
+ * with v_q = grad_out[b, ch, q] (grouping, gather) or v_q = grad_out[b, ch, i] * weight[b, i, t] (interpolation; the
+ * fp32 product rounded before the add, never fused).  References with idx outside [0, n) (interpolation: [0, m)) are
+ * ignored.  b * L and b * n (m) must be below 2^31.  Each call builds a reverse index of idx in the scratch (a counting
+ * sort: one memset, six launches) and sums it in one more launch; nothing synchronises with the host. */
+PRB_API size_t prb_group_points_grad_workspace_bytes(int b, int n, int npoints, int nsample);
+PRB_API int prb_group_points_grad_ws(int b, int c, int n, int npoints, int nsample, const float *grad_out,
+                                     const int *idx, float *grad_points, void *workspace, size_t workspace_bytes,
+                                     void *stream);
+
 /* three_nn_wrapper_fast, interpolate.cpp:14-23 (n unknown, m known; outputs d^2 and idx).
  * weight (b,n,3) may be NULL; when given, the inverse-distance weights of
  * pointnet2_modules.py:140-142 are emitted as well. */
@@ -148,6 +169,11 @@ PRB_API int prb_three_interpolate(int b, int c, int m, int n, const float *point
                           const float *weight, float *out, void *stream);
 PRB_API int prb_three_interpolate_grad(int b, int c, int n, int m, const float *grad_out, const int *idx,
                                const float *weight, float *grad_points, void *stream);
+/* ordered form of prb_three_interpolate_grad (see prb_group_points_grad_ws for the order) */
+PRB_API size_t prb_three_interpolate_grad_workspace_bytes(int b, int n, int m);
+PRB_API int prb_three_interpolate_grad_ws(int b, int c, int n, int m, const float *grad_out, const int *idx,
+                                          const float *weight, float *grad_points, void *workspace,
+                                          size_t workspace_bytes, void *stream);
 
 /* (B,C,N) <-> (B,N,C) layout change used in front of the fused kernels */
 PRB_API int prb_transpose_bcn_to_bnc(int b, int c, int n, const float *in, float *out, void *stream);
@@ -545,7 +571,13 @@ PRB_API int prb_stage_loss_backward(const prb_stage_loss_desc *desc, int rows, i
  * backward: from grad_out (b, out_stride_c, npoint) and the forward's z / stats / chosen: grad_weight[l]
  *           (c_out, c_in_l) written, grad_bias[l] (no BN) or grad_gamma[l] / grad_beta[l] (BN) written where non-NULL,
  *           and grad_feats (b, c_feat, n), when non-NULL, ACCUMULATED with atomics (the caller zeroes it).
- * Neither entry allocates or synchronises; all sums except the feature scatter are in a fixed order. */
+ * backward_det: as backward, but grad_feats, when non-NULL, is WRITTEN in a fixed order: layer 0's feature gradient
+ *           dA[r][3 + c] of every row r = (b * npoint + p) * nsample + s is staged in the workspace, then for every point j
+ *           grad_feats[b, c, j] = the sum over the rows of scene b with idx[r] == j, in increasing r, of dA[r][3 + c],
+ *           starting from +0.0f, each fp32 add rounded (points no row names get 0).  Scratch:
+ *           prb_sa_train_det_workspace_bytes, which needs the point count n for the reverse index of idx.
+ * None of the entries allocates or synchronises.  Every sum except backward's feature scatter is in a fixed order, so
+ * backward_det's results are the same bits on every call with the same inputs. */
 typedef struct prb_sa_train_desc {
     int num_layers;                             /* 1..3 */
     int c_in;                                   /* 3 + c_feat */
@@ -570,6 +602,12 @@ PRB_API int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n, i
                                   const float *stats, const unsigned char *chosen, const float *grad_out, int out_stride_c,
                                   int out_c_off, float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma,
                                   float *const *grad_beta, float *grad_feats, void *workspace, size_t workspace_bytes, void *stream);
+PRB_API size_t prb_sa_train_det_workspace_bytes(int b, int n, int npoint, int nsample, int c_feat, const prb_sa_train_desc *desc);
+PRB_API int prb_sa_train_backward_det(const prb_sa_train_desc *desc, int b, int n, int npoint, int nsample, int c_feat, const float *xyz,
+                                      const float *new_xyz, const float *feats_pm, const int *idx, const float *const *z,
+                                      const float *stats, const unsigned char *chosen, const float *grad_out, int out_stride_c,
+                                      int out_c_off, float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma,
+                                      float *const *grad_beta, float *grad_feats, void *workspace, size_t workspace_bytes, void *stream);
 
 /* --- training-mode FP module (csrc/sa_train.cu): three_interpolate + cat(skip) + SharedMLP of one PointnetFPModule,
  * forward and backward for autograd, with the layers of a prb_sa_train_desc (c_in = c_interp + c_skip, at most 2048;

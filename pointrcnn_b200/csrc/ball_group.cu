@@ -10,7 +10,7 @@
 // untouched when nothing hits.  Here: one warp per centre tests 32 points per step; ballot + popc
 // prefix keeps index order; the scene's points are staged through shared memory as SoA tiles shared by
 // all the warps of the CTA; a second radius over the same centres rides along for free (MSG layers).
-#include "common.cuh"
+#include "rev_index.cuh"
 
 namespace prb {
 
@@ -228,6 +228,29 @@ extern "C" int prb_group_points_grad(int b, int c, int n, int npoints, int nsamp
     return check_launch("group_points_grad_kernel");
 }
 
+// the ordered gradient: grad_points[b, c, j] += the sum of grad_out over the references of point j in increasing flat
+// index, through the reverse index of idx (rev_index.cuh)
+extern "C" size_t prb_group_points_grad_workspace_bytes(int b, int n, int npoints, int nsample) {
+    const long L = (long)npoints * nsample;
+    if (b <= 0 || n <= 0 || npoints <= 0 || nsample <= 0 || !rev_index_fits(b, L, n)) return 0;
+    return rev_index_bytes(b, (int)L, n);
+}
+
+extern "C" int prb_group_points_grad_ws(int b, int c, int n, int npoints, int nsample, const float *grad_out, const int *idx,
+                                        float *grad_points, void *workspace, size_t workspace_bytes, void *stream) {
+    PRB_REQUIRE(b >= 0 && c >= 0 && n >= 0 && npoints >= 0 && nsample > 0, "group_points_grad_ws: bad dimensions");
+    const long L = (long)npoints * nsample;
+    if (b == 0 || c == 0 || n == 0 || L == 0) return 0;
+    PRB_REQUIRE(rev_index_fits(b, L, n), "group_points_grad_ws: %d x %ld references over %d points", b, L, n);
+    PRB_REQUIRE(grad_out && idx && grad_points && workspace, "group_points_grad_ws: bad arguments");
+    const size_t need = rev_index_bytes(b, (int)L, n);
+    PRB_REQUIRE(workspace_bytes >= need, "group_points_grad_ws: workspace of %zu bytes < %zu", workspace_bytes, need);
+    const RevIndex R = rev_index_at(b, (int)L, n, workspace);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (int rc = rev_index_build(R, idx, s)) return rc;
+    return seg_sum(R, SEG_GROUP, c, grad_out, nullptr, true, grad_points, s);
+}
+
 // gather == grouping with nsample = 1
 extern "C" int prb_gather_points(int b, int c, int n, int npoints, const float *points, const int *idx, float *out,
                                  void *stream) {
@@ -236,6 +259,13 @@ extern "C" int prb_gather_points(int b, int c, int n, int npoints, const float *
 extern "C" int prb_gather_points_grad(int b, int c, int n, int npoints, const float *grad_out, const int *idx,
                                       float *grad_points, void *stream) {
     return prb_group_points_grad(b, c, n, npoints, 1, grad_out, idx, grad_points, stream);
+}
+extern "C" size_t prb_gather_points_grad_workspace_bytes(int b, int n, int npoints) {
+    return prb_group_points_grad_workspace_bytes(b, n, npoints, 1);
+}
+extern "C" int prb_gather_points_grad_ws(int b, int c, int n, int npoints, const float *grad_out, const int *idx, float *grad_points,
+                                         void *workspace, size_t workspace_bytes, void *stream) {
+    return prb_group_points_grad_ws(b, c, n, npoints, 1, grad_out, idx, grad_points, workspace, workspace_bytes, stream);
 }
 
 extern "C" int prb_transpose_bcn_to_bnc(int b, int c, int n, const float *in, float *out, void *stream) {

@@ -11,7 +11,7 @@
 // fewer than three points exist.
 #include <math_constants.h>
 
-#include "common.cuh"
+#include "rev_index.cuh"
 
 namespace prb {
 
@@ -161,4 +161,25 @@ extern "C" int prb_three_interpolate_grad(int b, int c, int n, int m, const floa
     dim3 grid(min(ceil_div(n, TI_THREADS), 64), ceil_div(c, TI_CH), b);
     three_interpolate_grad_kernel<<<grid, TI_THREADS, 0, (cudaStream_t)stream>>>(c, n, m, grad_out, idx, weight, grad_points);
     return check_launch("three_interpolate_grad_kernel");
+}
+
+// the ordered gradient: grad_points[b, c, k] += the sum of grad_out * weight over the taps q = 3 i + t naming known point k,
+// in increasing q, through the reverse index of idx (rev_index.cuh)
+extern "C" size_t prb_three_interpolate_grad_workspace_bytes(int b, int n, int m) {
+    if (b <= 0 || n <= 0 || m <= 0 || !rev_index_fits(b, 3L * n, m)) return 0;
+    return rev_index_bytes(b, 3 * n, m);
+}
+
+extern "C" int prb_three_interpolate_grad_ws(int b, int c, int n, int m, const float *grad_out, const int *idx, const float *weight,
+                                             float *grad_points, void *workspace, size_t workspace_bytes, void *stream) {
+    PRB_REQUIRE(b >= 0 && c >= 0 && n >= 0 && m >= 0, "three_interpolate_grad_ws: bad dimensions");
+    if (b == 0 || c == 0 || n == 0 || m == 0) return 0;
+    PRB_REQUIRE(rev_index_fits(b, 3L * n, m), "three_interpolate_grad_ws: %d x %d rows over %d points", b, n, m);
+    PRB_REQUIRE(grad_out && idx && weight && grad_points && workspace, "three_interpolate_grad_ws: bad arguments");
+    const size_t need = rev_index_bytes(b, 3 * n, m);
+    PRB_REQUIRE(workspace_bytes >= need, "three_interpolate_grad_ws: workspace of %zu bytes < %zu", workspace_bytes, need);
+    const RevIndex R = rev_index_at(b, 3 * n, m, workspace);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (int rc = rev_index_build(R, idx, s)) return rc;
+    return seg_sum(R, SEG_TAPS, c, grad_out, weight, true, grad_points, s);
 }

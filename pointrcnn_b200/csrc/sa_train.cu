@@ -10,14 +10,17 @@
 //             statistics, a, b); then one max-pool launch that records the chosen sample of every (group, channel)
 //   backward  per layer, last to first: the BN statistics sum(g), sum(g * xhat) (last layer: over the chosen rows only;
 //             inner layers: in the epilogue of the GEMM that produced their dA), a finalise launch (dgamma, dbeta / dbias),
-//             dA = dZ W (skipped for layer 0 without a feature gradient; layer 0 scatters into d features with atomics),
+//             dA = dZ W (skipped for layer 0 without a feature gradient; layer 0 scatters into d features with atomics, or in
+//             the ordered backward stages them for a per-point sum over the reverse index of idx),
 //             dW = dZ^T A as per-CTA partials over row ranges, reduced in a fixed order
 // dZ = a (g - sum(g)/n - xhat sum(g xhat)/n) (no BN: dZ = g) is formed on load.  GEMMs are mma.sync m16n8k8 TF32 with fp32
-// accumulation.  No float atomics except the feature scatter: parameter gradients, outputs and running statistics are the
-// same bits on every call with the same inputs.
+// accumulation.  No float atomics except the feature scatter of prb_sa_train_backward: parameter gradients, outputs and
+// running statistics are the same bits on every call with the same inputs, and so is the feature gradient of
+// prb_sa_train_backward_det, which stages layer 0's feature columns and sums them per point over a reverse index of idx.
 #include <algorithm>
 
 #include "mlp_dev.cuh"
+#include "rev_index.cuh"
 
 namespace prb {
 
@@ -448,6 +451,14 @@ struct DaScatterFeats {     // SA layer 0: the feature columns are scattered int
         }
     }
 };
+struct DaStageFeats {       // SA layer 0, ordered: the feature columns are stored (rows, c_feat) for the gather-sum
+    static constexpr bool kSums = false;
+    int c_feat;
+    float *stage;
+    __device__ void operator()(int r, int c, float v, float &, float &) const {
+        if (c >= 3) stage[(size_t)r * c_feat + (c - 3)] = v;
+    }
+};
 struct DaMasked {           // inner layer: masked by the previous layer's ReLU, stored as its g; g and xhat feed its BN sums
     static constexpr bool kSums = true;
     StLayer P;
@@ -617,116 +628,6 @@ __global__ void __launch_bounds__(kStThreads) fp_train_last_grad(int rows, int n
     }
 }
 
-// Reverse index of the taps: the references q = 3 r + t of known point j = b * m + idx[q] end up in list[off[j] ..
-// off[j + 1]) in increasing q.  Counts and slots use integer atomics; the per-point sort fixes the order.
-__global__ void __launch_bounds__(kStThreads) fp_rev_count(FpGeom F, int *cnt) {
-    const int q = blockIdx.x * kStThreads + threadIdx.x;
-    if (q < 3 * F.rows) atomicAdd(cnt + (q / 3 / F.n) * F.m + F.idx[q], 1);
-}
-
-constexpr int kScanItems = 4 * kStThreads;   // counts per block of the offset scan
-
-// exclusive prefix of v over the block; total receives the block's sum
-__device__ __forceinline__ int st_block_scan(int v, int &total) {
-    __shared__ int ws[kStThreads / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    int x = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-        const int y = __shfl_up_sync(0xffffffffu, x, o);
-        if (lane >= o) x += y;
-    }
-    if (lane == 31) ws[warp] = x;
-    __syncthreads();
-    if (warp == 0) {
-        int w = lane < kStThreads / 32 ? ws[lane] : 0;
-#pragma unroll
-        for (int o = 1; o < kStThreads / 32; o <<= 1) {
-            const int y = __shfl_up_sync(0xffffffffu, w, o);
-            if (lane >= o) w += y;
-        }
-        if (lane < kStThreads / 32) ws[lane] = w;
-    }
-    __syncthreads();
-    const int before = warp ? ws[warp - 1] : 0;
-    total = ws[kStThreads / 32 - 1];
-    __syncthreads();
-    return before + x - v;
-}
-
-// off[i] = the prefix of cnt within its block of kScanItems; tot[block] = the block's sum
-__global__ void __launch_bounds__(kStThreads) fp_scan_local(int K, const int *cnt, int *off, int *tot) {
-    const int base = blockIdx.x * kScanItems + threadIdx.x * 4;
-    int v[4], s = 0;
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        v[i] = base + i < K ? cnt[base + i] : 0;
-        s += v[i];
-    }
-    int total;
-    int x = st_block_scan(s, total);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        if (base + i < K) off[base + i] = x;
-        x += v[i];
-    }
-    if (threadIdx.x == 0) tot[blockIdx.x] = total;
-}
-
-// one block: tot -> its exclusive prefix; off[K] = the sum of all counts
-__global__ void __launch_bounds__(kStThreads) fp_scan_blocks(int nb, int *tot, int *off_end) {
-    int carry = 0;
-    for (int b0 = 0; b0 < nb; b0 += kStThreads) {
-        const int i = b0 + (int)threadIdx.x;
-        const int v = i < nb ? tot[i] : 0;
-        int total;
-        const int x = st_block_scan(v, total);
-        if (i < nb) tot[i] = carry + x;
-        carry += total;
-    }
-    if (threadIdx.x == 0) *off_end = carry;
-}
-
-__global__ void __launch_bounds__(kStThreads) fp_scan_add(int K, const int *tot, int *off) {
-    const int i = blockIdx.x * kStThreads + threadIdx.x;
-    if (i < K) off[i] += tot[i / kScanItems];
-}
-
-// each reference into a free slot of its point (cnt counts down to 0)
-__global__ void __launch_bounds__(kStThreads) fp_rev_fill(FpGeom F, const int *off, int *cnt, int *list) {
-    const int q = blockIdx.x * kStThreads + threadIdx.x;
-    if (q >= 3 * F.rows) return;
-    const int j = (q / 3 / F.n) * F.m + F.idx[q];
-    list[off[j] + atomicSub(cnt + j, 1) - 1] = q;
-}
-
-// every point's references in increasing order (heapsort: bounded work however many rows share a known point)
-__global__ void __launch_bounds__(kStThreads) fp_rev_sort(int K, const int *off, int *list) {
-    const int j = blockIdx.x * kStThreads + threadIdx.x;
-    if (j >= K) return;
-    int *a = list + off[j];
-    const int len = off[j + 1] - off[j];
-    auto sift = [a](int root, int end) {
-        for (;;) {
-            int ch = 2 * root + 1;
-            if (ch >= end) return;
-            if (ch + 1 < end && a[ch + 1] > a[ch]) ++ch;
-            if (a[root] >= a[ch]) return;
-            const int t = a[root];
-            a[root] = a[ch];
-            a[ch] = t;
-            root = ch;
-        }
-    };
-    for (int i = len / 2 - 1; i >= 0; --i) sift(i, len);
-    for (int e = len - 1; e > 0; --e) {
-        const int t = a[0];
-        a[0] = a[e];
-        a[e] = t;
-        sift(0, e);
-    }
-}
-
 // G = I^T dZ_0 (b m, c1): per known point the sum over its references in list order, one warp per point
 __global__ void __launch_bounds__(kStThreads) fp_train_gather_g(int K, const int *off, const int *list, const float *w, DzSrc D, float *G) {
     const int j = blockIdx.x * (kStThreads / 32) + (threadIdx.x >> 5);
@@ -872,6 +773,7 @@ int st_backward(const StackPlan &p, const prb_sa_train_desc *d, Dz dz, int npart
 
 struct StPlan : StackPlan {
     int P, gpp;            // parts / groups per part of the last layer's statistics pass
+    size_t off_stage, off_rev, det_total;   // the ordered backward's scratch after `total` (st_det_layout)
 };
 
 int st_plan(const prb_sa_train_desc *d, int b, int npoint, int ns, int c_feat, StPlan &p) {
@@ -890,6 +792,16 @@ int st_plan(const prb_sa_train_desc *d, int b, int npoint, int ns, int c_feat, S
     const int cmax = *std::max_element(p.cout, p.cout + p.L);
     const int cinner = p.L > 1 ? *std::max_element(p.cout, p.cout + p.L - 1) : 0;
     st_layout(p, (size_t)cmax * max(p.T, p.P), 0, (size_t)p.wparts[0] * p.cout[0] * p.cin[0], cinner);
+    return 0;
+}
+
+// the ordered backward: the staged layer-0 feature gradient (rows, c_feat) and the reverse index of idx over the n points
+int st_det_layout(StPlan &p, int b, int n, int npoint, int ns, int c_feat) {
+    PRB_REQUIRE(n >= 1 && rev_index_fits(b, (long)npoint * ns, n), "sa_train: %d scenes of %d points", b, n);
+    size_t at = p.total;
+    p.off_stage = st_take(at, (size_t)p.rows * c_feat * sizeof(float));
+    p.off_rev = st_take(at, rev_index_bytes(b, npoint * ns, n));
+    p.det_total = at;
     return 0;
 }
 
@@ -938,16 +850,22 @@ extern "C" int prb_sa_train_forward(const prb_sa_train_desc *desc, int b, int n,
     return check_launch("sa_train_pool");
 }
 
-extern "C" int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n, int npoint, int nsample, int c_feat, const float *xyz,
-                                     const float *new_xyz, const float *feats_pm, const int *idx, const float *const *z,
-                                     const float *stats, const unsigned char *chosen, const float *grad_out, int out_stride_c,
-                                     int out_c_off, float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma,
-                                     float *const *grad_beta, float *grad_feats, void *workspace, size_t workspace_bytes, void *stream) {
+namespace prb {
+
+int sa_train_backward(bool ordered, const prb_sa_train_desc *desc, int b, int n, int npoint, int nsample, int c_feat, const float *xyz,
+                      const float *new_xyz, const float *feats_pm, const int *idx, const float *const *z, const float *stats,
+                      const unsigned char *chosen, const float *grad_out, int out_stride_c, int out_c_off, float *const *grad_weight,
+                      float *const *grad_bias, float *const *grad_gamma, float *const *grad_beta, float *grad_feats, void *workspace,
+                      size_t workspace_bytes, void *stream) {
     StPlan p;
     if (int rc = st_plan(desc, b, npoint, nsample, c_feat, p)) return rc;
+    if (ordered) {
+        if (int rc = st_det_layout(p, b, n, npoint, nsample, c_feat)) return rc;
+    }
+    const size_t need = ordered ? p.det_total : p.total;
     PRB_REQUIRE(xyz && new_xyz && idx && z && stats && chosen && grad_out && grad_weight && (c_feat == 0 || feats_pm) && workspace,
                 "sa_train_backward: bad arguments");
-    PRB_REQUIRE(workspace_bytes >= p.total, "sa_train_backward: workspace of %zu bytes < %zu", workspace_bytes, p.total);
+    PRB_REQUIRE(workspace_bytes >= need, "sa_train_backward: workspace of %zu bytes < %zu", workspace_bytes, need);
     PRB_REQUIRE(out_c_off >= 0 && out_c_off + p.cout[p.L - 1] <= out_stride_c, "sa_train_backward: channels %d..%d outside %d", out_c_off,
                 out_c_off + p.cout[p.L - 1], out_stride_c);
     if (int rc = st_check_layers(p, desc, "sa_train_backward", z, grad_weight)) return rc;
@@ -963,7 +881,8 @@ extern "C" int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n
     sa_train_last_stats<<<p.P, kStThreads, 0, s>>>(G, dz(p.L - 1).L, p.gpp, p1, p2);
     if (int rc = check_launch("sa_train_last_stats")) return rc;
     if (int rc = st_backward(p, desc, dz, p.P, z, stats, grad_weight, grad_bias, grad_gamma, grad_beta, workspace, s)) return rc;
-    // layer 0: dW over the grouped rows; dA only for the feature columns, scattered into grad_feats
+    // layer 0: dW over the grouped rows; dA only for the feature columns, scattered into grad_feats (ordered: staged, then
+    // summed per point over the reverse index of idx)
     sa_train_dw_gemm<<<dim3(ceil_div(p.cout[0], 64), ceil_div(p.cin[0], 64), p.wparts[0]), kStThreads, 0, s>>>(dz(0), SaA0Src{G}, p.rows, p.cout[0],
                                                                                                             p.cin[0], p.wchunk[0], wpart);
     if (int rc = check_launch("sa_train_dw_gemm")) return rc;
@@ -971,9 +890,45 @@ extern "C" int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n
     sa_train_dw_reduce<<<ceil_div(count, kStThreads), kStThreads, 0, s>>>(p.wparts[0], count, p.cin[0], p.cin[0], wpart, grad_weight[0]);
     if (int rc = check_launch("sa_train_dw_reduce")) return rc;
     if (!grad_feats || c_feat == 0) return 0;
-    sa_train_da_gemm<<<dim3(p.T, ceil_div(p.cin[0], kStColTile)), kStThreads, 0, s>>>(dz(0), DaScatterFeats{G, grad_feats}, p.rows, p.cout[0],
-                                                                                      desc->weight[0], p.cin[0], p.cin[0], p.T, nullptr, nullptr);
-    return check_launch("sa_train_da_gemm");
+    const dim3 grid(p.T, ceil_div(p.cin[0], kStColTile));
+    if (!ordered) {
+        sa_train_da_gemm<<<grid, kStThreads, 0, s>>>(dz(0), DaScatterFeats{G, grad_feats}, p.rows, p.cout[0], desc->weight[0], p.cin[0], p.cin[0],
+                                                     p.T, nullptr, nullptr);
+        return check_launch("sa_train_da_gemm");
+    }
+    float *stage = st_at<float>(workspace, p.off_stage);
+    const RevIndex R = rev_index_at(b, npoint * nsample, n, st_at<void>(workspace, p.off_rev));
+    if (int rc = rev_index_build(R, idx, s)) return rc;
+    sa_train_da_gemm<<<grid, kStThreads, 0, s>>>(dz(0), DaStageFeats{c_feat, stage}, p.rows, p.cout[0], desc->weight[0], p.cin[0], p.cin[0],
+                                                 p.T, nullptr, nullptr);
+    if (int rc = check_launch("sa_train_da_gemm")) return rc;
+    return seg_sum(R, SEG_ROWS, c_feat, stage, nullptr, false, grad_feats, s);
+}
+
+}  // namespace prb
+
+extern "C" int prb_sa_train_backward(const prb_sa_train_desc *desc, int b, int n, int npoint, int nsample, int c_feat, const float *xyz,
+                                     const float *new_xyz, const float *feats_pm, const int *idx, const float *const *z,
+                                     const float *stats, const unsigned char *chosen, const float *grad_out, int out_stride_c,
+                                     int out_c_off, float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma,
+                                     float *const *grad_beta, float *grad_feats, void *workspace, size_t workspace_bytes, void *stream) {
+    return sa_train_backward(false, desc, b, n, npoint, nsample, c_feat, xyz, new_xyz, feats_pm, idx, z, stats, chosen, grad_out, out_stride_c,
+                             out_c_off, grad_weight, grad_bias, grad_gamma, grad_beta, grad_feats, workspace, workspace_bytes, stream);
+}
+
+extern "C" size_t prb_sa_train_det_workspace_bytes(int b, int n, int npoint, int nsample, int c_feat, const prb_sa_train_desc *desc) {
+    StPlan p;
+    if (st_plan(desc, b, npoint, nsample, c_feat, p) || st_det_layout(p, b, n, npoint, nsample, c_feat)) return 0;
+    return p.det_total;
+}
+
+extern "C" int prb_sa_train_backward_det(const prb_sa_train_desc *desc, int b, int n, int npoint, int nsample, int c_feat, const float *xyz,
+                                         const float *new_xyz, const float *feats_pm, const int *idx, const float *const *z,
+                                         const float *stats, const unsigned char *chosen, const float *grad_out, int out_stride_c,
+                                         int out_c_off, float *const *grad_weight, float *const *grad_bias, float *const *grad_gamma,
+                                         float *const *grad_beta, float *grad_feats, void *workspace, size_t workspace_bytes, void *stream) {
+    return sa_train_backward(true, desc, b, n, npoint, nsample, c_feat, xyz, new_xyz, feats_pm, idx, z, stats, chosen, grad_out, out_stride_c,
+                             out_c_off, grad_weight, grad_bias, grad_gamma, grad_beta, grad_feats, workspace, workspace_bytes, stream);
 }
 
 // ------------------------------------------------------------------------------------------------ FP module, host side
@@ -984,8 +939,7 @@ constexpr int kFpMaxIn = 2048;     // widest layer-0 input (interpolated + skip 
 struct FpPlan : StackPlan {
     int krows, KT;              // b m known rows, their row tiles
     int wparts_i, wchunk_i;     // dWi over the known rows
-    int scan_blocks;
-    size_t off_proj, off_cnt, off_off, off_tot, off_list;
+    size_t off_proj, off_rev;
 };
 
 int fp_plan(const prb_sa_train_desc *d, int b, int n, int m, int ci, int cs, FpPlan &p) {
@@ -998,16 +952,12 @@ int fp_plan(const prb_sa_train_desc *d, int b, int n, int m, int ci, int cs, FpP
     p.KT = ceil_div(p.krows, kStRowTile);
     st_wsplit(p.rows, p.cout[0], max(cs, 1), p.wchunk[0], p.wparts[0]);
     st_wsplit(p.krows, p.cout[0], ci, p.wchunk_i, p.wparts_i);
-    p.scan_blocks = ceil_div(p.krows, kScanItems);
     const int cmax = *std::max_element(p.cout, p.cout + p.L);
     const size_t wpart0 = std::max((size_t)p.wparts[0] * p.cout[0] * cs, (size_t)p.wparts_i * p.cout[0] * ci);
     // proj: the forward's P = F Wi^T, the backward's G = I^T dZ_0
     p.off_proj = st_layout(p, (size_t)cmax * p.T, (size_t)p.krows * p.cout[0] * sizeof(float), wpart0, cmax);
     size_t at = p.total;
-    p.off_cnt = st_take(at, (size_t)p.krows * sizeof(int));
-    p.off_off = st_take(at, (size_t)(p.krows + 1) * sizeof(int));
-    p.off_tot = st_take(at, (size_t)p.scan_blocks * sizeof(int));
-    p.off_list = st_take(at, (size_t)3 * p.rows * sizeof(int));
+    p.off_rev = st_take(at, rev_index_bytes(b, 3 * n, m));
     p.total = at;
     return 0;
 }
@@ -1062,26 +1012,12 @@ extern "C" int prb_fp_train_backward(const prb_sa_train_desc *desc, int b, int n
     double *p1 = st_at<double>(workspace, p.off_p1), *p2 = st_at<double>(workspace, p.off_p2);
     float *mg = st_at<float>(workspace, p.off_mg), *wpart = st_at<float>(workspace, p.off_wpart);
     float *G = st_at<float>(workspace, p.off_proj);
-    int *cnt = st_at<int>(workspace, p.off_cnt), *off = st_at<int>(workspace, p.off_off);
-    int *tot = st_at<int>(workspace, p.off_tot), *list = st_at<int>(workspace, p.off_list);
+    const RevIndex R = rev_index_at(b, 3 * n, m, st_at<void>(workspace, p.off_rev));
     const FpGeom F{p.rows, n, m, c_interp, c_skip, idx, weight, known_pm, skip};
     const int last = p.L - 1;
 
     // the reverse index depends only on the taps: build it first
-    if (cudaMemsetAsync(cnt, 0, (size_t)p.krows * sizeof(int), s) != cudaSuccess) return check_launch("fp_train_backward: memset");
-    const int qblocks = ceil_div(3 * p.rows, kStThreads);
-    fp_rev_count<<<qblocks, kStThreads, 0, s>>>(F, cnt);
-    if (int rc = check_launch("fp_rev_count")) return rc;
-    fp_scan_local<<<p.scan_blocks, kStThreads, 0, s>>>(p.krows, cnt, off, tot);
-    if (int rc = check_launch("fp_scan_local")) return rc;
-    fp_scan_blocks<<<1, kStThreads, 0, s>>>(p.scan_blocks, tot, off + p.krows);
-    if (int rc = check_launch("fp_scan_blocks")) return rc;
-    fp_scan_add<<<ceil_div(p.krows, kStThreads), kStThreads, 0, s>>>(p.krows, tot, off);
-    if (int rc = check_launch("fp_scan_add")) return rc;
-    fp_rev_fill<<<qblocks, kStThreads, 0, s>>>(F, off, cnt, list);
-    if (int rc = check_launch("fp_rev_fill")) return rc;
-    fp_rev_sort<<<ceil_div(p.krows, kStThreads), kStThreads, 0, s>>>(p.krows, off, list);
-    if (int rc = check_launch("fp_rev_sort")) return rc;
+    if (int rc = rev_index_build(R, idx, s)) return rc;
 
     const StGrad Lg{p.cout[last], desc->bn, z[last], stats + (size_t)last * ST_ROWS * kStMaxC, nullptr, grad_out, nullptr, p.cout[last], 0, mg};
     fp_train_last_grad<<<dim3(p.T, ceil_div(p.cout[last], 32)), kStThreads, 0, s>>>(p.rows, n, Lg, p.g(workspace, last), p1, p2);
@@ -1095,7 +1031,7 @@ extern "C" int prb_fp_train_backward(const prb_sa_train_desc *desc, int b, int n
     const int c1 = p.cout[0], cin0 = p.cin[0];
     const float *W0 = desc->weight[0];
     const DzSrc D = dz(0);
-    fp_train_gather_g<<<ceil_div(p.krows, kStThreads / 32), kStThreads, 0, s>>>(p.krows, off, list, weight, D, G);
+    fp_train_gather_g<<<ceil_div(p.krows, kStThreads / 32), kStThreads, 0, s>>>(p.krows, R.off, R.list, weight, D, G);
     if (int rc = check_launch("fp_train_gather_g")) return rc;
     const MatSrc Gs{p.krows, c1, c1, G};
     // dWi = G^T F

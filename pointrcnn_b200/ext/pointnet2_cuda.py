@@ -3,6 +3,11 @@
 Every function takes the reference's positional arguments (explicit dims + caller-allocated tensors),
 sets the device of the first tensor, launches on torch's current stream and raises RuntimeError on
 failure (the reference prints and exit(-1)s).
+
+The three gradient scatters (group_points_grad, gather_points_grad, three_interpolate_grad) add with float
+atomics, so their sums come in any order.  Under torch.use_deterministic_algorithms(True) (warn_only too)
+they take the ordered *_grad_ws entries instead: the same contract, the sums in a fixed order
+(include/pointrcnn_b200.h), scratch from torch's allocator.
 """
 import torch
 
@@ -32,6 +37,10 @@ def _i32(*tensors_and_sizes):
             raise RuntimeError("%s has %d elements, the given dimensions need %d" % (name, t.numel(), need))
 
 
+def _workspace(nbytes, like):
+    return torch.empty(nbytes, dtype=torch.uint8, device=like.device) if nbytes else None
+
+
 def ball_query_wrapper(b, n, m, radius, nsample, new_xyz, xyz, idx):
     C.require_cuda(new_xyz, xyz, idx); C.require_contig(new_xyz, xyz, idx)
     _f32((new_xyz, b * m * 3, "new_xyz"), (xyz, b * n * 3, "xyz")); _i32((idx, b * m * nsample, "idx"))
@@ -54,7 +63,14 @@ def group_points_grad_wrapper(b, c, n, npoints, nsample, grad_out, idx, grad_poi
     C.require_cuda(grad_out, idx, grad_points); C.require_contig(grad_out, idx, grad_points)
     _f32((grad_out, b * c * npoints * nsample, "grad_out"), (grad_points, b * c * n, "grad_points")); _i32((idx, b * npoints * nsample, "idx"))
     with _guard(grad_out):
-        C.check(C.lib().prb_group_points_grad(int(b), int(c), int(n), int(npoints), int(nsample), C.ptr(grad_out),
+        lib = C.lib()
+        if torch.are_deterministic_algorithms_enabled():
+            wsb = lib.prb_group_points_grad_workspace_bytes(int(b), int(n), int(npoints), int(nsample))
+            ws = _workspace(wsb, grad_out)
+            C.check(lib.prb_group_points_grad_ws(int(b), int(c), int(n), int(npoints), int(nsample), C.ptr(grad_out), C.ptr(idx),
+                                                 C.ptr(grad_points), C.ptr(ws), C.c_size_t(wsb), C.stream()), "group_points_grad_ws")
+        else:
+            C.check(lib.prb_group_points_grad(int(b), int(c), int(n), int(npoints), int(nsample), C.ptr(grad_out),
                                               C.ptr(idx), C.ptr(grad_points), C.stream()), "group_points_grad")
     return 1
 
@@ -72,7 +88,14 @@ def gather_points_grad_wrapper(b, c, n, npoints, grad_out, idx, grad_points):
     C.require_cuda(grad_out, idx, grad_points); C.require_contig(grad_out, idx, grad_points)
     _f32((grad_out, b * c * npoints, "grad_out"), (grad_points, b * c * n, "grad_points")); _i32((idx, b * npoints, "idx"))
     with _guard(grad_out):
-        C.check(C.lib().prb_gather_points_grad(int(b), int(c), int(n), int(npoints), C.ptr(grad_out), C.ptr(idx),
+        lib = C.lib()
+        if torch.are_deterministic_algorithms_enabled():
+            wsb = lib.prb_gather_points_grad_workspace_bytes(int(b), int(n), int(npoints))
+            ws = _workspace(wsb, grad_out)
+            C.check(lib.prb_gather_points_grad_ws(int(b), int(c), int(n), int(npoints), C.ptr(grad_out), C.ptr(idx), C.ptr(grad_points),
+                                                  C.ptr(ws), C.c_size_t(wsb), C.stream()), "gather_points_grad_ws")
+        else:
+            C.check(lib.prb_gather_points_grad(int(b), int(c), int(n), int(npoints), C.ptr(grad_out), C.ptr(idx),
                                                C.ptr(grad_points), C.stream()), "gather_points_grad")
     return 1
 
@@ -109,5 +132,12 @@ def three_interpolate_grad_wrapper(b, c, n, m, grad_out, idx, weight, grad_point
     C.require_cuda(grad_out, idx, weight, grad_points); C.require_contig(grad_out, idx, weight, grad_points)
     _f32((grad_out, b * c * n, "grad_out"), (weight, b * n * 3, "weight"), (grad_points, b * c * m, "grad_points")); _i32((idx, b * n * 3, "idx"))
     with _guard(grad_out):
-        C.check(C.lib().prb_three_interpolate_grad(int(b), int(c), int(n), int(m), C.ptr(grad_out), C.ptr(idx),
+        lib = C.lib()
+        if torch.are_deterministic_algorithms_enabled():
+            wsb = lib.prb_three_interpolate_grad_workspace_bytes(int(b), int(n), int(m))
+            ws = _workspace(wsb, grad_out)
+            C.check(lib.prb_three_interpolate_grad_ws(int(b), int(c), int(n), int(m), C.ptr(grad_out), C.ptr(idx), C.ptr(weight),
+                                                      C.ptr(grad_points), C.ptr(ws), C.c_size_t(wsb), C.stream()), "three_interpolate_grad_ws")
+        else:
+            C.check(lib.prb_three_interpolate_grad(int(b), int(c), int(n), int(m), C.ptr(grad_out), C.ptr(idx),
                                                    C.ptr(weight), C.ptr(grad_points), C.stream()), "three_interpolate_grad")

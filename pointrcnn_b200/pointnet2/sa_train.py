@@ -6,6 +6,8 @@ weight / bias, so autograd accumulates their .grad as for the torch path; the BN
 num_batches_tracked are updated in place by the forward, as BatchNorm2d does in training mode.  Saved for backward: the
 pre-activations Z of every layer, the per-channel statistics and the sample each pooled output took (`decisions`).
 Precision: TF32 tensor-core GEMMs with fp32 accumulation, the BN statistics summed in float64.
+Under torch.use_deterministic_algorithms(True) (warn_only too) the backward takes prb_sa_train_backward_det, whose feature
+gradient is summed per point in a fixed order instead of scattered with float atomics; every other result is the same.
 """
 import ctypes
 
@@ -199,8 +201,10 @@ class _SATrain(torch.autograd.Function):
         dev = xyz.device
         g_out = g_out.contiguous()
         c_total = g_out.size(1)
+        ordered = torch.are_deterministic_algorithms_enabled()
         if ctx.needs_input_grad[3] and c_feat > 0:
-            g_feats = torch.zeros((B, c_feat, N), dtype=torch.float32, device=dev)
+            # ordered: each scale WRITES its sum, so scales after the first go through a buffer and are added in scale order
+            g_feats = (torch.empty if ordered else torch.zeros)((B, c_feat, N), dtype=torch.float32, device=dev)
         grads, off = [], 0
         with torch.cuda.device(dev):
             for k, (s, idx, ns, d) in enumerate(zip(ctx.scales, idxs, ctx.nss, ctx.descs)):
@@ -208,11 +212,20 @@ class _SATrain(torch.autograd.Function):
                 z, stats, chosen = rest[:nl], rest[nl], rest[nl + 1]
                 rest = rest[nl + 2:]
                 bufs = _grad_buffers(params[k * 12:(k + 1) * 12], nl)
-                ws = torch.empty(L.prb_sa_train_workspace_bytes(B, npoint, ns, c_feat, ctypes.byref(d), 1), dtype=torch.uint8, device=dev)
-                C.check(L.prb_sa_train_backward(ctypes.byref(d), B, N, npoint, ns, c_feat, C.ptr(xyz), C.ptr(centres), C.ptr(feats_pm),
-                                                C.ptr(idx), _ptrs(z), C.ptr(stats), C.ptr(chosen), C.ptr(g_out), c_total, off,
-                                                *[_ptrs(b) for b in bufs], C.ptr(g_feats), C.ptr(ws), ws.numel(), C.stream()),
-                        "sa_train_backward")
+                if ordered:
+                    entry, name = L.prb_sa_train_backward_det, "sa_train_backward_det"
+                    wsb = L.prb_sa_train_det_workspace_bytes(B, N, npoint, ns, c_feat, ctypes.byref(d))
+                    g_k = g_feats if k == 0 or g_feats is None else torch.empty_like(g_feats)
+                else:
+                    entry, name = L.prb_sa_train_backward, "sa_train_backward"
+                    wsb = L.prb_sa_train_workspace_bytes(B, npoint, ns, c_feat, ctypes.byref(d), 1)
+                    g_k = g_feats
+                ws = torch.empty(wsb, dtype=torch.uint8, device=dev)
+                C.check(entry(ctypes.byref(d), B, N, npoint, ns, c_feat, C.ptr(xyz), C.ptr(centres), C.ptr(feats_pm), C.ptr(idx), _ptrs(z),
+                              C.ptr(stats), C.ptr(chosen), C.ptr(g_out), c_total, off, *[_ptrs(b) for b in bufs], C.ptr(g_k), C.ptr(ws),
+                              ws.numel(), C.stream()), name)
+                if g_k is not g_feats:
+                    g_feats.add_(g_k)
                 grads += _slot_grads(bufs, ctx.needs_input_grad[4 + k * 12:4 + (k + 1) * 12])
                 off += s.c_out[-1]
         return (None, None, None, g_feats) + tuple(grads)
