@@ -84,12 +84,26 @@ def grouping_ok(module, n_points):
     return True
 
 
+def tensor_stamp(tensors):
+    """[(tensor, version)] of the tensors a packed chain is built from, the tensors themselves held: a cache that compares
+    stamps with stamp_matches() sees a replaced tensor (a new nn.Parameter, load_state_dict(assign=True)) even when it
+    took the id() and the version of the one it replaced, and an in-place edit through its version counter.  Holding them
+    keeps a replaced parameter's storage alive until the cache's next call rebuilds the chain (or its module's _apply /
+    invalidate_fused drops it)."""
+    return [(t, None if t is None else t._version) for t in tensors]
+
+
+def stamp_matches(old, new):
+    return old is not None and len(old) == len(new) and all(a is b and va == vb for (a, va), (b, vb) in zip(old, new))
+
+
 class _FusedMLP:
     """The mlp_chain.Chain of one SharedMLP (folded BN, packed weights on the device), rebuilt whenever a parameter / buffer
-    version changes (optimizer step, load_state_dict, .to())."""
+    is replaced or its version changes (optimizer step, load_state_dict, in-place edits)."""
 
     def __init__(self):
         self.key = None
+        self.stamp = None
         self.chain = None
         self.proj = None
 
@@ -112,8 +126,9 @@ class _FusedMLP:
             if hasattr(layer, "bn"):
                 bn = layer.bn.bn
                 tensors += [bn.weight, bn.bias, bn.running_mean, bn.running_var]
-        key = (kind, split, str(device), _fold_scale(), project_known) + tuple((id(t), t._version) if t is not None else None for t in tensors)
-        if key == self.key:
+        key = (kind, split, str(device), _fold_scale(), project_known)
+        stamp = tensor_stamp(tensors)
+        if key == self.key and stamp_matches(self.stamp, stamp):
             return self.chain
         fold_scale = key[3]
         folded = [mlp_chain.fold(layer.conv, layer.bn.bn if hasattr(layer, "bn") else None, fold_scale) for layer in layers]
@@ -130,7 +145,7 @@ class _FusedMLP:
             ws[0] = torch.cat([torch.eye(c1), W0[:, c_known:]], dim=1)
             split = c1
         self.chain = mlp_chain.Chain(kind, split, ws, shifts, scales, device=device)
-        self.key = key
+        self.key, self.stamp = key, stamp
         return self.chain
 
 

@@ -23,10 +23,12 @@ def _layers(seq):
 
 
 class FusedRPNHeads:
-    """cache of the packed two-layer chain of (rpn_cls_layer, rpn_reg_layer); rebuilt when a parameter changes"""
+    """cache of the packed two-layer chain of (rpn_cls_layer, rpn_reg_layer); rebuilt when a parameter or buffer is
+    replaced or its version changes (pointnet2_modules.tensor_stamp)"""
 
     def __init__(self):
-        self.key = None
+        self.device = None
+        self.stamp = None
         self.chain = None
         self.n_cls = None
 
@@ -60,9 +62,10 @@ class FusedRPNHeads:
     def __call__(self, cls_seq, reg_seq, features):
         """features (B,C,N) -> rpn_cls (B,N,n_cls), rpn_reg (B,N,reg_channel), as lib/net/rpn.py:76-77"""
         tensors = [p for seq in (cls_seq, reg_seq) for p in list(seq.parameters()) + list(seq.buffers())]
-        key = (str(features.device),) + tuple((id(t), t._version) for t in tensors)
-        if key != self.key:
-            (self.chain, self.n_cls), self.key = self._build(cls_seq, reg_seq, features.device), key
+        stamp = pm.tensor_stamp(tensors)
+        if str(features.device) != self.device or not pm.stamp_matches(self.stamp, stamp):
+            self.chain, self.n_cls = self._build(cls_seq, reg_seq, features.device)
+            self.device, self.stamp = str(features.device), stamp
         B, Cc, N = features.shape
         rows = pm._point_major(features)            # (B,N,C): the twin written by the last FP launch, or one transpose
         out = self.chain.rows(rows.view(B * N, Cc)).view(B, N, -1)
@@ -71,7 +74,8 @@ class FusedRPNHeads:
 
 def rpn_heads(rpn_module, backbone_features):
     """eval-mode replacement of `rpn_cls_layer(f).transpose(1,2).contiguous()`, `rpn_reg_layer(f).transpose(...)`
-    for a reference lib.net.rpn.RPN instance (or anything with the same two attributes)"""
+    for a reference lib.net.rpn.RPN instance (or anything with the same two attributes).  The packed chain is cached on
+    `rpn_module`; invalidate_heads() drops it."""
     cache = rpn_module.__dict__.setdefault("_prb_heads", FusedRPNHeads())
     fused_ok = (not torch.is_grad_enabled()) and not rpn_module.training and pm._fused_enabled() and \
         FusedRPNHeads.supported(rpn_module.rpn_cls_layer, rpn_module.rpn_reg_layer)
@@ -79,3 +83,9 @@ def rpn_heads(rpn_module, backbone_features):
         return (rpn_module.rpn_cls_layer(backbone_features).transpose(1, 2).contiguous(),
                 rpn_module.rpn_reg_layer(backbone_features).transpose(1, 2).contiguous())
     return cache(rpn_module.rpn_cls_layer, rpn_module.rpn_reg_layer, backbone_features)
+
+
+def invalidate_heads(rpn_module):
+    """drop the packed heads chain rpn_heads() cached on `rpn_module`: after weights were edited through `.data`, which
+    bumps no version counter, and whenever the module's tensors are converted (RPNStage._apply)"""
+    rpn_module.__dict__.pop("_prb_heads", None)

@@ -14,7 +14,7 @@ import torch.nn as nn
 
 from ..backbone import Pointnet2MSG
 from ..pointnet2 import pytorch_utils as pt_utils
-from .heads import rpn_heads
+from .heads import invalidate_heads, rpn_heads
 from .proposal_layer import ProposalLayer
 
 # tools/cfgs/default.yaml:19
@@ -45,6 +45,17 @@ class RPNStage(nn.Module):
                                            pt_utils.Conv1d(128, reg_channel, activation=None))
         self.proposal_layer = ProposalLayer(mode=mode, cfg=cfg if cfg is not None else default_cfg())
         self.backbone_net.FP_modules[0].emit_point_major = True      # the fused heads read the point-major twin
+
+    def _apply(self, fn, *args, **kwargs):
+        invalidate_heads(self)         # see _PointnetSAModuleBase._apply; the backbone modules drop their own chains
+        return super()._apply(fn, *args, **kwargs)
+
+    def invalidate_fused(self):
+        """call after editing weights through `.data` (EMA, weight averaging): drops every packed chain of the stage"""
+        invalidate_heads(self)
+        for m in self.backbone_net.modules():
+            if hasattr(m, "invalidate_fused"):
+                m.invalidate_fused()
 
     def forward(self, pts_input, with_features=False):
         """pts_input (B,N,3+C) -> (rois (B,M,7), roi_scores_raw (B,M)) [+ rpn_cls, rpn_reg, backbone_xyz, backbone_features]"""
