@@ -14,10 +14,12 @@ import contextlib
 
 import numpy as np
 import torch
+from torch import nn
 
 from .. import config
 from ..parallel_utils import GradBucketReducer
 from ..rpn.stage import CLS_MEAN_SIZE, RPNStage
+from . import recipe
 from .losses import rcnn_loss, rpn_loss
 
 
@@ -33,20 +35,86 @@ def _sa_switch(sa_train, fp_train=None):
     return config.override(**kw) if kw else contextlib.nullcontext()
 
 
-class RPNTrainer:
+def _schedule(optimizer, total_steps, lr):
+    """the per-iteration schedule of a trainer's `optimizer` switch (None for "adam", whose schedule is per epoch); raises
+    ValueError for an unknown name or "adam_onecycle" without total_steps"""
+    if optimizer not in recipe.OPTIMIZERS:
+        raise ValueError("optimizer must be one of %s, not %r" % (", ".join(map(repr, recipe.OPTIMIZERS)), optimizer))
+    if optimizer == "adam":
+        return None
+    if total_steps is None:
+        raise ValueError("optimizer='adam_onecycle' needs total_steps (iterations per epoch * epochs)")
+    return recipe.OneCycle(total_steps, lr_max=lr)
+
+
+class _PointRCNNLayout(nn.Module):
+    """the reference's PointRCNN module tree over a trainer's stages: state-dict keys rpn.* (and rcnn_net.*), leaf modules in
+    the order the reference's parameter groups take them"""
+
+    def __init__(self, rpn, rcnn_net=None):
+        super().__init__()
+        self.rpn = rpn
+        if rcnn_net is not None:
+            self.rcnn_net = rcnn_net
+
+
+class _Recipe:
+    """the optimizer switch and the schedule hooks of both trainers (see train.recipe).  optimizer="adam": torch Adam with
+    L2 weight decay over the trainable parameters (cfgs OPTIMIZER: adam); its warm-up and step decay apply only through
+    the hooks.  "adam_onecycle": recipe.TrueWDAdam over the PointRCNN-layout groups with the OneCycle schedule of
+    total_steps iterations (the reference's default recipe)"""
+
+    def _build_optimizer(self, schedule, lr, weight_decay):
+        self.schedule, self.lr = schedule, lr
+        fused = self.device.type == "cuda"
+        if schedule is None:
+            self.opt = torch.optim.Adam(self.params, lr=lr, weight_decay=weight_decay, **({"fused": True} if fused else {}))
+        else:
+            self.opt = recipe.TrueWDAdam(recipe.param_groups(self.net), *schedule.initial, wd=weight_decay, fused=fused)
+
+    def _set_lr(self, lr):
+        for group in self.opt.param_groups:
+            group["lr"] = lr
+
+    def schedule_epoch(self, epoch, it):
+        """the start of `epoch`, `it` iterations into the run (Trainer.train): the BN momentum of `it` (the reference passes
+        the iteration count, not the epoch) and, for "adam" once the warm-up is over, the step decay of `epoch`"""
+        recipe.set_bn_momentum(self.net, recipe.bn_momentum(it))
+        if self.schedule is None and epoch >= recipe.WARMUP_EPOCH:
+            self._set_lr(self.lr * recipe.step_decay(epoch))
+
+    def schedule_iteration(self, it, epoch, iters_per_epoch):
+        """before the step of iteration `it`: OneCycle's lr and beta1, or for "adam" in the first WARMUP_EPOCH epochs the
+        cosine warm-up over WARMUP_EPOCH * iters_per_epoch iterations"""
+        if self.schedule is not None:
+            self.opt.set(*self.schedule(it))
+        elif epoch < recipe.WARMUP_EPOCH:
+            self._set_lr(recipe.warmup_lr(it, recipe.WARMUP_EPOCH * iters_per_epoch, self.lr))
+
+    def resume_schedule(self, it, epoch):
+        """after loading a checkpoint of iteration `it`, epoch `epoch`: the BN momentum the reference's resumed scheduler
+        constructor sets (last_epoch = epoch + 1, applied as epoch + 2) and OneCycle's values at `it`"""
+        recipe.set_bn_momentum(self.net, recipe.bn_momentum(epoch + 2))
+        if self.schedule is not None:
+            self.opt.set(*self.schedule(it))
+
+
+class RPNTrainer(_Recipe):
     """loss_impl: which stage-loss path forward_loss takes ("torch" / "device", see train.losses; None: the config switch).
     sa_train: which path the SA modules take in training ("torch" / "device", see pointnet2/sa_train.py; None: the config
-    switch).  fp_train: the same for the FP modules (see pointnet2/fp_train.py)"""
+    switch).  fp_train: the same for the FP modules (see pointnet2/fp_train.py).  optimizer / total_steps: see _Recipe;
+    self.net is the model in the PointRCNN layout (rpn.*) that checkpoints hold"""
 
     def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, loss_impl=None,
-                 sa_train=None, fp_train=None):
+                 sa_train=None, fp_train=None, optimizer="adam", total_steps=None):
+        schedule = _schedule(optimizer, total_steps, lr)
         torch.manual_seed(seed)                       # identical initial weights on every rank
         self.device = torch.device(device)
         self.model = RPNStage(input_channels=input_channels, mode="TRAIN").to(self.device).train()
+        self.net = _PointRCNNLayout(self.model)
         self.params = [p for p in self.model.parameters() if p.requires_grad]
         self.reducer = GradBucketReducer(self.params, world=world, bucket_mb=bucket_mb)
-        fused = self.device.type == "cuda"
-        self.opt = torch.optim.Adam(self.params, lr=lr, weight_decay=weight_decay, **({"fused": True} if fused else {}))
+        self._build_optimizer(schedule, lr, weight_decay)
         self.mean_size = torch.from_numpy(CLS_MEAN_SIZE[0]).to(self.device)
         self.loss_impl = loss_impl
         self.sa_train = sa_train
@@ -86,7 +154,7 @@ def synthetic_labels(pts_input, seed=0):
     return cls.to(pts_input.device), reg.to(pts_input.device)
 
 
-class RCNNTrainer:
+class RCNNTrainer(_Recipe):
     """One RCNN training step with the RPN fixed (the reference's second training phase: tools/train_rcnn.py --train_mode rcnn,
     cfg.RPN.FIXED): the RPN stage runs in eval mode without grad on the fused path and hands (rois, point features, mask,
     depth) to the RCNN stage, whose target layer samples 64 RoIs per scene; forward / backward of the RCNN network on the
@@ -94,20 +162,23 @@ class RCNNTrainer:
     ("torch": the reference's random calls, "device": one device pass without host reads; None: the config switch).  loss_impl:
     which stage-loss path every forward_loss* method takes ("torch" / "device", see train.losses; None: the config switch).
     sa_train: which path the RCNN network's SA modules take ("torch" / "device", see pointnet2/sa_train.py; None: the config
-    switch)."""
+    switch).  optimizer / total_steps: see _Recipe; self.net is the PointRCNN layout (rpn.*, rcnn_net.*) that checkpoints
+    hold, and recipe.load_part(self.net, path) loads a phase-1 checkpoint's RPN (--rpn_ckpt)."""
 
     def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, rpn_score_thresh=0.3,
-                 target_draw=None, loss_impl=None, sa_train=None):
+                 target_draw=None, loss_impl=None, sa_train=None, optimizer="adam", total_steps=None):
         from ..rcnn.stage import RCNNStage
+        schedule = _schedule(optimizer, total_steps, lr)
         torch.manual_seed(seed)
         self.device = torch.device(device)
         self.rpn = RPNStage(input_channels=input_channels, mode="TRAIN").to(self.device).eval()     # TRAIN quotas: 512 RoIs per scene
         for p in self.rpn.parameters():
             p.requires_grad_(False)
         self.model = RCNNStage(num_classes=2, input_channels=128).to(self.device).train()
+        self.net = _PointRCNNLayout(self.rpn, self.model)
         self.params = [p for p in self.model.parameters() if p.requires_grad]
         self.reducer = GradBucketReducer(self.params, world=world, bucket_mb=bucket_mb)
-        self.opt = torch.optim.Adam(self.params, lr=lr, weight_decay=weight_decay, **({"fused": True} if self.device.type == "cuda" else {}))
+        self._build_optimizer(schedule, lr, weight_decay)
         self.mean_size = torch.from_numpy(CLS_MEAN_SIZE[0]).to(self.device)
         self.rpn_score_thresh = rpn_score_thresh
         self.target_draw = target_draw
