@@ -66,6 +66,16 @@ def opt_n_threads(n):
 
 
 # ------------------------------------------------------------------ pointnet2 ops
+def dist2(a, b):
+    """fp32 squared distance of aligned point pairs (..., 3) in the reference kernels' FMA order"""
+    a, b = np.broadcast_arrays(_f32(a), _f32(b))
+    shape = a.shape[:-1]
+    a, b = _f32(a.reshape(-1, 3)), _f32(b.reshape(-1, 3))
+    out = np.empty(a.shape[0], dtype=np.float32)
+    lib().orc_dist2(a.shape[0], _p(a), _p(b), _p(out))
+    return out.reshape(shape)
+
+
 def fps(xyz, npoint, return_temp=False, temp0=None):
     """temp0: caller-initialised running minima (the reference's temp tensor is in/out); default 1e10 everywhere"""
     xyz = _f32(xyz)

@@ -52,6 +52,11 @@ static inline float dist2_ref(float ax, float ay, float az, float bx, float by, 
     return fmaf(dz, dz, t);
 }
 
+/* the squared distance above for n aligned pairs, so tests can certify fp32 boundary placements */
+ORC_API void orc_dist2(int n, const float *a, const float *b, float *out) {
+    for (int i = 0; i < n; ++i) out[i] = dist2_ref(a[i * 3], a[i * 3 + 1], a[i * 3 + 2], b[i * 3], b[i * 3 + 1], b[i * 3 + 2]);
+}
+
 /* cuda_utils.h:10-14 : largest power of two <= min(n, 1024), at least 1 */
 ORC_API int orc_opt_n_threads(int work_size) {
     int pow_2 = (int)(log((double)work_size) / log(2.0));

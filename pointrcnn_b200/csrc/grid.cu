@@ -648,7 +648,11 @@ __global__ void __launch_bounds__(GR_THREADS) three_nn_csr_kernel(const GridNnPa
     nn_store(p, ((size_t)scene * p.n + u) * 3, b1, b2, b3, i1, i2, i3);
 }
 
+// The reference starts its cascade at 1e40 (double), so only a finite distance ever enters: an inf (or NaN) distance
+// must not take an empty slot through the index tie-break, or a query at infinity would list points 0, 1, 2 instead of
+// the reference's 0, 0, 0.
 __device__ __forceinline__ void nn_insert_lex(float d, int k, float &b1, float &b2, float &b3, int &i1, int &i2, int &i3) {
+    if (!(d < CUDART_INF_F)) return;
     if (d < b1 || (d == b1 && k < i1)) {
         b3 = b2; i3 = i2; b2 = b1; i2 = i1; b1 = d; i1 = k;
     } else if (d < b2 || (d == b2 && k < i2)) {
