@@ -29,11 +29,12 @@
 extern "C" {
 #endif
 
-#define PRB_ABI_VERSION 7   /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
+#define PRB_ABI_VERSION 8   /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
                              * 5: ordered FPS, input pipeline / KITTI output group, prb_options.roipool_fused;
                              * 6: prb_rcnn_sample_rois / prb_rcnn_roi_targets take the recipe as values (the signatures of
                              *    the former _ex entries, which are gone);
-                             * 7: prb_fp_train_forward loses its `project` argument (layer 0 always runs projected) */
+                             * 7: prb_fp_train_forward loses its `project` argument (layer 0 always runs projected);
+                             * 8: the unread mlp_* fields are gone */
 #if defined(__GNUC__)
 #define PRB_API __attribute__((visibility("default")))
 #else
@@ -54,24 +55,9 @@ typedef struct prb_options {
     int fps_prune;     /* 0: never use the pruned single-CTA kernel; 1: for 4097..16384 points; 2: also 2049..4096 */
     int fps_threads;   /* threads per CTA of the rank kernel; 0 = heuristic */
     int fps_generic;   /* 1: force the generic (reference-shaped) kernel */
-    /* the chain kernels read only mlp_occ, mlp_sms and mlp_resident; the other mlp_* fields have no effect and keep the
-     * block's layout */
-    int mlp_gather;
-    int mlp_ng;
     int mlp_occ;       /* >= 1: at most this many chain-kernel CTAs per SM; 0 = as many as registers and shared memory allow */
     int mlp_sms;       /* size the persistent grid for this many SMs; 0 = all */
-    int mlp_atmem;
-    int mlp_sleepy;
-    int mlp_trace;
-    int mlp_pipeline;
-    int mlp_ne, mlp_ngw;
-    int mlp_zs, mlp_nbuf;
-    int mlp_brows;
-    int mlp_pool;
     int mlp_resident;  /* 1 (default): chain launches whose weights fit run on the resident-weight kernel; 0: always stream */
-    int mlp_lazy_ns;
-    int mlp_fill;
-    int mlp_tune;
     int roipool_exhaustive;  /* 1: roipool3d pass A tests every point against every box (no x-z binning) */
     int roipool_parts;     /* roipool3d pass B: CTAs per box (1..8); 0 = 1 */
     int roipool_stage_kb;  /* roipool3d pass B: shared staging area per CTA in KB (8..160); 0 = 48 */

@@ -38,14 +38,14 @@ class SATrainDesc(ctypes.Structure):
 
 class Options(ctypes.Structure):
     """struct prb_options (per-thread tuning block)"""
-    _fields_ = [(k, c_int) for k in ("fps_cluster", "fps_prune", "fps_threads", "fps_generic", "mlp_gather", "mlp_ng", "mlp_occ",
-                                     "mlp_sms", "mlp_atmem", "mlp_sleepy", "mlp_trace", "mlp_pipeline", "mlp_ne", "mlp_ngw", "mlp_zs",
-                                     "mlp_nbuf", "mlp_brows", "mlp_pool", "mlp_resident", "mlp_lazy_ns", "mlp_fill", "mlp_tune", "roipool_exhaustive", "roipool_parts", "roipool_stage_kb", "roipool_direct", "nn_walk", "nn_sort_queries", "grid_csr", "grid_debug")] + [("nn_cell", c_float), ("roipool_fused", c_int)]
+    _fields_ = [(k, c_int) for k in ("fps_cluster", "fps_prune", "fps_threads", "fps_generic", "mlp_occ", "mlp_sms", "mlp_resident",
+                                     "roipool_exhaustive", "roipool_parts", "roipool_stage_kb", "roipool_direct", "nn_walk",
+                                     "nn_sort_queries", "grid_csr", "grid_debug")] + [("nn_cell", c_float), ("roipool_fused", c_int)]
 
 
 @contextlib.contextmanager
 def options(**kw):
-    """with options(fps_cluster=2, mlp_gather=1): ...  -- overrides fields of THIS thread's prb_options for the block.
+    """with options(fps_prune=0, mlp_resident=0): ...  -- overrides fields of THIS thread's prb_options for the block.
     Thread-local inside the library (prb_set_thread_options): safe under nn.DataParallel worker threads."""
     L = lib()
     old, new = Options(), Options()
@@ -98,7 +98,7 @@ def lib():
         L.prb_fp_train_backward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P, P, c_size_t, P]
         L.prb_options_init.restype = None
         L.prb_get_thread_options.restype = None
-        if L.prb_abi_version() != 7:
+        if L.prb_abi_version() != 8:
             raise RuntimeError("pointrcnn_b200: ABI version mismatch")
         _lib = L
     return _lib

@@ -41,24 +41,9 @@ static prb_options make_defaults() {
     o.fps_prune = env_int("PRB_FPS_PRUNE", 1);
     o.fps_threads = env_int("PRB_FPS_THREADS", 0);
     o.fps_generic = env_int("PRB_FPS_GENERIC", 0);
-    o.mlp_gather = env_int("PRB_MLP_GATHER", 0);
-    o.mlp_ng = env_int("PRB_MLP_NG", 0);
     o.mlp_occ = env_int("PRB_MLP_OCC", 0);
     o.mlp_sms = env_int("PRB_MLP_SMS", 0);
-    o.mlp_atmem = env_int("PRB_MLP_ATMEM", 1);
-    o.mlp_sleepy = env_int("PRB_MLP_SLEEPY", 3);
-    o.mlp_trace = env_int("PRB_MLP_TRACE", 0);
-    o.mlp_pipeline = env_int("PRB_MLP_PIPELINE", 1);
-    o.mlp_ne = env_int("PRB_MLP_NE", 0);
-    o.mlp_ngw = env_int("PRB_MLP_NGW", 0);
-    o.mlp_zs = env_int("PRB_MLP_ZS", 0);
-    o.mlp_nbuf = env_int("PRB_MLP_NBUF", 0);
-    o.mlp_brows = env_int("PRB_MLP_BROWS", 0);
-    o.mlp_pool = env_int("PRB_MLP_POOL", 0);
     o.mlp_resident = env_int("PRB_MLP_RESIDENT", 1);
-    o.mlp_lazy_ns = env_int("PRB_MLP_LAZY_NS", 0);
-    o.mlp_fill = env_int("PRB_MLP_FILL", 1);
-    o.mlp_tune = env_int("PRB_MLP_TUNE", 1);
     o.roipool_exhaustive = env_int("PRB_ROIPOOL_EXHAUSTIVE", 0);
     o.roipool_parts = env_int("PRB_ROIPOOL_PARTS", 0);
     o.roipool_stage_kb = env_int("PRB_ROIPOOL_STAGE_KB", 0);

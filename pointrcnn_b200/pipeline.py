@@ -27,11 +27,9 @@ class _Slot:
 
 
 class BatchPipeline:
-    def __init__(self, fn, inflight=6, device=None, graphs=False, fps_cluster=None):
+    def __init__(self, fn, inflight=6, device=None, graphs=False):
         """fn: callable(batch_on_device) -> tensor or tuple of tensors; inflight: batches in flight (one stream and one
-        set of result buffers per slot); graphs: replay fn as a CUDA graph per slot.
-        (`fps_cluster` is accepted for compatibility and ignored: the pruned single-CTA sampling kernel takes every
-        scene of <= 16384 points; use `_cabi.options(fps_cluster=...)` around run() for larger scenes.)"""
+        set of result buffers per slot); graphs: replay fn as a CUDA graph per slot."""
         self.fn = fn
         self.device = torch.device(device if device is not None else "cuda", torch.cuda.current_device()) \
             if not isinstance(device, torch.device) else device
@@ -44,17 +42,7 @@ class BatchPipeline:
 
     # ------------------------------------------------------------------ one batch on one slot
     def _forward(self, slot, x):
-        """run fn on x (already on the slot's stream); returns the output tuple.
-        With several batches in flight the library runs in THROUGHPUT mode (`prb_options.mlp_fill = 0`): small single-layer
-        chain launches are not dealt to extra column groups just to fill idle SMs -- those SMs belong to the other batches
-        (baked into the graph at capture)."""
-        from . import _cabi
-        if len(self.slots) > 1 and _cabi.lib() is not None:
-            with _cabi.options(mlp_fill=0):
-                return self._forward_impl(slot, x)
-        return self._forward_impl(slot, x)
-
-    def _forward_impl(self, slot, x):
+        """run fn on x (already on the slot's stream); returns the output tuple."""
         if not self.graphs:
             out = self.fn(x)
             return out if isinstance(out, (tuple, list)) else (out,)

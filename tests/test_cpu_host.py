@@ -102,7 +102,7 @@ def test_cabi_library_exports_every_declared_symbol():
     assert len(names) >= 25
     for n in names:
         assert hasattr(lib, n), "libpointrcnn_b200.so does not export %s" % n
-    assert lib.prb_abi_version() == 7
+    assert lib.prb_abi_version() == 8
     assert lib.prb_launch_count() == 0
     # and the other way round: nothing is exported that the header does not declare
     import subprocess
@@ -255,4 +255,4 @@ def test_options_struct_matches_the_header():
     assert names == [f[0] for f in _cabi.Options._fields_]
     o = _cabi.Options()
     _cabi.lib().prb_options_init(ctypes.byref(o))
-    assert o.fps_prune == 1 and o.mlp_pipeline == 1 and abs(o.nn_cell - 1.6) < 1e-6
+    assert o.fps_prune == 1 and o.mlp_resident == 1 and abs(o.nn_cell - 1.6) < 1e-6

@@ -15,7 +15,7 @@ def test_stage_loss_symbols_resolve():
     for name in ("prb_stage_loss_workspace_bytes", "prb_stage_loss_forward", "prb_stage_loss_backward"):
         assert getattr(lib, name) is not None
     assert lib.prb_stage_loss_workspace_bytes(16 * 16384) > 0
-    assert lib.prb_abi_version() == 7
+    assert lib.prb_abi_version() == 8
 
 
 def test_descriptor_layout_matches_the_header():
