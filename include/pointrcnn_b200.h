@@ -29,12 +29,13 @@
 extern "C" {
 #endif
 
-#define PRB_ABI_VERSION 8   /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
-                             * 5: ordered FPS, input pipeline / KITTI output group, prb_options.roipool_fused;
+#define PRB_ABI_VERSION 9   /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
+                             * 5: ordered FPS, input pipeline / KITTI output group, a fused RoI-pooling switch in prb_options;
                              * 6: prb_rcnn_sample_rois / prb_rcnn_roi_targets take the recipe as values (the signatures of
                              *    the former _ex entries, which are gone);
                              * 7: prb_fp_train_forward loses its `project` argument (layer 0 always runs projected);
-                             * 8: the unread mlp_* fields are gone */
+                             * 8: the unread mlp_* fields are gone;
+                             * 9: the five RoI-pooling fields are gone */
 #if defined(__GNUC__)
 #define PRB_API __attribute__((visibility("default")))
 #else
@@ -58,17 +59,11 @@ typedef struct prb_options {
     int mlp_occ;       /* >= 1: at most this many chain-kernel CTAs per SM; 0 = as many as registers and shared memory allow */
     int mlp_sms;       /* size the persistent grid for this many SMs; 0 = all */
     int mlp_resident;  /* 1 (default): chain launches whose weights fit run on the resident-weight kernel; 0: always stream */
-    int roipool_exhaustive;  /* 1: roipool3d pass A tests every point against every box (no x-z binning) */
-    int roipool_parts;     /* roipool3d pass B: CTAs per box (1..8); 0 = 1 */
-    int roipool_stage_kb;  /* roipool3d pass B: shared staging area per CTA in KB (8..160); 0 = 48 */
-    int roipool_direct;    /* 1: roipool3d pass B takes boxes with many rows through scalar L1 gathers (first version) instead of chunked staging */
     int nn_walk;           /* three_nn on the grid: 0 = 27 unrolled cell walks (default), 1 = one convergent cursor loop per lane (slower) */
     int nn_sort_queries;   /* 1: three_nn groups the queries by grid cell before the search; measured: the sort costs what the locality saves */
     int grid_csr;      /* 1: hash grid as CSR runs (counting sort per scene) instead of linked lists; slower at the RPN shapes */
     int grid_debug;    /* 1: print (and synchronise for) the 3-NN grid's fallback counts */
     float nn_cell;     /* 3-NN grid cell edge in units of the mean point spacing (default 1.6) */
-    int roipool_fused;     /* 1: the binned assign pass of a box runs inside the copy kernel's CTA (no index list in HBM); 0 (default): two kernels --
-                            * measured: fused 0.167 ms, two kernels 0.156 ms at the configs[3] shape */
 } prb_options;
 PRB_API void prb_options_init(prb_options *o);                 /* library defaults */
 PRB_API int prb_set_thread_options(const prb_options *o);      /* NULL: back to the defaults */
@@ -277,10 +272,12 @@ PRB_API int prb_three_nn_grid(int b, int n, int m, const float *unknown, const f
 PRB_API int prb_roipool3d(int B, int N, int M, int C, int S, const float *xyz, const float *boxes3d,
                   const float *pts_feature, float *pooled, int *empty_flag,
                   const float *rois_canonical, void *stream);
-/* two-pass form (what the Python mirror calls): pass A reads a scene's points once per tile of boxes and writes the
- * per-box index lists into caller scratch (prb_roipool3d_workspace_bytes), pass B streams the pooled rows with
- * 128-bit stores.  zero_fill_empty != 0: the kernel zeroes the rows of empty boxes itself, so `pooled` may be
- * uninitialised (saves the caller's 558 MB memset at C4); 0: untouched, as the reference leaves them. */
+/* two-pass form (what the Python mirror calls): pass A writes the per-box index lists into caller scratch
+ * (prb_roipool3d_workspace_bytes), pass B streams the pooled rows with 128-bit stores.  For scenes of at most 262144
+ * points pass A bins the points into an x-z grid first and tests each box against the cells its footprint covers
+ * (three kernels in all); larger scenes test every point against every box (two kernels).  S is at most 3200, or 1600
+ * for scenes of more than 65536 points.  zero_fill_empty != 0: the kernel zeroes the rows of empty boxes itself, so
+ * `pooled` may be uninitialised (saves the caller's 558 MB memset at C4); 0: untouched, as the reference leaves them. */
 PRB_API size_t prb_roipool3d_workspace_bytes(int B, int N, int M, int S);
 PRB_API int prb_roipool3d_ws(int B, int N, int M, int C, int S, const float *xyz, const float *boxes3d,
                      const float *pts_feature, float *pooled, int *empty_flag, const float *rois_canonical,

@@ -131,26 +131,24 @@ __global__ void __launch_bounds__(RP_THREADS) roipool3d_kernel(int N, int M, int
 
 
 // ------------------------------------------------------------------------------------------------ two-pass form
-// Pass A (assign): one CTA per (scene, tile of RA_BOXES boxes).  The scene's points are read ONCE per tile (the
-// reference and the one-pass kernel above re-read all N points for every box: 2048 x 196 KB at C4).  Warp w owns the
-// contiguous point range [w*N/8, (w+1)*N/8): it appends the hits of every box to its own ordered list in shared memory
-// (ballot + popc prefix, no CTA barrier inside the scan); the lists are then concatenated in warp order, which IS
-// point-index order, and cut at S -> idx (B,M,S) int32 + cnt (B,M) in caller scratch.
+// Pass A (assign) writes each box's first S inside points in index order -> idx (B,M,S) int32 + cnt (B,M) in caller
+// scratch: binned (below) for scenes of at most RG_MAX_POINTS points, exhaustive for larger ones.
 // Pass B (copy): one CTA per box streams the S x (3+C) output as ONE flat array with 128-bit stores (rows are
-// 532 bytes at C4, so row-aligned stores are 4 bytes per lane); sources are read through L1 (a box holds a few dozen
-// distinct rows that are repeated cyclically).  Empty boxes set the flag and, when asked, zero their rows, so the caller
-// need not pre-zero the 558 MB output.
+// 532 bytes at C4, so row-aligned stores are 4 bytes per lane).  Empty boxes set the flag and, when asked, zero their
+// rows, so the caller need not pre-zero the 558 MB output.
+//
+// Pass A, exhaustive: one CTA per (scene, tile of RA_BOXES boxes).  The scene's points are read ONCE per tile (the
+// reference and the one-pass kernel above re-read all N points for every box).  Warp w owns the contiguous point range
+// [w*N/8, (w+1)*N/8): it appends the hits of every box to its own ordered list in shared memory (ballot + popc prefix, no
+// CTA barrier inside the scan); the lists are then concatenated in warp order, which IS point-index order, and cut at S.
 constexpr int RA_BOXES = 4;
 constexpr int RA_WARPS = 8;
 constexpr int RA_UNROLL = 4;     // points per lane per step: 12 coordinate loads in flight per lane
 
-// IdxT: unsigned short when the scene has <= 65536 points (half the shared memory -> twice the resident CTAs), else int
-template <typename IdxT>
 __global__ void __launch_bounds__(32 * RA_WARPS) roipool3d_assign_kernel(int N, int M, int S, const float *__restrict__ xyz,
                                                                         const float *__restrict__ boxes3d,
                                                                         int *__restrict__ idx_out, int *__restrict__ cnt_out) {
-    extern __shared__ unsigned char s_raw[];
-    IdxT *s_list = reinterpret_cast<IdxT *>(s_raw);      // [RA_BOXES][RA_WARPS][S]
+    extern __shared__ int s_list[];      // [RA_BOXES][RA_WARPS][S]
     __shared__ int s_cnt[RA_BOXES][RA_WARPS];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int box0 = blockIdx.x * RA_BOXES, scene = blockIdx.y;
@@ -182,7 +180,7 @@ __global__ void __launch_bounds__(32 * RA_WARPS) roipool3d_assign_kernel(int N, 
                 const unsigned hits = __ballot_sync(0xffffffffu, in);
                 if (hits) {
                     const int pos = cnt[b] + __popc(hits & ((1u << lane) - 1));
-                    if (in && pos < S) s_list[((size_t)b * RA_WARPS + warp) * S + pos] = (IdxT)k;
+                    if (in && pos < S) s_list[((size_t)b * RA_WARPS + warp) * S + pos] = k;
                     cnt[b] = min(S, cnt[b] + __popc(hits));
                 }
             }
@@ -200,7 +198,7 @@ __global__ void __launch_bounds__(32 * RA_WARPS) roipool3d_assign_kernel(int N, 
             const int c = s_cnt[b][w];
             const int take = min(c, S - off);
             int *dst = idx_out + ((size_t)scene * M + box0 + b) * S + off;
-            for (int j = tid; j < take; j += 32 * RA_WARPS) dst[j] = (int)s_list[((size_t)b * RA_WARPS + w) * S + j];
+            for (int j = tid; j < take; j += 32 * RA_WARPS) dst[j] = s_list[((size_t)b * RA_WARPS + w) * S + j];
             off += take;
             if (off >= S) break;
         }
@@ -208,7 +206,7 @@ __global__ void __launch_bounds__(32 * RA_WARPS) roipool3d_assign_kernel(int N, 
     }
 }
 
-// Pass A, binned (default for N <= RG_MAX_POINTS): the exhaustive pass above tests every point against every box
+// Pass A, binned (scenes of at most RG_MAX_POINTS points): the exhaustive pass above tests every point against every box
 // (B*N*M = 33.5 M predicates at C4, ~100 us).  Here the scene's points are first bucketed into an RG x RG grid over their
 // x-z bounding box (one CTA per scene: bounds, histogram, scan, scatter -> a point permutation grouped by cell, cells
 // row-major in z), and a box only tests the points of the cells its footprint touches.  Index ORDER is restored by a
@@ -303,16 +301,26 @@ __global__ void __launch_bounds__(RG_THREADS) roipool3d_bin_kernel(int N, const 
     }
 }
 
-// The binned assign pass of one box, by all threads of the CTA: set the bit of every inside point in s_bits (N bits, shared),
-// then warp 0 walks the bitmap and writes the first S set bits -- "the first S inside points in point-index order" -- to
-// list[] (global or shared).  Returns min(count, S) to every thread of warp 0 (other warps: undefined).  Ends with no barrier.
-__device__ __forceinline__ int assign_grid_box(int N, int S, const float *__restrict__ pts, const float *__restrict__ bx,
-                                               const int *__restrict__ sorted, const int *__restrict__ cstart, const SceneGrid g,
-                                               unsigned int *s_bits, int *list) {
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nthreads = blockDim.x;
+// One CTA per (scene, box): set the bit of every inside point in s_bits (N bits), then warp 0 walks the bitmap and writes
+// the first S set bits -- "the first S inside points in point-index order" -- and their count.
+constexpr int RGA_THREADS = 128;
+__global__ void __launch_bounds__(RGA_THREADS) roipool3d_assign_grid_kernel(int N, int M, int S, const float *__restrict__ xyz,
+                                                                           const float *__restrict__ boxes3d,
+                                                                           const int *__restrict__ sorted_idx,
+                                                                           const int *__restrict__ cell_start,
+                                                                           const SceneGrid *__restrict__ grids,
+                                                                           int *__restrict__ idx_out, int *__restrict__ cnt_out) {
+    extern __shared__ unsigned int s_bits[];          // ceil(N / 32) words
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const int box = blockIdx.x, scene = blockIdx.y;
+    const size_t bi = (size_t)scene * M + box;
+    const float *pts = xyz + (size_t)scene * N * 3;
+    const int *sorted = sorted_idx + (size_t)scene * N;
+    const int *cstart = cell_start + (size_t)scene * (RG_CELLS + 1);
+    const SceneGrid g = grids[scene];
     const int nwords = (N + 31) >> 5;
-    for (int i = tid; i < nwords; i += nthreads) s_bits[i] = 0u;
-    const BoxConst bc = make_box(bx);
+    for (int i = tid; i < nwords; i += RGA_THREADS) s_bits[i] = 0u;
+    const BoxConst bc = make_box(boxes3d + bi * 7);
     // conservative x-z footprint of the predicate (see above); NaN / Inf boxes degrade to "every cell" or "cell 0", both safe
     const float hl = (float)bc.half_l, hw = (float)bc.half_w, ac = fabsf(bc.cosa), as = fabsf(bc.sina);
     float ex = fminf(__fmaf_rn(ac, hl, as * hw), 10.f), ez = fminf(__fmaf_rn(as, hl, ac * hw), 10.f);
@@ -325,7 +333,7 @@ __device__ __forceinline__ int assign_grid_box(int N, int S, const float *__rest
     if (zc0 > zc1) { const int t = zc0; zc0 = zc1; zc1 = t; }
     __syncthreads();
     // a z-row of the footprint is one contiguous span of the permutation
-    for (int zc = zc0 + warp; zc <= zc1; zc += nthreads / 32) {
+    for (int zc = zc0 + warp; zc <= zc1; zc += RGA_THREADS / 32) {
         const int lo = cstart[zc * RG + xc0], hi = cstart[zc * RG + xc1 + 1];
         for (int e = lo + lane; e < hi; e += 32) {
             const int k = sorted[e];
@@ -334,7 +342,8 @@ __device__ __forceinline__ int assign_grid_box(int N, int S, const float *__rest
         }
     }
     __syncthreads();
-    if (warp != 0) return 0;
+    if (warp != 0) return;
+    int *list = idx_out + bi * S;
     int run = 0;
     for (int w0 = 0; w0 < nwords && run < S; w0 += 32) {
         unsigned word = w0 + lane < nwords ? s_bits[w0 + lane] : 0u;
@@ -351,30 +360,13 @@ __device__ __forceinline__ int assign_grid_box(int N, int S, const float *__rest
         }
         run += __shfl_sync(0xffffffffu, incl, 31);
     }
-    return min(run, S);
+    if (lane == 0) cnt_out[bi] = min(run, S);
 }
-
-constexpr int RGA_THREADS = 128;
-__global__ void __launch_bounds__(RGA_THREADS) roipool3d_assign_grid_kernel(int N, int M, int S, const float *__restrict__ xyz,
-                                                                           const float *__restrict__ boxes3d,
-                                                                           const int *__restrict__ sorted_idx,
-                                                                           const int *__restrict__ cell_start,
-                                                                           const SceneGrid *__restrict__ grids,
-                                                                           int *__restrict__ idx_out, int *__restrict__ cnt_out) {
-    extern __shared__ unsigned int s_bits[];          // ceil(N / 32) words
-    const int box = blockIdx.x, scene = blockIdx.y;
-    const int n = assign_grid_box(N, S, xyz + (size_t)scene * N * 3, boxes3d + ((size_t)scene * M + box) * 7,
-                                  sorted_idx + (size_t)scene * N, cell_start + (size_t)scene * (RG_CELLS + 1), grids[scene], s_bits,
-                                  idx_out + ((size_t)scene * M + box) * S);
-    if (threadIdx.x == 0) cnt_out[(size_t)scene * M + box] = n;
-}
-
-struct FusedAssign { const int *sorted_idx, *cell_start; const SceneGrid *grids; const float *boxes3d; };   // sorted_idx == nullptr: two-kernel form
 
 // Pass B.  A box usually holds far fewer than S points, so its S output rows are `cnt` distinct rows repeated cyclically:
 // flat, the output IS the cnt x (3+C) source block repeated -- out[e] = block[e mod (cnt*(3+C))].  The block is staged in
 // shared memory once (coalesced row reads, canonical transform applied there) and streamed out with 128-bit stores;
-// boxes with more points than the staging area holds take the direct path (sources through L1).
+// boxes with more points than the staging area holds take the direct paths below.
 constexpr int RB_STAGE_FLOATS = 12 * 1024;   // 48 KB: 92 rows of 133 floats.  Data dependent: a smaller area suits boxes that
                                              // hold a few points, 48 KB the ~60 points per enlarged RoI of the RCNN stage
 
@@ -382,34 +374,17 @@ __global__ void __launch_bounds__(RP_THREADS) roipool3d_copy_kernel(int N, int M
                                                                     const float *__restrict__ pts_feature,
                                                                     const int *__restrict__ idx_in, const int *__restrict__ cnt_in,
                                                                     float *__restrict__ pooled, int *__restrict__ empty_flag,
-                                                                    const float *__restrict__ rois, int zero_fill, int stage_floats, int opts_chunked,
-                                                                    const FusedAssign fa) {
-    extern __shared__ float s_blk[];          // stage_floats floats, then S ints (direct path / fused index list), then the fused pass's bitmap
-    int *s_idx = reinterpret_cast<int *>(s_blk + stage_floats);
-    __shared__ int s_cnt;
+                                                                    const float *__restrict__ rois, int zero_fill) {
+    extern __shared__ float s_blk[];          // RB_STAGE_FLOATS floats, then S ints (the direct paths' index list)
+    int *s_idx = reinterpret_cast<int *>(s_blk + RB_STAGE_FLOATS);
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int box = blockIdx.x, scene = blockIdx.y;
     const size_t bi = (size_t)scene * M + box;
-    // Fused form (prb_options.roipool_fused; measured SLOWER than two kernels, 0.167 vs 0.156 ms at the configs[3] shape -- the
-    // assign phase holds the CTA's 50 KB of shared memory idle while it chases pointers): this CTA first runs the binned assign pass of ITS box -- bitmap and index list stay in shared
-    // memory -- and copies straight away: one launch less, no index list in HBM, and the dependent loads of the assign pass
-    // (cell offsets -> permutation -> coordinates) hide behind the row streams of the SM's other CTAs.
-    if (fa.sorted_idx) {
-        const int n = assign_grid_box(N, S, xyz + (size_t)scene * N * 3, fa.boxes3d + bi * 7, fa.sorted_idx + (size_t)scene * N,
-                                      fa.cell_start + (size_t)scene * (RG_CELLS + 1), fa.grids[scene],
-                                      reinterpret_cast<unsigned int *>(s_idx + S), s_idx);
-        if (tid == 0) s_cnt = n;
-        __syncthreads();
-    }
-    const int cnt = fa.sorted_idx ? s_cnt : cnt_in[bi];
+    const int cnt = cnt_in[bi];
     const int W = 3 + C;
     const long total = (long)S * W;
     float *dst = pooled + bi * (size_t)total;
     const bool vec = (total & 3) == 0 && ((reinterpret_cast<uintptr_t>(dst) & 15) == 0);
-    // a box's output is dealt to gridDim.z CTAs (contiguous ranges of the flat row stream): twice the CTAs, half the tail
-    const int part = blockIdx.z, nparts = gridDim.z;
-    const long e_lo = vec ? 4 * ((total / 4) * part / nparts) : total * part / nparts;
-    const long e_hi = vec ? 4 * ((total / 4) * (part + 1) / nparts) : total * (part + 1) / nparts;
     // canonical transform constants (rcnn_net.py:146-152): xyz -= roi centre, rotate (x,z) by roi ry
     float rcx = 0.f, rcy = 0.f, rcz = 0.f, rcos = 1.f, rsin = 0.f;
     if (rois) {
@@ -423,23 +398,23 @@ __global__ void __launch_bounds__(RP_THREADS) roipool3d_copy_kernel(int N, int M
         return col == 0 ? __fmaf_rn(x, rcos, -__fmul_rn(z, rsin)) : (col == 1 ? y : __fmaf_rn(x, rsin, __fmul_rn(z, rcos)));
     };
     if (cnt == 0) {
-        if (tid == 0 && part == 0) empty_flag[bi] = 1;
+        if (tid == 0) empty_flag[bi] = 1;
         // The reference leaves the rows of an empty box zero -- and then applies the canonical transform to those zeros too
         // (rcnn_net.py:146-152 runs over every RoI).  With the transform fused, an empty box's xyz columns get the
         // transformed origin; without it the rows are zero-filled on request or left to the caller's memset.
         if (rois) {
             const float ex = canon(0.f, 0.f, 0.f, 0), ey = canon(0.f, 0.f, 0.f, 1), ez = canon(0.f, 0.f, 0.f, 2);
-            for (long e = e_lo + tid; e < e_hi; e += RP_THREADS) { const int c = (int)(e % W); dst[e] = c == 0 ? ex : (c == 1 ? ey : (c == 2 ? ez : 0.f)); }
+            for (long e = tid; e < total; e += RP_THREADS) { const int c = (int)(e % W); dst[e] = c == 0 ? ex : (c == 1 ? ey : (c == 2 ? ez : 0.f)); }
         } else if (zero_fill) {
-            if (vec) for (long e = e_lo + 4L * tid; e < e_hi; e += 4L * RP_THREADS) *reinterpret_cast<float4 *>(dst + e) = make_float4(0.f, 0.f, 0.f, 0.f);
-            else for (long e = e_lo + tid; e < e_hi; e += RP_THREADS) dst[e] = 0.f;
+            if (vec) for (long e = 4L * tid; e < total; e += 4L * RP_THREADS) *reinterpret_cast<float4 *>(dst + e) = make_float4(0.f, 0.f, 0.f, 0.f);
+            else for (long e = tid; e < total; e += RP_THREADS) dst[e] = 0.f;
         }
         return;
     }
     const float *pts = xyz + (size_t)scene * N * 3;
     const float *feat = pts_feature + (size_t)scene * N * C;
-    const int *idx = fa.sorted_idx ? s_idx : idx_in + bi * S;
-    if ((long)cnt * W <= stage_floats && vec) {
+    const int *idx = idx_in + bi * S;
+    if ((long)cnt * W <= RB_STAGE_FLOATS && vec) {
         // ---- stage the cnt distinct rows (warp per row, lanes along the row), then stream the block cyclically
         for (int j = warp; j < cnt; j += RP_WARPS) {
             const int k = idx[j];
@@ -454,8 +429,8 @@ __global__ void __launch_bounds__(RP_THREADS) roipool3d_copy_kernel(int N, int M
         __syncthreads();
         const int P = cnt * W;                       // period of the output, in floats
         const int step = (4 * RP_THREADS) % P;
-        int m = (int)((e_lo + 4 * tid) % P);
-        for (long e = e_lo + 4L * tid; e < e_hi; e += 4L * RP_THREADS) {
+        int m = (4 * tid) % P;
+        for (long e = 4L * tid; e < total; e += 4L * RP_THREADS) {
             float4 v;
             if (m + 3 < P) {
                 v = make_float4(s_blk[m], s_blk[m + 1], s_blk[m + 2], s_blk[m + 3]);
@@ -471,12 +446,8 @@ __global__ void __launch_bounds__(RP_THREADS) roipool3d_copy_kernel(int N, int M
         }
         return;
     }
-    // ---- direct path: many points in the box (or an unaligned output): sources through L1
-    if (fa.sorted_idx) {      // the list already sits in s_idx[0 .. cnt): extend it cyclically in place
-        for (int j = cnt + tid; j < S; j += RP_THREADS) s_idx[j] = s_idx[j % cnt];
-    } else {
-        for (int j = tid; j < S; j += RP_THREADS) s_idx[j] = idx[j < cnt ? j : j % cnt];
-    }
+    // ---- direct paths: many points in the box (or an unaligned output)
+    for (int j = tid; j < S; j += RP_THREADS) s_idx[j] = idx[j < cnt ? j : j % cnt];
     __syncthreads();
     auto value = [&](int row, int col) -> float {
         const int k = s_idx[row];
@@ -484,16 +455,16 @@ __global__ void __launch_bounds__(RP_THREADS) roipool3d_copy_kernel(int N, int M
         if (!rois) return __ldg(pts + (size_t)k * 3 + col);
         return canon(__ldg(pts + (size_t)k * 3), __ldg(pts + (size_t)k * 3 + 1), __ldg(pts + (size_t)k * 3 + 2), col);
     };
-    if (vec && W <= stage_floats / 2 && opts_chunked) {
+    if (vec && W <= RB_STAGE_FLOATS / 2) {
         // ---- chunked staging (boxes with more distinct rows than the staging area holds: the regime of real RoIs, ~60 and
         // more points per enlarged box): the output is produced in pieces of CH rows -- gather the piece's rows into shared
         // memory (warp per row, coalesced), stream the piece out with 128-bit stores -- instead of assembling every float4
         // from four scalar loads through L1.  Pieces are cut at multiples of 4 floats, so a piece needs one row more than
         // its length.
-        const int CH = stage_floats / W - 1;                    // whole rows per piece (>= 1)
+        const int CH = RB_STAGE_FLOATS / W - 1;                 // whole rows per piece (>= 1)
         const long piece = ((long)CH * W) & ~3L;
-        for (long f0 = e_lo; f0 < e_hi; f0 += piece) {
-            const long f1 = f0 + piece < e_hi ? f0 + piece : e_hi;
+        for (long f0 = 0; f0 < total; f0 += piece) {
+            const long f1 = f0 + piece < total ? f0 + piece : total;
             const int r0 = (int)(f0 / W), r1 = (int)((f1 - 1) / W);
             __syncthreads();                                     // the previous piece has been streamed out
             for (int j = r0 + warp; j <= r1; j += RP_WARPS) {
@@ -512,11 +483,12 @@ __global__ void __launch_bounds__(RP_THREADS) roipool3d_copy_kernel(int N, int M
                 *reinterpret_cast<float4 *>(dst + e) = make_float4(src[e], src[e + 1], src[e + 2], src[e + 3]);
         }
     } else if (vec) {
-        // thread t owns float4 units t, t + T, ...: (row, col) of the unit's first float advance by a constant stride
+        // rows wider than half the staging area: sources through L1.  Thread t owns float4 units t, t + T, ...: (row, col)
+        // of the unit's first float advance by a constant stride
         const int step = 4 * RP_THREADS;
         const int d_row = step / W, d_col = step % W;
-        int row = (int)((e_lo + 4 * tid) / W), col = (int)((e_lo + 4 * tid) % W);
-        for (long e = e_lo + 4L * tid; e < e_hi; e += step) {
+        int row = 4 * tid / W, col = 4 * tid % W;
+        for (long e = 4L * tid; e < total; e += step) {
             float v[4];
             int r = row, c = col;
 #pragma unroll
@@ -529,7 +501,7 @@ __global__ void __launch_bounds__(RP_THREADS) roipool3d_copy_kernel(int N, int M
             if (col >= W) { col -= W; ++row; }
         }
     } else {
-        for (long e = e_lo + tid; e < e_hi; e += RP_THREADS) dst[e] = value((int)(e / W), (int)(e % W));
+        for (long e = tid; e < total; e += RP_THREADS) dst[e] = value((int)(e / W), (int)(e % W));
     }
 }
 
@@ -551,48 +523,33 @@ extern "C" int prb_roipool3d_ws(int B, int N, int M, int C, int S, const float *
                 "roipool3d: bad arguments");
     if (B == 0 || M == 0) return 0;
     PRB_REQUIRE(workspace && workspace_bytes >= prb_roipool3d_workspace_bytes(B, N, M, S), "roipool3d: workspace too small");
-    const bool small_idx = N <= 65536;
-    const size_t smem_a = (size_t)RA_BOXES * RA_WARPS * S * (small_idx ? sizeof(unsigned short) : sizeof(int));
-    // staging area of pass B: boxes whose distinct rows do not fit take the direct path; a smaller area = more resident CTAs
-    int stage_kb = opts().roipool_stage_kb;
-    if (stage_kb < 8 || stage_kb > 160) stage_kb = RB_STAGE_FLOATS * 4 / 1024;
-    const int stage_floats = stage_kb * 256;
-    int parts = opts().roipool_parts;
-    if (parts < 1 || parts > 8) parts = 1;                                           // 2-4 CTAs per box: 0.134-0.140 ms (no gain)
-    size_t smem_b = (size_t)stage_floats * sizeof(float) + (size_t)S * sizeof(int);
-    FusedAssign fa = {nullptr, nullptr, nullptr, nullptr};
-    PRB_REQUIRE(smem_a <= 200 * 1024 && smem_b <= 200 * 1024, "roipool3d: sampled_pts_num %d too large", S);
+    // The largest S the entry accepts: 3200 up to 65536 points, 1600 above.  The exhaustive pass A keeps RA_BOXES x RA_WARPS
+    // x S int indices in shared memory, so it takes S <= 1600 within the 200 KB; the binned pass has no limit of its own.
+    PRB_REQUIRE(S <= (N <= 65536 ? 3200 : 1600), "roipool3d: sampled_pts_num %d too large", S);
     int *idx = reinterpret_cast<int *>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
     int *cnt = idx + (size_t)B * M * S;
     cudaStream_t st = (cudaStream_t)stream;
-    const size_t smem_bits = (size_t)((N + 31) / 32) * sizeof(unsigned int);
-    if (N > 0 && N <= RG_MAX_POINTS && opts().roipool_exhaustive == 0) {
+    if (N <= RG_MAX_POINTS) {
         int *sorted = cnt + (size_t)B * M;
         int *cstart = sorted + (size_t)B * N;
         SceneGrid *grids = reinterpret_cast<SceneGrid *>(((uintptr_t)(cstart + (size_t)B * (RG_CELLS + 1)) + 15) & ~(uintptr_t)15);
         roipool3d_bin_kernel<<<B, RG_THREADS, 0, st>>>(N, xyz, sorted, cstart, grids);
         if (int rc = check_launch("roipool3d_bin_kernel")) return rc;
-        if (opts().roipool_fused != 0 && parts == 1 && smem_b + smem_bits <= 200 * 1024) {
-            fa.sorted_idx = sorted; fa.cell_start = cstart; fa.grids = grids; fa.boxes3d = boxes3d;
-            smem_b += smem_bits;
-        } else {
-            roipool3d_assign_grid_kernel<<<dim3(M, B), RGA_THREADS, smem_bits, st>>>(N, M, S, xyz, boxes3d, sorted, cstart, grids, idx, cnt);
-            if (int rc = check_launch("roipool3d_assign_grid_kernel")) return rc;
-        }
-    } else if (small_idx) {
-        if (smem_a > 48 * 1024)
-            PRB_CUDA(cudaFuncSetAttribute(roipool3d_assign_kernel<unsigned short>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_a));
-        roipool3d_assign_kernel<unsigned short><<<dim3(ceil_div(M, RA_BOXES), B), 32 * RA_WARPS, smem_a, st>>>(N, M, S, xyz, boxes3d, idx, cnt);
+        const size_t smem_bits = (size_t)((N + 31) / 32) * sizeof(unsigned int);
+        roipool3d_assign_grid_kernel<<<dim3(M, B), RGA_THREADS, smem_bits, st>>>(N, M, S, xyz, boxes3d, sorted, cstart, grids, idx, cnt);
+        if (int rc = check_launch("roipool3d_assign_grid_kernel")) return rc;
     } else {
+        const size_t smem_a = (size_t)RA_BOXES * RA_WARPS * S * sizeof(int);
         if (smem_a > 48 * 1024)
-            PRB_CUDA(cudaFuncSetAttribute(roipool3d_assign_kernel<int>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_a));
-        roipool3d_assign_kernel<int><<<dim3(ceil_div(M, RA_BOXES), B), 32 * RA_WARPS, smem_a, st>>>(N, M, S, xyz, boxes3d, idx, cnt);
+            PRB_CUDA(cudaFuncSetAttribute(roipool3d_assign_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_a));
+        roipool3d_assign_kernel<<<dim3(ceil_div(M, RA_BOXES), B), 32 * RA_WARPS, smem_a, st>>>(N, M, S, xyz, boxes3d, idx, cnt);
+        if (int rc = check_launch("roipool3d_assign_kernel")) return rc;
     }
-    if (int rc = check_launch("roipool3d_assign_kernel")) return rc;   // (no launch since the last check on the binned path: returns 0)
+    const size_t smem_b = (size_t)RB_STAGE_FLOATS * sizeof(float) + (size_t)S * sizeof(int);
     if (smem_b > 48 * 1024)
         PRB_CUDA(cudaFuncSetAttribute(roipool3d_copy_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_b));
-    roipool3d_copy_kernel<<<dim3(M, B, parts), RP_THREADS, smem_b, st>>>(N, M, C, S, xyz, pts_feature, idx, cnt, pooled, empty_flag,
-                                                                        rois_canonical, zero_fill_empty, stage_floats, opts().roipool_direct ? 0 : 1, fa);
+    roipool3d_copy_kernel<<<dim3(M, B), RP_THREADS, smem_b, st>>>(N, M, C, S, xyz, pts_feature, idx, cnt, pooled, empty_flag,
+                                                                 rois_canonical, zero_fill_empty);
     return check_launch("roipool3d_copy_kernel");
 }
 

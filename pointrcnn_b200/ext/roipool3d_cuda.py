@@ -1,6 +1,6 @@
 """`roipool3d_cuda` -- same exports as lib/utils/roipool3d/src/roipool3d.cpp:198-203.
 
-`forward` / `forward_slow` run the one-pass H100 kernel.  The two CPU twins the reference exports for its
+`forward` / `forward_slow` run the two-pass H100 kernels.  The two CPU twins the reference exports for its
 dataloader (`pts_in_boxes3d_cpu`, `roipool3d_cpu`, roipool3d.cpp:97-195) are host functions by contract;
 they are restated here in numpy on top of the same predicate arithmetic.
 """
@@ -37,7 +37,8 @@ def forward(xyz, boxes3d, pts_feature, pooled_features, pooled_empty_flag, rois_
 
 
 def forward_one_pass(xyz, boxes3d, pts_feature, pooled_features, pooled_empty_flag, rois_canonical=None):
-    """the one-kernel form (prb_roipool3d: no scratch, every box rescans the scene) -- kept for A/B measurements"""
+    """the one-kernel form (prb_roipool3d: no scratch, every box rescans the scene): the exhaustive selection the tests
+    compare the two-pass `forward` against"""
     B, N = int(xyz.size(0)), int(xyz.size(1))
     M, Cf, S = int(boxes3d.size(1)), int(pts_feature.size(2)), int(pooled_features.size(2))
     with torch.cuda.device(xyz.device):

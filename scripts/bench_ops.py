@@ -43,19 +43,13 @@ pooled = torch.zeros((B, M, S, 3 + C), device=dev); empty = torch.zeros((B, M), 
 ms = timeit(lambda: roipool3d_cuda.forward(x, bx, f, pooled, empty))
 ms_c = timeit(lambda: roipool3d_cuda.forward(x, bx, f, pooled, empty, bx))
 ms_1p = timeit(lambda: roipool3d_cuda.forward_one_pass(x, bx, f, pooled, empty))
-from pointrcnn_b200 import _cabi
-with _cabi.options(roipool_exhaustive=1):
-    ms_ex = timeit(lambda: roipool3d_cuda.forward(x, bx, f, pooled, empty))
-with _cabi.options(roipool_fused=0):
-    ms_two = timeit(lambda: roipool3d_cuda.forward(x, bx, f, pooled, empty))
-    ms_two_c = timeit(lambda: roipool3d_cuda.forward(x, bx, f, pooled, empty, bx))
 ms_memset = timeit(lambda: pooled.zero_())
 from pointrcnn_b200.roipool3d import roipool3d_utils
 ms_util = timeit(lambda: roipool3d_utils.roipool3d_gpu(x, f, bx, 0.0, S))
 ms_ref = timeit(lambda: R.roipool3d(x, f, bx, S), iters=5)
 alg = (B * N * C * 4 + B * N * 12 + B * M * S * (3 + C) * 4)
 nonempty = int((empty == 0).sum())
-out["roipool3d_C4"] = {"ms": ms, "ms_with_canonical": ms_c, "ms_one_pass_kernel": ms_1p, "ms_exhaustive": ms_ex, "ms_two_kernel_form": ms_two, "ms_two_kernel_form_with_canonical": ms_two_c, "ms_memset_of_output": ms_memset,
+out["roipool3d_C4"] = {"ms": ms, "ms_with_canonical": ms_c, "ms_one_pass_kernel": ms_1p, "ms_memset_of_output": ms_memset,
                        "ms_roipool3d_gpu_wrapper_incl_alloc": ms_util, "ms_reference_kernels": ms_ref, "speedup": ms_ref / ms,
                        "algorithmic_MB": alg / 1e6, "achieved_GBs": alg / ms / 1e6, "peak_GBs": peaks["hbm_gbs"],
                        "frac": alg / ms / 1e6 / peaks["hbm_gbs"], "non_empty_boxes": nonempty, "of": B * M}

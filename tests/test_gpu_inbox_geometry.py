@@ -9,17 +9,29 @@ from oracle import refgpu as R
 
 pytestmark = pytest.mark.gpu
 
-from pointrcnn_b200 import _cabi as C  # noqa: E402
 from pointrcnn_b200.datasets.kitti_rcnn_dataset import generate_rpn_training_labels  # noqa: E402
 from pointrcnn_b200.ext import roipool3d_cuda  # noqa: E402
 
 HAVE_REF = R.available()
-# every form of the pooling entries: the one-pass kernel, the binned two-kernel default and its pass-B variants, the
-# exhaustive assign pass, the binned pass fused into the copy kernel
-FORMS = {"one_pass": None, "binned": {}, "exhaustive": dict(roipool_exhaustive=1), "fused": dict(roipool_fused=1),
-         "direct": dict(roipool_direct=1), "stage_kb8": dict(roipool_stage_kb=8), "parts3": dict(roipool_parts=3)}
-# (S, C): boxes that saturate S, a row width that is not a multiple of four floats (scalar stores), boxes that do not
-SHAPES = [(16, 2), (37, 2), (128, 5)]
+# both pooling entries: the one-pass kernel (every box scans the scene) and the two-pass form (binned pass A, pass B)
+FORMS = {"one_pass": roipool3d_cuda.forward_one_pass, "two_pass": roipool3d_cuda.forward}
+# (S, C): boxes that saturate S, a row width that is not a multiple of four floats (scalar stores), boxes that do not,
+# boxes with more distinct rows than pass B's staging area holds (chunked staging), rows wider than half of it (gathers)
+SHAPES = [(16, 2), (37, 2), (128, 5), (128, 130), (16, 6142)]
+STAGE_FLOATS = 12 * 1024                # RB_STAGE_FLOATS of csrc/roipool3d.cu
+# (S, C) -> the pass-B branch some box of these families must take.  Only the "cap" boxes hold more than 92 points.
+REACH = {(16, 2): ("staged", IR.FAMILIES), (37, 2): ("scalar", IR.FAMILIES), (128, 130): ("chunked", ("cap",)),
+         (16, 6142): ("direct", IR.FAMILIES)}
+
+
+def _pass_b_branch(cnt, S, C_):
+    """the branch of roipool3d_copy_kernel a non-empty box with cnt distinct rows takes"""
+    W = 3 + C_
+    if S * W % 4:
+        return "scalar"
+    if cnt * W <= STAGE_FLOATS:
+        return "staged"
+    return "chunked" if W <= STAGE_FLOATS // 2 else "direct"
 
 
 def _scenes(family, C_):
@@ -36,11 +48,7 @@ def _pool(form, x, bx, f, S, rois=None):
     B, M = bx.shape[:2]
     pooled = torch.zeros((B, M, S, 3 + f.shape[2]), device=x.device)
     empty = torch.zeros((B, M), dtype=torch.int32, device=x.device)
-    if FORMS[form] is None:
-        roipool3d_cuda.forward_one_pass(x, bx, f, pooled, empty, rois_canonical=rois)
-    else:
-        with C.options(**FORMS[form]):
-            roipool3d_cuda.forward(x, bx, f, pooled, empty, rois_canonical=rois)
+    FORMS[form](x, bx, f, pooled, empty, rois_canonical=rois)
     torch.cuda.synchronize()
     return pooled.cpu().numpy(), empty.cpu().numpy()
 
@@ -73,18 +81,22 @@ def _canonical_bound(pts, rois):
 
 @pytest.mark.parametrize("S,C_", SHAPES)
 @pytest.mark.parametrize("family", IR.FAMILIES)
-def test_roipool3d_every_form_against_float64(cuda, family, S, C_):
+def test_roipool3d_both_entries_against_float64(cuda, family, S, C_):
     xyz, boxes, feat = _scenes(family, C_)
     x, bx, f = (torch.from_numpy(a).to(cuda) for a in (xyz, boxes, feat))
-    first = None
+    out = {}
     for form in FORMS:
-        pooled, empty = _pool(form, x, bx, f, S)
-        _check_pooled(pooled, empty, xyz, boxes, feat, where="%s %s S=%d" % (family, form, S))
-        if first is None:
-            first = (pooled, empty)
-    pooled, empty = first
+        out[form] = _pool(form, x, bx, f, S)
+        _check_pooled(*out[form], xyz, boxes, feat, where="%s %s S=%d" % (family, form, S))
+    pooled, empty = out["two_pass"]
+    assert np.array_equal(empty, out["one_pass"][1]) and np.array_equal(pooled.view(np.uint32), out["one_pass"][0].view(np.uint32)), \
+        "%s: the two entries differ" % family
     if family not in ("degenerate",):
         assert (empty == 0).any(), "the family must fill boxes"
+    branch, families = REACH.get((S, C_), (None, ()))
+    if family in families:
+        taken = {_pass_b_branch(len(np.unique(pooled[b, m, :, 3])), S, C_) for b, m in zip(*np.nonzero(empty == 0))}
+        assert branch in taken, "%s S=%d C=%d: no box takes pass B's %s branch (%s)" % (family, S, C_, branch, taken)
     if HAVE_REF:
         rp, re = R.roipool3d(x, f, bx, S)
         rp, re = rp.cpu().numpy(), re.cpu().numpy()
@@ -94,7 +106,7 @@ def test_roipool3d_every_form_against_float64(cuda, family, S, C_):
 
 
 @pytest.mark.parametrize("family", ["random", "faces", "headings", "cap", "far", "degenerate"])
-def test_roipool3d_canonical_rows_against_float64(cuda, family):
+def test_roipool3d_canonical_rows_of_both_entries_against_float64(cuda, family):
     """with canonical RoIs the selection is the same, xyz lies within the derived bound of the float64 transform of the
     selected point, features stay bit copies, and empty boxes get the transformed zero rows"""
     S, C_ = 37, 2

@@ -463,18 +463,12 @@ def _roi_scene(B, N, M, C, seed):
 
 
 @pytest.mark.parametrize("B,N,M,C,S", [(2, 16384, 64, 130, 512), (1, 4096, 33, 5, 128), (2, 2000, 16, 0, 64)])
-def test_roipool3d_vs_reference_and_oracle(cuda, B, N, M, C, S):
+def test_roipool3d_two_pass_vs_reference_and_oracle(cuda, B, N, M, C, S):
     xyz, boxes, feat = _roi_scene(B, N, M, C, 41 + N)
     x, bx, f = T(xyz, cuda), T(boxes, cuda), T(feat, cuda)
     pooled = torch.zeros((B, M, S, 3 + C), device=cuda)
     empty = torch.zeros((B, M), dtype=torch.int32, device=cuda)
     roipool3d_cuda.forward(x, bx, f, pooled, empty)
-    from pointrcnn_b200 import _cabi
-    for alt in ({"roipool_direct": 1}, {"roipool_stage_kb": 8}, {"roipool_parts": 3}):   # scalar-gather path; tiny staging area
-        p2 = torch.zeros_like(pooled); e2 = torch.zeros_like(empty)                       # (every box chunked); 3 CTAs per box
-        with _cabi.options(**alt):
-            roipool3d_cuda.forward(x, bx, f, p2, e2)
-        assert torch.equal(p2, pooled) and torch.equal(e2, empty), "pass-B variant %r differs" % alt
     if HAVE_REF and C > 0:
         rp, re = R.roipool3d(x, f, bx, S)
         assert torch.equal(empty, re), "empty flags differ from the reference kernel"
@@ -489,12 +483,12 @@ def test_roipool3d_vs_reference_and_oracle(cuda, B, N, M, C, S):
     assert ge.sum() > 0 and (1 - ge).sum() > 0, "test should cover empty and non-empty boxes"
 
 
-@pytest.mark.parametrize("case", ["duplicates", "degenerate_line", "nan_inf", "huge_boxes", "tiny", "odd_n", "far_coordinates"])
-def test_roipool3d_binned_equals_exhaustive(cuda, case):
-    """the x-z binned assign pass (default) must select exactly the rows of the exhaustive scan: same predicate, the
-    footprint only prunes cells that cannot hold an inside point.  Degenerate clouds and boxes included."""
-    from pointrcnn_b200 import _cabi as C
-    rng = np.random.default_rng(len(case))
+@pytest.mark.parametrize("case", ["duplicates", "degenerate_line", "nan_inf", "huge_boxes", "tiny", "odd_n", "far_coordinates",
+                                  "large_scene", "no_points"])
+def test_roipool3d_two_pass_equals_one_pass(cuda, case):
+    """the two-pass entry must select exactly the rows of the one-pass kernel, which tests every point against every
+    box: the x-z binned assign pass only prunes cells that cannot hold an inside point, and scenes of more than
+    RG_MAX_POINTS points take the exhaustive assign pass.  Degenerate clouds and boxes included."""
     B, N, M, Cf, S = 2, 5000, 40, 7, 64
     xyz, boxes, feat = _roi_scene(B, N, M, Cf, 300 + len(case))
     if case == "duplicates":
@@ -518,21 +512,34 @@ def test_roipool3d_binned_equals_exhaustive(cuda, case):
         xyz, feat = xyz[:, :N].copy(), feat[:, :N].copy()
     elif case == "far_coordinates":
         xyz += np.float32(30000.0); boxes[:, :, 0:3] += np.float32(30000.0)     # coarse fp32 spacing around the boxes
+    elif case == "large_scene":
+        N = 54 * N                                                 # 270000 > RG_MAX_POINTS = 262144: the exhaustive assign pass
+        xyz, feat = np.tile(xyz, (1, 54, 1)), np.tile(feat, (1, 54, 1))       # each scene tiled: 54 copies of every point
     x, bx, f = T(xyz, cuda), T(boxes, cuda), T(feat, cuda)
+    forms = (roipool3d_cuda.forward, roipool3d_cuda.forward_one_pass)
+    if case == "no_points":
+        # torch gives a tensor without elements a NULL data pointer, which the entries refuse: call them with N = 0 and
+        # the pointers of real tensors
+        from pointrcnn_b200 import _cabi as C
+        L, P = C.lib(), C.ptr
+        ws = torch.empty(L.prb_roipool3d_workspace_bytes(B, 0, M, S), dtype=torch.uint8, device=cuda)
+        forms = (lambda x, bx, f, p, e: C.check(L.prb_roipool3d_ws(B, 0, M, Cf, S, P(x), P(bx), P(f), P(p), P(e), None, 0, P(ws),
+                                                                  C.c_size_t(ws.numel()), C.stream()), "roipool3d"),
+                 lambda x, bx, f, p, e: C.check(L.prb_roipool3d(B, 0, M, Cf, S, P(x), P(bx), P(f), P(p), P(e), None, C.stream()),
+                                                "roipool3d"))
     out = []
-    # binned as two kernels (default), exhaustive, binned with the assign pass fused into the copy kernel
-    for opt in (dict(roipool_exhaustive=0, roipool_fused=0), dict(roipool_exhaustive=1), dict(roipool_exhaustive=0, roipool_fused=1)):
+    for fwd in forms:
         pooled = torch.zeros((B, M, S, 3 + Cf), device=cuda)
         empty = torch.zeros((B, M), dtype=torch.int32, device=cuda)
-        with C.options(**opt):
-            roipool3d_cuda.forward(x, bx, f, pooled, empty)
+        fwd(x, bx, f, pooled, empty)
         torch.cuda.synchronize()
         out.append((pooled.cpu().numpy(), empty.cpu().numpy()))
-    assert np.array_equal(out[0][1], out[1][1]) and np.array_equal(out[2][1], out[1][1]), "empty flags differ"
+    assert np.array_equal(out[0][1], out[1][1]), "empty flags differ"
     assert np.array_equal(out[0][0].view(np.uint32), out[1][0].view(np.uint32)), "pooled rows differ (bitwise)"
-    assert np.array_equal(out[2][0].view(np.uint32), out[1][0].view(np.uint32)), "pooled rows differ (bitwise, fused form)"
-    if case in ("duplicates", "huge_boxes", "odd_n", "far_coordinates"):
+    if case in ("duplicates", "huge_boxes", "odd_n", "far_coordinates", "large_scene"):
         assert (out[0][1] == 0).sum() > 0, "case should have non-empty boxes"
+    if case == "no_points":
+        assert out[0][1].all() and not out[0][0].any(), "every box of a scene without points is empty"
 
 
 def test_roipool3d_utils_and_canonical(cuda):
