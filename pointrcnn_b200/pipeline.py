@@ -4,7 +4,8 @@ Furthest-point sampling is a dependency chain (4095 serial rounds for the first 
 scene (16 of 132 SMs), and nothing else of the SAME batch can run before it ends.  Consecutive batches are
 independent (the reference's eval loop processes them one after another), so batch i+1's sampling chain can
 overlap batch i's neighbour searches and tensor-core MLPs.  Results are identical to the sequential loop, bit for bit -- only the stream assignment
-differs (tests/test_gpu_mlp.py::test_batch_pipeline_matches_sequential).
+differs (tests/test_gpu_mlp.py::test_batch_pipeline_matches_sequential; at bench.py's batch, slot counts and RPN
+stage in tests/test_gpu_bench_paths.py).
 
 `graphs=True` captures `fn` once per slot (stream) into a CUDA graph and replays it: the ~45 native launches and the
 torch glue of one forward become one graph launch, which matters when batches are small (strong scaling: 2 scenes per
