@@ -408,6 +408,19 @@ PRB_API int prb_kitti_eval(int n_img, int num_classes, const int *classes, const
                            const int *gt_off, int n_gt, const double *dt, const int *dt_off, const int *dt_count, int n_dt,
                            int max_det, const long long *pair_off, long long n_pairs, double *overlaps, double *out,
                            void *workspace, size_t workspace_bytes, void *stream);
+/* the same statistics over num_sets (1..10) overlap sets per class, e.g. the ten of get_coco_eval_result
+ * (eval.py:681-740): min_overlaps HOST (num_sets, 3, num_classes), each in (0, 1); out (9*num_sets*num_classes*41*8 + 1 +
+ * 9*num_sets*num_classes) double with config q = ((metric*num_classes + class)*3 + difficulty)*num_sets + overlap set and
+ * the layout above.  score_thresh > 0 first keeps only the detections scoring >= score_thresh, in row order
+ * (kitti_common.filter_annos_low_score, evaluate.py:21-22), on the device: the result, the AOS flag and the overlaps are
+ * those of the filtered detections.  prb_kitti_eval is this entry with num_sets = 2 and no threshold.  The overlaps are
+ * computed once whatever num_sets is.  Seven launches (with the filter) and a memset, no host synchronisation. */
+PRB_API size_t prb_kitti_eval_sets_workspace_bytes(int n_img, int n_gt, int n_dt, int num_classes, int num_sets);
+PRB_API int prb_kitti_eval_sets(int n_img, int num_classes, const int *classes, int num_sets, const double *min_overlaps,
+                                double score_thresh, const double *gt, const int *gt_off, int n_gt, const double *dt,
+                                const int *dt_off, const int *dt_count, int n_dt, int max_det, const long long *pair_off,
+                                long long n_pairs, double *overlaps, double *out, void *workspace, size_t workspace_bytes,
+                                void *stream);
 /* the rows save_kitti_format would write for a batch of scenes (valid[k,j] && select[k,j], in row order) appended as
  * detection rows of image slot[k] (b, device int32), starting at row 0 of its range; dt_count[slot[k]] = their number.
  * boxes3d (b,m,7) [x,y,z,h,w,l,ry], scores (b,m), img_boxes (b,m,4), alpha (b,m), valid / select (b,m) int32, as

@@ -74,7 +74,7 @@ def lib():
         for name in ("prb_nms_workspace_bytes", "prb_mlp_packed_bytes", "prb_mlp_packed_bytes_ex",
                      "prb_sa_workspace_bytes", "prb_fp_workspace_bytes", "prb_rows_workspace_bytes", "prb_rows2_workspace_bytes", "prb_grid_workspace_bytes",
                      "prb_fps_workspace_bytes", "prb_fps_ordered_workspace_bytes", "prb_kitti_format_detections", "prb_rpn_proposals_workspace_bytes", "prb_roipool3d_workspace_bytes",
-                     "prb_kitti_eval_workspace_bytes", "prb_stage_loss_workspace_bytes", "prb_sa_train_workspace_bytes",
+                     "prb_kitti_eval_workspace_bytes", "prb_kitti_eval_sets_workspace_bytes", "prb_stage_loss_workspace_bytes", "prb_sa_train_workspace_bytes",
                      "prb_fp_train_workspace_bytes", "prb_sa_train_det_workspace_bytes", "prb_group_points_grad_workspace_bytes",
                      "prb_gather_points_grad_workspace_bytes", "prb_three_interpolate_grad_workspace_bytes"):
             getattr(L, name).restype = c_size_t

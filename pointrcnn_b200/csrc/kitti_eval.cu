@@ -3,13 +3,16 @@
 //
 // The annotations of every image sit in two row tables (ground truth and detections, kEvalCols doubles per row, ragged by
 // per-image offsets).  The stages follow eval.py's:
+//   filter      kitti_common.filter_annos_low_score (optional): the detections scoring >= score_thresh, in row order
 //   overlaps    calculate_iou_partly, per image a (dt x gt) matrix of the three metrics (:335-409)
 //   clean       clean_data per (class, difficulty): ignored_gt, ignored_dt, number of valid GT (:28-81)
 //   pass 1      compute_statistics_jit(compute_fp=False): the TP scores that are threshold candidates (:156-273)
 //   thresholds  get_thresholds on the sorted TP scores (:8-25)
 //   pass 2      fused_compute_statistics: tp / fp / fn / similarity per threshold (:285-332)
 //   finish      recall, precision, orientation similarity and their suffix maxima (:532-542)
-// A config is one (metric, class, difficulty, min_overlap).  Each (image, config) is one warp: the GT loop stays
+// A config is one (metric, class, difficulty, overlap set); the official table has two overlap sets per class
+// (get_official_eval_result), the COCO-style one ten (get_coco_eval_result, eval.py:681-740).  The overlaps do not depend on
+// the configs and are computed once.  Each (image, config) is one warp: the GT loop stays
 // sequential as in the reference, and the loop over detections is a warp reduction whose tie rule gives what the
 // sequential loop gives.  tp / fp / fn are integers; the similarity is summed per image in GT order and over images in
 // image order, so a result is the same, bit for bit, from run to run.
@@ -24,25 +27,27 @@ enum { C_X1 = 0, C_Y1, C_X2, C_Y2, C_ALPHA, C_TRUNC, C_OCC, C_L, C_H, C_W, C_X, 
 constexpr int kSamplePts = 41;
 constexpr int kMaxDetPerImage = 1024;     // one assignment bit per lane and 32 detections
 constexpr int kMaxEvalClasses = 8;
+constexpr int kMaxOverlapSets = 10;       // get_coco_eval_result's ten overlap thresholds per class
 constexpr int kCodeDontCare = 5;          // class codes: 0 car, 1 pedestrian, 2 cyclist, 3 van, 4 person_sitting, 5 DontCare
 constexpr int kOutPerThr = 8;             // tp, fp, fn, similarity, recall, precision, aos, threshold
 
 struct EvalCfg {
-    int nc;                                     // evaluated classes
-    int cls[kMaxEvalClasses];                   // their indices (0..2)
-    double min_ov[2][3][kMaxEvalClasses];       // [overlap set][metric][class]
+    int nc;                                                 // evaluated classes
+    int ns;                                                 // overlap sets
+    int cls[kMaxEvalClasses];                               // their indices (0..2)
+    double min_ov[kMaxOverlapSets][3][kMaxEvalClasses];     // [overlap set][metric][class]
 };
 
 struct ConfigId {
     int metric, c, diff, k;
 };
-// config q = ((metric * nc + c) * 3 + diff) * 2 + k: the metric-0 configs come first
-__device__ __forceinline__ ConfigId config_of(int q, int nc) {
+// config q = ((metric * nc + c) * 3 + diff) * ns + k: the metric-0 configs come first
+__device__ __forceinline__ ConfigId config_of(int q, int nc, int ns) {
     ConfigId r;
-    r.k = q & 1;
-    r.diff = (q >> 1) % 3;
-    r.c = (q / 6) % nc;
-    r.metric = q / (6 * nc);
+    r.k = q % ns;
+    r.diff = (q / ns) % 3;
+    r.c = (q / (3 * ns)) % nc;
+    r.metric = q / (3 * ns * nc);
     return r;
 }
 
@@ -67,6 +72,36 @@ __device__ __forceinline__ void bev_pre(const double *r, BoxPre &p, float &area)
     const float box[5] = {__fsub_rn(x, l * 0.5f), __fsub_rn(z, w * 0.5f), __fadd_rn(x, l * 0.5f), __fadd_rn(z, w * 0.5f), (float)r[C_RY]};
     box_pre(box, p);
     area = __fmul_rn(l, w);
+}
+
+// ------------------------------------------------------------------------------------------------ filter
+// filter_annos_low_score (kitti_common.py:190-201) in front of the other stages: the detections of image img with
+// score >= thresh, in row order, to the same rows of dt_f, and their number to count_f.  The rows after them, up to the
+// image's range, are zeroed.  A stable compaction leaves the assignment order and the AOS decision (the first image that
+// still has detections) as evaluating the filtered annotations gives them.  One warp per image.
+__global__ void __launch_bounds__(128) eval_filter_kernel(int n_img, double thresh, const double *__restrict__ dt,
+                                                          const int *__restrict__ dt_off, const int *__restrict__ dt_count,
+                                                          double *__restrict__ dt_f, int *__restrict__ count_f) {
+    const int img = blockIdx.x * 4 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (img >= n_img) return;
+    const int d0 = dt_off[img], cap = dt_off[img + 1] - d0;
+    const int nd = min(dt_count[img], min(cap, kMaxDetPerImage));
+    const double *src = dt + (size_t)d0 * kEvalCols;
+    double *dst = dt_f + (size_t)d0 * kEvalCols;
+    int n = 0;
+    for (int j0 = 0; j0 < nd; j0 += 32) {
+        const int j = j0 + lane;
+        const bool keep = j < nd && src[(size_t)j * kEvalCols + C_SCORE] >= thresh;
+        const unsigned bal = __ballot_sync(0xffffffffu, keep);
+        // the kept rows of these 32 in order, each copied by lanes 0..15, one field per lane
+        for (unsigned b = bal; b; b &= b - 1) {
+            const int s = __ffs(b) - 1;
+            if (lane < kEvalCols) dst[(size_t)n * kEvalCols + lane] = src[(size_t)(j0 + s) * kEvalCols + lane];
+            ++n;
+        }
+    }
+    for (size_t e = (size_t)n * kEvalCols + lane; e < (size_t)cap * kEvalCols; e += 32) dst[e] = 0.0;
+    if (lane == 0) count_f[img] = n;
 }
 
 // ------------------------------------------------------------------------------------------------ overlaps
@@ -168,7 +203,7 @@ __global__ void __launch_bounds__(256) eval_pass1_kernel(EvalCfg cfg, int n_img,
     const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (w >= n_img * nconf) return;
     const int q = w / n_img, img = w - q * n_img;
-    const ConfigId id = config_of(q, cfg.nc);
+    const ConfigId id = config_of(q, cfg.nc, cfg.ns);
     const double mo = cfg.min_ov[id.k][id.metric][id.c];
     const ImageView v = image_view(img, id.metric, id.c * 3 + id.diff, gt_off, dt_off, dt_count, pair_off, ov, n_pairs, ig_gt, n_gt, ig_dt, n_dt);
     unsigned assigned = 0;      // bit s: detection lane + 32 s
@@ -201,11 +236,11 @@ __global__ void __launch_bounds__(256) eval_pass1_kernel(EvalCfg cfg, int n_img,
 // power of two) and pick get_thresholds' ranks.  With the recall fixed between two picks, "take rank i" is monotone in i
 // (both rounded differences are monotone in the rounded recalls), so each pick is a binary search; the last rank is
 // always taken.  Same picks as the sequential loop, in the same double arithmetic.
-__global__ void __launch_bounds__(512) eval_thresholds_kernel(int nc, const int *__restrict__ nvalid, const int *__restrict__ tp_count,
+__global__ void __launch_bounds__(512) eval_thresholds_kernel(int nc, int ns, const int *__restrict__ nvalid, const int *__restrict__ tp_count,
                                                                double *__restrict__ tp_scores, int score_stride, double *__restrict__ thr,
                                                                int *__restrict__ nthr) {
     const int q = blockIdx.x, tid = threadIdx.x;
-    const ConfigId id = config_of(q, nc);
+    const ConfigId id = config_of(q, nc, ns);
     const int n = tp_count[q];
     double *s = tp_scores + (size_t)q * score_stride;
     int pad = 1;
@@ -258,7 +293,7 @@ __global__ void __launch_bounds__(256, 2) eval_pass2_kernel(EvalCfg cfg, int n_i
     const int w = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
     if (w >= n_img * nconf) return;
     const int q = w / n_img, img = w - q * n_img;
-    const ConfigId id = config_of(q, cfg.nc);
+    const ConfigId id = config_of(q, cfg.nc, cfg.ns);
     const double mo = cfg.min_ov[id.k][id.metric][id.c];
     const ImageView v = image_view(img, id.metric, id.c * 3 + id.diff, gt_off, dt_off, dt_count, pair_off, ov, n_pairs, ig_gt, n_gt, ig_dt, n_dt);
     // per lane: its detections' eligibility for the DontCare rule (metric 0), independent of the threshold
@@ -341,13 +376,13 @@ __device__ __forceinline__ double nan_max(double a, double b) { return (isnan(a)
 // one CTA per config, one thread per threshold: the similarity summed over images in image order, the rates in double,
 // suffix maxima over the thresholds.  out (nconf, 41, kOutPerThr), then the AOS flag (eval.py:636-641: the first
 // detection annotation with rows decides; AOS unless its first alpha is -10), then nthr (nconf)
-__global__ void __launch_bounds__(64) eval_finish_kernel(int nc, int n_img, const int *__restrict__ pr, const double *__restrict__ sim_img,
+__global__ void __launch_bounds__(64) eval_finish_kernel(int nc, int ns, int n_img, const int *__restrict__ pr, const double *__restrict__ sim_img,
                                                           const double *__restrict__ thr, const int *__restrict__ nthr,
                                                           const double *__restrict__ dt, const int *__restrict__ dt_off,
                                                           const int *__restrict__ dt_count, int nconf, double *__restrict__ out) {
     __shared__ double s_v[3][kSamplePts];
     const int q = blockIdx.x, t = threadIdx.x;
-    const ConfigId id = config_of(q, nc);
+    const ConfigId id = config_of(q, nc, ns);
     const int nt = nthr[q];
     double *o = out + (size_t)q * kSamplePts * kOutPerThr;
     if (t < kSamplePts) {
@@ -424,15 +459,16 @@ __global__ void __launch_bounds__(128, 4) eval_add_detections_kernel(int b, int 
 
 // ------------------------------------------------------------------------------------------------ workspace
 struct EvalWs {
-    size_t ig_gt, ig_dt, ints, n_ints, nvalid, tp_count, nthr, pr, tp_scores, thr, sim, total;
+    size_t ig_gt, ig_dt, ints, n_ints, nvalid, tp_count, nthr, pr, tp_scores, thr, sim, dt_f, count_f, total;
     int score_stride;
 };
 
 static size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
 
-static EvalWs eval_ws(int n_img, int n_gt, int n_dt, int nc) {
+// `filter`: room for the score-filtered detection table and counts, after everything else
+static EvalWs eval_ws(int n_img, int n_gt, int n_dt, int nc, int ns, bool filter) {
     EvalWs w;
-    const int ncl = 3 * nc, nconf = 18 * nc;
+    const int ncl = 3 * nc, nconf = 9 * ns * nc;
     int pad = 1;
     while (pad < n_gt) pad <<= 1;
     w.score_stride = pad;
@@ -448,7 +484,9 @@ static EvalWs eval_ws(int n_img, int n_gt, int n_dt, int nc) {
     off = align256(off + w.n_ints * sizeof(int));
     w.tp_scores = off; off = align256(off + (size_t)nconf * pad * sizeof(double));
     w.thr = off; off = align256(off + (size_t)nconf * kSamplePts * sizeof(double));
-    w.sim = off; off = align256(off + (size_t)6 * nc * kSamplePts * n_img * sizeof(double));
+    w.sim = off; off = align256(off + (size_t)3 * ns * nc * kSamplePts * n_img * sizeof(double));    // the metric-0 configs
+    w.dt_f = off; off = filter ? align256(off + (size_t)n_dt * kEvalCols * sizeof(double)) : off;
+    w.count_f = off; off = filter ? align256(off + (size_t)n_img * sizeof(int)) : off;
     w.total = off;
     return w;
 }
@@ -459,34 +497,45 @@ using namespace prb;
 
 extern "C" size_t prb_kitti_eval_workspace_bytes(int n_img, int n_gt, int n_dt, int num_classes) {
     if (n_img < 1 || n_gt < 0 || n_dt < 0 || num_classes < 1 || num_classes > kMaxEvalClasses) return 0;
-    return eval_ws(n_img, n_gt, n_dt, num_classes).total;
+    return eval_ws(n_img, n_gt, n_dt, num_classes, 2, false).total;
 }
 
-extern "C" int prb_kitti_eval(int n_img, int num_classes, const int *classes, const double *min_overlaps, const double *gt,
-                              const int *gt_off, int n_gt, const double *dt, const int *dt_off, const int *dt_count, int n_dt,
-                              int max_det, const long long *pair_off, long long n_pairs, double *overlaps, double *out,
-                              void *workspace, size_t workspace_bytes, void *stream) {
+extern "C" size_t prb_kitti_eval_sets_workspace_bytes(int n_img, int n_gt, int n_dt, int num_classes, int num_sets) {
+    if (n_img < 1 || n_gt < 0 || n_dt < 0 || num_classes < 1 || num_classes > kMaxEvalClasses || num_sets < 1 || num_sets > kMaxOverlapSets)
+        return 0;
+    return eval_ws(n_img, n_gt, n_dt, num_classes, num_sets, true).total;
+}
+
+extern "C" int prb_kitti_eval_sets(int n_img, int num_classes, const int *classes, int num_sets, const double *min_overlaps,
+                                   double score_thresh, const double *gt, const int *gt_off, int n_gt, const double *dt,
+                                   const int *dt_off, const int *dt_count, int n_dt, int max_det, const long long *pair_off,
+                                   long long n_pairs, double *overlaps, double *out, void *workspace, size_t workspace_bytes,
+                                   void *stream) {
     PRB_REQUIRE(n_img >= 1 && n_gt >= 0 && n_dt >= 0 && n_pairs >= 0 && classes && min_overlaps && gt_off && dt_off && dt_count &&
                     pair_off && out && (n_pairs == 0 || overlaps) && (n_gt == 0 || gt) && (n_dt == 0 || dt),
                 "kitti_eval: bad arguments");
     PRB_REQUIRE(num_classes >= 1 && num_classes <= kMaxEvalClasses, "kitti_eval: %d classes (1..%d)", num_classes, kMaxEvalClasses);
+    PRB_REQUIRE(num_sets >= 1 && num_sets <= kMaxOverlapSets, "kitti_eval: %d overlap sets (1..%d)", num_sets, kMaxOverlapSets);
     PRB_REQUIRE(max_det >= 0 && max_det <= kMaxDetPerImage, "kitti_eval: %d detection rows per image > %d", max_det, kMaxDetPerImage);
-    PRB_REQUIRE((long long)n_img * 18 * num_classes <= 0x7fffffffLL / 32, "kitti_eval: %d images is too many", n_img);
+    PRB_REQUIRE((long long)n_img * 9 * num_sets * num_classes <= 0x7fffffffLL / 32, "kitti_eval: %d images is too many", n_img);
     EvalCfg cfg;
     cfg.nc = num_classes;
+    cfg.ns = num_sets;
     for (int c = 0; c < num_classes; ++c) {
         PRB_REQUIRE(classes[c] >= 0 && classes[c] <= 2, "kitti_eval: class %d is not 0 (Car), 1 (Pedestrian) or 2 (Cyclist)", classes[c]);
         cfg.cls[c] = classes[c];
-        for (int k = 0; k < 2; ++k)
+        for (int k = 0; k < num_sets; ++k)
             for (int m = 0; m < 3; ++m) {
                 const double v = min_overlaps[(k * 3 + m) * num_classes + c];
                 PRB_REQUIRE(v > 0.0 && v < 1.0, "kitti_eval: min_overlap %g outside (0, 1)", v);
                 cfg.min_ov[k][m][c] = v;
             }
     }
-    const EvalWs w = eval_ws(n_img, n_gt, n_dt, num_classes);
+    // the reference's rule (evaluate.py:22): a threshold filters only when it is > 0
+    const bool filter = score_thresh > 0.0;
+    const EvalWs w = eval_ws(n_img, n_gt, n_dt, num_classes, num_sets, filter);
     PRB_REQUIRE(workspace && workspace_bytes >= w.total, "kitti_eval: workspace of %zu bytes < %zu", workspace_bytes, w.total);
-    const int nconf = 18 * num_classes, ncl = 3 * num_classes;
+    const int nconf = 9 * num_sets * num_classes, ncl = 3 * num_classes;
     cudaStream_t st = (cudaStream_t)stream;
     char *ws = (char *)workspace;
     signed char *ig_gt = (signed char *)(ws + w.ig_gt), *ig_dt = (signed char *)(ws + w.ig_dt);
@@ -495,6 +544,14 @@ extern "C" int prb_kitti_eval(int n_img, int num_classes, const int *classes, co
     double *tp_scores = (double *)(ws + w.tp_scores), *thr = (double *)(ws + w.thr), *sim = (double *)(ws + w.sim);
     PRB_CUDA(cudaMemsetAsync(ints, 0, w.n_ints * sizeof(int), st));
 
+    if (filter) {
+        double *dt_f = (double *)(ws + w.dt_f);
+        int *count_f = (int *)(ws + w.count_f);
+        eval_filter_kernel<<<ceil_div(n_img, 4), 128, 0, st>>>(n_img, score_thresh, dt, dt_off, dt_count, dt_f, count_f);
+        if (int rc = check_launch("eval_filter_kernel")) return rc;
+        dt = dt_f;
+        dt_count = count_f;
+    }
     eval_overlaps_kernel<<<n_img, 128, 0, st>>>(gt, gt_off, dt, dt_off, dt_count, pair_off, n_pairs, overlaps);
     if (int rc = check_launch("eval_overlaps_kernel")) return rc;
     const int rows = max(1, max(n_gt, n_dt));
@@ -504,13 +561,21 @@ extern "C" int prb_kitti_eval(int n_img, int num_classes, const int *classes, co
     eval_pass1_kernel<<<ceil_div(warps, 8), 256, 0, st>>>(cfg, n_img, nconf, dt, gt_off, dt_off, dt_count, pair_off, overlaps, n_pairs, ig_gt,
                                                           n_gt, ig_dt, n_dt, tp_count, tp_scores, w.score_stride);
     if (int rc = check_launch("eval_pass1_kernel")) return rc;
-    eval_thresholds_kernel<<<nconf, 512, 0, st>>>(num_classes, nvalid, tp_count, tp_scores, w.score_stride, thr, nthr);
+    eval_thresholds_kernel<<<nconf, 512, 0, st>>>(num_classes, num_sets, nvalid, tp_count, tp_scores, w.score_stride, thr, nthr);
     if (int rc = check_launch("eval_thresholds_kernel")) return rc;
     eval_pass2_kernel<<<ceil_div(warps, 8), 256, 0, st>>>(cfg, n_img, nconf, gt, dt, gt_off, dt_off, dt_count, pair_off, overlaps, n_pairs,
                                                           ig_gt, n_gt, ig_dt, n_dt, thr, nthr, pr, sim);
     if (int rc = check_launch("eval_pass2_kernel")) return rc;
-    eval_finish_kernel<<<nconf, 64, 0, st>>>(num_classes, n_img, pr, sim, thr, nthr, dt, dt_off, dt_count, nconf, out);
+    eval_finish_kernel<<<nconf, 64, 0, st>>>(num_classes, num_sets, n_img, pr, sim, thr, nthr, dt, dt_off, dt_count, nconf, out);
     return check_launch("eval_finish_kernel");
+}
+
+extern "C" int prb_kitti_eval(int n_img, int num_classes, const int *classes, const double *min_overlaps, const double *gt,
+                              const int *gt_off, int n_gt, const double *dt, const int *dt_off, const int *dt_count, int n_dt,
+                              int max_det, const long long *pair_off, long long n_pairs, double *overlaps, double *out,
+                              void *workspace, size_t workspace_bytes, void *stream) {
+    return prb_kitti_eval_sets(n_img, num_classes, classes, 2, min_overlaps, -1.0, gt, gt_off, n_gt, dt, dt_off, dt_count, n_dt, max_det,
+                               pair_off, n_pairs, overlaps, out, workspace, workspace_bytes, stream);
 }
 
 extern "C" int prb_kitti_eval_add_detections(int b, int m, const float *boxes3d, const float *scores, const float *img_boxes,

@@ -1,17 +1,24 @@
 """The KITTI AP metric on the device: tools/kitti_object_eval_python (eval.py:608-678 get_official_eval_result,
-evaluate.py:14-28 evaluate, kitti_common.py:293-346 get_label_annos) with the statistics in CUDA (`prb_kitti_eval`).
+eval.py:681-740 get_coco_eval_result, evaluate.py:14-28 evaluate, kitti_common.py:190-201 filter_annos_low_score and
+:293-346 get_label_annos) with the statistics in CUDA (`prb_kitti_eval_sets`).
 
 Two ways in:
-  - from annotations or files: `get_official_eval_result(gt_annos, dt_annos, current_classes)` and
-    `evaluate(label_path, result_path, label_split_file, current_class)` return the reference's (result_str, ret_dict);
-    `evaluate_annos` returns a KittiEvalResult with the full precision / recall / orientation arrays and mAP_R40 as well;
+  - from annotations or files: `get_official_eval_result(gt_annos, dt_annos, current_classes)` returns the reference's
+    (result_str, ret_dict), `get_coco_eval_result(...)` its COCO-style string (the AP averaged over ten overlap thresholds
+    per class), and `evaluate(label_path, result_path, label_split_file, current_class, coco, score_thresh)` either of
+    them for a directory of result files; `evaluate_annos` returns a KittiEvalResult with the full precision / recall /
+    orientation arrays and mAP_R40 as well;
   - in memory: `KittiEvaluator` takes `detections_device` output batch by batch without synchronising, and `result()`
     evaluates with one device-to-host copy.  With text_rounding=True its AP equals, bit for bit, the AP of the result
     files `write_kitti_batch` writes for the same batches.
+A score threshold > 0 drops the detections scoring below it on the device before the evaluation, as the reference's
+evaluate does on the host.
 
 Differences from the reference: any number of images works (the reference needs at least 50); BEV and 3D IoU come from the
 iou3d overlap in fp32 (a few 1e-6 from numba's clipper, so a pair right at a threshold may be decided differently); the
-orientation similarity is summed in another order (differences ~1e-12).
+orientation similarity is summed in another order (differences ~1e-12).  The reference's COCO path calls
+np.linspace with the float 10.0 as the number of samples, which numpy >= 1.18 refuses; here it is ten thresholds, as the
+call evidently means.
 """
 import ctypes
 import pathlib
@@ -27,6 +34,9 @@ NAME_TO_CLASS = {v: k for k, v in CLASS_TO_NAME.items()}
 # eval.py:609-615: [overlap set, metric (bbox, bev, 3d), class]
 MIN_OVERLAPS = np.array([[[0.7, 0.5, 0.5, 0.7, 0.5]] * 3,
                          [[0.7, 0.5, 0.5, 0.7, 0.5], [0.5, 0.25, 0.25, 0.5, 0.25], [0.5, 0.25, 0.25, 0.5, 0.25]]])
+# eval.py:688-694: per class (start, stop, number) of the COCO-style overlap thresholds
+CLASS_TO_RANGE = {0: [0.5, 0.95, 10], 1: [0.25, 0.7, 10], 2: [0.25, 0.7, 10], 3: [0.5, 0.95, 10], 4: [0.25, 0.7, 10]}
+MAX_OVERLAP_SETS = 10
 N_SAMPLE_PTS = 41
 MAX_DET_PER_IMAGE = 1024
 # row of the device tables (include/pointrcnn_b200.h)
@@ -114,10 +124,35 @@ def _offsets(counts):
     return off
 
 
+def filter_annos_low_score(annos, thresh):
+    """kitti_common.filter_annos_low_score on the host: every field of each annotation at the rows scoring >= thresh, in
+    order (the device applies the same rule with score_thresh)"""
+    out = []
+    for a in annos:
+        keep = [i for i, s in enumerate(a["score"]) if s >= thresh]
+        out.append({k: v[keep] for k, v in a.items()})
+    return out
+
+
+def official_min_overlaps(classes):
+    """get_official_eval_result's two overlap sets for the classes -> (2, 3, len(classes)) float64"""
+    return np.ascontiguousarray(MIN_OVERLAPS[:, :, list(classes)], np.float64)
+
+
+def coco_min_overlaps(classes):
+    """do_coco_style_eval's ten overlap sets for the classes -> (10, 3, len(classes)) float64: np.linspace over each class's
+    range, as numpy produces it (e.g. 0.8999999999999999 for Car's 0.9)"""
+    out = np.zeros([MAX_OVERLAP_SETS, 3, len(classes)])
+    for j, c in enumerate(classes):
+        start, stop, num = CLASS_TO_RANGE[c]
+        out[:, :, j] = np.linspace(np.float64(start), np.float64(stop), int(num))[:, None]
+    return out
+
+
 # ------------------------------------------------------------------------------------------------ device
-def _launch(classes, gt, gt_off, gt_counts, dt, dt_off, dt_count, dt_caps, device):
-    """prb_kitti_eval on the current stream -> (out, overlaps) device tensors; nothing waits for the GPU.
-    gt_counts / dt_caps are host arrays (row counts, rows owned per image)."""
+def _launch(classes, min_overlaps, gt, gt_off, gt_counts, dt, dt_off, dt_count, dt_caps, device, score_thresh=-1):
+    """prb_kitti_eval_sets on the current stream -> (out, overlaps) device tensors; nothing waits for the GPU.
+    min_overlaps: (sets, 3, len(classes)); gt_counts / dt_caps are host arrays (row counts, rows owned per image)."""
     lib = C.lib()
     n_img = len(gt_counts)
     if n_img < 1:
@@ -129,18 +164,22 @@ def _launch(classes, gt, gt_off, gt_counts, dt, dt_off, dt_count, dt_caps, devic
     pair_off = _offsets(gt_counts * dt_caps)
     n_pairs = int(pair_off[-1])
     cls = np.ascontiguousarray(classes, np.int32)
-    mo = np.ascontiguousarray(MIN_OVERLAPS[:, :, classes], np.float64)
-    nconf = 18 * nc
-    ws_bytes = lib.prb_kitti_eval_workspace_bytes(n_img, n_gt, n_dt, nc)
+    mo = np.ascontiguousarray(min_overlaps, np.float64)
+    ns = mo.shape[0]
+    if mo.shape != (ns, 3, nc):
+        raise ValueError("kitti_eval: min_overlaps of shape %s for %d classes (sets, 3, classes)" % (mo.shape, nc))
+    nconf = 9 * ns * nc
+    ws_bytes = lib.prb_kitti_eval_sets_workspace_bytes(n_img, n_gt, n_dt, nc, ns)
     with torch.cuda.device(device):
         pair_dev = torch.from_numpy(pair_off).to(device, non_blocking=True)
         ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
         ov = torch.empty(max(3 * n_pairs, 1), dtype=torch.float64, device=device)
         out = torch.empty(nconf * N_SAMPLE_PTS * 8 + 1 + nconf, dtype=torch.float64, device=device)
         P = ctypes.c_void_p
-        C.check(lib.prb_kitti_eval(n_img, nc, P(cls.ctypes.data), P(mo.ctypes.data), C.ptr(gt), C.ptr(gt_off), n_gt, C.ptr(dt), C.ptr(dt_off),
-                                   C.ptr(dt_count), n_dt, max_det, C.ptr(pair_dev), ctypes.c_longlong(n_pairs), C.ptr(ov), C.ptr(out), C.ptr(ws),
-                                   ctypes.c_size_t(ws_bytes), C.stream()), "kitti_eval")
+        C.check(lib.prb_kitti_eval_sets(n_img, nc, P(cls.ctypes.data), ns, P(mo.ctypes.data), ctypes.c_double(score_thresh), C.ptr(gt),
+                                        C.ptr(gt_off), n_gt, C.ptr(dt), C.ptr(dt_off), C.ptr(dt_count), n_dt, max_det, C.ptr(pair_dev),
+                                        ctypes.c_longlong(n_pairs), C.ptr(ov), C.ptr(out), C.ptr(ws), ctypes.c_size_t(ws_bytes), C.stream()),
+                "kitti_eval")
     return out, ov[:3 * n_pairs].view(3, n_pairs)
 
 
@@ -148,16 +187,21 @@ class KittiEvalResult:
     """precision / recall / orientation: (metric (bbox, bev, 3d), class, difficulty, overlap set, 41) float64, each metric's
     array as the reference's eval_class returns it (orientation only for bbox, zero without AOS); mAP_R11 / mAP_R40:
     (metric, class, difficulty, overlap set); mAP_aos (class, difficulty, overlap set) or None; counts: (..., 41, 4)
-    tp, fp, fn, similarity; thresholds (..., 41) and num_thresholds (...)"""
+    tp, fp, fn, similarity; thresholds (..., 41) and num_thresholds (...).  min_overlaps (overlap set, metric, class).
 
-    def __init__(self, classes, out):
+    The official evaluation (the two sets of get_official_eval_result) reports its (result_str, ret_dict); a COCO-style one
+    (coco=True, the ten sets of get_coco_eval_result) reports result_str only, ret_dict is None, and mAP_coco (metric,
+    class, difficulty) / mAP_aos_coco (class, difficulty) hold the R11 mAPs averaged over the sets."""
+
+    def __init__(self, classes, out, min_overlaps=None, coco=False):
         nc = len(classes)
-        nconf = 18 * nc
-        body = out[:nconf * N_SAMPLE_PTS * 8].reshape(3, nc, 3, 2, N_SAMPLE_PTS, 8)
         self.classes = list(classes)
-        self.min_overlaps = MIN_OVERLAPS[:, :, self.classes]
+        self.min_overlaps = official_min_overlaps(self.classes) if min_overlaps is None else np.asarray(min_overlaps, np.float64)
+        ns = self.min_overlaps.shape[0]
+        nconf = 9 * ns * nc
+        body = out[:nconf * N_SAMPLE_PTS * 8].reshape(3, nc, 3, ns, N_SAMPLE_PTS, 8)
         self.compute_aos = bool(out[nconf * N_SAMPLE_PTS * 8] != 0)
-        self.num_thresholds = out[nconf * N_SAMPLE_PTS * 8 + 1:].reshape(3, nc, 3, 2).astype(np.int64)
+        self.num_thresholds = out[nconf * N_SAMPLE_PTS * 8 + 1:].reshape(3, nc, 3, ns).astype(np.int64)
         self.counts = body[..., 0:4].copy()
         self.thresholds = body[..., 7].copy()
         self.recall = body[..., 4].copy()
@@ -168,7 +212,14 @@ class KittiEvalResult:
         self.mAP_R11 = _map_r11(self.precision)
         self.mAP_R40 = _map_r40(self.precision)
         self.mAP_aos = _map_r11(self.orientation[0]) if self.compute_aos else None
-        self.result_str, self.ret_dict = self._report()
+        self.coco = coco
+        if coco:
+            # do_coco_style_eval: each (class, difficulty, set) array of do_eval averaged over the sets
+            self.mAP_coco = np.stack([np.ascontiguousarray(m).mean(-1) for m in self.mAP_R11])
+            self.mAP_aos_coco = np.ascontiguousarray(self.mAP_aos).mean(-1) if self.compute_aos else None
+            self.result_str, self.ret_dict = self._coco_report(), None
+        else:
+            self.result_str, self.ret_dict = self._report()
 
     def _report(self):
         bbox, bev, d3 = self.mAP_R11
@@ -187,6 +238,21 @@ class KittiEvalResult:
             for d, diff in enumerate(("easy", "moderate", "hard")):
                 ret["Car_%s_%s" % (tag, diff)] = m[0, d, 0]
         return "".join(s + "\n" for s in lines), ret
+
+    def _coco_report(self):
+        bbox, bev, d3 = self.mAP_coco
+        lines = []
+        for j, c in enumerate(self.classes):
+            # eval.py:725-726: "start:step:stop", the step computed in float64 from the range
+            o_range = np.array(CLASS_TO_RANGE[c])[[0, 2, 1]]
+            o_range[1] = (o_range[2] - o_range[0]) / (o_range[1] - 1)
+            lines.append("{} coco AP@{:.2f}:{:.2f}:{:.2f}:".format(CLASS_TO_NAME[c], *o_range))
+            for tag, m in (("bbox AP", bbox), ("bev  AP", bev), ("3d   AP", d3)):
+                lines.append(f"{tag}:{m[j, 0]:.2f}, {m[j, 1]:.2f}, {m[j, 2]:.2f}")
+            if self.compute_aos:
+                a = self.mAP_aos_coco
+                lines.append(f"aos  AP:{a[j, 0]:.2f}, {a[j, 1]:.2f}, {a[j, 2]:.2f}")
+        return "".join(s + "\n" for s in lines)
 
 
 def _map_r11(prec):
@@ -209,19 +275,32 @@ def _device(device):
     return torch.device(device) if device is not None else torch.device("cuda", torch.cuda.current_device())
 
 
-def evaluate_annos(gt_annos, dt_annos, current_classes, device=None, return_overlaps=False):
+def _sets(classes, min_overlaps, coco):
+    """-> (min_overlaps (sets, 3, classes), coco flag) of an evaluation"""
+    if coco and min_overlaps is not None:
+        raise ValueError("kitti_eval: coco=True fixes the overlap sets; do not pass min_overlaps as well")
+    if coco:
+        return coco_min_overlaps(classes), True
+    return (official_min_overlaps(classes) if min_overlaps is None else np.asarray(min_overlaps, np.float64)), False
+
+
+def evaluate_annos(gt_annos, dt_annos, current_classes, device=None, return_overlaps=False, min_overlaps=None, score_thresh=-1,
+                   coco=False):
     """the whole evaluation of two annotation lists on the device -> KittiEvalResult (and the (3, pairs) overlap matrices,
-    (dt x gt) row-major per image, when asked)"""
+    (dt x gt) row-major per image, of the detections evaluated, when asked).  min_overlaps (sets, 3, classes): the overlap
+    sets, default the official two; coco=True: the ten COCO-style sets and report.  score_thresh > 0: only the
+    detections scoring >= score_thresh count (filter_annos_low_score, applied on the device)."""
     assert len(gt_annos) == len(dt_annos)
     classes = class_list(current_classes)
+    mo, coco = _sets(classes, min_overlaps, coco)
     dev = _device(device)
     gt, gt_counts = pack_annos(gt_annos)
     dt, dt_counts = pack_annos(dt_annos)
     up = lambda a, dt_=torch.float64: torch.from_numpy(np.ascontiguousarray(a)).to(device=dev, dtype=dt_)
     dt_count = up(dt_counts, torch.int32)
-    out, ov = _launch(classes, up(gt), up(_offsets(gt_counts), torch.int32), gt_counts, up(dt), up(_offsets(dt_counts), torch.int32), dt_count,
-                      dt_counts, dev)
-    res = KittiEvalResult(classes, out.cpu().numpy())
+    out, ov = _launch(classes, mo, up(gt), up(_offsets(gt_counts), torch.int32), gt_counts, up(dt), up(_offsets(dt_counts), torch.int32),
+                      dt_count, dt_counts, dev, score_thresh)
+    res = KittiEvalResult(classes, out.cpu().numpy(), mo, coco)
     return (res, ov.cpu().numpy()) if return_overlaps else res
 
 
@@ -231,13 +310,22 @@ def get_official_eval_result(gt_annos, dt_annos, current_classes):
     return r.result_str, r.ret_dict
 
 
-def evaluate(label_path, result_path, label_split_file, current_class=0):
-    """evaluate.py:14-28: every result file of result_path against the labels of the split's image ids"""
+def get_coco_eval_result(gt_annos, dt_annos, current_classes):
+    """eval.py:681-740 -> the same result string: per class the bbox / bev / 3d (and aos) R11 AP averaged over ten
+    overlap thresholds"""
+    return evaluate_annos(gt_annos, dt_annos, current_classes, coco=True).result_str
+
+
+def evaluate(label_path, result_path, label_split_file, current_class=0, coco=False, score_thresh=-1):
+    """evaluate.py:14-28: every result file of result_path against the labels of the split's image ids -> the COCO-style
+    result string (coco=True) or the official (result_str, ret_dict); score_thresh > 0 drops the detections scoring below
+    it first"""
     dt_annos = read_label_annos(result_path)
     with open(label_split_file, "r") as f:
         ids = [int(line) for line in f.readlines()]
     gt_annos = read_label_annos(label_path, ids)
-    return get_official_eval_result(gt_annos, dt_annos, current_class)
+    r = evaluate_annos(gt_annos, dt_annos, current_class, score_thresh=score_thresh, coco=coco)
+    return r.result_str if coco else (r.result_str, r.ret_dict)
 
 
 # ------------------------------------------------------------------------------------------------ in memory
@@ -304,10 +392,18 @@ class KittiEvaluator:
                                                       C.ptr(slot), 1 if text_rounding else 0, class_code(classes), C.ptr(self._dt),
                                                       C.ptr(self._dt_off), C.ptr(self._dt_count), C.stream()), "kitti_eval_add_detections")
 
-    def result(self, return_overlaps=False):
-        """evaluate everything added so far: the device stages and ONE device-to-host copy -> KittiEvalResult"""
+    def _evaluate_on_device(self, coco=False, score_thresh=-1):
+        """the device stages on the current stream -> (min_overlaps, coco, out, overlaps), out and overlaps on the device"""
+        mo, coco = _sets(self.classes, None, coco)
         caps = np.full(self.n_img, self._cap, np.int64)
-        out, ov = _launch(self.classes, self._gt, self._gt_off, self._gt_counts, self._dt.view(-1, COLS), self._dt_off, self._dt_count,
-                          caps, self.device)
-        res = KittiEvalResult(self.classes, out.cpu().numpy())
+        out, ov = _launch(self.classes, mo, self._gt, self._gt_off, self._gt_counts, self._dt.view(-1, COLS), self._dt_off, self._dt_count,
+                          caps, self.device, score_thresh)
+        return mo, coco, out, ov
+
+    def result(self, return_overlaps=False, coco=False, score_thresh=-1):
+        """evaluate everything added so far: the device stages and ONE device-to-host copy -> KittiEvalResult.
+        coco=True: the COCO-style evaluation; score_thresh > 0: only the detections scoring >= score_thresh, filtered on
+        the device"""
+        mo, coco, out, ov = self._evaluate_on_device(coco, score_thresh)
+        res = KittiEvalResult(self.classes, out.cpu().numpy(), mo, coco)
         return (res, ov) if return_overlaps else res

@@ -1,12 +1,16 @@
 """Time the device KITTI AP evaluation on a synthetic split the size of KITTI val.
 
-    python scripts/bench_kitti_eval.py [--images 3769] [--repeats 5] [--oracle-images 100] [--out result.json]
+    python scripts/bench_kitti_eval.py [--images 3769] [--repeats 5] [--oracle-images 100] [--coco] [--out result.json]
 
 The split: 3769 images with about as many label rows per image as KITTI's (Car / Van / Pedestrian / Cyclist / DontCare)
 and about 30 detections per image, added batch by batch (8 scenes per batch, the evaluation loop's batch) through
 KittiEvaluator.add_batch.  Reports the median wall time of result() (device stages + the one device-to-host copy), the
 add_batch time per batch, the library's launch count per result(), the card's name and power limit, and for context the
 numpy oracle's time on a subset of the images (CPU, not comparable to the GPU number).
+
+--coco also times result() for the ten COCO-style overlap sets (coco=True) and both evaluations with the device score
+filter (score_thresh=--score-thresh), each with its launch count: the overlaps are computed once whatever the number of
+sets, and the statistics stages scale with the number of configs (9 x sets x classes).
 """
 import argparse
 import json
@@ -53,6 +57,8 @@ def main():
     ap.add_argument("--images", type=int, default=3769)
     ap.add_argument("--repeats", type=int, default=5)
     ap.add_argument("--oracle-images", type=int, default=100)
+    ap.add_argument("--coco", action="store_true")
+    ap.add_argument("--score-thresh", type=float, default=0.5)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
     import torch
@@ -86,14 +92,20 @@ def main():
         fill(ev)
         torch.cuda.synchronize()
         add_ms.append((time.perf_counter() - t0) * 1e3 / ((a.images + B - 1) // B))
-    res_ms, launches = [], []
-    for _ in range(a.repeats):
-        torch.cuda.synchronize()
-        l0 = C.launch_count()
-        t0 = time.perf_counter()
-        r = ev.result()                           # ends in the device-to-host copy
-        res_ms.append((time.perf_counter() - t0) * 1e3)
-        launches.append(C.launch_count() - l0)
+
+    def timed(**kw):
+        ev.result(**kw)                           # warm-up of this variant
+        ms, launches = [], []
+        for _ in range(a.repeats):
+            torch.cuda.synchronize()
+            l0 = C.launch_count()
+            t0 = time.perf_counter()
+            r = ev.result(**kw)                   # ends in the device-to-host copy
+            ms.append((time.perf_counter() - t0) * 1e3)
+            launches.append(C.launch_count() - l0)
+        return r, ms, launches
+
+    r, res_ms, launches = timed()
     n_dt = int(ev._dt_count.sum().item())
     sub = min(a.oracle_images, a.images)
     # the oracle evaluates the same detections, read back from the device table
@@ -113,6 +125,16 @@ def main():
                add_batch_ms_per_batch_of_8=float(np.median(add_ms)), launches_per_result=launches[0],
                cpu_oracle_s=round(oracle_s, 2), cpu_oracle_images=sub, gpu=torch.cuda.get_device_name(0),
                nvidia_smi=smi.stdout.strip(), car_moderate_3d_ap=float(r.ret_dict["Car_3d_moderate"]))
+    if a.coco:
+        variants = {"coco": dict(coco=True), "official_score_thresh": dict(score_thresh=a.score_thresh),
+                    "coco_score_thresh": dict(coco=True, score_thresh=a.score_thresh)}
+        for name, kw in variants.items():
+            rv, ms, ln = timed(**kw)
+            out[name] = dict(result_ms_median=float(np.median(ms)), result_ms=[round(x, 3) for x in ms], launches_per_result=ln[0],
+                             car_moderate_3d_ap=float(rv.mAP_coco[2, 0, 1] if rv.coco else rv.ret_dict["Car_3d_moderate"]))
+        out["score_thresh"] = a.score_thresh
+        out["detections_above_score_thresh"] = int(((ev._dt[..., 14] >= a.score_thresh) &
+                                                    (torch.arange(ev._cap, device=dev)[None] < ev._dt_count[:, None])).sum().item())
     line = json.dumps(out)
     print(line)
     if a.out:
