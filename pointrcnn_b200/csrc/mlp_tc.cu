@@ -8,12 +8,14 @@
 // The reference materialises every (B,C,npoint,nsample) tensor in HBM between ~10 library kernels per
 // scale; here a 64-row tile never leaves the SM between its gather and its pooled output.
 //
-// Two kernels run a launch (one fused segment of a chain); they share the tile stages -- the row lookup, the layer-0
-// gather, the inner-layer epilogue and the final epilogues -- issue the same MMA sequence per K chunk, and give
+// Two kernels run a fused launch (layers of a chain at most 256 wide); they share the tile stages -- the row lookup, the
+// layer-0 gather, the inner-layer epilogue and the final epilogues -- issue the same MMA sequence per K chunk, and give
 // bit-identical outputs.  launch_chain picks one by shape:
 //   resident   every layer <= 128 wide; input / output one of SA -> max-pool, FP -> FP, rows -> rows; the packed weight
 //              image at most half of a CTA's shared memory; prb_options.mlp_resident != 0 (the default).
-//   streaming  every other launch.
+//   streaming  every other fused launch.
+// A layer wider than 256 runs alone on a third kernel, mlp_wide_kernel, as a dense GEMM over rows in global memory
+// (see there), with the same K order, k8 steps and epilogues.
 //
 // Resident kernel (mlp_resident_kernel; persistent CTAs of nwg warpgroups, no producer warp): at CTA start one thread
 // loads the segment's whole packed image with cp.async.bulk on one mbarrier, which every warpgroup waits on once.  Each
@@ -47,10 +49,12 @@
 // weight traffic halves.  The 128 accumulators per thread need more than the 168 registers 9 warps allow, so there the
 // producer is a whole warpgroup that hands its registers to the MMA warpgroups (setmaxnreg).  launch_chain holds the
 // per-launch timings the rule follows.
-// Chains whose activation buffer and weight stages do not fit in shared memory are split into several launches by
-// the host wrapper (rows materialised in between).
+// Chains with a layer wider than 256, or whose activation buffer and weight stages do not fit in shared memory, are split
+// into several launches by the host wrapper (rows materialised in between).
 // Precision: operands are rounded to TF32 (cvt.rn), products accumulate in fp32 -- the same contract as the
 // reference's cuDNN convolutions under torch's default allow_tf32=True (SURVEY.md 8c).
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <string.h>
 
 #include <vector>
@@ -748,6 +752,139 @@ __global__ void __launch_bounds__(NWG * 128, MINB) mlp_resident_kernel(const Cha
     if (tid == 0 && !w_ready) mbar_wait(s2u(&w_full), 0);   // no CTA exits with its weight copy in flight
 }
 
+// ------------------------------------------------------------------------------------------------ wide-layer kernel
+// One layer wider than WN_WIDE over rows already in global memory (row-major, tf32, K padded to a multiple of KC): the
+// layers of a chain wider than 256 run here, each as its own launch.  A CTA tile is WM_WIDE = 128 rows x 32 NS output
+// columns, where the layer's np columns are cut into two blocks of equal width (32 NS <= WN_WIDE = 256; where np / 32 is
+// odd, the second block's last 32 columns lie past the layer and are computed from whatever the B stage holds there and
+// never stored).  The persistent CTAs walk (row block, column block) tiles, the column blocks of a row block one after
+// another so its A rows are still in L2 for the second.  Warpgroup 2's one thread fills a ring of WIDE_NB stages, each one
+// K chunk of A (a TMA tensor-map load of 128 rows x 32 floats, SWIZZLE_128B, rows past the end zero) and of B (the
+// column block's slab of the packed image, at most 32 KB, one bulk copy); warpgroups 0 and 1 take rows 0-63 and 64-127
+// of the tile, one m64n(32 NS)k8 per K=8 step into 16 NS accumulators, and run the final epilogue while the producer
+// fills the ring with the next tile's chunks.  Per K chunk a 128 x 256 tile moves 48 KB for 2.1 MFLOP.
+// The K order and the epilogues are the fused kernels'.  Every chunk runs all four K=8 steps, with the MMA width fixed
+// at compile time: a runtime choice of either makes ptxas serialise the wgmma (C7520).  The fused kernels skip the K=8
+// steps past the end of a layer-0 segment; here they multiply the zeros of the gathered rows by the zeros of the packed
+// image, and adding those +0 products leaves every fp32 sum unchanged (only an all-zero sum of -0 products would become
+// +0).
+constexpr int WM_WIDE = 2 * TM, WN_WIDE = 256, WIDE_NB = 4;
+constexpr int WIDE_A_BYTES = WM_WIDE * KC * 4, WIDE_B_BYTES = WN_WIDE * KC * 4;
+constexpr int WIDE_STAGE_BYTES = WIDE_A_BYTES + WIDE_B_BYTES;
+constexpr int WIDE_THREADS = 3 * 128;
+
+// 2D TMA load of the box at (column c0, row r0) of the tensor map into shared memory, completing on the mbarrier
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap *map, int c0, int r0, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(r0), "r"(bar)
+                 : "memory");
+}
+
+template <int NS>
+__global__ void __launch_bounds__(WIDE_THREADS, 1) mlp_wide_kernel(const __grid_constant__ CUtensorMap amap, const ChainParams p) {
+    static_assert(NS >= 1 && NS <= NSUB_MAX, "mlp_wide_kernel: one m64n(32 NS)k8 per warpgroup and K=8 step");
+    constexpr int BW = 32 * NS;   // columns per block
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ uint64_t full[WIDE_NB], empty[WIDE_NB];
+    uint8_t *ring = smem_raw + ((1024u - (s2u(smem_raw) & 1023u)) & 1023u);
+    // [ring: WIDE_NB x (A | B) | per-warp pool maxima of both warpgroups | scale | shift | pool carry]
+    const int np = p.np[0], nch = p.nchunks[0];
+    float *red_all = reinterpret_cast<float *>(ring + (size_t)WIDE_NB * WIDE_STAGE_BYTES);
+    float *s_scale = red_all + 2 * 4 * RED_STRIDE;
+    float *s_shift = s_scale + np;
+    float *s_carry = s_shift + np;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    if (tid == 0) {
+        for (int i = 0; i < WIDE_NB; ++i) { mbar_init(s2u(&full[i]), 1); mbar_init(s2u(&empty[i]), 8); }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    load_scale_shift(p, s_scale, s_shift, tid, WIDE_THREADS);
+    __syncthreads();
+    const int ncb = (np + BW - 1) / BW;
+    const int num_tiles = (int)((p.total_rows + WM_WIDE - 1) / WM_WIDE) * ncb;
+
+    const int wg = __shfl_sync(0xffffffffu, warp >> 2, 0);
+    if (wg == 2) {
+        // ===================================================== producer: A and B of every K chunk of every tile
+        setmaxnreg_dec<PRODUCER_REGS>();
+        if (tid == 2 * 128) {
+            RingPos rb = {0, 0};
+            for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+                const int rblk = tile / ncb, col0 = (tile - rblk * ncb) * BW;
+                const uint32_t b_bytes = (uint32_t)min(BW, np - col0) * KC * 4;
+                for (int kc = 0; kc < nch; ++kc) {
+                    mbar_wait(s2u(&empty[rb.stage]), rb.phase ^ 1);
+                    const uint32_t stage = s2u(ring + (size_t)rb.stage * WIDE_STAGE_BYTES), bar = s2u(&full[rb.stage]);
+                    mbar_expect_tx(bar, WIDE_A_BYTES + b_bytes);
+                    tma_load_2d(stage, &amap, kc * KC, rblk * WM_WIDE, bar);
+                    bulk_g2s(stage + WIDE_A_BYTES, p.w[0] + ((size_t)kc * np + col0) * KC, b_bytes, bar);
+                    rb.advance(WIDE_NB);
+                }
+            }
+        }
+        return;
+    }
+
+    // ===================================================== MMA / epilogue warpgroups: rows 64 wg .. 64 wg + 63 of a tile
+    setmaxnreg_inc<MMA_REGS>();
+    const int wq = warp & 3, g = lane >> 2, t4 = lane & 3, tw = tid & 127;
+    float *red = red_all + wg * 4 * RED_STRIDE;
+    // an SA centre of 128 rows spans both warpgroups: warpgroup 0's pass leaves its maxima in s_carry for warpgroup 1's
+    const bool carry = p.mode_out == OUT_SA_MAX && p.ns > TM;
+    RingPos rb = {0, 0};
+    float acc[1][16 * NS];
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const int rblk = tile / ncb, col0 = (tile - rblk * ncb) * BW;
+        const int nsub = min(BW, np - col0) >> 5;   // the block's columns inside the layer
+        int prev_stage = -1;
+        for (int kc = 0; kc < nch; ++kc) {
+            mbar_wait(s2u(&full[rb.stage]), rb.phase);
+            const uint32_t stage = s2u(ring + (size_t)rb.stage * WIDE_STAGE_BYTES);
+            const uint64_t adesc[1] = {make_desc(stage + (uint32_t)wg * A_STAGE_BYTES)};
+            wgmma_fence();
+            mma_steps<NS, KC / 8, NS, 1>(acc, adesc, make_desc(stage + WIDE_A_BYTES), kc > 0 ? 1u : 0u);
+            wgmma_commit();
+            wgmma_wait<1>();     // the previous chunk's MMAs are done: release its stage
+            if (prev_stage >= 0 && lane == 0) mbar_arrive(s2u(&empty[prev_stage]));
+            prev_stage = (int)rb.stage;
+            rb.advance(WIDE_NB);
+        }
+        wgmma_wait<0>();
+        reg_fence(acc[0]);
+        if (lane == 0) mbar_arrive(s2u(&empty[prev_stage]));
+        if (p.mode_out == OUT_SA_MAX) {
+            if (carry && wg == 1) bar_mma();   // warpgroup 0's partial maxima are in s_carry
+            bar_wg_id(2 + wg);                 // every warp of the warpgroup is done with the previous tile's pool maxima
+        }
+        final_epilogue<NS>(p, acc[0], nsub, col0, wq, g, t4, tw, 2 * rblk + wg, s_scale, s_shift, red, s_carry, 2 + wg);
+        if (carry) {
+            if (wg == 0) bar_mma();
+            bar_mma();   // warpgroup 1 has read s_carry before warpgroup 0 writes the next tile's
+        }
+    }
+}
+
+// Layer 0's A operand of a chain whose first layer runs on the wide kernel: K chunk blockIdx.y of 64-row tile blockIdx.x,
+// gathered exactly as the fused kernels gather it into their A slots (tf32, padded segment order), written row-major
+// with `pitch` floats per row.  The columns past a segment's last K=8 step are written as zeros: the wide kernel runs
+// those steps, and their products must be +0.
+__global__ void __launch_bounds__(128) mlp_gather_kernel(const ChainParams p, float *rows, int pitch) {
+    __shared__ __align__(128) uint8_t A[A_STAGE_BYTES];
+    __shared__ TileRows M;
+    const int tile = blockIdx.x, kc = blockIdx.y, t = threadIdx.x;
+    load_tile_rows(p, tile, t, M);
+    __syncthreads();
+    const int ksteps = gather_chunk<128>(p, tile, kc, t, M, A);
+    __syncthreads();
+    for (int i = t; i < TM * 8; i += 128) {
+        const int r = i >> 3, j = i & 7;
+        const long R = (long)tile * TM + r;
+        if (R >= p.total_rows) continue;
+        const float4 v = j < 2 * ksteps ? *reinterpret_cast<const float4 *>(A + swz(r, j)) : make_float4(0.f, 0.f, 0.f, 0.f);
+        *reinterpret_cast<float4 *>(rows + (size_t)R * pitch + kc * KC + 4 * j) = v;
+    }
+}
+
 // ------------------------------------------------------------------------------------------------ host side
 static inline int round_up(int a, int b) { return (a + b - 1) / b * b; }
 
@@ -1007,10 +1144,68 @@ static int launch_chain(ChainParams &p, cudaStream_t st) {
     };
     // registers without spills: <2,2,1> 96 (two CTAs per SM), <4,1,1> 152; <4,1,2> 168 at launch, the MMA warpgroups
     // raised to 232 by setmaxnreg
+    PRB_REQUIRE(ns_max <= 4, "mlp: a fused launch of a layer %d wide (wider than %d runs on the wide kernel)", 64 * ns_max, WN_WIDE);
     if (T == 2) return go(mlp_chain_kernel<4, 1, 2>, chain_threads(4, 2));
     if (ns_max <= 2) return go(mlp_chain_kernel<2, 2, 1>, chain_threads(2, 1));
-    if (ns_max <= 4) return go(mlp_chain_kernel<4, 1, 1>, chain_threads(4, 1));
-    return go(mlp_chain_kernel<8, 1, 1>, chain_threads(8, 1));
+    return go(mlp_chain_kernel<4, 1, 1>, chain_threads(4, 1));
+}
+
+// cuTensorMapEncodeTiled from the driver the runtime uses (the library links only the runtime)
+static PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
+    static const PFN_cuTensorMapEncodeTiled_v12000 fn = [] {
+        void *f = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &f, 12000, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            f = nullptr;
+        return reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
+    }();
+    return fn;
+}
+
+// one layer wider than WN_WIDE (p.num_layers = 1) over a_rows: total_rows rows of a_pitch floats (a multiple of KC, the
+// layer's padded K), 16-byte aligned
+static int launch_wide(ChainParams &p, const float *a_rows, int a_pitch, cudaStream_t st) {
+    if (p.total_rows == 0) return 0;
+    PRB_REQUIRE(a_pitch % KC == 0 && a_pitch >= p.nchunks[0] * KC && (reinterpret_cast<uintptr_t>(a_rows) & 15) == 0,
+                "mlp_wide: rows of %d floats at %p cannot feed a layer of %d K chunks", a_pitch, (const void *)a_rows, p.nchunks[0]);
+    const PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
+    PRB_REQUIRE(encode, "mlp_wide: cuTensorMapEncodeTiled is not available from the driver");
+    CUtensorMap amap;
+    const cuuint64_t dims[2] = {(cuuint64_t)a_pitch, (cuuint64_t)p.total_rows};
+    const cuuint64_t strides[1] = {(cuuint64_t)a_pitch * sizeof(float)};
+    const cuuint32_t box[2] = {KC, WM_WIDE}, estr[2] = {1, 1};
+    const CUresult r = encode(&amap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float *>(a_rows), dims, strides, box, estr,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    PRB_REQUIRE(r == CUDA_SUCCESS, "mlp_wide: cuTensorMapEncodeTiled failed (%d)", (int)r);
+    const int np = p.np[0];
+    const size_t smem = 1024 /*alignment slack*/ + (size_t)WIDE_NB * WIDE_STAGE_BYTES + (size_t)(2 * 4 * RED_STRIDE + 3 * np) * sizeof(float);
+    // two column blocks of equal width (np <= MAX_NP = 2 WN_WIDE): a 384-wide layer as 2 x 192, not 256 + 128
+    const int ns = ((np >> 5) + 1) >> 1;
+    const long tiles = (p.total_rows + WM_WIDE - 1) / WM_WIDE * ((np + 32 * ns - 1) / (32 * ns));
+    int sms = num_sms();
+    if (const int v = opts().mlp_sms; v >= 1 && v < sms) sms = v;
+    auto go = [&](auto kern) -> int {
+        PRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<(int)(tiles < sms ? tiles : sms), WIDE_THREADS, smem, st>>>(amap, p);
+        return check_launch("mlp_wide_kernel");
+    };
+    static_assert(MAX_NP == 2 * WN_WIDE, "mlp_wide: two column blocks cover every layer");
+    switch (ns) {   // np in (WN_WIDE, MAX_NP]: 5 .. 8 subtiles per block
+        case 5: return go(mlp_wide_kernel<5>);
+        case 6: return go(mlp_wide_kernel<6>);
+        case 7: return go(mlp_wide_kernel<7>);
+        default: return go(mlp_wide_kernel<8>);
+    }
+}
+
+// layer 0's A operand as rows of `pitch` floats (the padded K of layer 0) for a wide first layer
+static int launch_gather(const ChainParams &p, float *rows, int pitch, cudaStream_t st) {
+    const long tiles = (p.total_rows + TM - 1) / TM;
+    if (tiles == 0) return 0;
+    mlp_gather_kernel<<<dim3((unsigned)tiles, (unsigned)p.nchunks[0]), 128, 0, st>>>(p, rows, pitch);
+    return check_launch("mlp_gather_kernel");
 }
 
 // can layers [l0, l1) run as one launch: the activations of the widest inner layer and two weight stages in shared memory
@@ -1027,20 +1222,35 @@ struct ChainIO {
     long rows;
 };
 
+// The launches of a chain: every layer wider than WN_WIDE alone on the wide kernel, the layers between them fused in as
+// few launches as shared memory allows (each the longest run from its first layer that fits).  Returns the end of the
+// launch that starts at layer l0.
+static int segment_end(const LayerGeom *g, int L, int l0) {
+    if (g[l0].np > WN_WIDE) return l0 + 1;
+    int l1 = l0 + 1;
+    while (l1 < L && g[l1].np <= WN_WIDE) ++l1;
+    while (l1 > l0 + 1 && !fits(g, l0, l1)) --l1;
+    return l1;
+}
+
+// Two ping-pong row buffers, each of the widest rows a launch of the chain reads from global memory: the output of
+// every launch but the last, and layer 0's gathered operand where the first layer is wide.  0 when the chain is one
+// fused launch.
 static size_t chain_workspace_bytes(long rows, int L, int kind, int c_in, int split, const int *c_out) {
     PackSegs ps;
     default_segs(kind, c_in, split, &ps);
     LayerGeom g[MAX_LAYERS];
     chain_geometry(L, ps.nseg, ps.width, c_out, g, nullptr);
-    // worst case: two ping-pong row buffers of the widest padded layer
-    int wmax = 0;
-    for (int l = 0; l < L; ++l) wmax = g[l].np > wmax ? g[l].np : wmax;
-    const bool split_needed = !fits(g, 0, L);
+    int wmax = g[0].np > WN_WIDE ? g[0].k_chunks * KC : 0;
+    for (int l0 = 0, l1; l0 < L; l0 = l1) {
+        l1 = segment_end(g, L, l0);
+        if (l1 < L && g[l1 - 1].np > wmax) wmax = g[l1 - 1].np;
+    }
     const size_t rows_pad = (size_t)((rows + TM - 1) / TM * TM);
-    return split_needed ? 2 * (rows_pad * wmax * sizeof(float) + 256) : 256;
+    return wmax ? 2 * (rows_pad * wmax * sizeof(float) + 256) : 256;
 }
 
-// run the whole chain, splitting where shared memory cannot hold a segment's activations and weight stages
+// run the whole chain as the launches segment_end picks, materialising rows between them
 static int run_chain(const ChainIO &io, const prb_mlp_desc *mlp, void *workspace, size_t workspace_bytes, cudaStream_t st) {
     const int L = mlp->num_layers;
     PRB_REQUIRE(io.rows < 0x7fffff00L, "mlp: %ld rows exceed the 2^31 row limit", io.rows);
@@ -1055,13 +1265,20 @@ static int run_chain(const ChainIO &io, const prb_mlp_desc *mlp, void *workspace
     for (int l = 0; l < L; ++l) { soff[l] = so; so += (size_t)g[l].np; }
 
     const long rows_pad = (io.rows + TM - 1) / TM * TM;
-    int l0 = 0;
+    // the next ping-pong buffer for rows of `width` floats
+    int pingpong = 0;
+    auto row_buffer = [&](int width, float **dst) -> int {
+        const size_t buf_bytes = (size_t)rows_pad * width * sizeof(float);
+        PRB_REQUIRE(workspace && workspace_bytes >= 2 * buf_bytes, "mlp: workspace too small (%zu < %zu)", workspace_bytes, 2 * buf_bytes);
+        *dst = (float *)((char *)workspace + (pingpong ? workspace_bytes / 2 / 256 * 256 : 0));
+        pingpong ^= 1;
+        return 0;
+    };
     const float *cur_rows = nullptr;
     int cur_pitch = 0;
-    int pingpong = 0;
-    while (l0 < L) {
-        int l1 = L;
-        while (l1 > l0 + 1 && !fits(g, l0, l1)) --l1;
+    for (int l0 = 0, l1; l0 < L; l0 = l1) {
+        l1 = segment_end(g, L, l0);
+        const bool wide = g[l0].np > WN_WIDE;
         ChainParams p = io.base;
         p.unit_scale = mlp->scale ? 0 : 1;
         p.linear_last = (l1 == L && (mlp->flags & 1)) ? 1 : 0;
@@ -1075,38 +1292,40 @@ static int run_chain(const ChainIO &io, const prb_mlp_desc *mlp, void *workspace
             p.scale[i] = mlp->scale ? mlp->scale + soff[l] : nullptr;
             p.shift[i] = mlp->shift + soff[l];
         }
-        if (l0 > 0) {  // continue from materialised rows
+        if (l0 == 0) {
+            p.nseg = ps.nseg;
+            for (int s = 0; s < ps.nseg; ++s) { p.seg_chunks[s] = round_up(ps.width[s], KC) / KC; p.seg_width[s] = ps.width[s]; }
+            if (wide) {   // gather layer 0's operand into rows first
+                float *dst = nullptr;
+                if (int rc = row_buffer(g[0].k_chunks * KC, &dst)) return rc;
+                if (int rc = launch_gather(p, dst, g[0].k_chunks * KC, st)) return rc;
+                cur_rows = dst;
+                cur_pitch = g[0].k_chunks * KC;
+            }
+        } else {  // continue from materialised rows
             p.mode_in = IN_DIRECT;
             p.x_rows = cur_rows;
             p.x_pitch = cur_pitch;
             p.x2_rows = nullptr;
             p.nseg = 1; p.seg_chunks[0] = g[l0].k_chunks; p.seg_width[0] = cur_pitch;
-        } else {
-            p.nseg = ps.nseg;
-            for (int s = 0; s < ps.nseg; ++s) { p.seg_chunks[s] = round_up(ps.width[s], KC) / KC; p.seg_width[s] = ps.width[s]; }
         }
-        if (l1 < L) {  // materialise this segment's activations as rows
-            size_t buf_bytes = (size_t)rows_pad * g[l1 - 1].np * sizeof(float);
-            PRB_REQUIRE(workspace && workspace_bytes >= 2 * buf_bytes, "mlp: workspace too small (%zu < %zu)", workspace_bytes, 2 * buf_bytes);
-            float *dst = (float *)((char *)workspace + (pingpong ? workspace_bytes / 2 / 256 * 256 : 0));
+        float *dst = nullptr;
+        if (l1 < L) {  // materialise this launch's activations as rows
+            if (int rc = row_buffer(g[l1 - 1].np, &dst)) return rc;
             p.mode_out = OUT_ROWS;
             p.round_out = 1;
             p.out_pm = nullptr;
             p.out = dst;
             p.out_pitch = g[l1 - 1].np;
             p.c_last = g[l1 - 1].np;
-            int rc = launch_chain(p, st);
-            if (rc) return rc;
-            cur_rows = dst;
-            cur_pitch = g[l1 - 1].np;
-            pingpong ^= 1;
         } else {
             // row-major output: write the padded width so the padding channels are defined (zero)
             p.c_last = p.mode_out == OUT_ROWS ? g[L - 1].np : mlp->c_out[L - 1];
-            int rc = launch_chain(p, st);
-            if (rc) return rc;
         }
-        l0 = l1;
+        const int rc = wide ? launch_wide(p, cur_rows, cur_pitch, st) : launch_chain(p, st);
+        if (rc) return rc;
+        cur_rows = dst;
+        cur_pitch = g[l1 - 1].np;
     }
     return 0;
 }

@@ -7,6 +7,10 @@ under `prb_options.mlp_resident = 1` (resident where the chain fits, the default
 settings alternated `--reps` times after a warm-up, `--iters` back-to-back launches per CUDA-event window.  Per launch it
 prints the median ms of each setting, TF/s over padded MACs (rows x K padded to 32 x N padded to 32, summed over layers)
 and the L2 weight traffic the streaming kernel needs (every 64-row tile reads the whole packed image).
+Then each chain call runs once more under torch.profiler, and every kernel it launches is listed with its device time:
+the gather, the fused segments and each layer wider than 256 on mlp_wide_kernel, which gets its TF/s over padded MACs
+and the L2 bytes its tiles read (per 128-row tile and column block, every K chunk of A, 16 KB, and of the column
+block's weights).
 Random weights, synthetic scenes: the work is that of a real batch.
 """
 import argparse
@@ -28,6 +32,7 @@ from pointrcnn_b200 import _cabi as C  # noqa: E402
 from pointrcnn_b200.backbone import Pointnet2MSG  # noqa: E402
 
 TM, KC = 64, 32
+WM, WN = 128, 256     # mlp_wide_kernel's tile rows and widest column block
 
 
 def _ru(a, b):
@@ -91,7 +96,34 @@ def main():
                  resident_spread_ms=max(ms[1]) - min(ms[1]), stream_spread_ms=max(ms[0]) - min(ms[0]))
         r["resident_tfs"] = 2 * macs / (r["resident_ms"] * 1e-3) / 1e12
         r["stream_tfs"] = 2 * macs / (r["stream_ms"] * 1e-3) / 1e12
+        r["launches"] = launches(launch, rows, ks, ns)
         results.append(r)
+
+    def launches(launch, rows, ks, ns):
+        """(kernel, ms per call, and for a wide layer TF/s and L2 MB) of every kernel one call launches, in order"""
+        torch.cuda.synchronize()
+        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+            for _ in range(args.iters):
+                launch()
+            torch.cuda.synchronize()
+        evs = sorted((e for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and "mlp_" in e.name),
+                     key=lambda e: e.time_range.start)
+        per = len(evs) // args.iters
+        wide = [(k, n) for k, n in zip(ks, ns) if n > WN]
+        out = []
+        for i in range(per):
+            name = evs[i].name.split("(")[0].replace("void ", "")
+            ms = statistics.median(e.device_time_total for e in evs[i::per]) / 1e3
+            row = dict(kernel=name, ms=ms)
+            if "mlp_wide_kernel" in name and wide:
+                k, n = wide.pop(0)
+                bw = 32 * ((n // 32 + 1) // 2)     # two column blocks of equal width
+                blocks = [min(bw, n - c) for c in range(0, n, bw)]
+                row["layer"] = "%d->%d" % (k, n)
+                row["tfs"] = 2 * rows * k * n / (ms * 1e-3) / 1e12
+                row["l2_mb"] = _ru(rows, WM) // WM * (k // KC) * sum(WM * KC * 4 + b * KC * 4 for b in blocks) / 1e6
+            out.append(row)
+        return out
 
     def c_out_of(d):
         return [d.c_out[i] for i in range(d.num_layers)]
@@ -149,6 +181,11 @@ def main():
         tot[1] += r["resident_ms"]
         tot[0] += r["stream_ms"]
     print("total: resident-where-fits %.3f ms, streamed %.3f ms" % (tot[1], tot[0]))
+    print("\nkernels per chain call (default options, torch.profiler device time, median of %d calls)" % args.iters)
+    for r in results:
+        for i, k in enumerate(r["launches"]):
+            extra = ("  layer %-9s %6.1f TF/s  L2 %7.1f MB" % (k["layer"], k["tfs"], k["l2_mb"])) if "tfs" in k else ""
+            print("%-34s %-44s %8.4f ms%s" % (r["chain"] if i == 0 else "", k["kernel"][:44], k["ms"], extra))
     if args.json:
         with open(args.json, "w") as f:
             json.dump(dict(card=card(), results=results), f, indent=1)
