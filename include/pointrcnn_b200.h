@@ -156,6 +156,50 @@ PRB_API int prb_three_interpolate_grad_ws(int b, int c, int n, int m, const floa
                                           const float *weight, float *grad_points, void *workspace,
                                           size_t workspace_bytes, void *stream);
 
+/* bfloat16 forms of grouping, gather and interpolation (torch.autocast training): the same layouts, sizes and index
+ * rules as the fp32 entries above, with the feature data (points, out, grad_out, grad_points) as bfloat16 bit patterns
+ * (uint16_t).  idx stays int32 and weight fp32.
+ *   - group / gather forward: copies, so exact.  Each thread moves 8 bfloat16 (16 bytes) per load of indices and per
+ *     store when npoints * nsample is a multiple of 8 and idx / out are 16-byte aligned, one element otherwise.
+ *   - three_interpolate forward: w0*f0 + w1*f1 + w2*f2 in fp32 on the exactly converted features, in the fp32 kernel's
+ *     order and contraction (fmaf(w2, f2, fmaf(w0, f0, w1 * f1))), rounded once to bfloat16 (to nearest even).  16-byte
+ *     stores when n is a multiple of 8 and idx / weight / out are 16-byte aligned.
+ *   - gradients: grad_out bfloat16 in, grad_points bfloat16 out.  Unlike the fp32 entries they WRITE grad_points (it need
+ *     not be zeroed, it is not read): every point's sum is formed in fp32 and rounded once to bfloat16 (to nearest even).
+ *     v_q is the fp32 value of grad_out[q] (grouping, gather) or its fp32 product with weight[q] (interpolation).
+ *     The plain entries add with float atomics into fp32 scratch (*_grad_bf16_workspace_bytes: b * c * n or b * c * m
+ *     floats, zeroed by the entry), then round: the fp32 sum of a point with k references comes in any order, so it lies
+ *     within (k - 1) * 2^-24 * sum |v_q| of the exact sum before the rounding.
+ *     The _ws entries sum in the order prb_group_points_grad_ws states, then round: the same bits on every call.  Their
+ *     scratch is that of the fp32 ordered entries (prb_group_points_grad_workspace_bytes,
+ *     prb_gather_points_grad_workspace_bytes, prb_three_interpolate_grad_workspace_bytes).
+ * No host synchronisation. */
+PRB_API int prb_group_points_bf16(int b, int c, int n, int npoints, int nsample, const uint16_t *points, const int *idx,
+                                  uint16_t *out, void *stream);
+PRB_API size_t prb_group_points_grad_bf16_workspace_bytes(int b, int c, int n);
+PRB_API int prb_group_points_grad_bf16(int b, int c, int n, int npoints, int nsample, const uint16_t *grad_out,
+                                       const int *idx, uint16_t *grad_points, void *workspace, size_t workspace_bytes,
+                                       void *stream);
+PRB_API int prb_group_points_grad_bf16_ws(int b, int c, int n, int npoints, int nsample, const uint16_t *grad_out,
+                                          const int *idx, uint16_t *grad_points, void *workspace, size_t workspace_bytes,
+                                          void *stream);
+/* nsample 1; the atomic entry's scratch is prb_group_points_grad_bf16_workspace_bytes(b, c, n) */
+PRB_API int prb_gather_points_bf16(int b, int c, int n, int npoints, const uint16_t *points, const int *idx,
+                                   uint16_t *out, void *stream);
+PRB_API int prb_gather_points_grad_bf16(int b, int c, int n, int npoints, const uint16_t *grad_out, const int *idx,
+                                        uint16_t *grad_points, void *workspace, size_t workspace_bytes, void *stream);
+PRB_API int prb_gather_points_grad_bf16_ws(int b, int c, int n, int npoints, const uint16_t *grad_out, const int *idx,
+                                           uint16_t *grad_points, void *workspace, size_t workspace_bytes, void *stream);
+PRB_API int prb_three_interpolate_bf16(int b, int c, int m, int n, const uint16_t *points, const int *idx,
+                                       const float *weight, uint16_t *out, void *stream);
+PRB_API size_t prb_three_interpolate_grad_bf16_workspace_bytes(int b, int c, int m);
+PRB_API int prb_three_interpolate_grad_bf16(int b, int c, int n, int m, const uint16_t *grad_out, const int *idx,
+                                            const float *weight, uint16_t *grad_points, void *workspace,
+                                            size_t workspace_bytes, void *stream);
+PRB_API int prb_three_interpolate_grad_bf16_ws(int b, int c, int n, int m, const uint16_t *grad_out, const int *idx,
+                                               const float *weight, uint16_t *grad_points, void *workspace,
+                                               size_t workspace_bytes, void *stream);
+
 /* (B,C,N) <-> (B,N,C) layout change used in front of the fused kernels */
 PRB_API int prb_transpose_bcn_to_bnc(int b, int c, int n, const float *in, float *out, void *stream);
 

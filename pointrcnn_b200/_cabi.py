@@ -76,7 +76,8 @@ def lib():
                      "prb_fps_workspace_bytes", "prb_fps_ordered_workspace_bytes", "prb_kitti_format_detections", "prb_rpn_proposals_workspace_bytes", "prb_roipool3d_workspace_bytes",
                      "prb_kitti_eval_workspace_bytes", "prb_kitti_eval_sets_workspace_bytes", "prb_stage_loss_workspace_bytes", "prb_sa_train_workspace_bytes",
                      "prb_fp_train_workspace_bytes", "prb_sa_train_det_workspace_bytes", "prb_group_points_grad_workspace_bytes",
-                     "prb_gather_points_grad_workspace_bytes", "prb_three_interpolate_grad_workspace_bytes"):
+                     "prb_gather_points_grad_workspace_bytes", "prb_three_interpolate_grad_workspace_bytes",
+                     "prb_group_points_grad_bf16_workspace_bytes", "prb_three_interpolate_grad_bf16_workspace_bytes"):
             getattr(L, name).restype = c_size_t
         P, I, F, U = c_void_p, c_int, c_float, ctypes.c_uint
         L.prb_rcnn_sample_rois.argtypes = [I, I, I, P, P, P, P, P, I, I, F, F, F, F, ctypes.c_double, I, I, I, I, I, F, U, P, P, P, P, P, P,

@@ -10,6 +10,8 @@
 // untouched when nothing hits.  Here: one warp per centre tests 32 points per step; ballot + popc
 // prefix keeps index order; the scene's points are staged through shared memory as SoA tiles shared by
 // all the warps of the CTA; a second radius over the same centres rides along for free (MSG layers).
+#include <stdint.h>
+
 #include "rev_index.cuh"
 
 namespace prb {
@@ -153,6 +155,57 @@ __global__ void __launch_bounds__(GP_THREADS) group_points_grad_kernel(int c, in
     }
 }
 
+// bfloat16 grouping (the same copy): each thread moves V consecutive references of its channel block.  V = 8 reads
+// their indices as two 16-byte loads and writes each channel's 8 values as one 16-byte store (the launcher picks it when L
+// is a multiple of 8 and idx / out are 16-byte aligned); V = 1 is the element-wise form for every other layout.
+template <int V>
+__global__ void __launch_bounds__(GP_THREADS) group_points_bf16_kernel(int c, int n, long L, const __nv_bfloat16 *__restrict__ points,
+                                                                       const int *__restrict__ idx, __nv_bfloat16 *__restrict__ out) {
+    const int scene = blockIdx.z, cb = blockIdx.y * GP_CH;
+    const int nch = min(GP_CH, c - cb);
+    const __nv_bfloat16 *src = points + ((size_t)scene * c + cb) * n;
+    const int *ix = idx + (size_t)scene * L;
+    __nv_bfloat16 *dst = out + ((size_t)scene * c + cb) * L;
+    for (long j = ((long)blockIdx.x * GP_THREADS + threadIdx.x) * V; j < L; j += (long)gridDim.x * GP_THREADS * V) {
+        int k[V];
+        if constexpr (V == 8) {
+            const int4 a = *reinterpret_cast<const int4 *>(ix + j), b = *reinterpret_cast<const int4 *>(ix + j + 4);
+            k[0] = a.x; k[1] = a.y; k[2] = a.z; k[3] = a.w; k[4] = b.x; k[5] = b.y; k[6] = b.z; k[7] = b.w;
+        } else {
+            k[0] = ix[j];
+        }
+#pragma unroll
+        for (int ch = 0; ch < GP_CH; ++ch) {
+            if (ch >= nch) continue;
+            const __nv_bfloat16 *row = src + (size_t)ch * n;
+            if constexpr (V == 8) {
+                __align__(16) __nv_bfloat16 v[8];
+#pragma unroll
+                for (int i = 0; i < 8; ++i) v[i] = __ldg(row + k[i]);
+                *reinterpret_cast<uint4 *>(dst + (size_t)ch * L + j) = *reinterpret_cast<const uint4 *>(v);
+            } else {
+                dst[(size_t)ch * L + j] = __ldg(row + k[0]);
+            }
+        }
+    }
+}
+
+// the atomic bfloat16 gradient, first pass: every reference adds its value, converted exactly, into fp32 sums (b, c, n)
+__global__ void __launch_bounds__(GP_THREADS) group_points_grad_bf16_kernel(int c, int n, long L, const __nv_bfloat16 *__restrict__ grad_out,
+                                                                            const int *__restrict__ idx, float *__restrict__ sums) {
+    const int scene = blockIdx.z, cb = blockIdx.y * GP_CH;
+    const int nch = min(GP_CH, c - cb);
+    const __nv_bfloat16 *g = grad_out + ((size_t)scene * c + cb) * L;
+    const int *ix = idx + (size_t)scene * L;
+    float *dst = sums + ((size_t)scene * c + cb) * n;
+    for (long j = (long)blockIdx.x * GP_THREADS + threadIdx.x; j < L; j += (long)gridDim.x * GP_THREADS) {
+        const int k = ix[j];
+#pragma unroll
+        for (int ch = 0; ch < GP_CH; ++ch)
+            if (ch < nch) atomicAdd(dst + (size_t)ch * n + k, __bfloat162float(g[(size_t)ch * L + j]));
+    }
+}
+
 // (B,C,N) -> (B,N,C) through a 32x33 shared tile
 __global__ void transpose_bcn_bnc_kernel(int c, int n, const float *__restrict__ in, float *__restrict__ out) {
     __shared__ float tile[32][33];
@@ -266,6 +319,80 @@ extern "C" size_t prb_gather_points_grad_workspace_bytes(int b, int n, int npoin
 extern "C" int prb_gather_points_grad_ws(int b, int c, int n, int npoints, const float *grad_out, const int *idx, float *grad_points,
                                          void *workspace, size_t workspace_bytes, void *stream) {
     return prb_group_points_grad_ws(b, c, n, npoints, 1, grad_out, idx, grad_points, workspace, workspace_bytes, stream);
+}
+
+// ------------------------------------------------------------------ bfloat16 grouping / gather (include/pointrcnn_b200.h)
+extern "C" int prb_group_points_bf16(int b, int c, int n, int npoints, int nsample, const uint16_t *points, const int *idx, uint16_t *out,
+                                     void *stream) {
+    PRB_REQUIRE(b >= 0 && c >= 0 && n > 0 && npoints >= 0 && nsample > 0 && points && idx && out, "group_points_bf16: bad arguments");
+    const long L = (long)npoints * nsample;
+    if (b == 0 || c == 0 || L == 0) return 0;
+    const auto *p = reinterpret_cast<const __nv_bfloat16 *>(points);
+    auto *o = reinterpret_cast<__nv_bfloat16 *>(out);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (L % 8 == 0 && (((uintptr_t)idx | (uintptr_t)out) & 15) == 0) {
+        group_points_bf16_kernel<8><<<gp_grid(b, c, L / 8), GP_THREADS, 0, s>>>(c, n, L, p, idx, o);
+        return check_launch("group_points_bf16_kernel<8>");
+    }
+    group_points_bf16_kernel<1><<<gp_grid(b, c, L), GP_THREADS, 0, s>>>(c, n, L, p, idx, o);
+    return check_launch("group_points_bf16_kernel<1>");
+}
+
+extern "C" size_t prb_group_points_grad_bf16_workspace_bytes(int b, int c, int n) {
+    if (b <= 0 || c <= 0 || n <= 0) return 0;
+    return (size_t)b * c * n * sizeof(float);
+}
+
+extern "C" int prb_group_points_grad_bf16(int b, int c, int n, int npoints, int nsample, const uint16_t *grad_out, const int *idx,
+                                          uint16_t *grad_points, void *workspace, size_t workspace_bytes, void *stream) {
+    PRB_REQUIRE(b >= 0 && c >= 0 && n > 0 && npoints >= 0 && nsample > 0, "group_points_grad_bf16: bad dimensions");
+    const long L = (long)npoints * nsample;
+    if (b == 0 || c == 0) return 0;
+    PRB_REQUIRE(grad_out && idx && grad_points && workspace, "group_points_grad_bf16: bad arguments");
+    const size_t need = prb_group_points_grad_bf16_workspace_bytes(b, c, n);
+    PRB_REQUIRE(workspace_bytes >= need, "group_points_grad_bf16: workspace of %zu bytes < %zu", workspace_bytes, need);
+    const cudaStream_t s = (cudaStream_t)stream;
+    float *sums = static_cast<float *>(workspace);
+    PRB_CUDA(cudaMemsetAsync(sums, 0, need, s));
+    if (L > 0) {
+        group_points_grad_bf16_kernel<<<gp_grid(b, c, L), GP_THREADS, 0, s>>>(c, n, L, reinterpret_cast<const __nv_bfloat16 *>(grad_out),
+                                                                               idx, sums);
+        if (int rc = check_launch("group_points_grad_bf16_kernel")) return rc;
+    }
+    return round_bf16((size_t)b * c * n, sums, grad_points, s);
+}
+
+extern "C" int prb_group_points_grad_bf16_ws(int b, int c, int n, int npoints, int nsample, const uint16_t *grad_out, const int *idx,
+                                             uint16_t *grad_points, void *workspace, size_t workspace_bytes, void *stream) {
+    PRB_REQUIRE(b >= 0 && c >= 0 && n >= 0 && npoints >= 0 && nsample > 0, "group_points_grad_bf16_ws: bad dimensions");
+    const long L = (long)npoints * nsample;
+    if (b == 0 || c == 0 || n == 0) return 0;
+    PRB_REQUIRE(grad_points, "group_points_grad_bf16_ws: bad arguments");
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (L == 0) {   // no reference: every sum is +0
+        PRB_CUDA(cudaMemsetAsync(grad_points, 0, (size_t)b * c * n * sizeof(uint16_t), s));
+        return 0;
+    }
+    PRB_REQUIRE(rev_index_fits(b, L, n), "group_points_grad_bf16_ws: %d x %ld references over %d points", b, L, n);
+    PRB_REQUIRE(grad_out && idx && workspace, "group_points_grad_bf16_ws: bad arguments");
+    const size_t need = rev_index_bytes(b, (int)L, n);
+    PRB_REQUIRE(workspace_bytes >= need, "group_points_grad_bf16_ws: workspace of %zu bytes < %zu", workspace_bytes, need);
+    const RevIndex R = rev_index_at(b, (int)L, n, workspace);
+    if (int rc = rev_index_build(R, idx, s)) return rc;
+    return seg_sum_bf16(R, SEG_GROUP, c, reinterpret_cast<const __nv_bfloat16 *>(grad_out), nullptr,
+                        reinterpret_cast<__nv_bfloat16 *>(grad_points), s);
+}
+
+extern "C" int prb_gather_points_bf16(int b, int c, int n, int npoints, const uint16_t *points, const int *idx, uint16_t *out, void *stream) {
+    return prb_group_points_bf16(b, c, n, npoints, 1, points, idx, out, stream);
+}
+extern "C" int prb_gather_points_grad_bf16(int b, int c, int n, int npoints, const uint16_t *grad_out, const int *idx, uint16_t *grad_points,
+                                           void *workspace, size_t workspace_bytes, void *stream) {
+    return prb_group_points_grad_bf16(b, c, n, npoints, 1, grad_out, idx, grad_points, workspace, workspace_bytes, stream);
+}
+extern "C" int prb_gather_points_grad_bf16_ws(int b, int c, int n, int npoints, const uint16_t *grad_out, const int *idx,
+                                              uint16_t *grad_points, void *workspace, size_t workspace_bytes, void *stream) {
+    return prb_group_points_grad_bf16_ws(b, c, n, npoints, 1, grad_out, idx, grad_points, workspace, workspace_bytes, stream);
 }
 
 extern "C" int prb_transpose_bcn_to_bnc(int b, int c, int n, const float *in, float *out, void *stream) {

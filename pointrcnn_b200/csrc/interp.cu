@@ -10,6 +10,7 @@
 // cascade initialised to +inf takes the same branches and (float)1e40 == +inf is what it stores when
 // fewer than three points exist.
 #include <math_constants.h>
+#include <stdint.h>
 
 #include "rev_index.cuh"
 
@@ -131,6 +132,77 @@ __global__ void __launch_bounds__(TI_THREADS) three_interpolate_grad_kernel(int 
     }
 }
 
+// bfloat16 interpolation: the fp32 kernel's arithmetic on the exactly converted values, rounded once to bfloat16.  Each
+// thread computes V consecutive output points of its channel block; V = 8 reads their taps and weights as 16-byte loads and
+// writes each channel's 8 values as one 16-byte store (the launcher picks it when n is a multiple of 8 and idx / weight / out
+// are 16-byte aligned).
+template <int V>
+__global__ void __launch_bounds__(TI_THREADS) three_interpolate_bf16_kernel(int c, int m, int n, const __nv_bfloat16 *__restrict__ points,
+                                                                            const int *__restrict__ idx, const float *__restrict__ weight,
+                                                                            __nv_bfloat16 *__restrict__ out) {
+    const int scene = blockIdx.z, cb = blockIdx.y * TI_CH;
+    const int nch = min(TI_CH, c - cb);
+    const __nv_bfloat16 *src = points + ((size_t)scene * c + cb) * m;
+    __nv_bfloat16 *dst = out + ((size_t)scene * c + cb) * n;
+    for (int j = (blockIdx.x * TI_THREADS + threadIdx.x) * V; j < n; j += gridDim.x * TI_THREADS * V) {
+        const size_t o = ((size_t)scene * n + j) * 3;
+        int k[3 * V];
+        float w[3 * V];
+        if constexpr (V == 8) {
+#pragma unroll
+            for (int i = 0; i < 6; ++i) {
+                const int4 a = reinterpret_cast<const int4 *>(idx + o)[i];
+                const float4 b = reinterpret_cast<const float4 *>(weight + o)[i];
+                k[4 * i] = a.x; k[4 * i + 1] = a.y; k[4 * i + 2] = a.z; k[4 * i + 3] = a.w;
+                w[4 * i] = b.x; w[4 * i + 1] = b.y; w[4 * i + 2] = b.z; w[4 * i + 3] = b.w;
+            }
+        } else {
+#pragma unroll
+            for (int t = 0; t < 3; ++t) { k[t] = idx[o + t]; w[t] = weight[o + t]; }
+        }
+#pragma unroll
+        for (int ch = 0; ch < TI_CH; ++ch) {
+            if (ch >= nch) continue;
+            const __nv_bfloat16 *row = src + (size_t)ch * m;
+            __align__(16) __nv_bfloat16 v[V];
+#pragma unroll
+            for (int i = 0; i < V; ++i) {
+                const float p0 = __bfloat162float(__ldg(row + k[3 * i])), p1 = __bfloat162float(__ldg(row + k[3 * i + 1])),
+                            p2 = __bfloat162float(__ldg(row + k[3 * i + 2]));
+                v[i] = __float2bfloat16_rn(__fmaf_rn(w[3 * i + 2], p2, __fmaf_rn(w[3 * i], p0, __fmul_rn(w[3 * i + 1], p1))));
+            }
+            if constexpr (V == 8)
+                *reinterpret_cast<uint4 *>(dst + (size_t)ch * n + j) = *reinterpret_cast<const uint4 *>(v);
+            else
+                dst[(size_t)ch * n + j] = v[0];
+        }
+    }
+}
+
+// the atomic bfloat16 gradient, first pass: the fp32 kernel's products and float atomics into fp32 sums (b, c, m)
+__global__ void __launch_bounds__(TI_THREADS) three_interpolate_grad_bf16_kernel(int c, int n, int m, const __nv_bfloat16 *__restrict__ grad_out,
+                                                                                 const int *__restrict__ idx, const float *__restrict__ weight,
+                                                                                 float *__restrict__ sums) {
+    const int scene = blockIdx.z, cb = blockIdx.y * TI_CH;
+    const int nch = min(TI_CH, c - cb);
+    const __nv_bfloat16 *g = grad_out + ((size_t)scene * c + cb) * n;
+    float *dst = sums + ((size_t)scene * c + cb) * m;
+    for (int j = blockIdx.x * TI_THREADS + threadIdx.x; j < n; j += gridDim.x * TI_THREADS) {
+        const size_t o = ((size_t)scene * n + j) * 3;
+        const int k0 = idx[o], k1 = idx[o + 1], k2 = idx[o + 2];
+        const float w0 = weight[o], w1 = weight[o + 1], w2 = weight[o + 2];
+#pragma unroll
+        for (int ch = 0; ch < TI_CH; ++ch)
+            if (ch < nch) {
+                const float gv = __bfloat162float(g[(size_t)ch * n + j]);
+                float *row = dst + (size_t)ch * m;
+                atomicAdd(row + k0, __fmul_rn(gv, w0));
+                atomicAdd(row + k1, __fmul_rn(gv, w1));
+                atomicAdd(row + k2, __fmul_rn(gv, w2));
+            }
+    }
+}
+
 }  // namespace prb
 
 using namespace prb;
@@ -182,4 +254,65 @@ extern "C" int prb_three_interpolate_grad_ws(int b, int c, int n, int m, const f
     const cudaStream_t s = (cudaStream_t)stream;
     if (int rc = rev_index_build(R, idx, s)) return rc;
     return seg_sum(R, SEG_TAPS, c, grad_out, weight, true, grad_points, s);
+}
+
+// ------------------------------------------------------------------ bfloat16 interpolation (include/pointrcnn_b200.h)
+extern "C" int prb_three_interpolate_bf16(int b, int c, int m, int n, const uint16_t *points, const int *idx, const float *weight,
+                                          uint16_t *out, void *stream) {
+    PRB_REQUIRE(b >= 0 && c >= 0 && m > 0 && n >= 0 && points && idx && weight && out, "three_interpolate_bf16: bad arguments");
+    if (b == 0 || c == 0 || n == 0) return 0;
+    const auto *p = reinterpret_cast<const __nv_bfloat16 *>(points);
+    auto *o = reinterpret_cast<__nv_bfloat16 *>(out);
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (n % 8 == 0 && (((uintptr_t)idx | (uintptr_t)weight | (uintptr_t)out) & 15) == 0) {
+        dim3 grid(min(ceil_div(n / 8, TI_THREADS), 64), ceil_div(c, TI_CH), b);
+        three_interpolate_bf16_kernel<8><<<grid, TI_THREADS, 0, s>>>(c, m, n, p, idx, weight, o);
+        return check_launch("three_interpolate_bf16_kernel<8>");
+    }
+    dim3 grid(min(ceil_div(n, TI_THREADS), 64), ceil_div(c, TI_CH), b);
+    three_interpolate_bf16_kernel<1><<<grid, TI_THREADS, 0, s>>>(c, m, n, p, idx, weight, o);
+    return check_launch("three_interpolate_bf16_kernel<1>");
+}
+
+extern "C" size_t prb_three_interpolate_grad_bf16_workspace_bytes(int b, int c, int m) {
+    if (b <= 0 || c <= 0 || m <= 0) return 0;
+    return (size_t)b * c * m * sizeof(float);
+}
+
+extern "C" int prb_three_interpolate_grad_bf16(int b, int c, int n, int m, const uint16_t *grad_out, const int *idx, const float *weight,
+                                               uint16_t *grad_points, void *workspace, size_t workspace_bytes, void *stream) {
+    PRB_REQUIRE(b >= 0 && c >= 0 && m > 0 && n >= 0, "three_interpolate_grad_bf16: bad dimensions");
+    if (b == 0 || c == 0) return 0;
+    PRB_REQUIRE(grad_out && idx && weight && grad_points && workspace, "three_interpolate_grad_bf16: bad arguments");
+    const size_t need = prb_three_interpolate_grad_bf16_workspace_bytes(b, c, m);
+    PRB_REQUIRE(workspace_bytes >= need, "three_interpolate_grad_bf16: workspace of %zu bytes < %zu", workspace_bytes, need);
+    const cudaStream_t s = (cudaStream_t)stream;
+    float *sums = static_cast<float *>(workspace);
+    PRB_CUDA(cudaMemsetAsync(sums, 0, need, s));
+    if (n > 0) {
+        dim3 grid(min(ceil_div(n, TI_THREADS), 64), ceil_div(c, TI_CH), b);
+        three_interpolate_grad_bf16_kernel<<<grid, TI_THREADS, 0, s>>>(c, n, m, reinterpret_cast<const __nv_bfloat16 *>(grad_out), idx, weight,
+                                                                       sums);
+        if (int rc = check_launch("three_interpolate_grad_bf16_kernel")) return rc;
+    }
+    return round_bf16((size_t)b * c * m, sums, grad_points, s);
+}
+
+extern "C" int prb_three_interpolate_grad_bf16_ws(int b, int c, int n, int m, const uint16_t *grad_out, const int *idx, const float *weight,
+                                                  uint16_t *grad_points, void *workspace, size_t workspace_bytes, void *stream) {
+    PRB_REQUIRE(b >= 0 && c >= 0 && n >= 0 && m >= 0, "three_interpolate_grad_bf16_ws: bad dimensions");
+    if (b == 0 || c == 0 || m == 0) return 0;
+    PRB_REQUIRE(grad_points, "three_interpolate_grad_bf16_ws: bad arguments");
+    const cudaStream_t s = (cudaStream_t)stream;
+    if (n == 0) {   // no tap: every sum is +0
+        PRB_CUDA(cudaMemsetAsync(grad_points, 0, (size_t)b * c * m * sizeof(uint16_t), s));
+        return 0;
+    }
+    PRB_REQUIRE(rev_index_fits(b, 3L * n, m), "three_interpolate_grad_bf16_ws: %d x %d rows over %d points", b, n, m);
+    PRB_REQUIRE(grad_out && idx && weight && workspace, "three_interpolate_grad_bf16_ws: bad arguments");
+    const size_t need = rev_index_bytes(b, 3 * n, m);
+    PRB_REQUIRE(workspace_bytes >= need, "three_interpolate_grad_bf16_ws: workspace of %zu bytes < %zu", workspace_bytes, need);
+    const RevIndex R = rev_index_at(b, 3 * n, m, workspace);
+    if (int rc = rev_index_build(R, idx, s)) return rc;
+    return seg_sum_bf16(R, SEG_TAPS, c, reinterpret_cast<const __nv_bfloat16 *>(grad_out), weight, reinterpret_cast<__nv_bfloat16 *>(grad_points), s);
 }

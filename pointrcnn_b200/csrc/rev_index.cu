@@ -1,4 +1,7 @@
 // rev_index.cu -- reverse index of a reference list and the fixed-order gather-sum over it; see rev_index.cuh.
+#include <algorithm>
+#include <type_traits>
+
 #include "rev_index.cuh"
 
 namespace prb {
@@ -116,10 +119,14 @@ __global__ void __launch_bounds__(kRiThreads) rev_sort(int K, const int *off, in
     }
 }
 
-// one thread per (source, block of kSegCh channels); grid (sources / kRiThreads, channel blocks, scenes)
-template <int KIND>
-__global__ void __launch_bounds__(kRiThreads) seg_sum_kernel(RevIndex R, int c, const float *__restrict__ g, const float *__restrict__ w,
-                                                             int accumulate, float *__restrict__ out) {
+__device__ __forceinline__ float seg_load(const float *p) { return __ldg(p); }
+__device__ __forceinline__ float seg_load(const __nv_bfloat16 *p) { return __bfloat162float(__ldg(p)); }
+
+// one thread per (source, block of kSegCh channels); grid (sources / kRiThreads, channel blocks, scenes).  T: the value
+// and output type (float: out = out + acc or acc; bfloat16: out = acc rounded once)
+template <int KIND, typename T>
+__global__ void __launch_bounds__(kRiThreads) seg_sum_kernel(RevIndex R, int c, const T *__restrict__ g, const float *__restrict__ w,
+                                                             int accumulate, T *__restrict__ out) {
     const int s = blockIdx.z, cb = blockIdx.y * kSegCh, j = blockIdx.x * kRiThreads + threadIdx.x;
     if (j >= R.n) return;
     const int nch = min(kSegCh, c - cb);
@@ -131,28 +138,33 @@ __global__ void __launch_bounds__(kRiThreads) seg_sum_kernel(RevIndex R, int c, 
     for (int e = e0; e < e1; ++e) {
         const int q = R.list[e], l = q - s * R.L;
         if constexpr (KIND == SEG_GROUP) {
-            const float *gv = g + ((size_t)s * c + cb) * R.L + l;
+            const T *gv = g + ((size_t)s * c + cb) * R.L + l;
 #pragma unroll
             for (int ch = 0; ch < kSegCh; ++ch)
-                if (ch < nch) acc[ch] = __fadd_rn(acc[ch], __ldg(gv + (size_t)ch * R.L));
+                if (ch < nch) acc[ch] = __fadd_rn(acc[ch], seg_load(gv + (size_t)ch * R.L));
         } else if constexpr (KIND == SEG_TAPS) {
             const int rows = R.L / 3;
-            const float *gv = g + ((size_t)s * c + cb) * rows + l / 3;
+            const T *gv = g + ((size_t)s * c + cb) * rows + l / 3;
             const float wq = __ldg(w + q);
 #pragma unroll
             for (int ch = 0; ch < kSegCh; ++ch)
-                if (ch < nch) acc[ch] = __fadd_rn(acc[ch], __fmul_rn(__ldg(gv + (size_t)ch * rows), wq));
+                if (ch < nch) acc[ch] = __fadd_rn(acc[ch], __fmul_rn(seg_load(gv + (size_t)ch * rows), wq));
         } else {
-            const float *gv = g + (size_t)q * c + cb;
+            const T *gv = g + (size_t)q * c + cb;
 #pragma unroll
             for (int ch = 0; ch < kSegCh; ++ch)
-                if (ch < nch) acc[ch] = __fadd_rn(acc[ch], __ldg(gv + ch));
+                if (ch < nch) acc[ch] = __fadd_rn(acc[ch], seg_load(gv + ch));
         }
     }
-    float *o = out + ((size_t)s * c + cb) * R.n + j;
+    T *o = out + ((size_t)s * c + cb) * R.n + j;
 #pragma unroll
-    for (int ch = 0; ch < kSegCh; ++ch)
-        if (ch < nch) o[(size_t)ch * R.n] = accumulate ? __fadd_rn(o[(size_t)ch * R.n], acc[ch]) : acc[ch];
+    for (int ch = 0; ch < kSegCh; ++ch) {
+        if (ch >= nch) continue;
+        if constexpr (std::is_same_v<T, float>)
+            o[(size_t)ch * R.n] = accumulate ? __fadd_rn(o[(size_t)ch * R.n], acc[ch]) : acc[ch];
+        else
+            o[(size_t)ch * R.n] = __float2bfloat16_rn(acc[ch]);
+    }
 }
 
 // the offset of `bytes` placed at `at`; `at` moves past them to the next 256-byte boundary
@@ -210,19 +222,40 @@ int rev_index_build(const RevIndex &R, const int *idx, cudaStream_t s) {
     return check_launch("rev_sort");
 }
 
-int seg_sum(const RevIndex &R, int kind, int c, const float *g, const float *w, bool accumulate, float *out, cudaStream_t s) {
+template <typename T>
+static int seg_sum_launch(const RevIndex &R, int kind, int c, const T *g, const float *w, bool accumulate, T *out, cudaStream_t s) {
     const dim3 grid(ceil_div(R.n, kRiThreads), ceil_div(c, kSegCh), R.b);
     switch (kind) {
     case SEG_GROUP:
-        seg_sum_kernel<SEG_GROUP><<<grid, kRiThreads, 0, s>>>(R, c, g, w, accumulate, out);
+        seg_sum_kernel<SEG_GROUP, T><<<grid, kRiThreads, 0, s>>>(R, c, g, w, accumulate, out);
         return check_launch("seg_sum_kernel<SEG_GROUP>");
     case SEG_TAPS:
-        seg_sum_kernel<SEG_TAPS><<<grid, kRiThreads, 0, s>>>(R, c, g, w, accumulate, out);
+        seg_sum_kernel<SEG_TAPS, T><<<grid, kRiThreads, 0, s>>>(R, c, g, w, accumulate, out);
         return check_launch("seg_sum_kernel<SEG_TAPS>");
     default:
-        seg_sum_kernel<SEG_ROWS><<<grid, kRiThreads, 0, s>>>(R, c, g, w, accumulate, out);
+        seg_sum_kernel<SEG_ROWS, T><<<grid, kRiThreads, 0, s>>>(R, c, g, w, accumulate, out);
         return check_launch("seg_sum_kernel<SEG_ROWS>");
     }
+}
+
+int seg_sum(const RevIndex &R, int kind, int c, const float *g, const float *w, bool accumulate, float *out, cudaStream_t s) {
+    return seg_sum_launch(R, kind, c, g, w, accumulate, out, s);
+}
+
+int seg_sum_bf16(const RevIndex &R, int kind, int c, const __nv_bfloat16 *g, const float *w, __nv_bfloat16 *out, cudaStream_t s) {
+    return seg_sum_launch(R, kind, c, g, w, false, out, s);
+}
+
+__global__ void __launch_bounds__(kRiThreads) round_bf16_kernel(size_t count, const float *__restrict__ in, __nv_bfloat16 *__restrict__ out) {
+    for (size_t i = (size_t)blockIdx.x * kRiThreads + threadIdx.x; i < count; i += (size_t)gridDim.x * kRiThreads)
+        out[i] = __float2bfloat16_rn(in[i]);
+}
+
+int round_bf16(size_t count, const float *in, void *out, cudaStream_t s) {
+    if (count == 0) return 0;
+    const unsigned blocks = (unsigned)std::min<size_t>((count + kRiThreads - 1) / kRiThreads, 4096);
+    round_bf16_kernel<<<blocks, kRiThreads, 0, s>>>(count, in, static_cast<__nv_bfloat16 *>(out));
+    return check_launch("round_bf16_kernel");
 }
 
 }  // namespace prb

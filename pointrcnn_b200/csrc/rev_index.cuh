@@ -5,9 +5,11 @@
 // idx[q], its references in list[off[j] .. off[j + 1]) in increasing q.  It is a counting sort: counts and slots use
 // integer atomics, and a per-source sort fixes the order, so the index is the same on every call.
 //
-// Users: the FP training backward (3 taps per unknown point), the ordered grouping / gather / interpolation gradients and
-// the SA training backward's feature gradient (nsample references per centre, 1 per gathered point).
+// Users: the FP training backward (3 taps per unknown point), the ordered grouping / gather / interpolation gradients (fp32
+// and bfloat16) and the SA training backward's feature gradient (nsample references per centre, 1 per gathered point).
 #pragma once
+#include <cuda_bf16.h>
+
 #include "common.cuh"
 
 namespace prb {
@@ -39,5 +41,13 @@ constexpr int kSegCh = 8;   // channels per thread of the gather-sum
 // out (b, c, n): for every source j of scene s and channel ch, acc = +0.0f, then acc = acc + v over the source's
 // references in increasing q (each add rounded to nearest, no contraction), then out = out + acc (accumulate) or out = acc.
 int seg_sum(const RevIndex &R, int kind, int c, const float *g, const float *w, bool accumulate, float *out, cudaStream_t s);
+
+// the same sum over bfloat16 values (each converted exactly to fp32; SEG_TAPS: the fp32 product with w rounded as above),
+// then out = acc rounded once to bfloat16 (to nearest even), written: out is not read
+int seg_sum_bf16(const RevIndex &R, int kind, int c, const __nv_bfloat16 *g, const float *w, __nv_bfloat16 *out, cudaStream_t s);
+
+// out[i] = in[i] rounded to bfloat16 (to nearest even) for i < count: the last pass of the atomic bfloat16 gradients, which
+// sum into fp32 scratch first
+int round_bf16(size_t count, const float *in, void *out, cudaStream_t s);
 
 }  // namespace prb

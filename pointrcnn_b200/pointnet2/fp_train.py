@@ -9,7 +9,9 @@ come from three_nn_weights (the fused path's 3-NN).  Saved for backward: the tap
 skip features, the pre-activations Z of every layer and the per-channel statistics.
 Layer 0 runs projected: the m known points go through the interpolated columns of layer 0 first, then the result is
 interpolated (n = 4 m at every RPN level, so this removes three quarters of that part of layer 0).
-Precision: TF32 tensor-core GEMMs with fp32 accumulation, the BN statistics summed in float64.
+Precision: TF32 tensor-core GEMMs with fp32 accumulation, the BN statistics summed in float64.  Under torch.autocast
+it computes in fp32 all the same (see sa_train.py): bfloat16 known / skip features are converted at entry, the outputs
+are fp32 and each input's gradient comes back in that input's dtype.
 """
 import ctypes
 
@@ -38,15 +40,15 @@ def faster_on_device(module, c_known, c_skip):
 
 def supported(module, unknown, known, unknow_feats, known_feats):
     """the whole rule but the switch, the need for an autograd graph and the shape rule: known points given, fp32 CUDA
-    inputs and contiguous fp32 CUDA parameters (sa_train._params_ok), coordinates without grad, and a SharedMLP as
-    sa_train._mlp_ok describes for c_known + c_skip (at most MAX_IN) input channels"""
+    coordinates without grad, fp32 or bfloat16 CUDA features, contiguous fp32 CUDA parameters (sa_train._params_ok), and a
+    SharedMLP as sa_train._mlp_ok describes for c_known + c_skip (at most MAX_IN) input channels"""
     if known is None or known_feats is None:
         return False
     for t in (unknown, known):
         if not t.is_cuda or t.dtype != torch.float32 or t.requires_grad:
             return False
     for t in (known_feats, unknow_feats):
-        if t is not None and (not t.is_cuda or t.dtype != torch.float32):
+        if t is not None and (not t.is_cuda or t.dtype not in sa_train.FEATURE_DTYPES):
             return False
     if not sa_train._params_ok(module.mlp):
         return False
@@ -58,6 +60,7 @@ class _FPTrain(torch.autograd.Function):
     """(known_feats, skip, *params) -> (out (B, C_last, n), out_pm (B, n, C_last) or None) of one FP module"""
 
     @staticmethod
+    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
     def forward(ctx, scale, geom, known_pm, known_feats, skip, *params):
         idx, weight, emit_pm = geom
         L = C.lib()
@@ -99,7 +102,7 @@ class _FPTrain(torch.autograd.Function):
         m, c_known = known_pm.size(1), known_pm.size(2)
         c_skip = 0 if skip is None else skip.size(1)
         dev = known_pm.device
-        g_out = g_out.contiguous()
+        g_out = g_out.float().contiguous()
         g_known = torch.empty((B, c_known, m), dtype=torch.float32, device=dev) if ctx.needs_input_grad[3] else None
         g_skip = torch.empty((B, c_skip, n), dtype=torch.float32, device=dev) if ctx.needs_input_grad[4] and c_skip > 0 else None
         bufs = sa_train._grad_buffers(params, nl)
@@ -115,7 +118,7 @@ class _FPTrain(torch.autograd.Function):
 def forward(module, idx, weight, known_pm, known_feats, skip, emit_pm):
     """the features (B, C_last, n) of FP module `module` through the device path, and their point-major twin (None unless
     emit_pm).  idx / weight (B, n, 3): three_nn_weights' taps; known_pm (B, m, c_known): known_feats point-major;
-    skip (B, c_skip, n) contiguous or None"""
+    skip (B, c_skip, n) contiguous or None; the features fp32 (sa_train.as_fp32)"""
     C.require_cuda(idx, weight, known_pm, known_feats, skip)
     scale = sa_train._Scale(module.mlp)
     out, out_pm = _FPTrain.apply(scale, (idx, weight, emit_pm), known_pm.detach(), known_feats, skip, *scale.params())

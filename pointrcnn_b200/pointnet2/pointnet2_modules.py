@@ -267,6 +267,7 @@ class _PointnetSAModuleBase(nn.Module):
         """the fused path's sampling and neighbour search, then sa_train's autograd Function over all scales"""
         xyz = xyz.contiguous()
         ret_xyz, centres, idxs, nss = self.fused_geometry(xyz, new_xyz)
+        features = sa_train.as_fp32(features)          # bfloat16 under autocast: the device path computes in fp32
         feats_pm = _point_major(features) if features is not None else None
         out, out_pm = sa_train.forward(self, xyz, features, feats_pm, centres, idxs, nss)
         return ret_xyz, _attach_pm(out, out_pm)
@@ -393,7 +394,8 @@ class PointnetFPModule(nn.Module):
     def _forward_train(self, unknown, known, unknow_feats, known_feats):
         """the fused path's 3-NN, then fp_train's autograd Function"""
         idx, weight = self.fused_geometry(unknown, known)
-        skip = unknow_feats.contiguous() if unknow_feats is not None else None
+        known_feats = sa_train.as_fp32(known_feats)    # bfloat16 under autocast: the device path computes in fp32
+        skip = sa_train.as_fp32(unknow_feats.contiguous()) if unknow_feats is not None else None
         out, out_pm = fp_train.forward(self, idx, weight, _point_major(known_feats), known_feats, skip, self.emit_point_major)
         return _attach_pm(out, out_pm) if out_pm is not None else out
 

@@ -5,6 +5,11 @@ and the QueryAndGroup / GroupAll modules, on top of the H100 `pointnet2_cuda` na
 Same names, argument order, output shapes/dtypes and zero-/1e10-fill obligations as the reference.
 Extras (used by the fused module paths, not part of the reference API): furthest_point_sample_xyz,
 ball_query_msg2, three_nn_weights.
+
+gather_operation, three_interpolate and grouping_operation also take bfloat16 features (what the SharedMLP convolutions
+return under torch.autocast): the output and the feature gradient are bfloat16 too, through the *_bf16 natives (copies;
+fp32 interpolation rounded once; gradients summed in fp32 and rounded once).  Indices, weights and coordinates stay
+int32 / float32; float32 features take the float32 natives as before, any other dtype raises.
 """
 from typing import Tuple
 
@@ -20,6 +25,19 @@ from ..ext import pointnet2_cuda as pointnet2
 
 def _cuda_empty(shape, dtype, like):
     return torch.empty(shape, dtype=dtype, device=like.device)
+
+
+def _feature_dtype(features):
+    """the output dtype of an index op: bfloat16 for bfloat16 features, else float32 (the natives refuse other dtypes)"""
+    return torch.bfloat16 if features.dtype == torch.bfloat16 else torch.float32
+
+
+def _grad_buffer(shape, grad_out):
+    """the feature gradient the scatter natives fill, in the dtype of the op's output (= of grad_out, = of the features):
+    bfloat16 uninitialised (the _bf16 natives write every element), else float32 zeros (they add into it)"""
+    if grad_out.dtype == torch.bfloat16:
+        return torch.empty(shape, dtype=torch.bfloat16, device=grad_out.device)
+    return torch.zeros(shape, dtype=torch.float32, device=grad_out.device)
 
 
 # Neighbour searches go through the hash grid (csrc/grid.cu) when the searched set is large enough to pay for the
@@ -143,7 +161,7 @@ class GatherOperation(Function):
         assert idx.is_contiguous()
         B, npoint = idx.size()
         _, Cc, N = features.size()
-        output = _cuda_empty((B, Cc, npoint), torch.float32, features)
+        output = _cuda_empty((B, Cc, npoint), _feature_dtype(features), features)
         pointnet2.gather_points_wrapper(B, Cc, N, npoint, features, idx, output)
         ctx.for_backwards = (idx, Cc, N)
         return output
@@ -152,7 +170,7 @@ class GatherOperation(Function):
     def backward(ctx, grad_out):
         idx, Cc, N = ctx.for_backwards
         B, npoint = idx.size()
-        grad_features = torch.zeros((B, Cc, N), dtype=torch.float32, device=grad_out.device)
+        grad_features = _grad_buffer((B, Cc, N), grad_out)
         pointnet2.gather_points_grad_wrapper(B, Cc, N, npoint, grad_out.contiguous(), idx, grad_features)
         return grad_features, None
 
@@ -208,7 +226,7 @@ class ThreeInterpolate(Function):
         B, c, m = features.size()
         n = idx.size(1)
         ctx.three_interpolate_for_backward = (idx, weight, m)
-        output = _cuda_empty((B, c, n), torch.float32, features)
+        output = _cuda_empty((B, c, n), _feature_dtype(features), features)
         pointnet2.three_interpolate_wrapper(B, c, m, n, features, idx, weight, output)
         return output
 
@@ -216,7 +234,7 @@ class ThreeInterpolate(Function):
     def backward(ctx, grad_out: torch.Tensor):
         idx, weight, m = ctx.three_interpolate_for_backward
         B, c, n = grad_out.size()
-        grad_features = torch.zeros((B, c, m), dtype=torch.float32, device=grad_out.device)
+        grad_features = _grad_buffer((B, c, m), grad_out)
         pointnet2.three_interpolate_grad_wrapper(B, c, n, m, grad_out.contiguous(), idx, weight, grad_features)
         return grad_features, None, None
 
@@ -232,7 +250,7 @@ class GroupingOperation(Function):
         assert idx.is_contiguous()
         B, nfeatures, nsample = idx.size()
         _, Cc, N = features.size()
-        output = _cuda_empty((B, Cc, nfeatures, nsample), torch.float32, features)
+        output = _cuda_empty((B, Cc, nfeatures, nsample), _feature_dtype(features), features)
         pointnet2.group_points_wrapper(B, Cc, N, nfeatures, nsample, features, idx, output)
         ctx.for_backwards = (idx, N)
         return output
@@ -241,7 +259,7 @@ class GroupingOperation(Function):
     def backward(ctx, grad_out: torch.Tensor):
         idx, N = ctx.for_backwards
         B, Cc, npoint, nsample = grad_out.size()
-        grad_features = torch.zeros((B, Cc, N), dtype=torch.float32, device=grad_out.device)
+        grad_features = _grad_buffer((B, Cc, N), grad_out)
         pointnet2.group_points_grad_wrapper(B, Cc, N, npoint, nsample, grad_out.contiguous(), idx, grad_features)
         return grad_features, None
 

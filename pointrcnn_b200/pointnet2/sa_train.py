@@ -8,6 +8,9 @@ pre-activations Z of every layer, the per-channel statistics and the sample each
 Precision: TF32 tensor-core GEMMs with fp32 accumulation, the BN statistics summed in float64.
 Under torch.use_deterministic_algorithms(True) (warn_only too) the backward takes prb_sa_train_backward_det, whose feature
 gradient is summed per point in a fixed order instead of scattered with float atomics; every other result is the same.
+Under torch.autocast the Function still computes in fp32: bfloat16 features are converted to fp32 before the point-major
+copy (fp32), the Function's forward casts its floating inputs to fp32 and runs with autocast off, and each input's
+gradient comes back in that input's dtype.  The outputs are fp32.
 """
 import ctypes
 
@@ -63,14 +66,22 @@ def _params_ok(module):
                for t in list(module.parameters()) + list(module.buffers()) if t.is_floating_point())
 
 
+FEATURE_DTYPES = (torch.float32, torch.bfloat16)     # bfloat16: the features of autocast training, converted at entry
+
+
+def as_fp32(t):
+    """`t` itself when None or float32, else its float32 copy (autograd returns the gradient in t's dtype)"""
+    return t if t is None or t.dtype == torch.float32 else t.float()
+
+
 def supported(module, xyz, features, new_xyz):
-    """the whole rule but the switch and the need for an autograd graph (the caller checks those): fp32 CUDA inputs and
-    contiguous fp32 CUDA parameters, coordinates without grad, and layout_ok"""
+    """the whole rule but the switch and the need for an autograd graph (the caller checks those): fp32 CUDA coordinates
+    without grad, fp32 or bfloat16 CUDA features, contiguous fp32 CUDA parameters, and layout_ok"""
     if not xyz.is_cuda or xyz.dtype != torch.float32 or xyz.requires_grad:
         return False
     if new_xyz is not None and new_xyz.requires_grad:
         return False
-    if features is not None and (not features.is_cuda or features.dtype != torch.float32):
+    if features is not None and (not features.is_cuda or features.dtype not in FEATURE_DTYPES):
         return False
     if not _params_ok(module.mlps):
         return False
@@ -151,6 +162,7 @@ class _SATrain(torch.autograd.Function):
     """(features, *params) -> (out (B, sum C_last, npoint), out_pm (B, npoint, sum C_last)) of one SA module"""
 
     @staticmethod
+    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
     def forward(ctx, scales, geom, feats_pm, features, *params):
         xyz, centres, idxs, nss = geom
         L = C.lib()
@@ -199,7 +211,7 @@ class _SATrain(torch.autograd.Function):
         npoint = centres.size(1)
         c_feat = ctx.c_feat
         dev = xyz.device
-        g_out = g_out.contiguous()
+        g_out = g_out.float().contiguous()
         c_total = g_out.size(1)
         ordered = torch.are_deterministic_algorithms_enabled()
         if ctx.needs_input_grad[3] and c_feat > 0:
@@ -232,7 +244,8 @@ class _SATrain(torch.autograd.Function):
 
 
 def forward(module, xyz, features, feats_pm, centres, idxs, nss):
-    """the pooled features (B, sum C_last, npoint) of `module` through the device path, and their point-major twin"""
+    """the pooled features (B, sum C_last, npoint) of `module` through the device path, and their point-major twin.
+    features / feats_pm: fp32 (as_fp32)"""
     C.require_cuda(xyz, centres, features, *idxs)
     scales = [_Scale(mlp) for mlp in module.mlps]
     params = [p for s in scales for p in s.params()]

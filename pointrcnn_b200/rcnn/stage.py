@@ -8,6 +8,8 @@ Same sub-module and parameter names as lib.net.rcnn_net.RCNNNet (`xyz_up_layer.l
 it is.  With the reference tree present, `dropin.activate()` + the unchanged lib/net/rcnn_net.py build the same thing on
 the same natives; this class exists so benches and GPU tests run on the box, where /root/reference does not exist.
 """
+import contextlib
+
 import torch
 import torch.nn as nn
 
@@ -136,7 +138,9 @@ class RCNNStage(nn.Module):
                 from ..rpn.proposal_target_layer import ProposalTargetLayer
                 self.proposal_target_layer = ProposalTargetLayer()
             target_layer = self.proposal_target_layer
-        with torch.no_grad(), config.override(**({"target_draw": target_draw} if target_draw is not None else {})):
+        # the targets are geometry, not network: fp32 under autocast too (the canonical rotation is a matmul)
+        fp32 = torch.autocast("cuda", enabled=False) if torch.is_autocast_enabled("cuda") else contextlib.nullcontext()
+        with torch.no_grad(), fp32, config.override(**({"target_draw": target_draw} if target_draw is not None else {})):
             target = target_layer(input_data)
             target["pts_input"] = torch.cat((target["sampled_pts"], target["pts_feature"]), dim=2)
         rcnn_cls, rcnn_reg = self.forward_pts(target["pts_input"])

@@ -12,8 +12,13 @@ pointrcnn_b200.config, "torch" unless changed):
   synchronisation, the same (total, terms) keys for the same options (each term a 0-d device tensor), and the gradients
   torch autograd derives for the mirror.  Values differ from the torch path in the last bits (float64 sums).  Without a
   foreground row the regression terms are exact zeros here, where the torch path leaves their keys out.  CUDA tensors only.
+
+Under torch.autocast both compute in fp32: rpn_loss / rcnn_loss cast their floating inputs to fp32 and run with autocast
+disabled (so the mirror's F.binary_cross_entropy stays legal and its terms match the device loss's), and the inputs'
+gradients come back in the inputs' dtypes.  Outside autocast nothing is cast.
 """
 import ctypes
+import functools
 
 import numpy as np
 import torch
@@ -133,6 +138,23 @@ def _impl(impl):
     return impl
 
 
+def _fp32_under_autocast(loss_fn):
+    """run `loss_fn` as it is outside CUDA autocast; inside, with autocast disabled and every floating CUDA tensor argument
+    below float64 cast to float32"""
+
+    def up(v):
+        return v.float() if torch.is_tensor(v) and v.is_cuda and v.is_floating_point() and v.dtype != torch.float64 else v
+
+    @functools.wraps(loss_fn)
+    def run(*args, **kwargs):
+        if not torch.is_autocast_enabled("cuda"):
+            return loss_fn(*args, **kwargs)
+        with torch.autocast("cuda", enabled=False):
+            return loss_fn(*[up(a) for a in args], **{k: up(v) for k, v in kwargs.items()})
+    return run
+
+
+@_fp32_under_autocast
 def rpn_loss(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, mean_size, loss_cls="SigmoidFocalLoss", focal_alpha=0.25, focal_gamma=2.0,
              fg_weight=15.0, loc_scope=3.0, loc_bin_size=0.5, num_head_bin=12, loc_xz_fine=True, loss_weight=(1.0, 1.0), impl=None):
     """get_rpn_loss (train_functions.py:55-120).  rpn_cls (B,N,1), rpn_reg (B,N,C), rpn_cls_label (B,N) in {-1,0,1},
@@ -173,6 +195,7 @@ def rpn_loss(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, mean_size, loss_cls
     return total, terms
 
 
+@_fp32_under_autocast
 def rcnn_loss(rcnn_cls, rcnn_reg, cls_label, reg_valid_mask, roi_boxes3d, gt_of_rois, mean_size, loss_cls="BinaryCrossEntropy",
               focal_alpha=0.25, focal_gamma=2.0, size_res_on_roi=False, loc_scope=1.5, loc_bin_size=0.5, num_head_bin=9,
               loc_y_by_bin=False, loc_y_scope=0.5, loc_y_bin_size=0.25, ce_weight=None, impl=None):
@@ -236,6 +259,7 @@ class _StageLoss(torch.autograd.Function):
     takes the upstream gradient of the total and of every slot of the vector (either may be absent) on the device"""
 
     @staticmethod
+    @torch.amp.custom_fwd(device_type="cuda", cast_inputs=torch.float32)
     def forward(ctx, cls, reg, desc, label, fg_mask, reg_label, mean_size, anchor_boxes, ce_weight):
         L = C.lib()
         rows = reg.shape[0]

@@ -9,6 +9,11 @@ eval-mode kernel: batch-statistics BatchNorm couples all tiles of a launch.  sa_
 supports through csrc/sa_train.cu instead, see pointnet2/sa_train.py.)  What this module adds over the reference's
 loop: no `.item()` inside the loss, per-rank processes instead of nn.DataParallel's per-step replicate / scatter / gather,
 and the bucketed all-reduce of `parallel_utils.GradBucketReducer` overlapped with backward.
+
+Mixed precision: call a trainer's step inside `with torch.autocast("cuda", dtype=torch.bfloat16):`.  The forward's
+convolutions then run with bfloat16 operands, the grouping / gather / interpolation natives move bfloat16 features, the
+device SA / FP / loss paths and both losses compute in fp32; backward, the all-reduce and the optimizer step run with
+autocast disabled, and parameters, gradients and optimizer state stay fp32 (INTEGRATION.md, "Training under autocast").
 """
 import contextlib
 
@@ -33,6 +38,11 @@ def _sa_switch(sa_train, fp_train=None):
             raise ValueError("%s must be 'torch', 'device' or None, not %r" % (name, value))
         kw[name] = value
     return config.override(**kw) if kw else contextlib.nullcontext()
+
+
+def _without_autocast():
+    """the backward / all-reduce / optimizer part of a step: with CUDA autocast disabled when the caller enabled it"""
+    return torch.autocast("cuda", enabled=False) if torch.is_autocast_enabled("cuda") else contextlib.nullcontext()
 
 
 def _schedule(optimizer, total_steps, lr):
@@ -132,11 +142,12 @@ class RPNTrainer(_Recipe):
     def step(self, pts_input, rpn_cls_label, rpn_reg_label, grad_norm_clip=None):
         self.reducer.reset()
         loss, terms = self.forward_loss(pts_input, rpn_cls_label, rpn_reg_label)
-        loss.backward()
-        self.reducer.finish()
-        if grad_norm_clip:
-            torch.nn.utils.clip_grad_norm_(self.params, grad_norm_clip)     # train_utils.py: clip_grad_norm_(.., GRAD_NORM_CLIP)
-        self.opt.step()
+        with _without_autocast():
+            loss.backward()
+            self.reducer.finish()
+            if grad_norm_clip:
+                torch.nn.utils.clip_grad_norm_(self.params, grad_norm_clip)     # train_utils.py: clip_grad_norm_(.., GRAD_NORM_CLIP)
+            self.opt.step()
         return loss.detach(), terms
 
 
@@ -234,9 +245,10 @@ class RCNNTrainer(_Recipe):
     def _step(self, forward_loss, args, grad_norm_clip):
         self.reducer.reset()
         loss, terms = forward_loss(*args)
-        loss.backward()
-        self.reducer.finish()
-        if grad_norm_clip:
-            torch.nn.utils.clip_grad_norm_(self.params, grad_norm_clip)
-        self.opt.step()
+        with _without_autocast():
+            loss.backward()
+            self.reducer.finish()
+            if grad_norm_clip:
+                torch.nn.utils.clip_grad_norm_(self.params, grad_norm_clip)
+            self.opt.step()
         return loss.detach(), terms
