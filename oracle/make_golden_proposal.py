@@ -44,7 +44,8 @@ def rpn_outputs(B, N, seed, far_empty=False):
     return scores.astype(np.float32), reg.astype(np.float32), xyz.astype(np.float32)
 
 
-def main():
+def install_reference():
+    """import the reference's ProposalLayer, cfg and decode_bbox_target with the CPU stand-ins described above"""
     from pointrcnn_b200 import dropin
     from oracle import oracle as O
     dropin._install_compat()
@@ -69,7 +70,12 @@ def main():
     from lib.config import cfg, cfg_from_file
     cfg_from_file(os.path.join(REF, "tools/cfgs/default.yaml"))
     from lib.rpn.proposal_layer import ProposalLayer
+    from lib.utils.bbox_transform import decode_bbox_target
+    return ProposalLayer, cfg, decode_bbox_target
 
+
+def main():
+    ProposalLayer, cfg, decode_bbox_target = install_reference()
     out = {}
     for name, mode, nms_type, dist_based, B, N, seed in CASES:
         cfg.RPN.NMS_TYPE = nms_type
@@ -82,7 +88,6 @@ def main():
         out[name + "_scores"] = sc.numpy()
         print(name, boxes.shape, "non-empty rows per scene:", [(sc[b] != 0).sum().item() for b in range(B)])
     # decode alone (all points of one case), to pin the arithmetic
-    from lib.utils.bbox_transform import decode_bbox_target
     scores, reg, xyz = rpn_outputs(2, 4096, 106)
     dec = decode_bbox_target(torch.from_numpy(xyz).view(-1, 3), torch.from_numpy(reg).view(-1, 76),
                              anchor_size=torch.from_numpy(cfg.CLS_MEAN_SIZE[0]), loc_scope=cfg.RPN.LOC_SCOPE,

@@ -19,14 +19,25 @@ from . import oracle as O
 F = np.float32
 
 
+def _argmax(a):
+    """torch.argmax over dim 1: the first maximum, and the first NaN when a row holds one (np.argmax agrees)"""
+    return np.argmax(a, axis=1)
+
+
+def descending(scores):
+    """torch.sort(descending=True)'s order where no two scores tie: NaN first, then the values from the largest"""
+    s = np.asarray(scores, dtype=F)
+    return np.lexsort((-np.where(np.isnan(s), F(0), s), ~np.isnan(s)))
+
+
 def decode_bbox_target(xyz, pred_reg, anchor_size, loc_scope, loc_bin_size, num_head_bin, get_xz_fine=True):
     """xyz (N,3), pred_reg (N,C) -> (N,7) [x, y, z, h, w, l, ry]; bbox_transform.py:40-121"""
     xyz = np.asarray(xyz, dtype=F)
     reg = np.asarray(pred_reg, dtype=F)
     anchor = np.asarray(anchor_size, dtype=F)
     nb = int(loc_scope / loc_bin_size) * 2                                   # :41
-    x_bin = np.argmax(reg[:, 0:nb], axis=1)                                  # :49
-    z_bin = np.argmax(reg[:, nb:2 * nb], axis=1)                             # :50
+    x_bin = _argmax(reg[:, 0:nb])                                           # :49
+    z_bin = _argmax(reg[:, nb:2 * nb])                                      # :50
     pos_x = x_bin.astype(F) * F(loc_bin_size) + F(loc_bin_size / 2) - F(loc_scope)   # :52
     pos_z = z_bin.astype(F) * F(loc_bin_size) + F(loc_bin_size / 2) - F(loc_scope)   # :53
     start = 2 * nb
@@ -38,13 +49,14 @@ def decode_bbox_target(xyz, pred_reg, anchor_size, loc_scope, loc_bin_size, num_
         start = 4 * nb
     pos_y = xyz[:, 1] + reg[:, start]                                        # :84
     start += 1
-    ry_bin = np.argmax(reg[:, start:start + num_head_bin], axis=1)           # :90
+    ry_bin = _argmax(reg[:, start:start + num_head_bin])                    # :90
     ry_res_norm = np.take_along_axis(reg[:, start + num_head_bin:start + 2 * num_head_bin], ry_bin[:, None], axis=1)[:, 0]
     angle_per_class = (2 * np.pi) / num_head_bin                             # :98
     ry_res = ry_res_norm * F(angle_per_class / 2)                            # :99
     ry = ry_bin.astype(F) * F(angle_per_class) + ry_res                      # :102
     two_pi = F(2 * np.pi)
-    m = np.fmod(ry, two_pi)                                                  # torch.remainder = fmod, then sign fix-up
+    with np.errstate(invalid="ignore"):                                      # an infinite or NaN ry gives NaN
+        m = np.fmod(ry, two_pi)                                              # torch.remainder = fmod, then sign fix-up
     m = np.where((m != 0) & (m < 0), m + two_pi, m).astype(F)
     ry = m
     ry = np.where(ry > F(np.pi), ry - two_pi, ry).astype(F)                  # :103
@@ -70,13 +82,14 @@ def boxes3d_to_bev(boxes3d):
 
 def _nms(boxes_bev, scores, thresh, nms_type):
     """iou3d_utils.py:56-87: sort by score (descending), NMS at the C++ boundary, map back"""
-    order = np.argsort(-scores, kind="stable")
+    order = descending(scores)
     keep = O.nms(np.ascontiguousarray(boxes_bev[order]), float(thresh), normal=(nms_type == "normal"))
     return order[keep]
 
 
-def distance_based_proposal(scores, proposals, order, pre_tot, post_tot, thresh, nms_type):
-    """proposal_layer.py:58-118"""
+def distance_based_proposal(scores, proposals, order, pre_tot, post_tot, thresh, nms_type, near_empty="raise"):
+    """proposal_layer.py:58-118.  With nothing in (0, 40] the reference stops on `assert i == 2`; near_empty="far_only"
+    is the device's rule instead: the near range contributes no rows and the far range its survivors, from row 0"""
     ranges = [0, 40.0, 80.0]
     pre = [0, int(pre_tot * 0.7), pre_tot - int(pre_tot * 0.7)]
     post = [0, int(post_tot * 0.7), post_tot - int(post_tot * 0.7)]
@@ -88,8 +101,10 @@ def distance_based_proposal(scores, proposals, order, pre_tot, post_tot, thresh,
         mask = (dist > ranges[i - 1]) & (dist <= ranges[i])
         if mask.sum() != 0:
             cs, cp = s_o[mask][:pre[i]], p_o[mask][:pre[i]]
+        elif i == 1 and near_empty == "far_only":
+            continue
         else:
-            assert i == 2
+            assert i == 2, "%d" % i
             cs, cp = s_o[first][pre[i - 1]:][:pre[i]], p_o[first][pre[i - 1]:][:pre[i]]
         keep = _nms(boxes3d_to_bev(cp), cs, thresh, nms_type)[:post[i]]
         s_list.append(cs[keep])
@@ -105,8 +120,11 @@ def score_based_proposal(scores, proposals, order, pre_tot, post_tot, thresh):
 
 
 def proposal_layer(rpn_scores, rpn_reg, xyz, anchor_size, loc_scope=3.0, loc_bin_size=0.5, num_head_bin=12, get_xz_fine=True,
-                   pre_nms_top_n=9000, post_nms_top_n=100, nms_thresh=0.8, nms_type="normal", distance_based=True):
-    """proposal_layer.py:15-56 -> (ret_bbox3d (B,post,7), ret_scores (B,post))"""
+                   pre_nms_top_n=9000, post_nms_top_n=100, nms_thresh=0.8, nms_type="normal", distance_based=True, order=None,
+                   near_empty="raise"):
+    """proposal_layer.py:15-56 -> (ret_bbox3d (B,post,7), ret_scores (B,post)).  order (B,N): the per-scene score order
+    to use instead of `descending` (the device's own torch.sort, so that how tied scores fall is the device's);
+    near_empty: see distance_based_proposal"""
     scores = np.asarray(rpn_scores, dtype=F)
     B, N = scores.shape
     prop = decode_bbox_target(np.asarray(xyz, F).reshape(-1, 3), np.asarray(rpn_reg, F).reshape(B * N, -1), anchor_size,
@@ -116,11 +134,12 @@ def proposal_layer(rpn_scores, rpn_reg, xyz, anchor_size, loc_scope=3.0, loc_bin
     ret_b = np.zeros((B, post_nms_top_n, 7), dtype=F)
     ret_s = np.zeros((B, post_nms_top_n), dtype=F)
     for k in range(B):
-        order = np.argsort(-scores[k], kind="stable")                          # :36 (ties: torch.sort is unstable; none in the tests)
+        # :36.  torch.sort need not order tied scores as `descending` does: tests with ties pass the device's order
+        o = descending(scores[k]) if order is None else np.asarray(order[k])
         if distance_based:
-            s, p = distance_based_proposal(scores[k], prop[k], order, pre_nms_top_n, post_nms_top_n, nms_thresh, nms_type)
+            s, p = distance_based_proposal(scores[k], prop[k], o, pre_nms_top_n, post_nms_top_n, nms_thresh, nms_type, near_empty)
         else:
-            s, p = score_based_proposal(scores[k], prop[k], order, pre_nms_top_n, post_nms_top_n, nms_thresh)
+            s, p = score_based_proposal(scores[k], prop[k], o, pre_nms_top_n, post_nms_top_n, nms_thresh)
         ret_b[k, :p.shape[0]] = p
         ret_s[k, :s.shape[0]] = s
     return ret_b, ret_s

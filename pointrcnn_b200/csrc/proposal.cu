@@ -35,12 +35,12 @@ __global__ void __launch_bounds__(256) decode_proposals_kernel(const DecodeParam
     const float *r = p.reg + i * p.c;
     const float *q = p.xyz + i * 3;
     const int nb = p.nb;
-    auto argmax = [&](int lo, int cnt) {          // first maximum, as torch.argmax
+    auto argmax = [&](int lo, int cnt) {          // first maximum, as torch.argmax: a NaN is the maximum
         int best = 0;
         float bv = __ldg(r + lo);
         for (int k = 1; k < cnt; ++k) {
             const float v = __ldg(r + lo + k);
-            if (v > bv) { bv = v; best = k; }
+            if (v > bv || (v != v && bv == bv)) { bv = v; best = k; }
         }
         return best;
     };

@@ -198,6 +198,30 @@ def check(got, exact, bnd):
     return bool((ratio <= 1).all()), float(ratio.max(initial=0.0)), int((ratio > 1).sum())
 
 
+# ------------------------------------------------------------------------------------------------------ the device anchor
+def anchor_iou(a_bev, b_bev):
+    """the device's BEV IoU matrix kernel (prb_boxes_iou_bev) on two CUDA (n, 5) tensors: the anchor every NMS consumer
+    must equal bit for bit, pinned to the reference's own kernel by test_gpu_iou_geometry.py"""
+    import torch
+    from pointrcnn_b200.ext import iou3d_cuda
+    out = torch.zeros((a_bev.shape[0], b_bev.shape[0]), dtype=torch.float32, device=a_bev.device)
+    iou3d_cuda.boxes_iou_bev_gpu(a_bev.contiguous(), b_bev.contiguous(), out)
+    return out
+
+
+def greedy(iou, thresh):
+    """greedy NMS in row order over an (n, n) IoU matrix, the suppressor first: keep i iff no kept k < i has
+    iou[k, i] > thresh (the kernels' comparison: a NaN IoU suppresses nothing) -> kept positions"""
+    hit = np.asarray(iou) > np.float32(thresh)
+    removed = np.zeros(hit.shape[0], bool)
+    kept = []
+    for i in range(hit.shape[0]):
+        if not removed[i]:
+            kept.append(i)
+            removed |= hit[i]
+    return kept
+
+
 # ------------------------------------------------------------------------------------------------------ pair families
 PLACES = ("near", "far")
 # families whose every pair must be classified ill-conditioned

@@ -37,10 +37,7 @@ def anchor_overlap(a_bev, b_bev):
     return out
 
 
-def anchor_iou(a_bev, b_bev):
-    out = torch.zeros((a_bev.shape[0], b_bev.shape[0]), dtype=torch.float32, device=a_bev.device)
-    iou3d_cuda.boxes_iou_bev_gpu(a_bev.contiguous(), b_bev.contiguous(), out)
-    return out
+anchor_iou = I.anchor_iou
 
 
 def same(x, y):
@@ -164,14 +161,6 @@ def test_nms_mask_is_the_anchor_iou_over_the_threshold(cuda, fams, thresh, norma
 
 
 # ------------------------------------------------------------------------------------------------ proposal NMS
-def _greedy(iou, thresh):
-    kept = []
-    for i in range(iou.shape[0]):
-        if all(not (iou[k, i] > np.float32(thresh)) for k in kept):       # the kernel's comparison: a NaN IoU suppresses nothing
-            kept.append(i)
-    return kept
-
-
 @pytest.mark.parametrize("thresh", [0.1, 0.7, 0.85])
 def test_proposal_nms_keeps_the_greedy_scan_over_the_anchor(cuda, fams, thresh):
     """the proposal kernel's in-kernel NMS (kept boxes and each 32-candidate chunk precomputed in shared memory, the
@@ -198,7 +187,7 @@ def test_proposal_nms_keeps_the_greedy_scan_over_the_anchor(cuda, fams, thresh):
     for s in range(b):
         o = order[s].cpu().numpy()
         bev = T(I.to_bev(boxes[s][o]), cuda)
-        want = _greedy(anchor_iou(bev, bev).cpu().numpy(), thresh)
+        want = I.greedy(anchor_iou(bev, bev).cpu().numpy(), thresh)
         pos = {float(v): k for k, v in enumerate(scores[s][o])}
         got = [pos[float(v)] for v in got_s[s] if v != 0]
         assert got == want, "scene %d: keep list of %d differs from the anchor's greedy scan of %d" % (s, len(got), len(want))
