@@ -305,9 +305,12 @@ def trimmed_gt(gt):
     return gt[:nz[-1] + 1] if nz.size else gt[:0]
 
 
-def sample_scene(scene, cfg=None, draw="numpy", iou="exact", rng=np.random, seed=0, scene_index=0, train=True, recipe="loader"):
+def sample_scene(scene, cfg=None, draw="numpy", iou="exact", rng=np.random, seed=0, scene_index=0, train=True, recipe="loader",
+                 iou3d=None):
     """scene: dict rpn_xyz (N,3), rpn_features (N,C), rpn_intensity (N,), seg_mask (N,), roi_boxes3d (M,7), gt_boxes3d (G,7),
-    and optionally pts_depth (N,) (the layer's input; else the norm of rpn_xyz).
+    and optionally pts_depth (N,) (the layer's input; else the norm of rpn_xyz).  iou3d: an (M, G) matrix that replaces the
+    IoU of the RoIs with the GT boxes (the columns of GT rows the layer trims are dropped); the jitter loop still computes
+    its own IoUs with `iou`.
     -> dict: status, branch, sel (R,3) [source RoI, GT, tries], iou (R,), rois / gt_of_rois (R,7) before augmentation,
     pooled_input / pooled_features / empty (the pool), pts_input / pts_features, cls_label, reg_valid_mask, gt_boxes3d_ct,
     roi_boxes3d, gt_boxes3d (after augmentation and the canonical transform)"""
@@ -330,8 +333,16 @@ def sample_scene(scene, cfg=None, draw="numpy", iou="exact", rng=np.random, seed
     out = dict(status=0)
     if len(rois_all) == 0 or len(gts_all) == 0:
         return _ignored(out, 2, R, S, E, feats.shape[1])
-    iou3d = iou_matrix(rois_all, gts_all, iou)
-    max_overlaps, gt_assignment = iou3d.max(axis=1), iou3d.argmax(axis=1)
+    if iou3d is None:
+        iou3d = iou_matrix(rois_all, gts_all, iou)
+    else:
+        iou3d = np.asarray(iou3d)
+        assert iou3d.shape[0] == len(rois_all) and iou3d.shape[1] >= len(gts_all), (iou3d.shape, len(rois_all), len(gts_all))
+        iou3d = iou3d[:, :len(gts_all)]
+    # the first maximum (a NaN if the row holds one) and its value, as torch.max(dim=1) returns them; numpy's max can
+    # return a later 0.0 for a leading -0.0, which the loader's reference never reports (its rows always try the jitter)
+    gt_assignment = iou3d.argmax(axis=1)
+    max_overlaps = iou3d[np.arange(len(iou3d)), gt_assignment]
     fg_thresh = min(c["REG_FG_THRESH"], c["CLS_FG_THRESH"])
     fg_inds = np.nonzero(max_overlaps >= fg_thresh)[0]
     if rc["gt_max_fg"]:
@@ -339,6 +350,7 @@ def sample_scene(scene, cfg=None, draw="numpy", iou="exact", rng=np.random, seed
         fg_inds = np.concatenate((fg_inds, roi_assignment[max_iou_of_gt > 0].reshape(-1)), axis=0)
     easy = np.nonzero(max_overlaps < c["CLS_BG_THRESH_LO"])[0]
     hard = np.nonzero((max_overlaps < c["CLS_BG_THRESH"]) & (max_overlaps >= c["CLS_BG_THRESH_LO"]))[0]
+    out["candidates"] = dict(max_overlaps=max_overlaps, gt_assignment=gt_assignment, fg=fg_inds, easy=easy, hard=hard, n_gt=len(gts_all))
     fg_num, bg_num = fg_inds.size, hard.size + easy.size
     fg_quota = int(np.round(c["FG_RATIO"] * R))
     if fg_num > 0 and bg_num > 0:

@@ -146,14 +146,15 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
     if (n == 0 || ng == 0) {
         st = 2;
     } else {
-        // max_overlaps / gt_assignment, max_iou_of_gt / roi_assignment: numpy's first-max argmax
+        // max_overlaps / gt_assignment, max_iou_of_gt / roi_assignment: numpy's first-max argmax, where the first NaN is
+        // the maximum (so a row or column holding a NaN joins no list)
         const float *I = iou + (size_t)scene * m * g;
         for (int i = tid; i < n; i += kRsThreads) {
             float best = I[(size_t)i * g];
             int arg = 0;
             for (int j = 1; j < ng; ++j) {
                 const float v = I[(size_t)i * g + j];
-                if (v > best) { best = v; arg = j; }
+                if (v > best || (v != v && best == best)) { best = v; arg = j; }
             }
             s_maxov[i] = best;
             s_gtas[i] = arg;
@@ -163,7 +164,7 @@ __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
             int arg = 0;
             for (int i = 1; i < n; ++i) {
                 const float v = I[(size_t)i * g + j];
-                if (v > best) { best = v; arg = i; }
+                if (v > best || (v != v && best == best)) { best = v; arg = i; }
             }
             s_roias[j] = best > 0.f ? arg : -1;
         }
