@@ -29,13 +29,14 @@
 extern "C" {
 #endif
 
-#define PRB_ABI_VERSION 9   /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
+#define PRB_ABI_VERSION 10  /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
                              * 5: ordered FPS, input pipeline / KITTI output group, a fused RoI-pooling switch in prb_options;
                              * 6: prb_rcnn_sample_rois / prb_rcnn_roi_targets take the recipe as values (the signatures of
                              *    the former _ex entries, which are gone);
                              * 7: prb_fp_train_forward loses its `project` argument (layer 0 always runs projected);
                              * 8: the unread mlp_* fields are gone;
-                             * 9: the five RoI-pooling fields are gone */
+                             * 9: the five RoI-pooling fields are gone;
+                             * 10: the hash-grid fields other than nn_sort_queries are gone */
 #if defined(__GNUC__)
 #define PRB_API __attribute__((visibility("default")))
 #else
@@ -47,8 +48,8 @@ PRB_API const char *prb_last_error(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches) */
 PRB_API unsigned long long prb_launch_count(void);
 
-/* Per-thread tuning block.  Every heuristic the kernels' launchers apply can be overridden here; 0 / the value
- * prb_options_init() fills in means "library default".  The block is THREAD-LOCAL (each nn.DataParallel worker
+/* Per-thread tuning block of the FPS, MLP-chain and 3-NN grid launchers: each field overrides one of their heuristics;
+ * 0 / the value prb_options_init() fills in means "library default".  The block is THREAD-LOCAL (each nn.DataParallel worker
  * thread owns one), nothing is process-global, and no entry point reads the environment per call: PRB_*
  * environment variables only seed the values prb_options_init() returns, once, when first used. */
 typedef struct prb_options {
@@ -59,11 +60,7 @@ typedef struct prb_options {
     int mlp_occ;       /* >= 1: at most this many chain-kernel CTAs per SM; 0 = as many as registers and shared memory allow */
     int mlp_sms;       /* size the persistent grid for this many SMs; 0 = all */
     int mlp_resident;  /* 1 (default): chain launches whose weights fit run on the resident-weight kernel; 0: always stream */
-    int nn_walk;           /* three_nn on the grid: 0 = 27 unrolled cell walks (default), 1 = one convergent cursor loop per lane (slower) */
     int nn_sort_queries;   /* 1: three_nn groups the queries by grid cell before the search; measured: the sort costs what the locality saves */
-    int grid_csr;      /* 1: hash grid as CSR runs (counting sort per scene) instead of linked lists; slower at the RPN shapes */
-    int grid_debug;    /* 1: print (and synchronise for) the 3-NN grid's fallback counts */
-    float nn_cell;     /* 3-NN grid cell edge in units of the mean point spacing (default 1.6) */
 } prb_options;
 PRB_API void prb_options_init(prb_options *o);                 /* library defaults */
 PRB_API int prb_set_thread_options(const prb_options *o);      /* NULL: back to the defaults */

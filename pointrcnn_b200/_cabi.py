@@ -39,7 +39,7 @@ class SATrainDesc(ctypes.Structure):
 class Options(ctypes.Structure):
     """struct prb_options (per-thread tuning block)"""
     _fields_ = [(k, c_int) for k in ("fps_cluster", "fps_prune", "fps_threads", "fps_generic", "mlp_occ", "mlp_sms", "mlp_resident",
-                                     "nn_walk", "nn_sort_queries", "grid_csr", "grid_debug")] + [("nn_cell", c_float)]
+                                     "nn_sort_queries")]
 
 
 @contextlib.contextmanager
@@ -98,7 +98,7 @@ def lib():
         L.prb_fp_train_backward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P, P, c_size_t, P]
         L.prb_options_init.restype = None
         L.prb_get_thread_options.restype = None
-        if L.prb_abi_version() != 9:
+        if L.prb_abi_version() != 10:
             raise RuntimeError("pointrcnn_b200: ABI version mismatch")
         _lib = L
     return _lib

@@ -28,22 +28,10 @@ constexpr int BQ_CAP = 128;   // candidates per centre handled on the grid path
 
 struct GridView {
     int table_size;           // power of two
-    const int *heads;         // (b, table_size), -1 = empty                      (linked-list form, tables > GB_MAX_TABLE)
-    const float4 *nodes;      // linked lists: (b, n) {x, y, z, next index as int bits}, node i = point i
-                              // CSR form:     (b, n) {x, y, z, point index as int bits}, grouped by hash bucket
+    const int *heads;         // (b, table_size) first node of every hash bucket's list, -1 = empty
+    const float4 *nodes;      // (b, n) {x, y, z, next index as int bits}, node i = point i
     const double *inv_h;      // (b) 1 / cell edge
-    const int2 *range;        // CSR form: (b, table_size) [first, last) node of every bucket
 };
-
-// The CSR form (prb_options.grid_csr, off by default): one CTA per scene counts the points of every hash bucket in shared memory, scans, and scatters
-// the points grouped by bucket.  A bucket is then a contiguous run of 16-byte nodes: its loads are independent of each
-// other, where a linked list is one L2 round trip per candidate.  Order inside a bucket is arbitrary (atomics) and does
-// not matter: both searches are order independent by construction (see above).
-// Not the default at the RPN shapes.  With 2n buckets a bucket holds 0-2 points, so there is no chain to chase, while the single-CTA
-// counting sort adds a serial build per level and the 27 range pairs cost the 3-NN kernel its occupancy.  Kept for dense
-// clouds (many points per cell), where runs do win.
-constexpr int GB_THREADS = 1024;
-constexpr int GB_MAX_TABLE = 32768;      // 128 KB of shared counters
 
 __device__ __forceinline__ int cell_coord(float v, double inv_h) { return (int)floor((double)v * inv_h); }
 __device__ __forceinline__ unsigned cell_hash(int cx, int cy, int cz, int mask) {
@@ -111,6 +99,13 @@ __global__ void __launch_bounds__(256) grid_insert_kernel(int n, int table_size,
     const int nxt = atomicExch(heads + (size_t)scene * table_size + hsh, i);
     nodes[(size_t)scene * n + i] = make_float4(p[0], p[1], p[2], __int_as_float(nxt));
 }
+
+// prb_options.nn_sort_queries (off by default): one CTA per scene counts the 3-NN queries of every hash bucket in shared
+// memory, scans, and scatters the queries grouped by bucket, so that a warp of three_nn_grid_kernel holds queries of one
+// or two cells.  Measured: the sort costs what the locality saves.  Order inside a bucket is arbitrary (atomics) and
+// does not matter: every query's answer is its own.
+constexpr int GB_THREADS = 1024;
+constexpr int GB_MAX_TABLE = 32768;      // 128 KB of shared counters
 
 __global__ void __launch_bounds__(GB_THREADS) grid_build_csr_kernel(int n, int table_size, const float *__restrict__ xyz,
                                                                    const double *__restrict__ inv_h, int2 *__restrict__ range,
@@ -283,91 +278,6 @@ __global__ void __launch_bounds__(GR_THREADS) ball_query_grid_kernel(const GridB
     }
 }
 
-// CSR form: lanes 0..26 look their cell's bucket up, the 27 runs are flattened into one list of node positions (shared
-// memory, no global access), and ALL 32 lanes then test candidates side by side: ceil(total / 32) batches of independent
-// 16-byte loads instead of one dependent chain per cell.  Hits keep their squared distance, the ranking below reads it back.
-constexpr int BQ_LIST = 512;      // candidate positions per centre on the grid path
-template <int NR>
-__global__ void __launch_bounds__(GR_THREADS) ball_query_csr_kernel(const GridBqParams<NR> p) {
-    __shared__ int s_cand[GR_WARPS][BQ_CAP];
-    __shared__ float s_d2[GR_WARPS][BQ_CAP];
-    __shared__ int s_pos[GR_WARPS][BQ_LIST];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int scene = blockIdx.y;
-    const int centre = blockIdx.x * GR_WARPS + warp;
-    if (centre >= p.m) return;                       // whole warp
-    const float *q = p.new_xyz + ((size_t)scene * p.m + centre) * 3;
-    const float cx = q[0], cy = q[1], cz = q[2];
-    const float4 *nodes = p.g.nodes + (size_t)scene * p.n;
-    const double ih = p.g.inv_h[scene];
-    float rmax = p.r2[0];
-#pragma unroll
-    for (int r = 1; r < NR; ++r) rmax = fmaxf(rmax, p.r2[r]);
-    // lane l < 27 owns neighbour cell l; duplicates of a hash bucket are taken once (lowest lane keeps it)
-    int first = 0, cnt_l = 0;
-    if (lane < 27) {
-        const int bx = cell_coord(cx, ih) + lane % 3 - 1, by = cell_coord(cy, ih) + (lane / 3) % 3 - 1, bz = cell_coord(cz, ih) + lane / 9 - 1;
-        const unsigned hsh = cell_hash(bx, by, bz, p.g.table_size - 1);
-        const unsigned same = __match_any_sync(0x07ffffffu, hsh);
-        if ((int)(__ffs(same) - 1) == lane) {
-            const int2 rg = __ldg(p.g.range + (size_t)scene * p.g.table_size + hsh);
-            first = rg.x; cnt_l = rg.y - rg.x;
-        }
-    }
-    int incl = cnt_l;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const int t = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += t; }
-    const int total = __shfl_sync(0xffffffffu, incl, 31);
-    if (total > BQ_LIST) {                           // dense cloud: the scan kernel's early exit is the fast path there
-        if (lane == 0) p.overflow[1 + atomicAdd(p.overflow, 1)] = scene * p.m + centre;
-        return;
-    }
-    for (int e = 0, o = incl - cnt_l; e < cnt_l; ++e) s_pos[warp][o + e] = first + e;
-    __syncwarp();
-    int cnt = 0;                                     // warp-uniform number of candidates inside the largest radius
-    for (int t0 = 0; t0 < total; t0 += 32) {
-        const int t = t0 + lane;
-        bool hit = false;
-        int k = 0;
-        float d2 = 0.f;
-        if (t < total) {
-            const float4 nd = __ldg(nodes + s_pos[warp][t]);
-            d2 = dist2_ref(cx - nd.x, cy - nd.y, cz - nd.z);
-            hit = d2 < rmax;
-            k = __float_as_int(nd.w);
-        }
-        const unsigned hm = __ballot_sync(0xffffffffu, hit);
-        const int pos = cnt + __popc(hm & ((1u << lane) - 1));
-        if (hit && pos < BQ_CAP) { s_cand[warp][pos] = k; s_d2[warp][pos] = d2; }
-        cnt += __popc(hm);
-    }
-    __syncwarp();
-    if (cnt > BQ_CAP) {
-        if (lane == 0) p.overflow[1 + atomicAdd(p.overflow, 1)] = scene * p.m + centre;
-        return;
-    }
-    // rank the hits of each radius by point index; slot k takes the hit of rank k, the tail repeats rank 0
-#pragma unroll
-    for (int r = 0; r < NR; ++r) {
-        int *out = p.idx[r] + ((size_t)scene * p.m + centre) * p.ns[r];
-        int nh = 0, lowest = 0x7fffffff;
-        for (int c0 = 0; c0 < cnt; c0 += 32) {
-            const int c = c0 + lane;
-            const int me = (c < cnt && s_d2[warp][c] < p.r2[r]) ? s_cand[warp][c] : -1;
-            int rank = 0;                            // number of hits of this radius with a smaller index
-            for (int e = 0; e < cnt; ++e) {          // broadcast reads
-                const int o = s_cand[warp][e];
-                rank += (s_d2[warp][e] < p.r2[r] && o < me) ? 1 : 0;
-            }
-            if (me >= 0 && rank < p.ns[r]) out[rank] = me;
-            nh += __popc(__ballot_sync(0xffffffffu, me >= 0));
-            lowest = min(lowest, __reduce_min_sync(0xffffffffu, me >= 0 ? me : 0x7fffffff));
-        }
-        if (nh > 0)
-            for (int sl = nh + lane; sl < p.ns[r]; sl += 32) out[sl] = lowest;
-    }
-}
-
 // brute-force scan for the centres on the overflow list (same code path as ball_query_kernel, one warp per centre)
 template <int NR>
 __global__ void __launch_bounds__(GR_THREADS) ball_query_overflow_kernel(const GridBqParams<NR> p) {
@@ -470,6 +380,8 @@ __global__ void __launch_bounds__(GR_THREADS) three_nn_grid_kernel(const GridNnP
     // All 27 bucket heads are fetched up front (independent loads); the cells are then walked centre-out and a cell
     // whose nearest face is farther than the current third distance is skipped (its points can neither beat nor tie
     // it: the per-axis gaps are shrunk by 0.999 so that rounding on either side cannot make the bound optimistic).
+    // The 27 unrolled walks diverge, and that helps: the diverged lane groups of a warp cover each other's dependent L2
+    // loads, where one convergent cursor loop per lane measured slower.
     int hd[27];
 #pragma unroll
     for (int c = 0; c < 27; ++c)
@@ -497,147 +409,6 @@ __global__ void __launch_bounds__(GR_THREADS) three_nn_grid_kernel(const GridNnP
             nn_insert(d, j, b1, b2, b3, i1, i2, i3);
             j = __float_as_int(nd.w);
             if (++walked > 2048) over = true;
-        }
-    }
-    const float hb = p.h[scene] * 0.9999f;
-    if (over || !(b3 < hb * hb)) {   // something outside the 3x3x3 block could be closer (or tie): brute force decides
-        p.overflow[1 + atomicAdd(p.overflow, 1)] = scene * p.n + u;
-        return;
-    }
-    nn_store(p, ((size_t)scene * p.n + u) * 3, b1, b2, b3, i1, i2, i3);
-}
-
-// The same search as ONE convergent loop per lane (prb_options.nn_walk = 1; MEASURED SLOWER, see the end of this comment).
-// ncu on the kernel above at the
-// finest RPN level (262144 queries): issue slots 78 % busy with 7 of 32 lanes active per instruction -- 27 unrolled cell
-// bodies, each with its own list walk, so lanes that skip a cell or walk a shorter list idle through everybody else's code.
-// Here a lane keeps a cursor (next cell in centre-out order, current node): every iteration either advances the cursor to
-// the next cell that can still hold a better neighbour, or processes one node; all lanes run the same short body.  Bucket
-// heads live in shared memory ([cell][thread], conflict free), the visiting order in a 27-entry shared table.  Same cells,
-// same order per query, same pruning and certification: identical results.
-// Slower than the unrolled kernel: the divergence of the
-// unrolled form is not waste: with independent thread scheduling the diverged lane groups of a warp cover each other's
-// dependent L2 loads like extra warps would; the convergent loop waits for every load with all 32 lanes.
-__global__ void __launch_bounds__(GR_THREADS) three_nn_walk_kernel(const GridNnParams p) {
-    __shared__ int s_hd[27][GR_THREADS];
-    __shared__ int s_order[27];
-    const int scene = blockIdx.y, tid = threadIdx.x;
-    const int t_ = blockIdx.x * GR_THREADS + tid;
-    if (tid < 27) {
-        constexpr int kOrder[27] = {13, 12, 14, 10, 16, 4, 22, 9, 11, 15, 17, 3, 5, 21, 23, 1, 7, 19, 25, 0, 2, 6, 8, 18, 20, 24, 26};
-        int v = 0;
-#pragma unroll
-        for (int i = 0; i < 27; ++i) v = tid == i ? kOrder[i] : v;
-        s_order[tid] = v;
-    }
-    const bool live = t_ < p.n;
-    int u = live ? t_ : 0;
-    float ux = 0.f, uy = 0.f, uz = 0.f;
-    if (live) {
-        if (p.qnodes) {
-            const float4 qn = __ldg(p.qnodes + (size_t)scene * p.n + t_);
-            ux = qn.x; uy = qn.y; uz = qn.z; u = __float_as_int(qn.w);
-        } else {
-            const float *q = p.unknown + ((size_t)scene * p.n + u) * 3;
-            ux = q[0]; uy = q[1]; uz = q[2];
-        }
-    }
-    const float4 *nodes = p.g.nodes + (size_t)scene * p.m;
-    const int *heads = p.g.heads + (size_t)scene * p.g.table_size;
-    const double ih = p.g.inv_h[scene];
-    const int cx = cell_coord(ux, ih), cy = cell_coord(uy, ih), cz = cell_coord(uz, ih);
-#pragma unroll
-    for (int c = 0; c < 27; ++c)
-        s_hd[c][tid] = live ? __ldg(heads + cell_hash(cx + c % 3 - 1, cy + (c / 3) % 3 - 1, cz + c / 9 - 1, p.g.table_size - 1)) : -1;
-    float glo[3], ghi[3];         // squared gaps to the low / high faces of my cell (0 for the middle slab)
-    {
-        const double hd_ = 1.0 / ih;
-        const double f[3] = {(double)ux - (double)cx * hd_, (double)uy - (double)cy * hd_, (double)uz - (double)cz * hd_};
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            const float lo = (float)fmax(f[a] - 1e-9, 0.0) * 0.999f, hi = (float)fmax(hd_ - f[a] - 1e-9, 0.0) * 0.999f;
-            glo[a] = lo * lo; ghi[a] = hi * hi;
-        }
-    }
-    __syncthreads();
-    float b1 = CUDART_INF_F, b2 = CUDART_INF_F, b3 = CUDART_INF_F;
-    int i1 = -1, i2 = -1, i3 = -1;
-    int walked = 0, t = 0, j = -1;
-    bool over = false, done = !live;
-    while (!done) {
-        if (j < 0) {                         // next cell, centre-out, that can still hold a closer (or tying) point
-            while (t < 27) {
-                const int c = s_order[t++];
-                const int ox = c % 3, oy = (c / 3) % 3, oz = c / 9;
-                const float lb = (ox == 0 ? glo[0] : ox == 2 ? ghi[0] : 0.f) + (oy == 0 ? glo[1] : oy == 2 ? ghi[1] : 0.f) +
-                                 (oz == 0 ? glo[2] : oz == 2 ? ghi[2] : 0.f);
-                if (lb > b3) continue;
-                j = s_hd[c][tid];
-                if (j >= 0) break;
-            }
-            if (j < 0) { done = true; continue; }
-        }
-        const float4 nd = __ldg(nodes + j);
-        nn_insert(dist2_ref(ux - nd.x, uy - nd.y, uz - nd.z), j, b1, b2, b3, i1, i2, i3);
-        j = __float_as_int(nd.w);
-        if (++walked > 2048) { over = true; done = true; }
-    }
-    if (!live) return;
-    const float hb = p.h[scene] * 0.9999f;
-    if (over || !(b3 < hb * hb)) {   // something outside the 3x3x3 block could be closer (or tie): brute force decides
-        p.overflow[1 + atomicAdd(p.overflow, 1)] = scene * p.n + u;
-        return;
-    }
-    nn_store(p, ((size_t)scene * p.n + u) * 3, b1, b2, b3, i1, i2, i3);
-}
-
-// CSR form of the kernel above: same walk order, pruning and certification rule; a bucket is a contiguous run, read four
-// nodes at a time (independent loads) instead of one dependent load per candidate
-__global__ void __launch_bounds__(GR_THREADS) three_nn_csr_kernel(const GridNnParams p) {
-    const int scene = blockIdx.y;
-    const int u = blockIdx.x * GR_THREADS + threadIdx.x;
-    if (u >= p.n) return;
-    const float *q = p.unknown + ((size_t)scene * p.n + u) * 3;
-    const float ux = q[0], uy = q[1], uz = q[2];
-    const float4 *nodes = p.g.nodes + (size_t)scene * p.m;
-    const int2 *range = p.g.range + (size_t)scene * p.g.table_size;
-    const double ih = p.g.inv_h[scene];
-    const int cx = cell_coord(ux, ih), cy = cell_coord(uy, ih), cz = cell_coord(uz, ih);
-    float b1 = CUDART_INF_F, b2 = CUDART_INF_F, b3 = CUDART_INF_F;
-    int i1 = -1, i2 = -1, i3 = -1;
-    int walked = 0;
-    bool over = false;
-    int2 rg[27];
-#pragma unroll
-    for (int c = 0; c < 27; ++c)
-        rg[c] = __ldg(range + cell_hash(cx + c % 3 - 1, cy + (c / 3) % 3 - 1, cz + c / 9 - 1, p.g.table_size - 1));
-    float gap[3][3];
-    {
-        const double hd_ = 1.0 / ih;
-        const double f[3] = {(double)ux - (double)cx * hd_, (double)uy - (double)cy * hd_, (double)uz - (double)cz * hd_};
-#pragma unroll
-        for (int a = 0; a < 3; ++a) {
-            const float lo = (float)fmax(f[a] - 1e-9, 0.0) * 0.999f, hi = (float)fmax(hd_ - f[a] - 1e-9, 0.0) * 0.999f;
-            gap[a][0] = lo * lo; gap[a][1] = 0.f; gap[a][2] = hi * hi;
-        }
-    }
-    constexpr int kOrder[27] = {13, 12, 14, 10, 16, 4, 22, 9, 11, 15, 17, 3, 5, 21, 23, 1, 7, 19, 25, 0, 2, 6, 8, 18, 20, 24, 26};
-#pragma unroll
-    for (int t = 0; t < 27; ++t) {
-        const int c = kOrder[t];
-        const float lb = gap[0][c % 3] + gap[1][(c / 3) % 3] + gap[2][c / 9];
-        if (lb > b3) continue;
-        for (int j = rg[c].x; j < rg[c].y && !over; j += 4) {
-            const int nq = min(4, rg[c].y - j);
-            float4 nd[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-                if (e < nq) nd[e] = __ldg(nodes + j + e);
-#pragma unroll
-            for (int e = 0; e < 4; ++e)
-                if (e < nq) nn_insert(dist2_ref(ux - nd[e].x, uy - nd[e].y, uz - nd[e].z), __float_as_int(nd[e].w), b1, b2, b3, i1, i2, i3);
-            walked += nq;
-            if (walked > 2048) over = true;
         }
     }
     const float hb = p.h[scene] * 0.9999f;
@@ -721,54 +492,38 @@ static int table_size_for(int n) {
 
 struct GridWs {
     int table;
-    int *heads, *overflow;
-    float4 *nodes;
-    float4 *qnodes;     // (b, n_queries)
-    int2 *qrange;       // (b, table)
-    double *inv_h;
-    float *h;
+    double *inv_h;      // (b)
+    float *h;           // (b)
+    float4 *nodes;      // (b, n_points)
+    int *heads;         // (b, table)
+    float4 *qnodes;     // (b, n_queries) the queries grouped by bucket (nn_sort_queries)
+    int2 *qrange;       // (b, table) their runs
+    int *overflow;      // count + up to b * n_queries entries
+    size_t bytes;       // from ws to the end of the overflow list
 };
 
-static size_t grid_ws_bytes(int b, int n_points, int n_queries) {
-    const size_t t = (size_t)table_size_for(n_points);
-    // t * 8: CSR ranges (or list heads); second t * 8 + n_queries * 16: the queries grouped by bucket (three_nn)
-    return (size_t)b * t * 16 + (size_t)b * n_points * 16 + (size_t)b * n_queries * 16 + ((size_t)b * n_queries + 64) * 4 + (size_t)b * 16 + 4096;
-}
-
+// The one layout of the grid workspace.  carve(nullptr, ...) measures it, so the size the caller allocates and the
+// regions carved from it cannot disagree.
 static GridWs carve(void *ws, int b, int n_points, int n_queries) {
     GridWs g;
     g.table = table_size_for(n_points);
-    char *c = (char *)(((uintptr_t)ws + 255) & ~(uintptr_t)255);
+    const uintptr_t base = (uintptr_t)ws;
+    uintptr_t c = (base + 255) & ~(uintptr_t)255;
     g.inv_h = (double *)c; c += (((size_t)b * 8 + 255) & ~(size_t)255);
     g.h = (float *)c; c += (((size_t)b * 4 + 255) & ~(size_t)255);
     g.nodes = (float4 *)c; c += (size_t)b * n_points * 16;
-    g.heads = (int *)c; c += (size_t)b * g.table * 8;     // linked-list heads (int) or CSR ranges (int2) live here
+    g.heads = (int *)c; c += (size_t)b * g.table * 4;
     g.qnodes = (float4 *)c; c += (size_t)b * n_queries * 16;
     g.qrange = (int2 *)c; c += (size_t)b * g.table * 8;
-    g.overflow = (int *)c;
-    (void)n_queries;
+    g.overflow = (int *)c; c += ((size_t)b * n_queries + 64) * 4;
+    g.bytes = c - base;
     return g;
 }
 
-static bool use_csr(int table) { return table <= GB_MAX_TABLE && opts().grid_csr != 0; }
+static GridView view_of(const GridWs &w) { return GridView{w.table, w.heads, w.nodes, w.inv_h}; }
 
-static GridView view_of(const GridWs &w, bool csr) {
-    GridView v;
-    v.table_size = w.table; v.heads = csr ? nullptr : w.heads; v.nodes = w.nodes; v.inv_h = w.inv_h;
-    v.range = csr ? reinterpret_cast<const int2 *>(w.heads) : nullptr;
-    return v;
-}
-
-// hash the points of every scene into the table: CSR runs (one CTA per scene) or, for tables beyond the shared-memory
-// counters, linked lists
-static int build_grid(int b, int n, const float *xyz, const GridWs &w, bool csr, cudaStream_t st) {
-    if (csr) {
-        const size_t smem = (size_t)w.table * sizeof(int);
-        if (smem > 48 * 1024)
-            PRB_CUDA(cudaFuncSetAttribute(grid_build_csr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        grid_build_csr_kernel<<<b, GB_THREADS, smem, st>>>(n, w.table, xyz, w.inv_h, reinterpret_cast<int2 *>(w.heads), w.nodes);
-        return check_launch("grid_build_csr_kernel");
-    }
+// hash the points of every scene into the table: one linked list per bucket
+static int build_grid(int b, int n, const float *xyz, const GridWs &w, cudaStream_t st) {
     grid_insert_kernel<<<dim3(ceil_div(n, 256), b), 256, 0, st>>>(n, w.table, xyz, w.inv_h, w.heads, w.nodes);
     return check_launch("grid_insert_kernel");
 }
@@ -779,7 +534,8 @@ using namespace prb;
 
 extern "C" {
 
-PRB_API size_t prb_grid_workspace_bytes(int b, int n_points, int n_queries) { return grid_ws_bytes(b, n_points, n_queries) + 1024; }
+// the layout plus the slack that aligns it on any base
+PRB_API size_t prb_grid_workspace_bytes(int b, int n_points, int n_queries) { return carve(nullptr, b, n_points, n_queries).bytes + 255; }
 
 // ball query for one or two radii through the hash grid; same outputs as prb_ball_query / prb_ball_query_msg2
 PRB_API int prb_ball_query_grid(int b, int n, int m, int nr, const float *radius, const int *nsample, const float *new_xyz,
@@ -794,20 +550,18 @@ PRB_API int prb_ball_query_grid(int b, int n, int m, int nr, const float *radius
     float rmax = radius[0];
     for (int r = 1; r < nr; ++r) rmax = radius[r] > rmax ? radius[r] : rmax;
     PRB_REQUIRE(rmax > 0.f, "ball_query_grid: radius must be positive");
-    const bool csr = use_csr(w.table);
-    if (!csr) PRB_CUDA(cudaMemsetAsync(w.heads, 0xff, (size_t)b * w.table * 4, st));
+    PRB_CUDA(cudaMemsetAsync(w.heads, 0xff, (size_t)b * w.table * 4, st));
     PRB_CUDA(cudaMemsetAsync(w.overflow, 0, 4, st));
     grid_set_cell_kernel<<<ceil_div(b, 128), 128, 0, st>>>(b, (double)rmax * 1.0001, w.inv_h, w.h);
     if (int rc = check_launch("grid_set_cell_kernel")) return rc;
-    if (int rc = build_grid(b, n, xyz, w, csr, st)) return rc;
+    if (int rc = build_grid(b, n, xyz, w, st)) return rc;
     const dim3 grid(ceil_div(m, GR_WARPS), b);
     const int ogrid = 2 * num_sms();
     if (nr == 1) {
         GridBqParams<1> p;
         p.b = b; p.n = n; p.m = m; p.r2[0] = radius[0] * radius[0]; p.ns[0] = nsample[0]; p.idx[0] = idx[0];
-        p.new_xyz = new_xyz; p.xyz = xyz; p.g = view_of(w, csr); p.overflow = w.overflow;
-        if (csr) ball_query_csr_kernel<1><<<grid, GR_THREADS, 0, st>>>(p);
-        else ball_query_grid_kernel<1><<<grid, GR_THREADS, 0, st>>>(p);
+        p.new_xyz = new_xyz; p.xyz = xyz; p.g = view_of(w); p.overflow = w.overflow;
+        ball_query_grid_kernel<1><<<grid, GR_THREADS, 0, st>>>(p);
         if (int rc = check_launch("ball_query_grid_kernel<1>")) return rc;
         ball_query_overflow_kernel<1><<<ogrid, GR_THREADS, 0, st>>>(p);
         return check_launch("ball_query_overflow_kernel<1>");
@@ -815,9 +569,8 @@ PRB_API int prb_ball_query_grid(int b, int n, int m, int nr, const float *radius
     GridBqParams<2> p;
     p.b = b; p.n = n; p.m = m;
     for (int r = 0; r < 2; ++r) { p.r2[r] = radius[r] * radius[r]; p.ns[r] = nsample[r]; p.idx[r] = idx[r]; }
-    p.new_xyz = new_xyz; p.xyz = xyz; p.g = view_of(w, csr); p.overflow = w.overflow;
-    if (csr) ball_query_csr_kernel<2><<<grid, GR_THREADS, 0, st>>>(p);
-    else ball_query_grid_kernel<2><<<grid, GR_THREADS, 0, st>>>(p);
+    p.new_xyz = new_xyz; p.xyz = xyz; p.g = view_of(w); p.overflow = w.overflow;
+    ball_query_grid_kernel<2><<<grid, GR_THREADS, 0, st>>>(p);
     if (int rc = check_launch("ball_query_grid_kernel<2>")) return rc;
     ball_query_overflow_kernel<2><<<ogrid, GR_THREADS, 0, st>>>(p);
     return check_launch("ball_query_overflow_kernel<2>");
@@ -833,23 +586,19 @@ PRB_API int prb_three_nn_grid(int b, int n, int m, const float *unknown, const f
     PRB_REQUIRE((long)b * m < 0x7fffffffL && (long)b * n < 0x7fffffffL, "three_nn_grid: too many points");
     cudaStream_t st = (cudaStream_t)stream;
     GridWs w = carve(workspace, b, m, n);
-    const bool csr = use_csr(w.table);
-    if (!csr) PRB_CUDA(cudaMemsetAsync(w.heads, 0xff, (size_t)b * w.table * 4, st));
+    PRB_CUDA(cudaMemsetAsync(w.heads, 0xff, (size_t)b * w.table * 4, st));
     PRB_CUDA(cudaMemsetAsync(w.overflow, 0, 4, st));
-    // cell edge = factor * mean point spacing.  A query is certified only if its third neighbour is closer than one
+    // cell edge = 1.6 x mean point spacing.  A query is certified only if its third neighbour is closer than one
     // cell, everything else falls back to the exhaustive scan; the centre-out walk skips cells beyond the current
     // third distance.
-    double factor = opts().nn_cell > 0.2f && opts().nn_cell < 50.f ? (double)opts().nn_cell : 1.6;
-    grid_cell_from_bbox_kernel<<<b, 256, 0, st>>>(m, known, factor, w.inv_h, w.h);
+    grid_cell_from_bbox_kernel<<<b, 256, 0, st>>>(m, known, 1.6, w.inv_h, w.h);
     if (int rc = check_launch("grid_cell_from_bbox_kernel")) return rc;
-    if (int rc = build_grid(b, m, known, w, csr, st)) return rc;
+    if (int rc = build_grid(b, m, known, w, st)) return rc;
     GridNnParams p;
     p.b = b; p.n = n; p.m = m; p.unknown = unknown; p.known = known; p.dist2 = dist2; p.weight = weight; p.idx = idx;
-    p.g = view_of(w, csr); p.h = w.h; p.overflow = w.overflow;
+    p.g = view_of(w); p.h = w.h; p.overflow = w.overflow;
     p.qnodes = nullptr;
-    if (!csr && w.table <= GB_MAX_TABLE && opts().nn_sort_queries) {
-        // group the QUERIES by hash bucket of the same grid (counting sort, one CTA per scene): a warp then holds queries of one
-        // or two cells and its 27 head loads / node walks hit L1 instead of pulling one L2 sector per lane
+    if (w.table <= GB_MAX_TABLE && opts().nn_sort_queries) {
         const size_t smem = (size_t)w.table * sizeof(int);
         if (smem > 48 * 1024)
             PRB_CUDA(cudaFuncSetAttribute(grid_build_csr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -857,18 +606,10 @@ PRB_API int prb_three_nn_grid(int b, int n, int m, const float *unknown, const f
         if (int rc = check_launch("grid_build_csr_kernel(queries)")) return rc;
         p.qnodes = w.qnodes;
     }
-    if (csr) three_nn_csr_kernel<<<dim3(ceil_div(n, GR_THREADS), b), GR_THREADS, 0, st>>>(p);
-    else if (opts().nn_walk == 1) three_nn_walk_kernel<<<dim3(ceil_div(n, GR_THREADS), b), GR_THREADS, 0, st>>>(p);
-    else three_nn_grid_kernel<<<dim3(ceil_div(n, GR_THREADS), b), GR_THREADS, 0, st>>>(p);
+    three_nn_grid_kernel<<<dim3(ceil_div(n, GR_THREADS), b), GR_THREADS, 0, st>>>(p);
     if (int rc = check_launch("three_nn_grid_kernel")) return rc;
     three_nn_overflow_kernel<<<4 * num_sms(), GR_THREADS, 0, st>>>(p);
     if (int rc = check_launch("three_nn_overflow_kernel")) return rc;
-    if (opts().grid_debug) {   // diagnostics only: synchronises
-        int cnt = 0;
-        PRB_CUDA(cudaMemcpyAsync(&cnt, w.overflow, 4, cudaMemcpyDeviceToHost, st));
-        PRB_CUDA(cudaStreamSynchronize(st));
-        fprintf(stderr, "[prb] three_nn_grid b=%d n=%d m=%d cell factor %.2f: %d of %ld queries left to the exhaustive scan\n", b, n, m, factor, cnt, (long)b * n);
-    }
     return 0;
 }
 

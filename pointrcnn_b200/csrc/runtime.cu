@@ -44,12 +44,7 @@ static prb_options make_defaults() {
     o.mlp_occ = env_int("PRB_MLP_OCC", 0);
     o.mlp_sms = env_int("PRB_MLP_SMS", 0);
     o.mlp_resident = env_int("PRB_MLP_RESIDENT", 1);
-    o.nn_walk = env_int("PRB_NN_WALK", 0);
     o.nn_sort_queries = env_int("PRB_NN_SORT_QUERIES", 0);
-    o.grid_csr = env_int("PRB_GRID_CSR", 0);
-    o.grid_debug = env_int("PRB_GRID_DEBUG", 0);
-    o.nn_cell = 1.6f;
-    if (const char *e = getenv("PRB_NN_CELL")) { float v = (float)atof(e); if (v > 0.2f && v < 50.f) o.nn_cell = v; }
     return o;
 }
 static const prb_options &defaults() {

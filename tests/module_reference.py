@@ -34,6 +34,8 @@ the terms that lie between the module and the packed image:
 A layer with input a (bound e), folded weight Wt = inv W, weight error Wr = rho |Wt| and M = |Wt| + Wr:
     bound = gamma(K_pad) (|a| + e) M^T + e M^T + |a| Wr^T + shift bound, then the epilogue and TF32 roundings above.
 """
+import gc
+
 import torch
 
 import mlp_reference as R
@@ -228,10 +230,17 @@ def seeded(module, seed):
 def replace_parameter(module, name, data):
     """module.<name> replaced by nn.Parameter(data), with `data` allocated by the caller while the old parameter is still
     alive: the new Parameter object then takes the slot the old one frees, so when nothing else holds the old parameter
-    the new one has its id() (and, like it if it was fresh, version 0).  Returns whether the id() was reused."""
+    the new one has its id() (and, like it if it was fresh, version 0).  Returns whether the id() was reused.  The cyclic
+    collector is held off meanwhile: a collection between the two steps frees other objects whose slots come first."""
     old_id = id(getattr(module, name))
-    delattr(module, name)
-    setattr(module, name, torch.nn.Parameter(data))
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        delattr(module, name)
+        setattr(module, name, torch.nn.Parameter(data))
+    finally:
+        if enabled:
+            gc.enable()
     return id(getattr(module, name)) == old_id
 
 

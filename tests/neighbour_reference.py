@@ -280,6 +280,22 @@ def nn_cell_edge(n, m, seed):
     return _f32(unknown), known, len(pockets)
 
 
+def nn_stack(n, m, seed, stack=2100, k=8):
+    """(unknown (n,3), known (m,3), k) for the 3-NN grid's walk cap: the known bounding box pinned to the scope, so h is
+    known here, and `stack` known points in the middle of one cell, more than the 2048 nodes a query walks before it
+    leaves itself to the exhaustive scan; the first k queries sit in that cell"""
+    rng = np.random.default_rng(seed)
+    known = _f32(SCOPE_LO + (SCOPE_HI - SCOPE_LO) * rng.random((m, 3)))
+    known[0], known[1] = SCOPE_LO, SCOPE_HI
+    h = nn_cell(known)
+    centre = (np.floor(np.array([1.0, 1.0, 30.0]) / h) + 0.5) * h
+    known[2:2 + stack] = _f32(centre + rng.uniform(-0.3, 0.3, (stack, 3)) * h)
+    known = known[np.concatenate([[0, 1], 2 + rng.permutation(m - 2)])]
+    q = _f32(centre + rng.uniform(-0.3, 0.3, (k, 3)) * h)
+    unknown = np.concatenate([q, _f32(SCOPE_LO + (SCOPE_HI - SCOPE_LO) * rng.random((n - k, 3)))])
+    return _f32(unknown), _f32(known), k
+
+
 # ------------------------------------------------------------------------------------------------ caps
 CAP_SIZES = (15, 16, 17, 31, 32, 33, 63, 64, 65, 127, 128, 129, 200)
 
@@ -287,7 +303,7 @@ CAP_SIZES = (15, 16, 17, 31, 32, 33, 63, 64, 65, 127, 128, 129, 200)
 def caps(n, seed, radii=(0.1, 0.5)):
     """one centre per cluster size: `size` points strictly inside the smaller radius (so inside both), nothing else in
     reach; plus a centre with a 600-point stack in a corner cell of its 3x3x3 block (outside the radius) that overflows
-    the list walk and the CSR position list.  Returns (cloud, centres, sizes) with size -1 for the stack centre"""
+    the list walk's cap of 512 nodes.  Returns (cloud, centres, sizes) with size -1 for the stack centre"""
     rng = np.random.default_rng(seed)
     r0, rmax = min(radii), max(radii)
     h = bq_cell(rmax)

@@ -68,7 +68,7 @@ def test_caps_clusters_hit_every_dispatch_boundary(caps):
         else:
             cells = np.floor(cloud.astype(np.float64) / h).astype(np.int64)
             block = np.all(np.abs(cells - np.floor(c.astype(np.float64) / h)) <= 1, axis=1)
-            assert block.sum() > 512 and (d < F32(rmax) * F32(rmax)).sum() == 0, "walk / CSR list overflow, no hit"
+            assert block.sum() > 512 and (d < F32(rmax) * F32(rmax)).sum() == 0, "list walk overflow, no hit"
     assert {32, 33, 128, 129, 16, 17}.issubset(sizes)
 
 

@@ -115,14 +115,14 @@ def _bq(x, c, radii, nss):
 
 
 @pytest.mark.parametrize("level", list(BQ_SHAPES) + ["rcnn128", "rcnn32"])
-@pytest.mark.parametrize("path", ["grid", "grid_csr", "brute_msg2", "brute_single"])
+@pytest.mark.parametrize("path", ["grid", "brute_msg2", "brute_single"])
 def test_ball_query_bits_on_adversarial_families(cuda, bq_cases, level, path):
     xyz, cen, radii, nss, want = bq_cases[level]
     x, c = T(xyz, cuda), T(cen, cuda)
     old = pu.GRID_MIN_POINTS_BQ
     pu.GRID_MIN_POINTS_BQ = 1 if path.startswith("grid") else old
     try:
-        with _cabi.options(grid_csr=int(path == "grid_csr")), config.override(disable_grid=path.startswith("brute")):
+        with config.override(disable_grid=path.startswith("brute")):
             if path == "brute_single":
                 got = [pu.ball_query(r, ns, x, c) for r, ns in zip(radii, nss)]
             else:
@@ -135,17 +135,15 @@ def test_ball_query_bits_on_adversarial_families(cuda, bq_cases, level, path):
         assert bad[0].size == 0, "r=%g: %d centres differ, first (scene, centre) %s" % (r, bad[0].size, list(zip(*bad))[:4])
 
 
-def test_ball_query_batch_equals_per_scene(cuda, bq_cases):
+def test_ball_query_grid_batch_equals_per_scene(cuda, bq_cases):
     """overflow-list entries and workspace offsets are per scene: the batch answer is each scene's own answer"""
     xyz, cen, radii, nss, _ = bq_cases["sa1"]
     x, c = T(xyz, cuda), T(cen, cuda)
-    for csr in (0, 1):
-        with _cabi.options(grid_csr=csr):
-            full = _bq(x, c, radii, nss)
-            for s in (0, 2, 5, 8, 15):                        # shell, caps, far1e6, nonfinite, lidar
-                one = _bq(x[s:s + 1].contiguous(), c[s:s + 1].contiguous(), radii, nss)
-                for a, b in zip(full, one):
-                    assert torch.equal(a[s:s + 1], b), (csr, s)
+    full = _bq(x, c, radii, nss)
+    for s in (0, 2, 5, 8, 15):                                # shell, caps, far1e6, nonfinite, lidar
+        one = _bq(x[s:s + 1].contiguous(), c[s:s + 1].contiguous(), radii, nss)
+        for a, b in zip(full, one):
+            assert torch.equal(a[s:s + 1], b), s
 
 
 # ------------------------------------------------------------------------------------------------ three_nn
@@ -162,13 +160,18 @@ def nn_cases():
         if m >= 512:                                          # certification pockets and cell-boundary queries
             for s, seed in ((6, 1), (7, 2)):
                 unknown[s], known[s], _ = NR.nn_cell_edge(n, m, seed)
+        if (n, m) == (16384, 4096):                           # the walk cap: more than 2048 known points in a query's cell
+            unknown[8], known[8], k = NR.nn_stack(n, m, 3)
+            inv_h = 1.0 / NR.nn_cell(known[8])
+            cells = np.floor(known[8].astype(np.float64) * inv_h)
+            for q in np.floor(unknown[8, :k].astype(np.float64) * inv_h):
+                assert (cells == q).all(axis=1).sum() > 2048
         d2, idx = O.three_nn(unknown, known)
         out[(n, m)] = (unknown, known, d2, idx)
     return out
 
 
-NN_MODES = {"plain": {}, "sorted_queries": {"nn_sort_queries": 1}, "walk": {"nn_walk": 1}, "csr": {"grid_csr": 1},
-            "cell_0.5": {"nn_cell": 0.5}, "cell_4.0": {"nn_cell": 4.0}, "brute": None}
+NN_MODES = {"plain": {}, "sorted_queries": {"nn_sort_queries": 1}, "brute": None}
 
 
 @pytest.mark.parametrize("n,m", NN_SHAPES)
@@ -185,8 +188,7 @@ def test_three_nn_bits_on_adversarial_families(cuda, nn_cases, n, m, mode):
     np.testing.assert_allclose(w.cpu().numpy(), O.interp_weights(d2), rtol=2e-6, atol=1e-7, equal_nan=True)
 
 
-@pytest.mark.parametrize("mode", ["plain", "csr"])
-def test_three_nn_grid_query_at_infinity_lists_point_zero(cuda, mode):
+def test_three_nn_grid_query_at_infinity_lists_point_zero(cuda):
     """every distance from a query at infinity is inf (or NaN), so the reference's cascade, started at 1e40, takes none of
     them and answers indices (0, 0, 0) at distance inf.  The grid sends such a query to its exhaustive kernel, which
     used to fill its empty slots through the index tie-break (inf == inf) and answer (0, 1, 2)."""
@@ -197,8 +199,7 @@ def test_three_nn_grid_query_at_infinity_lists_point_zero(cuda, mode):
     unknown[0, 17, 2] = np.inf
     d2, idx = O.three_nn(unknown, known)
     assert (idx[0, [5, 9, 17]] == 0).all() and np.isinf(d2[0, [5, 9, 17]]).all()
-    with _cabi.options(**NN_MODES[mode]):
-        got_d2, got_idx, _ = pu.three_nn_weights(T(unknown, cuda), T(known, cuda))
+    got_d2, got_idx, _ = pu.three_nn_weights(T(unknown, cuda), T(known, cuda))
     assert np.array_equal(got_idx.cpu().numpy(), idx)
     assert np.array_equal(got_d2.cpu().numpy(), d2)
 

@@ -636,9 +636,7 @@ def test_iou3d_utils_api(cuda):
     ("cube", 300, 40, (0.2,), (16,)),                # tiny set through the grid, single radius
     ("kitti", 5000, 777, (2.0, 4.0), (16, 32)),      # n not a power of two, big balls
 ])
-@pytest.mark.parametrize("csr", [0, 1])                # linked lists (default) / CSR runs
-def test_ball_query_grid_path_exact(cuda, kind, N, M, radii, nss, csr):
-    from pointrcnn_b200 import _cabi
+def test_ball_query_grid_path_exact(cuda, kind, N, M, radii, nss):
     xyz = _cloud(kind, 2, N, 51 + N)
     fidx = O.fps(xyz, M)
     new_xyz = np.stack([xyz[b][fidx[b]] for b in range(2)])
@@ -646,33 +644,30 @@ def test_ball_query_grid_path_exact(cuda, kind, N, M, radii, nss, csr):
     old = pu.GRID_MIN_POINTS_BQ
     pu.GRID_MIN_POINTS_BQ = 1
     try:
-        with _cabi.options(grid_csr=csr):
-            if len(radii) == 2:
-                got = pu.ball_query_msg2(radii, nss, x, c)
-            else:
-                got = [pu.ball_query(radii[0], nss[0], x, c)]
+        if len(radii) == 2:
+            got = pu.ball_query_msg2(radii, nss, x, c)
+        else:
+            got = [pu.ball_query(radii[0], nss[0], x, c)]
     finally:
         pu.GRID_MIN_POINTS_BQ = old
     for g, r, ns in zip(got, radii, nss):
         assert np.array_equal(g.cpu().numpy(), O.ball_query(r, ns, xyz, new_xyz)), "grid ball query differs (r=%g)" % r
 
 
-@pytest.mark.parametrize("cell", [None, 0.5, 4.0])     # default edge; tiny cells (most queries go to the exhaustive scan); big cells
 @pytest.mark.parametrize("kind,n,m", [("kitti", 8192, 2048), ("cube", 2000, 500), ("dup", 1024, 256), ("cube", 100, 5),
                                       ("kitti", 300, 3), ("dup", 4096, 64)])
-@pytest.mark.parametrize("mode", ["sorted_queries", "plain", "cursor_loop", "csr"])     # queries grouped by cell; default; convergent cursor loop; CSR
-def test_three_nn_grid_path_exact(cuda, kind, n, m, cell, mode):
-    grid_opts = {"sorted_queries": {"nn_sort_queries": 1}, "plain": {}, "cursor_loop": {"nn_walk": 1}, "csr": {"grid_csr": 1}}[mode]
+@pytest.mark.parametrize("mode", ["sorted_queries", "plain"])     # queries grouped by cell; default
+def test_three_nn_grid_path_exact(cuda, kind, n, m, mode):
+    from pointrcnn_b200 import _cabi
     unknown = _cloud(kind, 2, n, 61 + n)
     known = np.ascontiguousarray(unknown[:, ::max(1, n // m)][:, :m])
     if kind == "kitti":
         unknown[0, :10] += 300.0         # far-away queries: third neighbour beyond one cell -> brute-force list
     d2, idx = O.three_nn(unknown, known)
-    from pointrcnn_b200 import _cabi
     old = pu.GRID_MIN_POINTS_NN
     pu.GRID_MIN_POINTS_NN = 1
     try:
-        with _cabi.options(**grid_opts, **({} if cell is None else {"nn_cell": cell})):
+        with _cabi.options(nn_sort_queries=int(mode == "sorted_queries")):
             got_d2, got_idx, w = pu.three_nn_weights(T(unknown, cuda), T(known, cuda))
     finally:
         pu.GRID_MIN_POINTS_NN = old
