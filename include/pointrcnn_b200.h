@@ -29,14 +29,15 @@
 extern "C" {
 #endif
 
-#define PRB_ABI_VERSION 10  /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
+#define PRB_ABI_VERSION 11  /* 3: prb_options (per-thread tuning block; no per-call environment reads); 4: mlp_tune, prb_mlp_rows2;
                              * 5: ordered FPS, input pipeline / KITTI output group, a fused RoI-pooling switch in prb_options;
                              * 6: prb_rcnn_sample_rois / prb_rcnn_roi_targets take the recipe as values (the signatures of
                              *    the former _ex entries, which are gone);
                              * 7: prb_fp_train_forward loses its `project` argument (layer 0 always runs projected);
                              * 8: the unread mlp_* fields are gone;
                              * 9: the five RoI-pooling fields are gone;
-                             * 10: the hash-grid fields other than nn_sort_queries are gone */
+                             * 10: the hash-grid fields other than nn_sort_queries are gone;
+                             * 11: the four fps_* fields are gone */
 #if defined(__GNUC__)
 #define PRB_API __attribute__((visibility("default")))
 #else
@@ -48,15 +49,11 @@ PRB_API const char *prb_last_error(void);
 /* number of kernels this library has launched in this process (bench.py's gpu_launches) */
 PRB_API unsigned long long prb_launch_count(void);
 
-/* Per-thread tuning block of the FPS, MLP-chain and 3-NN grid launchers: each field overrides one of their heuristics;
+/* Per-thread tuning block of the MLP-chain and 3-NN grid launchers: each field overrides one of their heuristics;
  * 0 / the value prb_options_init() fills in means "library default".  The block is THREAD-LOCAL (each nn.DataParallel worker
  * thread owns one), nothing is process-global, and no entry point reads the environment per call: PRB_*
  * environment variables only seed the values prb_options_init() returns, once, when first used. */
 typedef struct prb_options {
-    int fps_cluster;   /* CTAs per scene of the cluster FPS kernel (1,2,4,8); 0 = heuristic */
-    int fps_prune;     /* 0: never use the pruned single-CTA kernel; 1: for 4097..16384 points; 2: also 2049..4096 */
-    int fps_threads;   /* threads per CTA of the rank kernel; 0 = heuristic */
-    int fps_generic;   /* 1: force the generic (reference-shaped) kernel */
     int mlp_occ;       /* >= 1: at most this many chain-kernel CTAs per SM; 0 = as many as registers and shared memory allow */
     int mlp_sms;       /* size the persistent grid for this many SMs; 0 = all */
     int mlp_resident;  /* 1 (default): chain launches whose weights fit run on the resident-weight kernel; 0: always stream */

@@ -38,13 +38,12 @@ class SATrainDesc(ctypes.Structure):
 
 class Options(ctypes.Structure):
     """struct prb_options (per-thread tuning block)"""
-    _fields_ = [(k, c_int) for k in ("fps_cluster", "fps_prune", "fps_threads", "fps_generic", "mlp_occ", "mlp_sms", "mlp_resident",
-                                     "nn_sort_queries")]
+    _fields_ = [(k, c_int) for k in ("mlp_occ", "mlp_sms", "mlp_resident", "nn_sort_queries")]
 
 
 @contextlib.contextmanager
 def options(**kw):
-    """with options(fps_prune=0, mlp_resident=0): ...  -- overrides fields of THIS thread's prb_options for the block.
+    """with options(mlp_resident=0): ...  -- overrides fields of THIS thread's prb_options for the block.
     Thread-local inside the library (prb_set_thread_options): safe under nn.DataParallel worker threads."""
     L = lib()
     old, new = Options(), Options()
@@ -98,7 +97,7 @@ def lib():
         L.prb_fp_train_backward.argtypes = [P, I, I, I, I, I, P, P, P, P, P, P, P, P, P, P, P, P, P, P, c_size_t, P]
         L.prb_options_init.restype = None
         L.prb_get_thread_options.restype = None
-        if L.prb_abi_version() != 10:
+        if L.prb_abi_version() != 11:
             raise RuntimeError("pointrcnn_b200: ABI version mismatch")
         _lib = L
     return _lib

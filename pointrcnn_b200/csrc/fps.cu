@@ -17,8 +17,8 @@
 // warp inside a CTA, lowest CTA inside a cluster.  One __syncthreads per round.  A scene is spread
 // over a thread-block cluster of CS CTAs (CS*THREADS*PPT >= n): each CTA's winner -- distance, rank AND
 // coordinates, 32 bytes -- goes to every peer with two st.async stores that complete a transaction count on the
-// peer's mbarrier (no cluster barrier in the loop).  A CTA mirrors only its OWN points in shared memory (<= 48 KB, so several clusters share an
-// SM); the winner's coordinates travel with the message.  new_xyz is emitted on the fly.
+// peer's mbarrier (no cluster barrier in the loop).  A CTA mirrors only its OWN points in shared memory (<= 96 KB); the
+// winner's coordinates travel with the message.  new_xyz is emitted on the fly.
 #include <limits.h>
 #include <math_constants.h>
 
@@ -29,7 +29,6 @@ namespace prb {
 struct FpsParams {
     int b, n, m;
     int S, logS, Q;      // reference block size, its log2, ceil(n/S)
-    int use_smem_xyz;    // rank-ordered xyz copy fits in shared memory
     const float *xyz;    // (b,n,3)
     float *temp;         // (b,n)
     int *idx;            // (b,m)
@@ -104,7 +103,7 @@ template <int THREADS, int PPT, int CS>
 __global__ void __launch_bounds__(THREADS, 1) fps_rank_kernel(const FpsParams p) {
     constexpr int W = THREADS / 32;
     constexpr int CAP = THREADS * PPT;               // ranks owned by this CTA
-    extern __shared__ __align__(16) float s_pts[];   // xyz of MY ranks (3 floats per rank), optional for CS == 1
+    extern __shared__ __align__(16) float s_pts[];   // xyz of MY ranks (3 floats per rank)
     __shared__ int2 s_wkey[2][kMaxWarps];            // per-warp (dist bits, rank), double buffered
     __shared__ FpsMsg s_slot[2][kMaxCluster];        // per-CTA winners (cluster exchange), double buffered
     __shared__ __align__(8) uint64_t s_bar[2];
@@ -141,11 +140,9 @@ __global__ void __launch_bounds__(THREADS, 1) fps_rank_kernel(const FpsParams p)
             px[i] = py[i] = pz[i] = 0.f;
             pd[i] = -1.f;
         }
-        if (p.use_smem_xyz) {
-            s_pts[(tid * PPT + i) * 3 + 0] = px[i];
-            s_pts[(tid * PPT + i) * 3 + 1] = py[i];
-            s_pts[(tid * PPT + i) * 3 + 2] = pz[i];
-        }
+        s_pts[(tid * PPT + i) * 3 + 0] = px[i];
+        s_pts[(tid * PPT + i) * 3 + 1] = py[i];
+        s_pts[(tid * PPT + i) * 3 + 2] = pz[i];
     }
     __syncthreads();
     if (CS > 1) cluster_sync_all();
@@ -186,12 +183,7 @@ __global__ void __launch_bounds__(THREADS, 1) fps_rank_kernel(const FpsParams p)
         int r = (int)__reduce_min_sync(0xffffffffu, kv.x == cm ? (unsigned)kv.y : 0xffffffffu);   // winning rank, uniform in the CTA
 
         if (CS == 1) {
-            if (p.use_smem_xyz) {
-                cx = s_pts[r * 3 + 0]; cy = s_pts[r * 3 + 1]; cz = s_pts[r * 3 + 2];
-            } else {
-                int k = rank_to_k(r, S, logS, Q);
-                cx = xyz[k * 3 + 0]; cy = xyz[k * 3 + 1]; cz = xyz[k * 3 + 2];
-            }
+            cx = s_pts[r * 3 + 0]; cy = s_pts[r * 3 + 1]; cz = s_pts[r * 3 + 2];
         } else {
             // my CTA's winner (with its coordinates) goes to every CTA of the cluster: two 16-byte st.async per peer
             if (warp == 0 && lane < CS) {
@@ -274,8 +266,9 @@ __global__ void __launch_bounds__(1024, 1) fps_generic_kernel(const FpsParams p)
 }
 
 template <int THREADS, int PPT, int CS>
-static int launch_rank(const FpsParams &p, size_t smem, cudaStream_t stream) {
+static int launch_rank(const FpsParams &p, cudaStream_t stream) {
     auto kern = fps_rank_kernel<THREADS, PPT, CS>;
+    constexpr size_t smem = (size_t)THREADS * PPT * 3 * sizeof(float);   // the CTA's slice of the scene
     // static shared memory counts against the 48 KB default too
     if (smem + 2048 > 48 * 1024) PRB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     cudaLaunchConfig_t cfg = {};
@@ -294,23 +287,22 @@ static int launch_rank(const FpsParams &p, size_t smem, cudaStream_t stream) {
     return check_launch("fps_rank_kernel");
 }
 
-template <int CS>
-static int dispatch_cs(const FpsParams &p, int threads, int ppt, size_t smem, cudaStream_t st) {
-#define PRB_FPS_CASE(T, P) \
-    if (threads == T && ppt == P) return launch_rank<T, P, CS>(p, smem, st);
-    if (CS == 1) {
-        PRB_FPS_CASE(128, 1) PRB_FPS_CASE(128, 2) PRB_FPS_CASE(128, 4)
-        PRB_FPS_CASE(256, 8)
-        PRB_FPS_CASE(1024, 4) PRB_FPS_CASE(1024, 8)
-    }
-    PRB_FPS_CASE(256, 4) PRB_FPS_CASE(512, 2) PRB_FPS_CASE(512, 4) PRB_FPS_CASE(512, 8) PRB_FPS_CASE(512, 16)
+// the (CS, threads, ppt) triples fps_run's configuration reaches, one line per cluster size
+static int dispatch_rank(const FpsParams &p, int cs, int threads, int ppt, cudaStream_t st) {
+#define PRB_FPS_CASE(C, T, P) \
+    if (cs == C && threads == T && ppt == P) return launch_rank<T, P, C>(p, st);
+    PRB_FPS_CASE(1, 128, 1) PRB_FPS_CASE(1, 128, 2) PRB_FPS_CASE(1, 128, 4) PRB_FPS_CASE(1, 256, 4)
+    PRB_FPS_CASE(1, 512, 4) PRB_FPS_CASE(1, 512, 8) PRB_FPS_CASE(1, 512, 16)
+    PRB_FPS_CASE(2, 512, 8) PRB_FPS_CASE(2, 512, 16)
+    PRB_FPS_CASE(4, 512, 4) PRB_FPS_CASE(4, 512, 8) PRB_FPS_CASE(4, 512, 16)
+    PRB_FPS_CASE(8, 256, 4) PRB_FPS_CASE(8, 512, 4) PRB_FPS_CASE(8, 512, 8) PRB_FPS_CASE(8, 512, 16)
 #undef PRB_FPS_CASE
-    set_error("fps: no kernel instance for threads=%d ppt=%d cs=%d", threads, ppt, CS);
+    set_error("fps: no kernel instance for cs=%d threads=%d ppt=%d", cs, threads, ppt);
     return -1;
 }
 
 // ------------------------------------------------------------------------------------------------------------
-// Pruned FPS (n in (2048, 16384]): one CTA per scene, exact.
+// Pruned FPS (n in (4096, 16384]): one CTA per scene, exact.
 //
 // A round only changes temp[k] where |p_k - p_last|^2 < temp[k], i.e. inside the new sample's Voronoi cell (~n/j
 // points in round j).  Points are pre-sorted into spatially compact GROUPS of 32 (k-d ordered cells, counting sort
@@ -323,6 +315,8 @@ static int dispatch_cs(const FpsParams &p, int threads, int ppt, size_t smem, cu
 // Layout: group g = slot * 16 + warp (neighbouring groups go to different warps); lane l of warp w keeps temp and
 // rank of point l of its NS groups in registers (static indexing: the slot loop is unrolled and predicated on the
 // ballot of the box tests, where lane j tests slot j); coordinates live in shared memory as three planes.
+constexpr int kPrunedWarps = 16;
+
 struct FpsSorted {
     float *sx, *sy, *sz, *st;   // (b, np) sorted coordinates and running min distance (pads: st = -1)
     int *srank;                 // (b, np) reference rank of the sorted point (pads: 0xffff)
@@ -496,11 +490,10 @@ __device__ __forceinline__ float redux_min_f32(float v) {
         if (lane == (J)) { gval = mx; gpay = mp; }                                                           \
     } break;
 
-// W warps x NS slots per lane cover the W * NS groups of a scene: <32,16> is the default for 16384 points.  <16,32> (1024
-// threads, prb_options.fps_threads = 1024: fewer touched slots on the busiest warp but a wider CTA arg-max and twice the
-// instruction issue per round) is an option, not the default: the round is bound by the fixed arg-max / barrier chain.
-template <int NS, int W>
-__global__ void __launch_bounds__(32 * W, 1) fps_pruned_kernel(const FpsParams p, const FpsSorted s) {
+// W warps x NS slots per lane cover the W * NS groups of a scene: NS = 32 for 16384 points, 16 for 8192.
+template <int NS>
+__global__ void __launch_bounds__(32 * kPrunedWarps, 1) fps_pruned_kernel(const FpsParams p, const FpsSorted s) {
+    constexpr int W = kPrunedWarps;
     constexpr int NP = W * NS * 32;
     extern __shared__ __align__(16) float s_pl[];       // three planes of NP floats
     __shared__ uint2 s_w[2][W];                         // per-warp winner {temp bits, (0x3fff - rank) << 14 | position}
@@ -605,28 +598,26 @@ using namespace prb;
 
 // pruned path: slots per lane for n points (0 = not applicable)
 static int pruned_slots(int n) {
-    const int mode = opts().fps_prune;   // 0 off, 1 n > 4096, 2 n > 2048
-    if (mode == 0 || n > 16384) return 0;
+    if (n > 16384) return 0;
     if (n > 8192) return 32;
     if (n > 4096) return 16;
-    if (n > 2048 && mode >= 2) return 8;
     return 0;
 }
 
-template <int NS, int W>
+template <int NS>
 static int launch_pruned(const FpsParams &p, const FpsSorted &s, cudaStream_t st) {
-    const size_t smem = (size_t)3 * W * NS * 32 * sizeof(float);
+    const size_t smem = (size_t)3 * kPrunedWarps * NS * 32 * sizeof(float);
     if (smem + 1024 > 48 * 1024)
-        PRB_CUDA(cudaFuncSetAttribute(fps_pruned_kernel<NS, W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        PRB_CUDA(cudaFuncSetAttribute(fps_pruned_kernel<NS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     fps_sort_kernel<<<p.b, 1024, 0, st>>>(p, s);
     if (int rc = check_launch("fps_sort_kernel")) return rc;
-    fps_pruned_kernel<NS, W><<<p.b, 32 * W, smem, st>>>(p, s);
+    fps_pruned_kernel<NS><<<p.b, 32 * kPrunedWarps, smem, st>>>(p, s);
     return check_launch("fps_pruned_kernel");
 }
 
 extern "C" size_t prb_fps_workspace_bytes(int b, int n) {
     const int ns = pruned_slots(n);
-    return ns ? (size_t)b * 16 * ns * 32 * 5 * sizeof(float) + 256 : 0;
+    return ns ? (size_t)b * kPrunedWarps * ns * 32 * 5 * sizeof(float) + 256 : 0;
 }
 
 extern "C" int prb_furthest_point_sampling(int b, int n, int m, const float *xyz, float *temp, int *idx,
@@ -657,69 +648,35 @@ static int fps_run(int b, int n, int m, const float *xyz, float *temp, int *idx,
 
     // exact pruned kernel (one CTA per scene) when the caller lent scratch memory
     if (const int ns = pruned_slots(n); ns && workspace && m > 1) {
-        const size_t np = (size_t)16 * ns * 32;
+        const size_t np = (size_t)kPrunedWarps * ns * 32;
         PRB_REQUIRE(workspace_bytes >= (size_t)b * np * 5 * sizeof(float) + 256, "fps: workspace of %zu bytes is too small", workspace_bytes);
         FpsSorted s;
         float *w = reinterpret_cast<float *>(((uintptr_t)workspace + 255) & ~(uintptr_t)255);
         s.sx = w; s.sy = w + b * np; s.sz = w + 2 * b * np; s.st = w + 3 * b * np;
         s.srank = reinterpret_cast<int *>(w + 4 * b * np);
         s.np = (int)np;
-        const int thr = opts().fps_threads;            // 0 / 512: 16 warps (default); 1024: 32 warps x half the slots
-        switch (ns) {
-            case 8: return thr == 1024 ? launch_pruned<4, 32>(p, s, st) : launch_pruned<8, 16>(p, s, st);
-            case 16: return thr == 1024 ? launch_pruned<8, 32>(p, s, st) : launch_pruned<16, 16>(p, s, st);
-            default: return thr == 1024 ? launch_pruned<16, 32>(p, s, st) : launch_pruned<32, 16>(p, s, st);
-        }
+        return ns == 16 ? launch_pruned<16>(p, s, st) : launch_pruned<32>(p, s, st);
     }
 
     // configuration: cluster size, threads per CTA, points per thread
     // A cluster of CS CTAs per scene cuts the per-round compute CS-fold; each CTA mirrors only its own slice of the
-    // scene in shared memory (<= 48 KB); large batches use smaller clusters so that CTAs do not start sharing SMs.
-    int cs = opts().fps_cluster;
-    if (cs != 0 && n_pad < 4096) cs = 1;       // the override is meant for the big levels only
-    if (cs == 0) {
-        cs = 1;
-        if (n_pad >= 8192) {
-            cs = (long)b * 8 <= num_sms() / 2 ? 8 : 4;
-            while (cs > 1 && (long)b * cs > 2L * num_sms()) cs >>= 1;
-        }
+    // scene in shared memory (<= 96 KB); large batches use smaller clusters so that CTAs do not start sharing SMs.
+    int cs = 1;
+    if (n_pad >= 8192) {
+        cs = (long)b * 8 <= num_sms() / 2 ? 8 : 4;
+        while (cs > 1 && (long)b * cs > 2L * num_sms()) cs >>= 1;
     }
     while (cs < 8 && ceil_div(n_pad, cs) > 8192) cs <<= 1;  // keep the register-resident path
-    while (cs > 1 && (n_pad % (cs * 128)) != 0) cs >>= 1;
-    int P = ceil_div(n_pad, cs);
-    int threads = opts().fps_threads;
-    if (threads == 0) {
-        threads = 128;
-        while (threads < 512 && threads * 4 < P) threads <<= 1;
-        if (threads * 16 < P) threads = 1024;
-    }
-    int ppt = 1;
-    while (threads * ppt < P) ppt <<= 1;
-    bool generic = (ppt > 16) || (threads == 1024 && ppt > 8) || opts().fps_generic;
-    // round (threads, ppt) to an instantiated pair
-    if (!generic) {
-        if (threads == 128 && ppt > 4) { threads = 256; ppt = ppt / 2; }
-        if (threads == 256 && ppt < 4) ppt = 4;
-        if (threads == 256 && ppt > 8) { threads = 512; ppt = ppt / 2; }
-        if (threads == 512 && ppt < 2) ppt = 2;
-        if (threads == 1024 && ppt < 4) ppt = 4;
-    }
-    if (generic) {
+    const int P = ceil_div(n_pad, cs);
+    if (P > 8192) {                                          // more than 65536 points
         fps_generic_kernel<<<b, p.S < 32 ? 32 : p.S, 0, st>>>(p);
         return check_launch("fps_generic_kernel");
     }
-    // shared copy of the CTA's own coordinates: whole (padded) scene for a single CTA, one slice in a cluster
-    size_t smem_pts = (size_t)threads * ppt * 3 * sizeof(float);
-    p.use_smem_xyz = (cs > 1 || smem_pts <= 200 * 1024) ? 1 : 0;
-    size_t smem = p.use_smem_xyz ? smem_pts : 0;
-    switch (cs) {
-        case 1: return dispatch_cs<1>(p, threads, ppt, smem, st);
-        case 2: return dispatch_cs<2>(p, threads, ppt, smem, st);
-        case 4: return dispatch_cs<4>(p, threads, ppt, smem, st);
-        case 8: return dispatch_cs<8>(p, threads, ppt, smem, st);
-    }
-    set_error("fps: bad cluster size %d", cs);
-    return -1;
+    int threads = 128;
+    while (threads < 512 && threads * 4 < P) threads <<= 1;
+    int ppt = 1;
+    while (threads * ppt < P) ppt <<= 1;
+    return dispatch_rank(p, cs, threads, ppt, st);
 }
 
 // ------------------------------------------------------------------------------------------------------------

@@ -37,10 +37,6 @@ static int env_int(const char *name, int dflt) {
 // process defaults: built-in values, overridden ONCE (first use) by PRB_* environment variables for experiment scripts
 static prb_options make_defaults() {
     prb_options o;
-    o.fps_cluster = env_int("PRB_FPS_CS", 0);
-    o.fps_prune = env_int("PRB_FPS_PRUNE", 1);
-    o.fps_threads = env_int("PRB_FPS_THREADS", 0);
-    o.fps_generic = env_int("PRB_FPS_GENERIC", 0);
     o.mlp_occ = env_int("PRB_MLP_OCC", 0);
     o.mlp_sms = env_int("PRB_MLP_SMS", 0);
     o.mlp_resident = env_int("PRB_MLP_RESIDENT", 1);

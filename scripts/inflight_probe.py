@@ -7,19 +7,17 @@ net = bench.build_model(dev)
 pool = [torch.from_numpy(bench.make_scenes(16 * i, 16)).to(dev) for i in range(8)]
 with torch.no_grad():
     for F in (1, 2, 3):
-        for cs in ("0", "2", "4"):
-            os.environ["PRB_FPS_CS"] = cs
-            streams = [torch.cuda.Stream() for _ in range(F)]
-            for i in range(6):
-                with torch.cuda.stream(streams[i % F]): net(pool[i % 8])
-            torch.cuda.synchronize()
-            K = 24
-            t0 = torch.cuda.Event(enable_timing=True); t1 = torch.cuda.Event(enable_timing=True)
-            t0.record()
-            for s in streams: s.wait_event(t0)
-            for i in range(K):
-                with torch.cuda.stream(streams[i % F]): net(pool[i % 8])
-            for s in streams: torch.cuda.current_stream().wait_stream(s)
-            t1.record(); torch.cuda.synchronize()
-            ms = t0.elapsed_time(t1) / K
-            print("inflight", F, "fps_cs", cs, "ms/batch %.3f" % ms, "scenes/s %.0f" % (16 / ms * 1e3), flush=True)
+        streams = [torch.cuda.Stream() for _ in range(F)]
+        for i in range(6):
+            with torch.cuda.stream(streams[i % F]): net(pool[i % 8])
+        torch.cuda.synchronize()
+        K = 24
+        t0 = torch.cuda.Event(enable_timing=True); t1 = torch.cuda.Event(enable_timing=True)
+        t0.record()
+        for s in streams: s.wait_event(t0)
+        for i in range(K):
+            with torch.cuda.stream(streams[i % F]): net(pool[i % 8])
+        for s in streams: torch.cuda.current_stream().wait_stream(s)
+        t1.record(); torch.cuda.synchronize()
+        ms = t0.elapsed_time(t1) / K
+        print("inflight", F, "ms/batch %.3f" % ms, "scenes/s %.0f" % (16 / ms * 1e3), flush=True)

@@ -94,7 +94,7 @@ def test_oracle_roipool_matches_reference_cpu_twin_semantics():
 
 
 # ------------------------------------------------------------------------------------------------ C ABI
-def test_cabi_library_exports_every_declared_symbol_at_abi_10():
+def test_cabi_library_exports_every_declared_symbol_at_abi_11():
     from pointrcnn_b200 import _cabi
     lib = _cabi.lib()
     hdr = open(os.path.join(ROOT, "include", "pointrcnn_b200.h")).read()
@@ -102,7 +102,7 @@ def test_cabi_library_exports_every_declared_symbol_at_abi_10():
     assert len(names) >= 25
     for n in names:
         assert hasattr(lib, n), "libpointrcnn_b200.so does not export %s" % n
-    assert lib.prb_abi_version() == 10
+    assert lib.prb_abi_version() == 11
     assert lib.prb_launch_count() == 0
     # and the other way round: nothing is exported that the header does not declare
     import subprocess
@@ -242,7 +242,7 @@ def test_unfused_module_math_on_cpu_group_all():
     np.testing.assert_allclose(out[:, :, 0].numpy(), want, rtol=1e-5, atol=1e-5)
 
 
-def test_options_struct_matches_the_header_at_abi_10():
+def test_options_struct_matches_the_header_at_abi_11():
     """ctypes mirror of struct prb_options: same fields, same order as include/pointrcnn_b200.h"""
     import re
     from pointrcnn_b200 import _cabi
@@ -255,4 +255,4 @@ def test_options_struct_matches_the_header_at_abi_10():
     assert names == [f[0] for f in _cabi.Options._fields_]
     o = _cabi.Options()
     _cabi.lib().prb_options_init(ctypes.byref(o))
-    assert o.fps_prune == 1 and o.mlp_resident == 1
+    assert (o.mlp_occ, o.mlp_sms, o.mlp_resident, o.nn_sort_queries) == (0, 0, 1, 0)

@@ -15,11 +15,11 @@ from pointrcnn_b200.pointnet2 import sa_train
 from pointrcnn_b200.pointnet2.pointnet2_modules import PointnetSAModule, PointnetSAModuleMSG
 
 
-def test_sa_train_symbols_resolve_at_abi_10():
+def test_sa_train_symbols_resolve_at_abi_11():
     lib = C.lib()
     for name in ("prb_sa_train_workspace_bytes", "prb_sa_train_forward", "prb_sa_train_backward"):
         assert getattr(lib, name) is not None
-    assert lib.prb_abi_version() == 10
+    assert lib.prb_abi_version() == 11
     d = C.SATrainDesc(num_layers=3, c_in=4)
     d.c_out[:] = [16, 16, 32]
     fwd = lib.prb_sa_train_workspace_bytes(16, 4096, 32, 1, ctypes.byref(d), 0)

@@ -10,12 +10,12 @@ from pointrcnn_b200 import config
 from pointrcnn_b200.train import losses as L
 
 
-def test_stage_loss_symbols_resolve_at_abi_10():
+def test_stage_loss_symbols_resolve_at_abi_11():
     lib = C.lib()
     for name in ("prb_stage_loss_workspace_bytes", "prb_stage_loss_forward", "prb_stage_loss_backward"):
         assert getattr(lib, name) is not None
     assert lib.prb_stage_loss_workspace_bytes(16 * 16384) > 0
-    assert lib.prb_abi_version() == 10
+    assert lib.prb_abi_version() == 11
 
 
 def test_descriptor_layout_matches_the_header():

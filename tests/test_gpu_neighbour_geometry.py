@@ -1,7 +1,7 @@
 """FPS, ball query and 3-NN on the device, bit for bit against the CPU oracle, on the adversarial families of
 tests/neighbour_reference.py at the batch-16 shapes of the network: every scene batch mixes one scene of each family
-with ray-cast LiDAR scenes.  Every kernel path a prb_option selects is compared with the same oracle result, computed
-once per module."""
+with ray-cast LiDAR scenes.  Every kernel path a prb_option or the batch size selects is compared with the same oracle
+result, computed once per module."""
 import numpy as np
 import pytest
 import torch
@@ -215,10 +215,13 @@ def test_three_nn_batch_equals_per_scene(cuda, nn_cases):
 
 
 # ------------------------------------------------------------------------------------------------ FPS
+FPS_SHAPES = [(16384, 4096), (8192, 2048), (32768, 1024), (4097, 1024), (70000, 512)]
+
+
 @pytest.fixture(scope="module")
 def fps_cases():
     out = {}
-    for n, m in ((16384, 4096), (4097, 1024)):
+    for n, m in FPS_SHAPES:
         xyz, _ = batch(n, 1, (0.5, 1.0), 500 + n)
         xyz[3] = NR.sphere_around_zero(n, 3)                  # a tie of n - 1 points in the first round
         want, temp = O.fps(xyz, m, return_temp=True)
@@ -226,27 +229,44 @@ def fps_cases():
     return out
 
 
-FPS_OPTS = {"default": {}, "prune1": {"fps_prune": 1}, "prune2": {"fps_prune": 2}, "prune_1024": {"fps_prune": 1, "fps_threads": 1024},
-            "cluster1": {"fps_prune": 0, "fps_cluster": 1}, "cluster2": {"fps_prune": 0, "fps_cluster": 2},
-            "cluster4": {"fps_prune": 0, "fps_cluster": 4}, "cluster8": {"fps_prune": 0, "fps_cluster": 8},
-            "generic": {"fps_prune": 0, "fps_generic": 1}}
+def fps_plain(x, m):
+    """(idx, new_xyz, temp) of prb_furthest_point_sampling: no scratch, so no scene takes the pruned kernel"""
+    b, n, _ = x.shape
+    temp = torch.full((b, n), 1e10, device=x.device)
+    idx = torch.empty((b, m), dtype=torch.int32, device=x.device)
+    new_xyz = torch.empty((b, m, 3), device=x.device)
+    _cabi.check(_cabi.lib().prb_furthest_point_sampling(b, n, m, _cabi.ptr(x), _cabi.ptr(temp), _cabi.ptr(idx), _cabi.ptr(new_xyz),
+                                                        _cabi.stream()), "furthest_point_sampling")
+    return idx, new_xyz, temp
 
 
-@pytest.mark.parametrize("n,m", [(16384, 4096), (4097, 1024)])
-@pytest.mark.parametrize("variant", list(FPS_OPTS))
-def test_fps_bits_on_adversarial_families(cuda, fps_cases, n, m, variant):
+# How each path runs the batch, by point count (132 SMs).  "ws": the entries that lend scratch -- the pruned kernel for
+# 4097-16384 points.  The plain entry's rank kernel, with CS CTAs per scene: "plain_b16" -- CS 4; "plain_b8", the first 8
+# scenes -- CS 8; "plain_tiled", the 16 scenes repeated to 96 -- CS 2 up to 16384 points, CS 4 at 32768.
+# 4097 points run one CTA per scene (512 threads x 16 ranks) and 70000 the generic kernel, whatever the path.
+@pytest.mark.parametrize("n,m", FPS_SHAPES)
+@pytest.mark.parametrize("path", ["ws", "plain_b16", "plain_b8", "plain_tiled"])
+def test_fps_bits_on_adversarial_families(cuda, fps_cases, n, m, path):
     xyz, want, want_temp = fps_cases[(n, m)]
+    if path == "plain_b8":
+        xyz, want, want_temp = xyz[:8], want[:8], want_temp[:8]
+    elif path == "plain_tiled":
+        reps = 3 * torch.cuda.get_device_properties(0).multi_processor_count // 4 // B
+        xyz, want, want_temp = (np.tile(a, (reps,) + (1,) * (a.ndim - 1)) for a in (xyz, want, want_temp))
+    b = len(xyz)
     x = T(xyz, cuda)
-    with _cabi.options(**FPS_OPTS[variant]):
+    if path == "ws":
         idx, new_xyz = pu.furthest_point_sample_xyz(x, m, ordered=False)
-        temp = torch.full((B, n), 1e10, device=cuda)
-        idx2 = torch.empty((B, m), dtype=torch.int32, device=cuda)
-        pointnet2_cuda.furthest_point_sampling_wrapper(B, n, m, x, temp, idx2)
+        temp = torch.full((b, n), 1e10, device=cuda)
+        idx2 = torch.empty((b, m), dtype=torch.int32, device=cuda)
+        pointnet2_cuda.furthest_point_sampling_wrapper(b, n, m, x, temp, idx2)
+        assert torch.equal(idx, idx2)
+    else:
+        idx, new_xyz, temp = fps_plain(x, m)
     got = idx.cpu().numpy()
     bad = np.where(np.any(got != want, axis=1))[0]
     assert bad.size == 0, "scenes %s differ from the oracle" % bad.tolist()
-    assert torch.equal(idx, idx2)
-    assert np.array_equal(new_xyz.cpu().numpy(), np.stack([xyz[b][want[b]] for b in range(B)]), equal_nan=True)
+    assert np.array_equal(new_xyz.cpu().numpy(), np.stack([xyz[s][want[s]] for s in range(b)]), equal_nan=True)
     assert np.array_equal(temp.cpu().numpy(), want_temp, equal_nan=True)
 
 

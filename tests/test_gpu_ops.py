@@ -4,6 +4,7 @@
 Calls go through the reference-named extension modules / Python wrappers, i.e. through the C ABI.
 """
 import os
+import re
 
 import numpy as np
 import pytest
@@ -43,8 +44,8 @@ FPS_CASES = [
     (7, 128, 32, "dup"),
     (2, 300, 50, "kitti"),        # n not a power of two: S=256, Q=2, holes in the rank space
     (2, 1500, 100, "dup"),        # S=1024, Q=2
-    (1, 20000, 64, "kitti"),      # rank copy does not fit shared memory
-    (2, 16384, 300, "dup"),       # cluster + ties
+    (1, 20000, 64, "kitti"),      # above the pruned kernel's 16384 points: 8-CTA cluster, 512x8
+    (2, 16384, 300, "dup"),       # pruned + ties
     (1, 70, 70, "cube"),          # m == n, tiny
 ]
 
@@ -71,17 +72,83 @@ def test_fps_index_exact(cuda, B, N, M, kind):
         assert np.array_equal(ref_temp.cpu().numpy(), want_temp), "oracle temp != reference temp"
 
 
-@pytest.mark.parametrize("opt", [{"fps_cluster": 1}, {"fps_cluster": 2}, {"fps_cluster": 4}, {"fps_cluster": 8},
-                                 {"fps_generic": 1}, {"fps_cluster": 1, "fps_threads": 1024}, {"fps_prune": 1},
-                                 {"fps_prune": 2, "fps_threads": 1024}])     # pruned kernel, 32 warps x half the slots
-def test_fps_all_kernel_variants_agree(cuda, opt):
-    from pointrcnn_b200 import _cabi
-    xyz = synth.dup_cloud(2, 8192, 5, unique=3000)
-    want = O.fps(xyz, 512)
-    opt = dict({"fps_prune": 0}, **opt)     # the cluster / generic kernels unless the case asks for pruning
-    with _cabi.options(**opt):              # per-thread prb_options, not the process environment
-        got = pu.furthest_point_sample(T(xyz, cuda), 512)
-    assert np.array_equal(got.cpu().numpy(), want)
+def _fps_entry(x, m, ws, t0=None):
+    """(idx, new_xyz, temp) of prb_furthest_point_sampling (ws=False: no scratch, so every scene takes a rank or the
+    generic kernel) or of prb_furthest_point_sampling_ws with the scratch it asks for (pruned kernel for 4097-16384 points)"""
+    from pointrcnn_b200 import _cabi as C
+    lib = C.lib()
+    b, n, _ = x.shape
+    temp = torch.full((b, n), 1e10, device=x.device) if t0 is None else T(t0.copy(), x.device)
+    idx = torch.empty((b, m), dtype=torch.int32, device=x.device)
+    new_xyz = torch.empty((b, m, 3), device=x.device)
+    if ws:
+        wsb = lib.prb_fps_workspace_bytes(b, n)
+        w = torch.empty(wsb, dtype=torch.uint8, device=x.device)
+        C.check(lib.prb_furthest_point_sampling_ws(b, n, m, C.ptr(x), C.ptr(temp), C.ptr(idx), C.ptr(new_xyz), C.ptr(w),
+                                                   C.c_size_t(wsb), C.stream()), "furthest_point_sampling_ws")
+    else:
+        C.check(lib.prb_furthest_point_sampling(b, n, m, C.ptr(x), C.ptr(temp), C.ptr(idx), C.ptr(new_xyz), C.stream()),
+                "furthest_point_sampling")
+    return idx, new_xyz, temp
+
+
+# (id, cluster size the batch size is chosen for, n, m, scratch lent to the _ws entry): rows that reach every FPS kernel
+# the library compiles through its default selection (fps_run).  The rank kernel runs CS CTAs per scene, each holding
+# threads x ranks-per-thread of the n_pad = S*ceil(n/S) ranks; above 65536 points the generic kernel runs, and the _ws
+# entry takes the pruned kernel for 4097-16384 points.
+FPS_TABLE = [
+    ("cs1-128x1", 1, 100, 64, False), ("cs1-128x2", 1, 200, 64, False), ("cs1-128x4", 1, 500, 128, False),
+    ("cs1-256x4", 1, 1000, 256, False), ("cs1-512x4", 1, 2000, 512, False), ("cs1-512x8", 1, 4000, 512, False),
+    ("cs1-512x16", 1, 7000, 512, False),
+    ("cs8-256x4", 8, 8192, 512, False), ("cs8-512x4", 8, 16000, 512, False), ("cs8-512x8", 8, 30000, 512, False),
+    ("cs8-512x16", 8, 65536, 512, False),
+    ("cs4-512x4", 4, 8000, 256, False), ("cs4-512x8", 4, 16384, 256, False), ("cs4-512x16", 4, 30000, 256, False),
+    ("cs2-512x8", 2, 8192, 256, False), ("cs2-512x16", 2, 12000, 256, False),
+    ("generic", 8, 70000, 512, False),
+    ("pruned16", 1, 6000, 512, True), ("pruned32", 1, 16384, 512, True),
+]
+
+
+def _fps_batch(cs):
+    """the batch size a row runs at.  For 8192 ranks or more fps_run gives each scene CS = 8 CTAs while 8b <= SMs/2,
+    else 4, halves CS while b*CS > 2 SMs, then doubles it while a CTA would hold more than 8192 ranks; fewer ranks run
+    one CTA per scene at any batch size."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    return {1: 3, 8: 1, 4: sms // 4, 2: 3 * sms // 4}[cs]
+
+
+@pytest.mark.parametrize("cs,n,m,ws", [r[1:] for r in FPS_TABLE], ids=[r[0] for r in FPS_TABLE])
+def test_fps_all_kernel_variants_agree(cuda, cs, n, m, ws):
+    """every FPS kernel, reached by batch size and point count through the public entries: indices, new_xyz and temp
+    equal the oracle's (and the reference kernel's) bit for bit on a duplicate-heavy cloud"""
+    b = _fps_batch(cs)
+    xyz = synth.dup_cloud(b, n, 5)
+    want, want_temp = O.fps(xyz, m, return_temp=True)
+    x = T(xyz, cuda)
+    idx, new_xyz, temp = _fps_entry(x, m, ws)
+    assert np.array_equal(idx.cpu().numpy(), want)
+    assert np.array_equal(new_xyz.cpu().numpy(), np.stack([xyz[s][want[s]] for s in range(b)]))
+    assert np.array_equal(temp.cpu().numpy(), want_temp)
+    if HAVE_REF:
+        ref, ref_temp = R.fps(x, m, return_temp=True)
+        assert torch.equal(idx, ref) and torch.equal(temp, ref_temp)
+
+
+def test_fps_table_launches_every_fps_kernel(cuda):
+    """the rows of FPS_TABLE launch exactly the sampling kernels the library compiles: 16 rank kernel instances, the two
+    pruned instances with their sort kernel, and the generic kernel"""
+    xs = [T(synth.u_kitti(_fps_batch(cs), n, 7), cuda) for _, cs, n, _, _ in FPS_TABLE]
+    with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+        for x, (_, _, _, m, ws) in zip(xs, FPS_TABLE):
+            _fps_entry(x, m, ws)
+        torch.cuda.synchronize()
+    seen = {re.search(r"fps_\w+(<[^>]*>)?", e.name).group(0) for e in prof.events()
+            if e.device_type == torch.autograd.DeviceType.CUDA and "fps_" in e.name}
+    rank = ["fps_rank_kernel<%d, %d, %d>" % k for k in ((128, 1, 1), (128, 2, 1), (128, 4, 1), (256, 4, 1), (512, 4, 1),
+                                                       (512, 8, 1), (512, 16, 1), (256, 4, 8), (512, 4, 8), (512, 8, 8),
+                                                       (512, 16, 8), (512, 4, 4), (512, 8, 4), (512, 16, 4), (512, 8, 2),
+                                                       (512, 16, 2))]
+    assert seen == set(rank + ["fps_pruned_kernel<16>", "fps_pruned_kernel<32>", "fps_sort_kernel", "fps_generic_kernel"])
 
 
 ORDERED_CASES = [
@@ -223,7 +290,7 @@ def test_backbone_takes_the_ordered_shortcut(cuda):
     assert torch.equal(f_a, f_b) and torch.equal(xyz_a, xyz_b)
 
 
-def test_options_are_thread_local(cuda):
+def test_options_are_thread_local_at_abi_11(cuda):
     """SURVEY 8(b): natives are re-entered from nn.DataParallel worker threads; one thread's prb_options must not leak"""
     import threading
     from pointrcnn_b200 import _cabi
@@ -232,14 +299,14 @@ def test_options_are_thread_local(cuda):
     def worker():
         o = _cabi.Options()
         _cabi.lib().prb_get_thread_options(ctypes.byref(o))
-        seen["worker"] = (o.fps_cluster, o.fps_prune)
+        seen["worker"] = (o.mlp_resident, o.mlp_sms)
     import ctypes
-    with _cabi.options(fps_cluster=8, fps_prune=0):
+    with _cabi.options(mlp_resident=0, mlp_sms=8):
         t = threading.Thread(target=worker); t.start(); t.join()
         o = _cabi.Options()
         _cabi.lib().prb_get_thread_options(ctypes.byref(o))
-        seen["main"] = (o.fps_cluster, o.fps_prune)
-    assert seen["main"] == (8, 0) and seen["worker"] != (8, 0)
+        seen["main"] = (o.mlp_resident, o.mlp_sms)
+    assert seen["main"] == (0, 8) and seen["worker"] != (0, 8)
 
 
 def test_fps_temp_writeback_and_m_edge(cuda):
@@ -255,9 +322,11 @@ def test_fps_temp_writeback_and_m_edge(cuda):
     assert torch.count_nonzero(one) == 0
 
 
-@pytest.mark.parametrize("N,M,prune", [(6000, 300, 1), (16384, 1000, 1), (3000, 200, 2)])
-def test_fps_pruned_kernel_resumes_from_caller_temp(cuda, N, M, prune):
-    """temp is in/out (sampling_gpu.cu:105-111): a caller-initialised temp steers the sampling and gets the final minima"""
+@pytest.mark.parametrize("N,M", [(6000, 300), (16384, 1000), (3000, 200)])
+@pytest.mark.parametrize("entry", ["ws", "plain"])
+def test_fps_pruned_kernel_resumes_from_caller_temp(cuda, N, M, entry):
+    """temp is in/out (sampling_gpu.cu:105-111): a caller-initialised temp steers the sampling and gets the final minima.
+    The wrapper lends scratch (pruned kernel for 6000 and 16384 points); the plain entry runs the rank kernels."""
     from pointrcnn_b200.ext import pointnet2_cuda
     xyz = synth.u_kitti(2, N, 17)
     rng = np.random.default_rng(5)
@@ -265,11 +334,12 @@ def test_fps_pruned_kernel_resumes_from_caller_temp(cuda, N, M, prune):
     t0[:, ::7] = 1e10
     want, want_temp = O.fps(xyz, M, return_temp=True, temp0=t0)
     x = T(xyz, cuda)
-    temp = T(t0.copy(), cuda)
-    idx = torch.empty((2, M), dtype=torch.int32, device=cuda)
-    from pointrcnn_b200 import _cabi
-    with _cabi.options(fps_prune=prune):
+    if entry == "ws":
+        temp = T(t0.copy(), cuda)
+        idx = torch.empty((2, M), dtype=torch.int32, device=cuda)
         pointnet2_cuda.furthest_point_sampling_wrapper(2, N, M, x, temp, idx)
+    else:
+        idx, _, temp = _fps_entry(x, M, False, t0)
     assert np.array_equal(idx.cpu().numpy(), want)
     assert np.array_equal(temp.cpu().numpy(), want_temp)
     if HAVE_REF:
