@@ -515,6 +515,39 @@ PRB_API int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *
                                  int aug_flip, float rot_lo, float rot_hi, float flip_prob, int pts_raw_ry, float reg_fg_thresh,
                                  float cls_fg_thresh, float cls_bg_thresh, unsigned seed, float *gt_boxes_ct, int *cls_label,
                                  int *reg_valid_mask, void *stream);
+/* The same two stages with the seed read from device memory (`seed`: one unsigned, read at kernel start) instead of passed
+ * by value; with *seed equal to the value, the outputs are the host-seed entries' bit for bit.  A CUDA graph that captured
+ * them draws new samples on each replay when the captured sequence also advances *seed. */
+PRB_API int prb_rcnn_sample_rois_dseed(int b, int m, int g, const float *iou, const float *rois, const int *roi_count,
+                                       const float *gt_boxes, const int *gt_count, int roi_per_image, int fg_per_image,
+                                       float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh, float cls_bg_thresh_lo,
+                                       double hard_bg_ratio, int aug_method, int gt_max_fg, int fg_aug_times, int bg_aug_times,
+                                       int kept_src_iou, float pool_extra_width, const unsigned *seed, float *rois_out,
+                                       float *gt_out, float *iou_out, float *pool_boxes, int *sel, int *status, void *stream);
+PRB_API int prb_rcnn_roi_targets_dseed(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
+                                       const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
+                                       int aug_flip, float rot_lo, float rot_hi, float flip_prob, int pts_raw_ry, float reg_fg_thresh,
+                                       float cls_fg_thresh, float cls_bg_thresh, const unsigned *seed, float *gt_boxes_ct,
+                                       int *cls_label, int *reg_valid_mask, void *stream);
+
+/* ------------------------------------------------------------------ optimizer step ------
+ * prb_adam_true_wd_step: the step of the fastai OptimWrapper(true_wd=True) around Adam for n fp32 tensors, one launch, no
+ * host synchronisation.  hyper (device, 3 doubles): lr, beta1, beta2.  Per element, in this order: p *= (float)(1 -
+ * weight_decay * lr) (the factor in double, rounded once); then torch's fused Adam arithmetic in fp32 with weight decay 0:
+ * m = fma(b1, m, fma(-b1, g, g)), v = fma(b2, v, fma(-b2, g*g, g*g)), p -= (lr / (1 - b1^t)) * m / (sqrt(v) / sqrt(1 -
+ * b2^t) + eps), where b1, b2, lr, eps are rounded to float and t = *step.  The caller increments every step counter before
+ * the call, as torch does.  Each tensor: contiguous device fp32 param / grad / exp_avg / exp_avg_sq of numel elements and
+ * its fp32 step counter; `tensors` is a device array.  n <= 65535. */
+typedef struct prb_adam_tensor {
+    float *param;
+    const float *grad;
+    float *exp_avg;
+    float *exp_avg_sq;
+    const float *step;
+    long long numel;
+} prb_adam_tensor;
+PRB_API int prb_adam_true_wd_step(int n, const prb_adam_tensor *tensors, const double *hyper, double weight_decay, double eps,
+                                  void *stream);
 
 /* ------------------------------------------------------------------ evaluation statistics ------
  * The recall, segmentation IoU and classification accuracy of tools/eval_rcnn.py's three evaluation loops

@@ -82,6 +82,9 @@ def lib():
         L.prb_rcnn_sample_rois.argtypes = [I, I, I, P, P, P, P, P, I, I, F, F, F, F, ctypes.c_double, I, I, I, I, I, F, U, P, P, P, P, P, P,
                                            P]
         L.prb_rcnn_roi_targets.argtypes = [I, I, I, I, P, P, P, P, P, I, I, I, I, F, F, F, I, F, F, F, U, P, P, P, P]
+        L.prb_rcnn_sample_rois_dseed.argtypes = [P if t is U else t for t in L.prb_rcnn_sample_rois.argtypes]
+        L.prb_rcnn_roi_targets_dseed.argtypes = [P if t is U else t for t in L.prb_rcnn_roi_targets.argtypes]
+        L.prb_adam_true_wd_step.argtypes = [I, P, P, ctypes.c_double, ctypes.c_double, P]
         L.prb_eval_box_recall.argtypes = [I, I, P, P, I, P, P, I, ctypes.POINTER(F), P, P, P, P]
         L.prb_eval_cls_acc.argtypes = [I, I, P, P, P, F, F, F, P, P, P]
         L.prb_stage_loss_workspace_bytes.argtypes = [I]

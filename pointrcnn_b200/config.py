@@ -42,6 +42,11 @@ _DEFAULTS = dict(
 _local = threading.local()
 
 
+def names():
+    """every switch, in a fixed order"""
+    return tuple(sorted(_DEFAULTS))
+
+
 def get(name):
     ov = getattr(_local, "ov", None)
     if ov and name in ov:

@@ -108,7 +108,9 @@ struct RsCfg {
 __global__ void __launch_bounds__(kRsThreads) rcnn_sample_kernel(
     int m, int g, RsCfg cf, const float *__restrict__ iou, const float *__restrict__ rois, const int *__restrict__ roi_count,
     const float *__restrict__ gts, const int *__restrict__ gt_count, float *__restrict__ rois_out, float *__restrict__ gt_out,
-    float *__restrict__ iou_out, float *__restrict__ pool_boxes, int *__restrict__ sel, int *__restrict__ status) {
+    float *__restrict__ iou_out, float *__restrict__ pool_boxes, int *__restrict__ sel, int *__restrict__ status,
+    const unsigned *__restrict__ seed_dev) {
+    if (seed_dev) cf.seed = *seed_dev;       // the device-seed entry: a counter a captured graph advances between replays
     extern __shared__ __align__(16) unsigned char s_raw[];
     float *s_maxov = reinterpret_cast<float *>(s_raw);        // m
     int *s_gtas = reinterpret_cast<int *>(s_maxov + m);       // m
@@ -296,7 +298,8 @@ struct RtCfg {
 __global__ void __launch_bounds__(kRtThreads) rcnn_targets_kernel(
     int R, int S, int W, RtCfg cf, float *__restrict__ rows, float *__restrict__ rois, float *__restrict__ gts,
     const float *__restrict__ iou, const int *__restrict__ empty, float *__restrict__ gt_ct, int *__restrict__ cls_label,
-    int *__restrict__ reg_valid) {
+    int *__restrict__ reg_valid, const unsigned *__restrict__ seed_dev) {
+    if (seed_dev) cf.seed = *seed_dev;
     const int k = blockIdx.x, scene = k / R, r = k - scene * R, tid = threadIdx.x;
     float rb[7], gb[7];
 #pragma unroll
@@ -372,12 +375,12 @@ __global__ void __launch_bounds__(kRtThreads) rcnn_targets_kernel(
 
 using namespace prb;
 
-extern "C" int prb_rcnn_sample_rois(int b, int m, int g, const float *iou, const float *rois, const int *roi_count,
-                                    const float *gt_boxes, const int *gt_count, int roi_per_image, int fg_per_image,
-                                    float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh, float cls_bg_thresh_lo,
-                                    double hard_bg_ratio, int aug_method, int gt_max_fg, int fg_aug_times, int bg_aug_times,
-                                    int kept_src_iou, float pool_extra_width, unsigned seed, float *rois_out, float *gt_out,
-                                    float *iou_out, float *pool_boxes, int *sel, int *status, void *stream) {
+static int rcnn_sample_rois(int b, int m, int g, const float *iou, const float *rois, const int *roi_count, const float *gt_boxes,
+                            const int *gt_count, int roi_per_image, int fg_per_image, float reg_fg_thresh, float cls_fg_thresh,
+                            float cls_bg_thresh, float cls_bg_thresh_lo, double hard_bg_ratio, int aug_method, int gt_max_fg,
+                            int fg_aug_times, int bg_aug_times, int kept_src_iou, float pool_extra_width, unsigned seed,
+                            const unsigned *seed_dev, float *rois_out, float *gt_out, float *iou_out, float *pool_boxes, int *sel,
+                            int *status, void *stream) {
     PRB_REQUIRE(b > 0 && m >= 0 && g >= 0 && rois_out && gt_out && iou_out && pool_boxes && sel && status && (m == 0 || rois) &&
                     (g == 0 || gt_boxes) && (m == 0 || g == 0 || iou),
                 "rcnn_sample_rois: bad arguments");
@@ -395,15 +398,15 @@ extern "C" int prb_rcnn_sample_rois(int b, int m, int g, const float *iou, const
     const size_t smem = (size_t)(6 * m + 3 * g) * 4;
     PRB_CUDA(cudaFuncSetAttribute(rcnn_sample_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(smem > 0 ? smem : 4)));
     rcnn_sample_kernel<<<b, kRsThreads, smem, (cudaStream_t)stream>>>(m, g, cf, iou, rois, roi_count, gt_boxes, gt_count, rois_out,
-                                                                       gt_out, iou_out, pool_boxes, sel, status);
+                                                                       gt_out, iou_out, pool_boxes, sel, status, seed_dev);
     return check_launch("rcnn_sample_kernel");
 }
 
-extern "C" int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
-                                    const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
-                                    int aug_flip, float rot_lo, float rot_hi, float flip_prob, int pts_raw_ry, float reg_fg_thresh,
-                                    float cls_fg_thresh, float cls_bg_thresh, unsigned seed, float *gt_boxes_ct, int *cls_label,
-                                    int *reg_valid_mask, void *stream) {
+static int rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes, const float *iou,
+                            const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling, int aug_flip, float rot_lo,
+                            float rot_hi, float flip_prob, int pts_raw_ry, float reg_fg_thresh, float cls_fg_thresh,
+                            float cls_bg_thresh, unsigned seed, const unsigned *seed_dev, float *gt_boxes_ct, int *cls_label,
+                            int *reg_valid_mask, void *stream) {
     PRB_REQUIRE(b > 0 && roi_per_image > 0 && S > 0 && W >= 3 && rows && rois && gt_boxes && iou && empty_flag && gt_boxes_ct &&
                     cls_label && reg_valid_mask,
                 "rcnn_roi_targets: bad arguments");
@@ -413,6 +416,53 @@ extern "C" int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, floa
     RtCfg cf{aug_data != 0, aug_rotation != 0, aug_scaling != 0, aug_flip != 0, pts_raw_ry != 0, rot_lo, rot_hi, flip_prob,
              reg_fg_thresh, cls_fg_thresh, cls_bg_thresh, seed};
     rcnn_targets_kernel<<<b * roi_per_image, kRtThreads, 0, (cudaStream_t)stream>>>(roi_per_image, S, W, cf, rows, rois, gt_boxes, iou,
-                                                                                      empty_flag, gt_boxes_ct, cls_label, reg_valid_mask);
+                                                                                      empty_flag, gt_boxes_ct, cls_label, reg_valid_mask,
+                                                                                      seed_dev);
     return check_launch("rcnn_targets_kernel");
+}
+
+extern "C" int prb_rcnn_sample_rois(int b, int m, int g, const float *iou, const float *rois, const int *roi_count,
+                                    const float *gt_boxes, const int *gt_count, int roi_per_image, int fg_per_image,
+                                    float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh, float cls_bg_thresh_lo,
+                                    double hard_bg_ratio, int aug_method, int gt_max_fg, int fg_aug_times, int bg_aug_times,
+                                    int kept_src_iou, float pool_extra_width, unsigned seed, float *rois_out, float *gt_out,
+                                    float *iou_out, float *pool_boxes, int *sel, int *status, void *stream) {
+    return rcnn_sample_rois(b, m, g, iou, rois, roi_count, gt_boxes, gt_count, roi_per_image, fg_per_image, reg_fg_thresh,
+                            cls_fg_thresh, cls_bg_thresh, cls_bg_thresh_lo, hard_bg_ratio, aug_method, gt_max_fg, fg_aug_times,
+                            bg_aug_times, kept_src_iou, pool_extra_width, seed, nullptr, rois_out, gt_out, iou_out, pool_boxes, sel,
+                            status, stream);
+}
+
+extern "C" int prb_rcnn_sample_rois_dseed(int b, int m, int g, const float *iou, const float *rois, const int *roi_count,
+                                          const float *gt_boxes, const int *gt_count, int roi_per_image, int fg_per_image,
+                                          float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh, float cls_bg_thresh_lo,
+                                          double hard_bg_ratio, int aug_method, int gt_max_fg, int fg_aug_times, int bg_aug_times,
+                                          int kept_src_iou, float pool_extra_width, const unsigned *seed, float *rois_out,
+                                          float *gt_out, float *iou_out, float *pool_boxes, int *sel, int *status, void *stream) {
+    PRB_REQUIRE(seed, "rcnn_sample_rois_dseed: seed is NULL");
+    return rcnn_sample_rois(b, m, g, iou, rois, roi_count, gt_boxes, gt_count, roi_per_image, fg_per_image, reg_fg_thresh,
+                            cls_fg_thresh, cls_bg_thresh, cls_bg_thresh_lo, hard_bg_ratio, aug_method, gt_max_fg, fg_aug_times,
+                            bg_aug_times, kept_src_iou, pool_extra_width, 0u, seed, rois_out, gt_out, iou_out, pool_boxes, sel,
+                            status, stream);
+}
+
+extern "C" int prb_rcnn_roi_targets(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
+                                    const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
+                                    int aug_flip, float rot_lo, float rot_hi, float flip_prob, int pts_raw_ry, float reg_fg_thresh,
+                                    float cls_fg_thresh, float cls_bg_thresh, unsigned seed, float *gt_boxes_ct, int *cls_label,
+                                    int *reg_valid_mask, void *stream) {
+    return rcnn_roi_targets(b, roi_per_image, S, W, rows, rois, gt_boxes, iou, empty_flag, aug_data, aug_rotation, aug_scaling, aug_flip,
+                            rot_lo, rot_hi, flip_prob, pts_raw_ry, reg_fg_thresh, cls_fg_thresh, cls_bg_thresh, seed, nullptr,
+                            gt_boxes_ct, cls_label, reg_valid_mask, stream);
+}
+
+extern "C" int prb_rcnn_roi_targets_dseed(int b, int roi_per_image, int S, int W, float *rows, float *rois, float *gt_boxes,
+                                          const float *iou, const int *empty_flag, int aug_data, int aug_rotation, int aug_scaling,
+                                          int aug_flip, float rot_lo, float rot_hi, float flip_prob, int pts_raw_ry,
+                                          float reg_fg_thresh, float cls_fg_thresh, float cls_bg_thresh, const unsigned *seed,
+                                          float *gt_boxes_ct, int *cls_label, int *reg_valid_mask, void *stream) {
+    PRB_REQUIRE(seed, "rcnn_roi_targets_dseed: seed is NULL");
+    return rcnn_roi_targets(b, roi_per_image, S, W, rows, rois, gt_boxes, iou, empty_flag, aug_data, aug_rotation, aug_scaling, aug_flip,
+                            rot_lo, rot_hi, flip_prob, pts_raw_ry, reg_fg_thresh, cls_fg_thresh, cls_bg_thresh, 0u, seed, gt_boxes_ct,
+                            cls_label, reg_valid_mask, stream);
 }

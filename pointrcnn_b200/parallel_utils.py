@@ -46,7 +46,11 @@ class GradBucketReducer:
     compute stream wait for the side stream (the averaged gradients are then in place for the optimizer step).
     Over NVSwitch a 12 MB reduction is latency-bound (tens of microseconds): bucket count trades launch latency against
     overlap, 4 MB buckets give 3-4 collectives per RPN step.  Works on CPU / gloo as well (no streams: collectives run
-    inline) for the world-size-2 tests."""
+    inline) for the world-size-2 tests.
+
+    Under CUDA-graph capture (the trainers' cuda_graph=True) the side stream is the fork / join capture needs: reset()'s
+    zeroing of the buckets, the event waits and the collectives the hooks enqueue are captured with the step, and a replay
+    re-runs exactly those; the hooks and their Python bookkeeping run only while capturing."""
 
     def __init__(self, params, world=None, bucket_mb=4.0, process_group=None):
         self.params = [p for p in params if p.requires_grad]

@@ -78,6 +78,13 @@ class RCNNStage(nn.Module):
         self._fused_rows = None
         return super()._apply(fn, *args, **kwargs)
 
+    def invalidate_fused(self):
+        """call after editing weights without bumping their versions (`.data` edits, CUDA graph replays): drops the packed
+        row chains and every SA module's chain"""
+        self._fused_rows = None
+        for m in self.SA_modules:
+            m.invalidate_fused()
+
     def _rows_fusable(self, pts_input):
         if config.get("disable_fused") or not pts_input.is_cuda or pts_input.dtype != torch.float32 or not pts_input.is_contiguous():
             return False

@@ -79,12 +79,14 @@ def layer_recipe(cfg):
                   flip_prob=0.5, pts_raw_ry=1, **_shared(cfg))
 
 
-def run(recipe, xyz, feat, rois, gts, counts, seed):
+def run(recipe, xyz, feat, rois, gts, counts, seed, seed_dev=None):
     """the recipe on one batch, on the current stream and without a host synchronisation: prb_boxes_iou3d (skipped when M
     or G is 0), prb_rcnn_sample_rois, prb_roipool3d_ws on the enlarged sampled boxes, prb_rcnn_roi_targets.
     xyz (B,N,3), feat (B,N,F), rois (B,M,7), gts (B,G,7): contiguous float32 CUDA tensors; counts (2,B) int32
-    [roi_count; gt_count], required by a recipe with counts and ignored otherwise.  -> dict of the raw outputs, R =
-    ROI_PER_IMAGE, S = NUM_POINTS: pooled (B,R,S,3+F) transformed rows, empty (B,R) int32, pool_boxes (B,R,7) the boxes the
+    [roi_count; gt_count], required by a recipe with counts and ignored otherwise.  seed_dev: None, or a CUDA int32 tensor
+    whose first element the sample and targets launches read as the seed in place of `seed` (the _dseed entries: a
+    captured graph that advances it draws anew on every replay).  -> dict of the raw outputs, R = ROI_PER_IMAGE, S =
+    NUM_POINTS: pooled (B,R,S,3+F) transformed rows, empty (B,R) int32, pool_boxes (B,R,7) the boxes the
     rows were pooled from, rois / gts (B,R,7) after augmentation, iou (B,R) before it, sel (B,R,3) int32, status (B) int32, gt_ct (B*R,7), cls / reg (B*R) int32"""
     if recipe.counts and counts is None:
         raise ValueError("rcnn targets: this recipe takes the RoI and GT counts")
@@ -93,7 +95,6 @@ def run(recipe, xyz, feat, rois, gts, counts, seed):
     R, S, F_ = rc.roi_per_image, rc.num_points, feat.shape[2]
     W = 3 + F_
     dev = rois.device
-    seed &= 0xffffffff
     L, st = C.lib(), C.stream()
     f = lambda *shp: torch.empty(shp, dtype=torch.float32, device=dev)
     i32 = lambda *shp: torch.empty(shp, dtype=torch.int32, device=dev)
@@ -103,11 +104,14 @@ def run(recipe, xyz, feat, rois, gts, counts, seed):
     rois_out, gt_out, iou_out, pool_boxes = f(B, R, 7), f(B, R, 7), f(B, R), f(B, R, 7)
     sel, status = i32(B, R, 3), i32(B)
     roi_count, gt_count = (counts[0], counts[1]) if rc.counts else (None, None)
-    C.check(L.prb_rcnn_sample_rois(B, M, G, C.ptr(iou), C.ptr(rois), C.ptr(roi_count), C.ptr(gts), C.ptr(gt_count), R, rc.fg_per_image,
-                                   rc.reg_fg_thresh, rc.cls_fg_thresh, rc.cls_bg_thresh, rc.cls_bg_thresh_lo, rc.hard_bg_ratio,
-                                   rc.aug_method, rc.gt_max_fg, rc.fg_aug_times, rc.bg_aug_times, rc.kept_src_iou, rc.pool_extra_width,
-                                   seed, C.ptr(rois_out), C.ptr(gt_out), C.ptr(iou_out), C.ptr(pool_boxes), C.ptr(sel), C.ptr(status),
-                                   st), "rcnn_sample_rois")
+    if seed_dev is None:
+        sample, finish, seed = L.prb_rcnn_sample_rois, L.prb_rcnn_roi_targets, seed & 0xffffffff
+    else:
+        sample, finish, seed = L.prb_rcnn_sample_rois_dseed, L.prb_rcnn_roi_targets_dseed, C.ptr(seed_dev)
+    C.check(sample(B, M, G, C.ptr(iou), C.ptr(rois), C.ptr(roi_count), C.ptr(gts), C.ptr(gt_count), R, rc.fg_per_image, rc.reg_fg_thresh,
+                   rc.cls_fg_thresh, rc.cls_bg_thresh, rc.cls_bg_thresh_lo, rc.hard_bg_ratio, rc.aug_method, rc.gt_max_fg,
+                   rc.fg_aug_times, rc.bg_aug_times, rc.kept_src_iou, rc.pool_extra_width, seed, C.ptr(rois_out), C.ptr(gt_out),
+                   C.ptr(iou_out), C.ptr(pool_boxes), C.ptr(sel), C.ptr(status), st), "rcnn_sample_rois")
     pooled = f(B, R, S, W)
     empty = torch.zeros((B, R), dtype=torch.int32, device=dev)
     wsb = L.prb_roipool3d_workspace_bytes(B, N, R, S)
@@ -115,8 +119,7 @@ def run(recipe, xyz, feat, rois, gts, counts, seed):
     C.check(L.prb_roipool3d_ws(B, N, R, F_, S, C.ptr(xyz), C.ptr(pool_boxes), C.ptr(feat), C.ptr(pooled), C.ptr(empty), None, 1,
                                C.ptr(ws), C.c_size_t(wsb), st), "roipool3d")
     gt_ct, cls, reg = f(B * R, 7), i32(B * R), i32(B * R)
-    C.check(L.prb_rcnn_roi_targets(B, R, S, W, C.ptr(pooled), C.ptr(rois_out), C.ptr(gt_out), C.ptr(iou_out), C.ptr(empty), rc.aug_data,
-                                   rc.aug_rotation, rc.aug_scaling, rc.aug_flip, rc.rot_lo, rc.rot_hi, rc.flip_prob, rc.pts_raw_ry,
-                                   rc.reg_fg_thresh, rc.cls_fg_thresh, rc.cls_bg_thresh, seed, C.ptr(gt_ct), C.ptr(cls), C.ptr(reg), st),
-            "rcnn_roi_targets")
+    C.check(finish(B, R, S, W, C.ptr(pooled), C.ptr(rois_out), C.ptr(gt_out), C.ptr(iou_out), C.ptr(empty), rc.aug_data, rc.aug_rotation,
+                   rc.aug_scaling, rc.aug_flip, rc.rot_lo, rc.rot_hi, rc.flip_prob, rc.pts_raw_ry, rc.reg_fg_thresh, rc.cls_fg_thresh,
+                   rc.cls_bg_thresh, seed, C.ptr(gt_ct), C.ptr(cls), C.ptr(reg), st), "rcnn_roi_targets")
     return dict(pooled=pooled, empty=empty, pool_boxes=pool_boxes, rois=rois_out, gts=gt_out, iou=iou_out, sel=sel, status=status, gt_ct=gt_ct, cls=cls, reg=reg)

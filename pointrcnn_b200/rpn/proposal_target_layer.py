@@ -23,9 +23,10 @@ With draw="device" (or draw=None and config switch target_draw = "device") the w
 host read: rcnn/targets.py runs prb_boxes_iou3d, csrc/rcnn_sample.cu's sample stage, prb_roipool3d_ws and the targets
 stage in the layer's recipe (targets.layer_recipe).  Random draws are counter-based hashes of
 (seed, scene, stage, row, try, slot): the reference's distribution, not its stream.  The seed is the layer's call
-counter unless forward(..., seed=) gives one.  Extra output keys: sample_status (B) int32 (0 ok, 1 no fg and no bg RoI --
-the reference stops in pdb --, 2 no GT -- the reference raises; such a scene's rows have cls_label -1 and
-reg_valid_mask 0) and sample_index (B * ROI_PER_IMAGE, 3) int32 [source RoI, GT, jitter tries].
+counter unless forward(..., seed=) gives one.  After use_device_seed() the seed is a device int32 counter instead, which
+each call reads and then advances on the device, so a CUDA graph that captured the call draws anew on every replay.
+Extra output keys: sample_status (B) int32 (0 ok, 1 no fg and no bg RoI -- the reference stops in pdb --, 2 no GT -- the
+reference raises; such a scene's rows have cls_label -1 and reg_valid_mask 0) and sample_index (B * ROI_PER_IMAGE, 3) int32 [source RoI, GT, jitter tries].
 """
 import numpy as np
 import torch
@@ -65,6 +66,12 @@ class ProposalTargetLayer(nn.Module):
         self.cfg = cfg
         self.draw = draw
         self.calls = 0
+        self.seed_counter = None
+
+    def use_device_seed(self, device):
+        """draw="device" calls without seed= read their seed from a device int32 counter, started at the call count, and
+        advance it on the device"""
+        self.seed_counter = torch.full((1,), self.calls, dtype=torch.int32, device=device)
 
     def _pts_feature(self, input_dict):
         """[intensity?, seg_mask, pts_depth / 70 - 0.5?, rpn_features] (:19-32)"""
@@ -79,10 +86,11 @@ class ProposalTargetLayer(nn.Module):
         draw = self.draw or config.get("target_draw")
         if draw not in DRAWS:
             raise ValueError("target_draw must be one of %s, not %r" % (DRAWS, draw))
+        explicit = seed is not None
         seed = self.calls if seed is None else seed
         self.calls += 1
         if draw == "device":
-            return self.forward_device(input_dict, seed)
+            return self.forward_device(input_dict, seed if explicit or self.seed_counter is None else None)
         cfg = self.cfg
         roi_boxes3d, gt_boxes3d = input_dict['roi_boxes3d'], input_dict['gt_boxes3d']
         batch_rois, batch_gt_of_rois, batch_roi_iou = self.sample_rois_for_rcnn(roi_boxes3d, gt_boxes3d)
@@ -120,7 +128,7 @@ class ProposalTargetLayer(nn.Module):
     def forward_device(self, input_dict, seed):
         """forward() in four device launches and no host read: 3D IoU of every (RoI, GT) pair, the sample stage (selection +
         jitter loop), RoI pooling on the enlarged jittered boxes, the targets stage (augmentation, labels, canonical
-        transform).  Same keys and shapes as the torch path, plus sample_status and sample_index."""
+        transform).  seed None: the device counter's value, which the call then advances.  Same keys and shapes as the torch path, plus sample_status and sample_index."""
         recipe = targets.layer_recipe(self.cfg)
         rois = input_dict['roi_boxes3d'][:, :, 0:7].contiguous().float()
         gts = input_dict['gt_boxes3d'][:, :, 0:7].contiguous().float()
@@ -128,7 +136,10 @@ class ProposalTargetLayer(nn.Module):
         C.require_cuda(rois, gts, xyz)
         with torch.cuda.device(rois.device):
             feat = self._pts_feature(input_dict).contiguous().float()
-            o = targets.run(recipe, xyz, feat, rois, gts, None, seed)
+            counter = self.seed_counter if seed is None else None
+            o = targets.run(recipe, xyz, feat, rois, gts, None, 0 if seed is None else seed, seed_dev=counter)
+            if counter is not None:
+                counter.add_(1)
         rows = o["pooled"].view(-1, recipe.num_points, o["pooled"].shape[3])
         return {'sampled_pts': rows[:, :, 0:3], 'pts_feature': rows[:, :, 3:], 'cls_label': o["cls"].long(), 'reg_valid_mask': o["reg"].long(),
                 'gt_of_rois': o["gt_ct"], 'gt_iou': o["iou"].view(-1), 'roi_boxes3d': o["rois"].view(-1, 7), 'sample_status': o["status"],

@@ -118,37 +118,100 @@ class TrueWDAdam:
     """OptimWrapper.create(partial(Adam, betas=(0.9, 0.99)), lr, layer_groups, wd=wd, true_wd=True, bn_wd=True): a
     torch.optim.Adam with weight_decay=0 over `groups`, preceded in step() by the decoupled decay p *= 1 - wd * lr.  The
     schedule writes lr and beta1 into every group (set()); state_dict() is the inner Adam's, as the reference's checkpoints
-    hold it.  Not AdamW: its decay lives in the groups, and a reference optimizer_state (weight_decay=0) would switch it off."""
+    hold it.  Not AdamW: its decay lives in the groups, and a reference optimizer_state (weight_decay=0) would switch it off.
 
-    def __init__(self, groups, lr, mom, wd=WEIGHT_DECAY, fused=False):
+    graph=True (for CUDA parameters): every group's lr and betas are 1-element float64 CUDA tensors (views of one
+    [lr, beta1, beta2] tensor) that set() fills in place, and step() is one prb_adam_true_wd_step launch that reads them on
+    the device, so a CUDA graph that captured it follows the schedule.  It computes the bits the eager step computes (the
+    decay factor from the double lr, then torch's fused Adam arithmetic).  state_dict() holds Python floats either way."""
+
+    def __init__(self, groups, lr, mom, wd=WEIGHT_DECAY, fused=False, graph=False):
         self.opt = torch.optim.Adam([{"params": g, "lr": 0} for g in groups], betas=(0.9, BETA2), **({"fused": True} if fused else {}))
         self.wd = wd
+        self.graph = graph
+        self._table = None
+        if graph:
+            dev = next(p.device for g in groups for p in g)
+            self.hyper = torch.tensor([0.0, 0.9, BETA2], dtype=torch.float64, device=dev)
+            self._install_hyper()
         self.set(lr, mom)
+
+    def _install_hyper(self):
+        for group in self.opt.param_groups:
+            group["lr"], group["betas"] = self.hyper[0:1], (self.hyper[1:2], self.hyper[2:3])
 
     @property
     def param_groups(self):
         return self.opt.param_groups
 
     def set(self, lr, mom):
+        if self.graph:
+            self.hyper[0:1].fill_(lr)
+            self.hyper[1:2].fill_(mom)
+            return
         for group in self.opt.param_groups:
             group["lr"], group["betas"] = lr, (mom, group["betas"][1])
 
     @torch.no_grad()
     def step(self):
+        if self.graph:
+            return self._step_device()
         for group in self.opt.param_groups:
             ps = [p for p in group["params"] if p.requires_grad]
             if ps:
                 torch._foreach_mul_(ps, 1 - self.wd * group["lr"])
         self.opt.step()
 
+    def _tensors(self):
+        """the trained parameters (requires_grad) with their Adam state, created as torch's fused Adam creates it"""
+        out = []
+        for group in self.opt.param_groups:
+            for p in group["params"]:
+                if not p.requires_grad:
+                    continue
+                if p.grad is None or p.dtype != torch.float32 or not (p.is_contiguous() and p.grad.is_contiguous()):
+                    raise ValueError("TrueWDAdam(graph=True) steps contiguous fp32 parameters that all have a gradient")
+                st = self.opt.state[p]
+                if not st:
+                    st["step"] = torch.zeros((), dtype=torch.float32, device=p.device)
+                    st["exp_avg"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                    st["exp_avg_sq"] = torch.zeros_like(p, memory_format=torch.preserve_format)
+                out.append((p, st))
+        return out
+
+    def _step_device(self):
+        from .. import _cabi as C
+        if self._table is None:
+            ts = self._tensors()
+            rows = [[p.data_ptr(), p.grad.data_ptr(), st["exp_avg"].data_ptr(), st["exp_avg_sq"].data_ptr(), st["step"].data_ptr(),
+                     p.numel()] for p, st in ts]
+            self._table = (torch.tensor(rows, dtype=torch.int64).reshape(-1, 6).to(self.hyper.device), [st["step"] for _, st in ts])
+        table, steps = self._table
+        if steps:
+            torch._foreach_add_(steps, 1)
+        eps = self.opt.param_groups[0]["eps"]
+        with torch.cuda.device(self.hyper.device):
+            C.check(C.lib().prb_adam_true_wd_step(len(steps), C.ptr(table), C.ptr(self.hyper), float(self.wd), float(eps), C.stream()),
+                    "adam_true_wd_step")
+
     def zero_grad(self, set_to_none=True):
         self.opt.zero_grad(set_to_none)
 
     def state_dict(self):
-        return self.opt.state_dict()
+        sd = self.opt.state_dict()
+        if self.graph:
+            lr, b1, b2 = self.hyper.tolist()
+            for group in sd["param_groups"]:
+                group["lr"], group["betas"] = lr, (b1, b2)
+        return sd
 
     def load_state_dict(self, state_dict):
         self.opt.load_state_dict(state_dict)
+        if self.graph:
+            g = self.opt.param_groups[0]
+            self.hyper.copy_(torch.tensor([float(g["lr"]), float(g["betas"][0]), float(g["betas"][1])], dtype=torch.float64))
+            self._install_hyper()
+            self._table = None
 
 
 def _load(path):
@@ -204,7 +267,8 @@ def fit(trainer, batches_per_epoch, epochs, start_it=0, start_epoch=0, ckpt_dir=
     loss and loss terms stay on the device and reach the host in one copy at the epoch's end.
     -> one dict per epoch: {'loss': (iters,) array, term name: (iters,) array}.  Row k of every array is iteration k of
     the epoch; a term an iteration did not return (the torch loss path has no regression terms without a foreground
-    point) is NaN there."""
+    point) is NaN there.  A trainer built with cuda_graph=True replays its captured step here; its steps return fresh
+    tensors, so every row holds its own iteration, and the schedule hooks reach the replays through device tensors."""
     it = start_it
     history = []
     for epoch in range(start_epoch, epochs):

@@ -10,6 +10,18 @@ supports through csrc/sa_train.cu instead, see pointnet2/sa_train.py.)  What thi
 loop: no `.item()` inside the loss, per-rank processes instead of nn.DataParallel's per-step replicate / scatter / gather,
 and the bucketed all-reduce of `parallel_utils.GradBucketReducer` overlapped with backward.
 
+CUDA graphs (cuda_graph=True, both trainers' step()): the first call runs eager (it creates the optimizer state and warms
+cuDNN and the allocator), the next captures the whole step -- forward, loss, backward, the bucketed all-reduce, gradient
+clipping and the optimizer step -- into a torch.cuda.CUDAGraph and replays it once, and later calls copy their inputs
+into the graph's static buffers and replay it.  One graph per key of what a replay cannot change (input shapes and
+dtypes, grad_norm_clip, the autocast state and dtype, torch's deterministic flag, the BatchNorm momenta, the config
+switches), so a new key captures again.  The returned loss and terms are fresh tensors, not the graph's outputs.  The
+schedule reaches replays through device tensors (lr, and beta1 of "adam_onecycle"), the RCNN target layer through a
+device seed counter; after a replay the trained modules' fused eval caches are dropped.  Loading a checkpoint
+(recipe.load_checkpoint, load_part) drops the graphs: the next step runs eager again and the one after captures.  A step
+that cannot be captured (torch loss path, torch target draw, autocast with its weight-cast cache, a CPU device) raises
+ValueError before anything is captured (INTEGRATION.md, "Training steps as CUDA graphs").
+
 Mixed precision: call a trainer's step inside `with torch.autocast("cuda", dtype=torch.bfloat16):`.  The forward's
 convolutions then run with bfloat16 operands, the grouping / gather / interpolation natives move bfloat16 features, the
 device SA / FP / loss paths and both losses compute in fp32; backward, the all-reduce and the optimizer step run with
@@ -43,6 +55,26 @@ def _sa_switch(sa_train, fp_train=None):
 def _without_autocast():
     """the backward / all-reduce / optimizer part of a step: with CUDA autocast disabled when the caller enabled it"""
     return torch.autocast("cuda", enabled=False) if torch.is_autocast_enabled("cuda") else contextlib.nullcontext()
+
+
+def _resolved(value, switch):
+    return value or config.get(switch)
+
+
+def _graph_refusal(device, loss_impl, target_draw=False):
+    """why a cuda_graph=True trainer cannot capture its step (None: it can); target_draw False: no target layer.  The
+    trainers check the values they were given at construction, and the resolved ones (a switch left to None follows the
+    config) at every step, before anything is captured"""
+    if device.type != "cuda":
+        return "cuda_graph=True needs a CUDA device, not %s" % device
+    if _resolved(loss_impl, "loss_impl") != "device":
+        return "cuda_graph=True needs loss_impl='device': the torch loss path reads boolean masks on the host"
+    if target_draw is not False and _resolved(target_draw, "target_draw") != "device":
+        return "cuda_graph=True needs target_draw='device': the torch target layer reads its samples on the host"
+    if torch.is_autocast_enabled("cuda") and torch.is_autocast_cache_enabled():
+        return ("cuda_graph=True under autocast needs torch.autocast(..., cache_enabled=False): a cached weight cast "
+                "cannot be captured")
+    return None
 
 
 def _schedule(optimizer, total_steps, lr):
@@ -79,12 +111,100 @@ class _Recipe:
         fused = self.device.type == "cuda"
         if schedule is None:
             self.opt = torch.optim.Adam(self.params, lr=lr, weight_decay=weight_decay, **({"fused": True} if fused else {}))
+            if self._graph_mode():
+                self._lr_tensor = torch.full((1,), lr, dtype=torch.float32, device=self.device)
+                self._graph_groups()
+                self.opt.register_load_state_dict_post_hook(lambda opt: self._graph_groups(reload=True))
         else:
-            self.opt = recipe.TrueWDAdam(recipe.param_groups(self.net), *schedule.initial, wd=weight_decay, fused=fused)
+            self.opt = recipe.TrueWDAdam(recipe.param_groups(self.net), *schedule.initial, wd=weight_decay, fused=fused,
+                                         graph=self._graph_mode())
+
+    def _graph_mode(self):
+        return getattr(self, "cuda_graph", False)
+
+    def _graph_groups(self, reload=False):
+        """cuda_graph with optimizer="adam": torch's fused Adam reading lr from a float32 CUDA tensor (capturable, as torch
+        requires for capture).  reload: after load_state_dict, which puts the file's float lr and flags in the groups"""
+        for group in self.opt.param_groups:
+            if reload:
+                self._lr_tensor.fill_(float(group["lr"]))
+            group["lr"], group["capturable"] = self._lr_tensor, True
 
     def _set_lr(self, lr):
+        if self._graph_mode():
+            self._lr_tensor.fill_(lr)
+            return
         for group in self.opt.param_groups:
             group["lr"] = lr
+
+    def _init_graphs(self, cuda_graph):
+        self.cuda_graph = bool(cuda_graph)
+        self._graphs = {}
+        self._warm = False
+        self._stream = None
+        if self.cuda_graph:
+            self.net.register_load_state_dict_post_hook(lambda module, keys: self.drop_graphs())
+
+    def drop_graphs(self):
+        """forget every captured step: the next step() runs eager again (it rebuilds what the load replaced: optimizer
+        state, packed eval weights) and the one after captures.  Loading a state dict into self.net does this"""
+        self._graphs.clear()
+        self._warm = False
+
+    def graph_key(self, inputs, grad_norm_clip):
+        """everything a replay of the captured step cannot change: input shapes and dtypes, the clip, the CUDA autocast
+        state and dtype, torch's deterministic flag (and warn_only), the BatchNorm momenta that cuDNN and the device
+        SA / FP kernels take as host values, and the config switches the step reads while it is traced (a switch the
+        trainer was given counts with its own value)"""
+        autocast = (torch.is_autocast_enabled("cuda"), torch.get_autocast_dtype("cuda") if torch.is_autocast_enabled("cuda") else None)
+        momenta = tuple(m.momentum for m in self.model.modules() if isinstance(m, recipe.BN_TYPES))
+        own = {k: getattr(self, k, None) for k in ("sa_train", "fp_train", "loss_impl", "target_draw")}
+        switches = tuple((k, own.get(k) or config.get(k)) for k in config.names())
+        return (tuple((tuple(t.shape), t.dtype) for t in inputs), grad_norm_clip, autocast,
+                torch.are_deterministic_algorithms_enabled(), torch.is_deterministic_algorithms_warn_only_enabled(), momenta,
+                switches)
+
+    def _run_step(self, forward_loss, args, grad_norm_clip):
+        self.reducer.reset()
+        loss, terms = forward_loss(*args)
+        with _without_autocast():
+            loss.backward()
+            self.reducer.finish()
+            if grad_norm_clip:
+                torch.nn.utils.clip_grad_norm_(self.params, grad_norm_clip)     # train_utils.py: clip_grad_norm_(.., GRAD_NORM_CLIP)
+            self.opt.step()
+        return loss.detach(), terms
+
+    def _graphed_step(self, forward_loss, inputs, grad_norm_clip):
+        """one step of a cuda_graph trainer: eager on the first call, then capture (once per graph_key) and replay"""
+        refusal = _graph_refusal(self.device, self.loss_impl, getattr(self, "target_draw", False))
+        if refusal:
+            raise ValueError(refusal)
+        if not self._warm:
+            # on the capture stream: autograd keeps each parameter's gradient accumulator, with the stream it was created
+            # on, for as long as anything holds this step's graph, and a capture may not join work on another stream
+            self._warm = True
+            if self._stream is None:
+                self._stream = torch.cuda.Stream(self.device)
+            self._stream.wait_stream(torch.cuda.current_stream(self.device))
+            with torch.cuda.stream(self._stream):
+                loss, terms = self._run_step(forward_loss, inputs, grad_norm_clip)
+            torch.cuda.current_stream(self.device).wait_stream(self._stream)
+            return loss, {k: v.detach() for k, v in terms.items()}
+        key = self.graph_key(inputs, grad_norm_clip)
+        entry = self._graphs.get(key)
+        if entry is None:
+            static = tuple(t.detach().clone() for t in inputs)
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph, stream=self._stream):
+                loss, terms = self._run_step(forward_loss, static, grad_norm_clip)
+            entry = self._graphs[key] = (graph, static, (loss, {k: v.detach() for k, v in terms.items()}))
+        graph, static, (loss, terms) = entry
+        for dst, src in zip(static, inputs):
+            dst.copy_(src, non_blocking=True)
+        graph.replay()
+        self.model.invalidate_fused()             # replays change parameters and BN buffers without bumping their versions
+        return loss.clone(), {k: v.clone() for k, v in terms.items()}
 
     def schedule_epoch(self, epoch, it):
         """the start of `epoch`, `it` iterations into the run (Trainer.train): the BN momentum of `it` (the reference passes
@@ -113,11 +233,17 @@ class RPNTrainer(_Recipe):
     """loss_impl: which stage-loss path forward_loss takes ("torch" / "device", see train.losses; None: the config switch).
     sa_train: which path the SA modules take in training ("torch" / "device", see pointnet2/sa_train.py; None: the config
     switch).  fp_train: the same for the FP modules (see pointnet2/fp_train.py).  optimizer / total_steps: see _Recipe;
-    self.net is the model in the PointRCNN layout (rpn.*) that checkpoints hold"""
+    self.net is the model in the PointRCNN layout (rpn.*) that checkpoints hold.  cuda_graph: replay step() as a CUDA
+    graph (see the module docstring; needs loss_impl="device")"""
 
     def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, loss_impl=None,
-                 sa_train=None, fp_train=None, optimizer="adam", total_steps=None):
+                 sa_train=None, fp_train=None, optimizer="adam", total_steps=None, cuda_graph=False):
         schedule = _schedule(optimizer, total_steps, lr)
+        if cuda_graph:
+            refusal = _graph_refusal(torch.device(device), loss_impl or "device", False)
+            if refusal:
+                raise ValueError(refusal)
+        self.cuda_graph = bool(cuda_graph)
         torch.manual_seed(seed)                       # identical initial weights on every rank
         self.device = torch.device(device)
         self.model = RPNStage(input_channels=input_channels, mode="TRAIN").to(self.device).train()
@@ -130,6 +256,7 @@ class RPNTrainer(_Recipe):
         self.sa_train = sa_train
         self.fp_train = fp_train
         _sa_switch(sa_train, fp_train)
+        self._init_graphs(cuda_graph)
 
     def forward_loss(self, pts_input, rpn_cls_label, rpn_reg_label):
         m = self.model
@@ -140,15 +267,11 @@ class RPNTrainer(_Recipe):
         return rpn_loss(rpn_cls, rpn_reg, rpn_cls_label, rpn_reg_label, self.mean_size, impl=self.loss_impl)
 
     def step(self, pts_input, rpn_cls_label, rpn_reg_label, grad_norm_clip=None):
-        self.reducer.reset()
-        loss, terms = self.forward_loss(pts_input, rpn_cls_label, rpn_reg_label)
-        with _without_autocast():
-            loss.backward()
-            self.reducer.finish()
-            if grad_norm_clip:
-                torch.nn.utils.clip_grad_norm_(self.params, grad_norm_clip)     # train_utils.py: clip_grad_norm_(.., GRAD_NORM_CLIP)
-            self.opt.step()
-        return loss.detach(), terms
+        """one training step -> (loss, loss terms); with cuda_graph a captured replay after the first call"""
+        inputs = (pts_input, rpn_cls_label, rpn_reg_label)
+        if self.cuda_graph:
+            return self._graphed_step(self.forward_loss, inputs, grad_norm_clip)
+        return self._run_step(self.forward_loss, inputs, grad_norm_clip)
 
 
 def synthetic_labels(pts_input, seed=0):
@@ -174,12 +297,22 @@ class RCNNTrainer(_Recipe):
     which stage-loss path every forward_loss* method takes ("torch" / "device", see train.losses; None: the config switch).
     sa_train: which path the RCNN network's SA modules take ("torch" / "device", see pointnet2/sa_train.py; None: the config
     switch).  optimizer / total_steps: see _Recipe; self.net is the PointRCNN layout (rpn.*, rcnn_net.*) that checkpoints
-    hold, and recipe.load_part(self.net, path) loads a phase-1 checkpoint's RPN (--rpn_ckpt)."""
+    hold, and recipe.load_part(self.net, path) loads a phase-1 checkpoint's RPN (--rpn_ckpt).  gt_rows: a GT capacity;
+    step() pads gt_boxes3d to that many rows with zero rows (the target layer trims them as padding, so nothing changes)
+    and raises ValueError for a batch with more.  cuda_graph: replay step() as a CUDA graph (see the module docstring;
+    needs loss_impl="device" and target_draw="device"); step_jit and step_offline, whose point and RoI counts vary per
+    batch, still run eager."""
 
     def __init__(self, input_channels=1, device="cuda", world=1, lr=0.002, weight_decay=0.001, bucket_mb=4.0, seed=0, rpn_score_thresh=0.3,
-                 target_draw=None, loss_impl=None, sa_train=None, optimizer="adam", total_steps=None):
+                 target_draw=None, loss_impl=None, sa_train=None, optimizer="adam", total_steps=None, gt_rows=None, cuda_graph=False):
         from ..rcnn.stage import RCNNStage
+        from ..rpn.proposal_target_layer import ProposalTargetLayer
         schedule = _schedule(optimizer, total_steps, lr)
+        if cuda_graph:
+            refusal = _graph_refusal(torch.device(device), loss_impl or "device", target_draw or "device")
+            if refusal:
+                raise ValueError(refusal)
+        self.cuda_graph = bool(cuda_graph)
         torch.manual_seed(seed)
         self.device = torch.device(device)
         self.rpn = RPNStage(input_channels=input_channels, mode="TRAIN").to(self.device).eval()     # TRAIN quotas: 512 RoIs per scene
@@ -195,7 +328,12 @@ class RCNNTrainer(_Recipe):
         self.target_draw = target_draw
         self.loss_impl = loss_impl
         self.sa_train = sa_train
+        self.gt_rows = gt_rows
         _sa_switch(sa_train)
+        self._init_graphs(cuda_graph)
+        if self.cuda_graph:
+            self.model.proposal_target_layer = ProposalTargetLayer()
+            self.model.proposal_target_layer.use_device_seed(self.device)
 
     @torch.no_grad()
     def rpn_outputs(self, pts_input, gt_boxes3d):
@@ -231,24 +369,25 @@ class RCNNTrainer(_Recipe):
                          impl=self.loss_impl)
 
     def step_offline(self, batch, grad_norm_clip=None):
-        """one offline-recipe training step (tools/train_rcnn.py --train_mode rcnn_offline) on a prepared batch"""
-        return self._step(self.forward_loss_offline, (batch,), grad_norm_clip)
+        """one offline-recipe training step (tools/train_rcnn.py --train_mode rcnn_offline) on a prepared batch; eager also
+        with cuda_graph (the RoI count varies per batch)"""
+        return self._run_step(self.forward_loss_offline, (batch,), grad_norm_clip)
 
     def step_jit(self, batch, grad_norm_clip=None):
         """one training step of tools/train_rcnn.py --train_mode rcnn_offline with ROI_SAMPLE_JIT (the target layer inside
-        the network) on a prepare_jit_batch batch"""
-        return self._step(self.forward_loss_jit, (batch,), grad_norm_clip)
+        the network) on a prepare_jit_batch batch; eager also with cuda_graph (the point and RoI counts vary per batch)"""
+        return self._run_step(self.forward_loss_jit, (batch,), grad_norm_clip)
 
     def step(self, pts_input, gt_boxes3d, grad_norm_clip=None):
-        return self._step(self.forward_loss, (pts_input, gt_boxes3d), grad_norm_clip)
-
-    def _step(self, forward_loss, args, grad_norm_clip):
-        self.reducer.reset()
-        loss, terms = forward_loss(*args)
-        with _without_autocast():
-            loss.backward()
-            self.reducer.finish()
-            if grad_norm_clip:
-                torch.nn.utils.clip_grad_norm_(self.params, grad_norm_clip)
-            self.opt.step()
-        return loss.detach(), terms
+        """one online training step with the RPN fixed -> (loss, loss terms); with cuda_graph a captured replay after the
+        first call"""
+        if self.gt_rows is not None:
+            B, G = gt_boxes3d.shape[0], gt_boxes3d.shape[1]
+            if G > self.gt_rows:
+                raise ValueError("a batch with %d GT rows exceeds gt_rows=%d" % (G, self.gt_rows))
+            if G < self.gt_rows:
+                gt_boxes3d = torch.cat([gt_boxes3d, gt_boxes3d.new_zeros((B, self.gt_rows - G) + tuple(gt_boxes3d.shape[2:]))], dim=1)
+        inputs = (pts_input, gt_boxes3d)
+        if self.cuda_graph:
+            return self._graphed_step(self.forward_loss, inputs, grad_norm_clip)
+        return self._run_step(self.forward_loss, inputs, grad_norm_clip)
